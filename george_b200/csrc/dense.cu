@@ -398,15 +398,13 @@ struct bgp_dense {
   double t_ms[2] = {0, 0};
 };
 
-// outer block width (a multiple of DN_NB); BGP_DENSE_OB overrides the default for tuning runs
+// outer block width (a multiple of DN_NB); BGP_DENSE_OB overrides the default for tuning runs and for tests that run
+// every update level at small n.  Read at every compute(), like the other diagnostic switches.
 static int64_t dense_outer_block() {
-  static int64_t ob = 0;
-  if (ob == 0) {
-    ob = DN_OB;
-    if (const char* e = getenv("BGP_DENSE_OB")) {
-      const long v = atol(e);
-      if (v >= DN_NB && v <= 4096 && v % DN_NB == 0) ob = v;
-    }
+  int64_t ob = DN_OB;
+  if (const char* e = getenv("BGP_DENSE_OB")) {
+    const long v = atol(e);
+    if (v >= DN_NB && v <= 4096 && v % DN_NB == 0) ob = v;
   }
   return ob;
 }
@@ -417,13 +415,10 @@ static int64_t dense_outer_block() {
 // rank-OB update touches everything to the right.  Almost all flops therefore run as GEMMs with K = OB, whose
 // read-modify-write epilogue of C is amortised over 16x more tensor work than at K = 64.
 static int64_t dense_mid_block(int64_t OB) {
-  static int64_t mb = 0;
-  if (mb == 0) {
-    mb = DN_MB;
-    if (const char* e = getenv("BGP_DENSE_MB")) {
-      const long v = atol(e);
-      if (v >= DN_NB && v % DN_NB == 0) mb = v;
-    }
+  int64_t mb = DN_MB;
+  if (const char* e = getenv("BGP_DENSE_MB")) {
+    const long v = atol(e);
+    if (v >= DN_NB && v % DN_NB == 0) mb = v;
   }
   return (mb < OB && OB % mb == 0) ? mb : OB;
 }

@@ -11,6 +11,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
+#include <cstring>
 #include <vector>
 
 #include "common.cuh"
@@ -156,6 +157,25 @@ static int hodlr_solve_dev(bgp_hodlr* h, double* b, int64_t nrhs, int64_t ldb, c
 static int hodlr_exchange_finish(bgp_hodlr* h);
 static int hodlr_finish_top_impl(bgp_hodlr* h, bool allreduce);
 
+// The leaf solve stages a (max_leaf x cols) column group in shared memory: leaves of up to 3200 rows take the default
+// 8 columns, larger ones (a tree whose root is one leaf, N < 2 min_size) the widest of 4, 2, 1 that fits.
+constexpr size_t LS_SMEM_MAX = 200 * 1024;
+constexpr int LS_MAX_LEAF = (int)(LS_SMEM_MAX / sizeof(double));  // 25600 rows: one column still fits
+
+static bool leaf_solve_fits(int max_leaf, int cols) { return sizeof(double) * (size_t)max_leaf * cols <= LS_SMEM_MAX; }
+
+template <int COLS>
+static int leaf_solve_launch(bgp_hodlr* h, double* X, int64_t ldx, const int* ncols_by_depth, int ncols_fixed,
+                             int max_cols, cudaStream_t s) {
+  const dim3 grid((unsigned)h->leaves.size(), (unsigned)((max_cols + COLS - 1) / COLS));
+  const size_t smem = sizeof(double) * (size_t)h->max_leaf * COLS;
+  // (the attribute is per device / context: set it on every call, it is cheap)
+  cudaFuncSetAttribute(leaf_solve_kernel<COLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
+  leaf_solve_kernel<COLS><<<grid, LS_THREADS, smem, s>>>(h->d_leaves.p, h->d_L.p, X, ldx, ncols_by_depth, ncols_fixed, h->max_leaf);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
 static int launch_leaf_solve(bgp_hodlr* h, double* X, int64_t ldx, const int* ncols_by_depth, int ncols_fixed,
                              int max_cols, cudaStream_t s) {
   const int nl = (int)h->leaves.size();
@@ -164,21 +184,16 @@ static int launch_leaf_solve(bgp_hodlr* h, double* X, int64_t ldx, const int* nc
   // instantiation for calls with more than 8 columns (the up-sweep): it streams the leaf factor once per 32 columns
   // instead of once per 8, but at four times the serial work per CTA it measured slower on H100 (up-sweep 3.42 vs 3.36 ms,
   // Matern32 N = 262144) — kept as an experiment.
-  int wide = 0;
-  if (const char* e = getenv("BGP_LEAF_COLS")) wide = (atoi(e) > LS_COLS && max_cols > LS_COLS) ? 1 : 0;
-  const int cols = wide ? LS_COLS_WIDE : LS_COLS;
-  dim3 grid(nl, (max_cols + cols - 1) / cols);
-  const size_t smem = sizeof(double) * (size_t)h->max_leaf * cols;
-  if (smem > 200 * 1024) { set_error("leaf size %d too large for the leaf solve kernel", h->max_leaf); return BGP_ERR_INVALID; }
-  if (wide) {
-    cudaFuncSetAttribute(leaf_solve_kernel<LS_COLS_WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    leaf_solve_kernel<LS_COLS_WIDE><<<grid, LS_THREADS, smem, s>>>(h->d_leaves.p, h->d_L.p, X, ldx, ncols_by_depth, ncols_fixed, h->max_leaf);
-  } else {
-    cudaFuncSetAttribute(leaf_solve_kernel<LS_COLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    leaf_solve_kernel<LS_COLS><<<grid, LS_THREADS, smem, s>>>(h->d_leaves.p, h->d_L.p, X, ldx, ncols_by_depth, ncols_fixed, h->max_leaf);
-  }
-  BGP_LAUNCH_CHECK();
-  return BGP_OK;
+  const int m = h->max_leaf;
+  if (const char* e = getenv("BGP_LEAF_COLS"))
+    if (atoi(e) > LS_COLS && max_cols > LS_COLS && leaf_solve_fits(m, LS_COLS_WIDE))
+      return leaf_solve_launch<LS_COLS_WIDE>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+  if (leaf_solve_fits(m, LS_COLS)) return leaf_solve_launch<LS_COLS>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+  if (leaf_solve_fits(m, 4)) return leaf_solve_launch<4>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+  if (leaf_solve_fits(m, 2)) return leaf_solve_launch<2>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+  if (leaf_solve_fits(m, 1)) return leaf_solve_launch<1>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+  set_error("leaf size %d too large for the leaf solve kernel (at most %d rows)", m, LS_MAX_LEAF);  // compute() rejects it first
+  return BGP_ERR_INVALID;
 }
 
 // one internal level: W = V^T X (both halves), small solve, X -= U T.   factor: up-sweep (X = U panel) vs plain solve
@@ -611,12 +626,20 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
     loff += (int64_t)nd.size * nd.size;
     h->max_leaf = std::max(h->max_leaf, nd.size);
   }
+  if (h->max_leaf > LS_MAX_LEAF) {
+    set_error("leaf size %d too large: the leaf solve handles at most %d rows (N=%lld, min_size=%d); lower min_size",
+              h->max_leaf, LS_MAX_LEAF, (long long)n, o.min_size);
+    return BGP_ERR_INVALID;
+  }
   BGP_TRY(h->d_leaves.reserve(std::max(nl, 1), sA));
   BGP_TRY(h->d_L.reserve((size_t)std::max<int64_t>(loff, 1), sA));
   BGP_TRY(h->d_leaf_logdet.reserve(std::max(nl, 1), sA));
   if (nl) {
     BGP_CUDA(cudaMemcpyAsync(h->d_leaves.p, hleaves.data(), sizeof(LeafDesc) * nl, cudaMemcpyHostToDevice, sA));
-    if (h->max_leaf <= 768) {
+    // BGP_LEAF_FACTOR=generic: the CUDA-core kernel at any leaf size (tests compare the two LDL^T implementations)
+    const char* lf_env = getenv("BGP_LEAF_FACTOR");
+    const bool generic = lf_env && strcmp(lf_env, "generic") == 0;
+    if (h->max_leaf <= 768 && !generic) {
       const int ldp = lf_panel_ld(h->max_leaf);
       const size_t smem = sizeof(double) * (size_t)LF_NB * ldp;
       // (the attribute is per device / context: set it on every call, it is cheap)
@@ -1196,9 +1219,11 @@ int bgp_selftest_lu(int32_t n, int32_t nrhs, const double* S_host, double* R_hos
 }
 
 int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n, int32_t k, const double* A_host,
-                      int64_t lda, const double* B_host, int64_t ldb, double* C_host, int64_t ldc, int32_t atomic_add) {
+                      int64_t lda, const double* B_host, int64_t ldb, double* C_host, int64_t ldc, int32_t mode) {
   BGP_TRY(require_device());
   if (m <= 0 || n <= 0 || k <= 0) { set_error("bgp_selftest_gemm: bad sizes"); return BGP_ERR_INVALID; }
+  if (mode & ~(GD_ATOMIC_ADD | GD_LOWER)) { set_error("bgp_selftest_gemm: bad mode %d", mode); return BGP_ERR_INVALID; }
+  if (a_kcontig && !b_kcontig) { set_error("bgp_selftest_gemm: the (A K-contiguous) x (B N-contiguous) variant is not built"); return BGP_ERR_INVALID; }
   cudaStream_t s = 0;
   const size_t na = (size_t)(a_kcontig ? m : k) * lda, nb = (size_t)(b_kcontig ? n : k) * ldb, nc = (size_t)n * ldc;
   DevBuf<double> dA, dB, dC;
@@ -1208,12 +1233,12 @@ int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n
   BGP_CUDA(cudaMemcpyAsync(dB.p, B_host, sizeof(double) * nb, cudaMemcpyHostToDevice, s));
   BGP_CUDA(cudaMemcpyAsync(dC.p, C_host, sizeof(double) * nc, cudaMemcpyHostToDevice, s));
   GemmDesc g;
-  g.A = dA.p; g.B = dB.p; g.C = dC.p; g.M = m; g.N = n; g.K = k; g.mode = atomic_add ? GD_ATOMIC_ADD : GD_SUB;
+  g.A = dA.p; g.B = dB.p; g.C = dC.p; g.M = m; g.N = n; g.K = k; g.mode = mode;
   g.lda = lda; g.ldb = ldb; g.ldc = ldc;
   BGP_CUDA(cudaMemcpyAsync(dd.p, &g, sizeof(g), cudaMemcpyHostToDevice, s));
-  if (a_kcontig && b_kcontig) BGP_TRY((gemm_dmma_launch<true, true>(dd.p, 1, m, n, nullptr, s)));
-  else if (!a_kcontig && b_kcontig) BGP_TRY((gemm_dmma_launch<false, true>(dd.p, 1, m, n, nullptr, s)));
-  else { set_error("bgp_selftest_gemm: only the (A K-contiguous | M-contiguous) x (B K-contiguous) variants are built here"); return BGP_ERR_INVALID; }
+  if (a_kcontig) BGP_TRY((gemm_dmma_launch<true, true>(dd.p, 1, m, n, nullptr, s)));
+  else if (b_kcontig) BGP_TRY((gemm_dmma_launch<false, true>(dd.p, 1, m, n, nullptr, s)));
+  else BGP_TRY((gemm_dmma_launch<false, false>(dd.p, 1, m, n, nullptr, s)));
   BGP_CUDA(cudaMemcpyAsync(C_host, dC.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;

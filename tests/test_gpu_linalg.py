@@ -40,6 +40,40 @@ def test_dmma_gemm_variants(gpu, m, n, k, a_k):
         np.testing.assert_allclose(got, want, rtol=0, atol=1e-11 * max(1.0, np.sqrt(k)))
 
 
+GD_LOWER = 256
+
+
+@pytest.mark.parametrize("n,e,b,cend", [
+    (2100, 64, 0, 256),      # rank-64 update inside the first MB block
+    (2100, 256, 0, 2048),    # rank-MB update up to the OB boundary
+    (2100, 2048, 0, 2100),   # rank-OB update, ragged 52-row remainder
+    (4161, 2048, 0, 4161),   # rank-OB update of a 2113-row trailing matrix
+    (4161, 4096, 2048, 4161),  # second OB block, 65-row remainder
+    (700, 640, 512, 700),    # rank-128 update of a 60-row tail (small-OB blocking)
+    (577, 576, 512, 577),    # last panel of width 1
+    (129, 64, 0, 128)])      # one row below the update's columns
+def test_dmma_gemm_cholesky_update(gpu, n, e, b, cend):
+    """The <A M-contiguous, B N-contiguous> variant with the lower-only output: exactly the descriptors dense_potrf
+    issues, C[e:n, e:cend) -= L[e:n, b:e) L[e:cend, b:e)^T with A and B the same panel.  Entries above the diagonal
+    are left untouched, in the lower-only and in the full mode."""
+    from george_b200 import _lib
+    lib = _lib.load()
+    rng = np.random.default_rng(n + e + cend)
+    M, N, K = n - e, cend - e, e - b
+    P = np.asfortranarray(rng.normal(size=(M, K)))  # rows e.., columns b..e of the factor (leading dimension M)
+    C0 = np.asfortranarray(rng.normal(size=(M, N)))
+    full = C0 - P @ P[:N].T
+    lower = np.tril(np.ones((M, N), dtype=bool))
+    for mode in (0, GD_LOWER):
+        Cf = C0.copy(order="F")
+        _lib.check(lib.bgp_selftest_gemm(0, 0, M, N, K, _lib.ptr(P), M, _lib.ptr(P), M, _lib.ptr(Cf), M, mode))
+        if mode == GD_LOWER:
+            assert np.array_equal(Cf[~lower], C0[~lower])
+            np.testing.assert_allclose(Cf[lower], full[lower], rtol=0, atol=1e-11 * np.sqrt(K))
+        else:
+            np.testing.assert_allclose(Cf, full, rtol=0, atol=1e-11 * np.sqrt(K))
+
+
 @pytest.mark.parametrize("n,nrhs", [(1, 1), (31, 3), (32, 1), (33, 5), (64, 64), (150, 1), (257, 200), (700, 130)])
 def test_blocked_lu_vs_lapack(gpu, n, nrhs):
     from george_b200 import _lib
