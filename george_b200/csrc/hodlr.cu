@@ -1175,6 +1175,26 @@ int bgp_hodlr_node_pivots(const bgp_hodlr_t* hc, int64_t node, int32_t* rows, in
   return BGP_OK;
 }
 
+// The node's columns [vcol, vcol + rank) of its level's V panel, rows [start, start + size): the up-sweep reads this
+// panel but never writes it (the U panel is the copy it solves in place), so these are the ACA's factors as it left them.
+int bgp_hodlr_node_factors(const bgp_hodlr_t* h, int64_t node, double* out) {
+  if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  if (!h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (h->opts.shard_count > 1) { set_error("node factors are not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  if (node < 0 || node >= (int64_t)h->nodes.size() || h->nodes[node].is_leaf) {
+    set_error("node %lld is not an internal node", (long long)node);
+    return BGP_ERR_INDEX;
+  }
+  const HNode& nd = h->nodes[node];
+  if (nd.rank == 0) return BGP_OK;
+  const LevelInfo& L = h->levels[nd.depth];
+  const PanelSet& ps = h->pset(L);
+  const double* src = ps.vbase() + (int64_t)L.vcol * ps.ld + nd.start;
+  BGP_CUDA(cudaMemcpy2D(out, sizeof(double) * nd.size, src, sizeof(double) * ps.ld, sizeof(double) * nd.size, nd.rank,
+                        cudaMemcpyDeviceToHost));
+  return BGP_OK;
+}
+
 int bgp_hodlr_last_timing(const bgp_hodlr_t* h, double* ms5) {
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
   for (int i = 0; i < 5; ++i) ms5[i] = h->t_ms[i];

@@ -86,7 +86,9 @@ __global__ void __launch_bounds__(LU_PANEL_THREADS) lu_panel_kernel(const LuNode
       if (a > best) { best = a; bi = i; }
     }
     lu_block_argmax(best, bi, red, redi);
-    const int p = bi;
+    // nothing comparable below the diagonal (every entry NaN): no interchange, the NaN pivot carries into log|det| and
+    // the solve, as small_solve_kernel does.  Without this the sentinel index would be used as a row.
+    const int p = bi == 0x7fffffff ? col : bi;
     if (threadIdx.x == 0) nd.piv[col] = p;
     // row interchange inside the panel; stage the new pivot row
     if (threadIdx.x < nb) {

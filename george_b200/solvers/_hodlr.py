@@ -160,6 +160,18 @@ class HODLRSolver(object):
         _lib.check(self._lib.bgp_hodlr_node_pivots(self._ptr, node, _lib.ptr(rows), _lib.ptr(cols)))
         return rows[:rank], cols[:rank]
 
+    def factors(self, node):
+        """``(Vl, Ur)``: the ACA factors of internal node ``node`` (pre-order index), ``(half, rank)`` and
+        ``(size - half, rank)``, with ``K[right, left] ~ Ur @ Vl.T`` (``include/bgp.h: bgp_hodlr_node_factors``)."""
+        self._require_computed()
+        nodes = self.nodes()
+        if not 0 <= node < len(nodes):
+            raise IndexError("node index out of range")
+        nd = nodes[node]
+        out = np.zeros((nd["size"], nd["rank"]), dtype=np.float64, order="F")
+        _lib.check(self._lib.bgp_hodlr_node_factors(self._ptr, node, _lib.ptr(out)))
+        return out[:nd["half"]], out[nd["half"]:]
+
     def timing(self):
         t = (C.c_double * 5)()
         _lib.check(self._lib.bgp_hodlr_last_timing(self._ptr, t))

@@ -268,6 +268,14 @@ int bgp_hodlr_num_nodes(const bgp_hodlr_t* h, int64_t* out);
 int bgp_hodlr_node_info(const bgp_hodlr_t* h, bgp_hodlr_node_info_t* out /* num_nodes */);
 /* ACA pivots of node `node` (pre-order index): rows[k], cols[k] for k < rank, block-relative. */
 int bgp_hodlr_node_pivots(const bgp_hodlr_t* h, int64_t node, int32_t* rows, int32_t* cols);
+/* Diagnostics: the low-rank factors of internal node `node` as the ACA left them (they are not modified afterwards).
+ * out: host buffer (size x rank, column-major, ld size; size and rank from bgp_hodlr_node_info).  Rows [0, half) hold
+ * V_[0] (normalised residual rows, indexed by the left half's columns), rows [half, size) hold U_[1] (residual columns,
+ * indexed by the right half's rows), so the block K[right, left] ~ out[half:, :] out[:half, :]^T.  A dense-fallback node
+ * (exhaust_mode = DENSE) holds V = I and U = the block itself.  Nothing is written for rank 0.  Single-GPU only:
+ * BGP_ERR_INVALID on a sharded factorisation; BGP_ERR_INDEX for a leaf or an out-of-range node; BGP_ERR_NOT_COMPUTED
+ * before compute. */
+int bgp_hodlr_node_factors(const bgp_hodlr_t* h, int64_t node, double* out);
 /* Device-event timings of the last compute, ms: [0] leaves (build+factor; stream A, CONCURRENT with [1]),
  * [1] ACA (stream B, from the start of compute), [2] up-sweep (panel finalisation + leaf solves + level sweeps, from the
  * moment both streams have drained), [3] total compute, [4] last solve.  [3] ~ max([0], [1]) + host gap + [2]. */

@@ -75,6 +75,23 @@ def residual_ld(K, X, B):
     return float(np.sqrt(np.sum(R * R)) / (nk * nx))
 
 
+def residual_ld_blocked(K, X, B, rows=512):
+    """``residual_ld`` with K converted to longdouble ``rows`` rows at a time: the same sums (to longdouble rounding)
+    without a longdouble copy of the whole matrix (1 GB at n = 8194)."""
+    K = np.asarray(K, dtype=np.float64)
+    n = K.shape[0]
+    X = np.asarray(X, dtype=LD).reshape(n, -1)
+    B = np.asarray(B, dtype=LD).reshape(n, -1)
+    r2 = LD(0)
+    k2 = LD(0)
+    for i0 in range(0, n, rows):
+        Kb = K[i0:i0 + rows].astype(LD)
+        R = Kb @ X - B[i0:i0 + rows]
+        r2 += np.sum(R * R)
+        k2 += np.sum(Kb * Kb)
+    return float(np.sqrt(r2) / (np.sqrt(k2) * np.sqrt(np.sum(X * X))))
+
+
 def rel_max(A, Ref):
     """``max|A - Ref| / max|Ref|``, evaluated in longdouble."""
     Ref = np.asarray(Ref, dtype=LD)

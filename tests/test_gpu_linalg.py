@@ -97,6 +97,29 @@ def test_blocked_lu_vs_lapack(gpu, n, nrhs):
     assert abs(ld.value - np.linalg.slogdet(S)[1]) <= 1e-11 * max(1.0, abs(ld.value)) * max(1.0, np.log10(cond))
 
 
+@pytest.mark.parametrize("n,col", [(144, 5), (162, 161)])
+def test_blocked_lu_with_a_nan_column_returns_nan(gpu, n, col):
+    """A Woodbury matrix whose trailing column is NaN below the diagonal (what non-finite kernel values or noise produce)
+    has no comparable pivot candidate there.  The panel kernel keeps the row in place and the NaN reaches log|det| and
+    the solve, as the shared-memory path does; it used to take the arg-max's 'nothing found' sentinel as a row index.
+    The handle stays usable afterwards."""
+    from george_b200 import _lib
+    lib = _lib.load()
+    S = np.eye(n)
+    S[col:, col] = np.nan
+    Sf = np.asfortranarray(S)
+    Rf = np.asfortranarray(np.ones((n, 3)))
+    ld = C.c_double(0.0)
+    _lib.check(lib.bgp_selftest_lu(n, 3, _lib.ptr(Sf), _lib.ptr(Rf), C.byref(ld)))
+    assert np.isnan(ld.value)
+    assert np.all(np.isnan(Rf[col]))
+    # the device is still healthy: a regular system right after
+    S = np.eye(n) + 0.1 * np.random.default_rng(n).normal(size=(n, n)) / np.sqrt(n)
+    Sf, Rf = np.asfortranarray(S), np.asfortranarray(np.ones((n, 1)))
+    _lib.check(lib.bgp_selftest_lu(n, 1, _lib.ptr(Sf), _lib.ptr(Rf), C.byref(ld)))
+    np.testing.assert_allclose(Rf[:, 0], np.linalg.solve(S, np.ones(n)), rtol=0, atol=1e-12)
+
+
 def test_big_rank_levels_match_oracle(gpu, oracle):
     """ExpSquared + ExpSine2 at N = 16384: the reference algorithm's ranks reach ~75 at the top (2r > 142), so the top
     levels take the blocked-LU / DMMA path and the lower ones the shared-memory path."""

@@ -55,6 +55,23 @@ def test_residual_of_extended_solve(n, nrhs):
     assert hiprec.residual_ld(K, Xf, B) <= 1e-15
 
 
+@pytest.mark.parametrize("n,nrhs,rows", [(1, 1, 512), (300, 9, 64), (300, 9, 300), (1031, 2, 512)])
+def test_blocked_residual_matches_unblocked(n, nrhs, rows):
+    """The row-blocked residual (for matrices whose longdouble copy does not fit) sums the same terms; both agree with a
+    float64 evaluation to float64 rounding, and with each other to longdouble rounding."""
+    K = _spd(n, 3 * n)
+    rng = np.random.default_rng(n + rows)
+    X = rng.normal(size=(n, nrhs))
+    B = K @ X + 1e-8 * rng.normal(size=(n, nrhs))  # a residual far above float64 rounding
+    full = hiprec.residual_ld(K, X, B)
+    blocked = hiprec.residual_ld_blocked(K, X, B, rows=rows)
+    assert abs(blocked - full) <= 1e-15 * full
+    f64 = np.linalg.norm(K @ X - B) / (np.linalg.norm(K) * np.linalg.norm(X))
+    assert abs(blocked - f64) <= 1e-3 * f64  # (the float64 product K @ X carries ~1e-14 of that residual's size)
+    if n <= 300:  # an extended-precision solution: the residual is at longdouble rounding
+        assert hiprec.residual_ld_blocked(K, hiprec.solve_ld(hiprec.chol_ld(K), B), B, rows=rows) <= 1e-17
+
+
 def test_not_positive_definite_index():
     K = np.eye(5)
     K[1, 3] = K[3, 1] = 1.0
