@@ -22,6 +22,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libbgp_b200.so")
 
 BGP_OK, BGP_ERR_INVALID, BGP_ERR_DIM, BGP_ERR_NOT_COMPUTED, BGP_ERR_LINALG = 0, 1, 2, 3, 4
 BGP_ERR_CUDA, BGP_ERR_NO_DEVICE, BGP_ERR_RANK_CAPACITY, BGP_ERR_INDEX, BGP_ERR_NOMEM = 5, 6, 7, 8, 9
+BGP_PREDICT_VAR, BGP_PREDICT_COV = 0, 1
 
 
 class BGPError(RuntimeError):
@@ -63,6 +64,8 @@ SIGNATURES = {
     "bgp_kmat_gradient_contract": (C.c_int, [_specp, _p, _p, _i64, _p, _p]),
     "bgp_dense_grad_terms": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_grad_terms": (C.c_int, [_p, _p, _p, _p, _p, _p]),
+    "bgp_dense_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
+    "bgp_hodlr_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
     "bgp_dense_create": (C.c_int, [C.POINTER(_p)]),
     "bgp_dense_destroy": (None, [_p]),
     "bgp_dense_compute": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),

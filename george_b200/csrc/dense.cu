@@ -23,6 +23,15 @@ int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const uns
                               int64_t n, const double* M, int64_t ldm, const double* alpha, double ca, double cm,
                               double* g_dev, double* diag_dev, DevBuf<double>& scratch, cudaStream_t s);
 int fill_identity_launch(double* A, int64_t n, cudaStream_t s);
+int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
+                             int64_t n2, double* out, int64_t ld, cudaStream_t s);
+int kmat_diagonal_launch(const DevProgram* dprog, const double* x1, const double* x2, int64_t n, double* out,
+                         cudaStream_t s);
+int64_t predict_chunk_cols(int64_t n, int64_t multiple);
+int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
+                       double* var, DevBuf<double>& scratch, cudaStream_t s);
+int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
+                     bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
 
 constexpr int DN_NB = 64;   // inner panel width (diagonal block in shared memory)
 constexpr int DN_MB = 256;  // middle block of the delayed-update hierarchy (see dense_potrf)
@@ -535,6 +544,44 @@ static int dense_potrs_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
   return BGP_OK;
 }
 
+// X (n x nrhs, column-major ldx) <- L^-1 X: the forward half of dense_potrs_dev (predictive variance / covariance need
+// only W = L^-1 K(x, x*), since K(x*, x) K^-1 K(x, x*) = W^T W).  Few right-hand sides go through the one-launch step
+// kernels, which leave the result in d_tmp; it is copied back into X.
+static int dense_trsm_fwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
+  const int64_t n = h->n;
+  const double* L = h->d_A.p;
+  cudaStream_t s = h->s;
+  if (nrhs <= DS_MAX_RHS) {
+    BGP_TRY(h->d_tmp.reserve((size_t)n * DS_MAX_RHS, s));
+    double* Y = h->d_tmp.p;
+    for (int64_t k0 = 0; k0 < n; k0 += DN_NB) {
+      const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
+      const int64_t rem = n - k0 - nb;
+      const unsigned g = (unsigned)std::max<int64_t>(1, (rem + DS_ROWS - 1) / DS_ROWS);
+      const int nr = (int)nrhs;
+      if (nr == 1) trsv_fwd_step_kernel<1><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr);
+      else if (nr <= 4) trsv_fwd_step_kernel<4><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr);
+      else trsv_fwd_step_kernel<DS_MAX_RHS><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr);
+      BGP_LAUNCH_CHECK();
+    }
+    BGP_CUDA(cudaMemcpy2DAsync(X, sizeof(double) * ldx, Y, sizeof(double) * n, sizeof(double) * n, nrhs,
+                               cudaMemcpyDeviceToDevice, s));
+    return BGP_OK;
+  }
+  const unsigned cb = (unsigned)((nrhs + 127) / 128);
+  for (int64_t k0 = 0; k0 < n; k0 += DN_NB) {
+    const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
+    trsv_block_kernel<<<cb, 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 0);
+    BGP_LAUNCH_CHECK();
+    const int64_t rem = n - k0 - nb;
+    if (rem <= 0) break;
+    dim3 grid((unsigned)((rem + GM_T - 1) / GM_T), (unsigned)((nrhs + GM_T - 1) / GM_T));
+    gemm_sub_kernel<0, 0><<<grid, 256, 0, s>>>(rem, nrhs, nb, L + k0 * n + k0 + nb, n, X + k0, ldx, X + k0 + nb, ldx, 0, nullptr);
+    BGP_LAUNCH_CHECK();
+  }
+  return BGP_OK;
+}
+
 extern "C" {
 
 int bgp_dense_create(bgp_dense_t** out) {
@@ -709,6 +756,58 @@ int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r,
                                     diag_out ? ddiag : nullptr, h->d_gscratch, s));
   if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
   if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  return BGP_OK;
+}
+
+int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
+                      double* out) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (!h->has_inputs) { set_error("the factor was imported: the handle holds no kernel/coordinates"); return BGP_ERR_NOT_COMPUTED; }
+  if (what != BGP_PREDICT_VAR && what != BGP_PREDICT_COV) { set_error("invalid prediction kind %d", what); return BGP_ERR_INVALID; }
+  if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
+  DevProgram P;
+  BGP_TRY(build_dev_program(spec, &P));
+  if (P.ndim != h->ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", P.ndim, h->ndim); return BGP_ERR_DIM; }
+  if (ns == 0) return BGP_OK;
+  const int64_t n = h->n;
+  const int nd = h->ndim;
+  cudaStream_t s = h->s;
+  DevBuf<DevProgram> dprog;
+  DevBuf<double> dxs, dW, dkd, dvar, dC, scratch;
+  DevBuf<GemmDesc> ddesc;
+  BGP_TRY(upload_program(P, dprog, s));
+  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
+  if (what == BGP_PREDICT_VAR) {
+    // workspace n*c + O(c): var_j = k(x*_j, x*_j) - ||L^-1 K(x, x*_j)||^2, chunk by chunk
+    BGP_TRY(dxs.alloc((size_t)c * nd, s));
+    BGP_TRY(dW.alloc((size_t)n * c, s));
+    BGP_TRY(dkd.alloc((size_t)c, s));
+    BGP_TRY(dvar.alloc((size_t)c, s));
+    for (int64_t j0 = 0; j0 < ns; j0 += c) {
+      const int64_t nc = std::min(c, ns - j0);
+      BGP_CUDA(cudaMemcpyAsync(dxs.p, xs + j0 * nd, sizeof(double) * nc * nd, cudaMemcpyHostToDevice, s));
+      BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p, nc, h->d_x.p, n, dW.p, n, s));  // K(x, x*_chunk), N x nc
+      BGP_TRY(dense_trsm_fwd_dev(h, dW.p, nc, n));
+      BGP_TRY(kmat_diagonal_launch(dprog.p, dxs.p, dxs.p, nc, dkd.p, s));
+      BGP_TRY(predict_var_launch(dW.p, dW.p, n, n, nc, dkd.p, dvar.p, scratch, s));
+      BGP_CUDA(cudaMemcpyAsync(out + j0, dvar.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));
+    }
+  } else {
+    // every W chunk stays resident (n*ns), then C = K** - W^T W (lower, mirrored: exactly symmetric)
+    BGP_TRY(dxs.alloc((size_t)ns * nd, s));
+    BGP_TRY(dW.alloc((size_t)n * ns, s));
+    BGP_TRY(dC.alloc((size_t)ns * ns, s));
+    BGP_CUDA(cudaMemcpyAsync(dxs.p, xs, sizeof(double) * ns * nd, cudaMemcpyHostToDevice, s));
+    BGP_TRY(kmat_symmetric_launch_auto(P, dprog.p, dxs.p, ns, nullptr, dC.p, ns, s));
+    for (int64_t j0 = 0; j0 < ns; j0 += c) {
+      const int64_t nc = std::min(c, ns - j0);
+      BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p + j0 * nd, nc, h->d_x.p, n, dW.p + j0 * n, n, s));
+      BGP_TRY(dense_trsm_fwd_dev(h, dW.p + j0 * n, nc, n));
+    }
+    BGP_TRY(predict_gemm_sub(dW.p, n, dW.p, n, ns, ns, n, true, dC.p, ns, scratch, ddesc, s));
+    BGP_CUDA(cudaMemcpyAsync(out, dC.p, sizeof(double) * ns * ns, cudaMemcpyDeviceToHost, s));
+  }
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;
 }

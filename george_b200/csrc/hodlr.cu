@@ -27,6 +27,17 @@ int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const uns
                               int64_t n, const double* M, int64_t ldm, const double* alpha, double ca, double cm,
                               double* g_dev, double* diag_dev, DevBuf<double>& scratch, cudaStream_t s);
 int fill_identity_launch(double* A, int64_t n, cudaStream_t s);
+int kmat_symmetric_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x, int64_t n,
+                               const double* diag_add, double* out, int64_t ld, cudaStream_t s);
+int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
+                             int64_t n2, double* out, int64_t ld, cudaStream_t s);
+int kmat_diagonal_launch(const DevProgram* dprog, const double* x1, const double* x2, int64_t n, double* out,
+                         cudaStream_t s);
+int64_t predict_chunk_cols(int64_t n, int64_t multiple);
+int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
+                       double* var, DevBuf<double>& scratch, cudaStream_t s);
+int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
+                     bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
 bool comm_ready();
 int comm_rank();
 int comm_world();
@@ -1141,6 +1152,65 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
                                     diag_out ? ddiag : nullptr, h->d_gscratch, s));
   if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
   if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  return BGP_OK;
+}
+
+// GP.predict's variance / covariance on the stored factorisation.  The test points are streamed in chunks of a multiple
+// of 64 columns, so W = K^-1 B is solved in the same 64-column groups as apply_inverse and matches it bit for bit.
+int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
+                      double* out) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (h->opts.shard_count > 1) { set_error("predict is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  if (what != BGP_PREDICT_VAR && what != BGP_PREDICT_COV) { set_error("invalid prediction kind %d", what); return BGP_ERR_INVALID; }
+  if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
+  DevProgram P;
+  BGP_TRY(build_dev_program(spec, &P));
+  if (P.ndim != h->ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", P.ndim, h->ndim); return BGP_ERR_DIM; }
+  if (ns == 0) return BGP_OK;
+  const int64_t n = h->n;
+  const int nd = h->ndim;
+  cudaStream_t s = h->sA;
+  DevBuf<DevProgram> dprog;
+  DevBuf<double> dxs, dB, dW, dkd, dvar, dC, scratch;
+  DevBuf<GemmDesc> ddesc;
+  BGP_TRY(upload_program(P, dprog, s));
+  const int64_t c = std::min(ns, predict_chunk_cols(n, 64));
+  BGP_TRY(dW.alloc((size_t)n * c, s));
+  if (what == BGP_PREDICT_VAR) {
+    // workspace 2*n*c + O(c): var_j = k(x*_j, x*_j) - B_j . (K^-1 B)_j, chunk by chunk
+    BGP_TRY(dxs.alloc((size_t)c * nd, s));
+    BGP_TRY(dB.alloc((size_t)n * c, s));
+    BGP_TRY(dkd.alloc((size_t)c, s));
+    BGP_TRY(dvar.alloc((size_t)c, s));
+    for (int64_t j0 = 0; j0 < ns; j0 += c) {
+      const int64_t nc = std::min(c, ns - j0);
+      BGP_CUDA(cudaMemcpyAsync(dxs.p, xs + j0 * nd, sizeof(double) * nc * nd, cudaMemcpyHostToDevice, s));
+      BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p, nc, h->d_x.p, n, dB.p, n, s));
+      BGP_CUDA(cudaMemcpyAsync(dW.p, dB.p, sizeof(double) * n * nc, cudaMemcpyDeviceToDevice, s));
+      BGP_TRY(hodlr_solve_dev(h, dW.p, nc, n, s, 0));
+      BGP_TRY(kmat_diagonal_launch(dprog.p, dxs.p, dxs.p, nc, dkd.p, s));
+      BGP_TRY(predict_var_launch(dB.p, dW.p, n, n, nc, dkd.p, dvar.p, scratch, s));
+      BGP_CUDA(cudaMemcpyAsync(out + j0, dvar.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));
+    }
+  } else {
+    // B = K(x, x*) stays resident (n*ns), W one chunk (n*c): C[:, chunk] = K**[:, chunk] - B^T W_chunk, in the
+    // reference's orientation (K_h^-1 is symmetric only to tol)
+    BGP_TRY(dxs.alloc((size_t)ns * nd, s));
+    BGP_TRY(dB.alloc((size_t)n * ns, s));
+    BGP_TRY(dC.alloc((size_t)ns * ns, s));
+    BGP_CUDA(cudaMemcpyAsync(dxs.p, xs, sizeof(double) * ns * nd, cudaMemcpyHostToDevice, s));
+    BGP_TRY(kmat_symmetric_launch_auto(P, dprog.p, dxs.p, ns, nullptr, dC.p, ns, s));
+    BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p, ns, h->d_x.p, n, dB.p, n, s));
+    for (int64_t j0 = 0; j0 < ns; j0 += c) {
+      const int64_t nc = std::min(c, ns - j0);
+      BGP_CUDA(cudaMemcpyAsync(dW.p, dB.p + j0 * n, sizeof(double) * n * nc, cudaMemcpyDeviceToDevice, s));
+      BGP_TRY(hodlr_solve_dev(h, dW.p, nc, n, s, 0));
+      // column-major C (ld ns): rows j0.. of the chunk are output COLUMNS j of the row-major result
+      BGP_TRY(predict_gemm_sub(dW.p, n, dB.p, n, nc, ns, n, false, dC.p + j0, ns, scratch, ddesc, s));
+    }
+    BGP_CUDA(cudaMemcpyAsync(out, dC.p, sizeof(double) * ns * ns, cudaMemcpyDeviceToHost, s));
+  }
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;
 }

@@ -437,6 +437,16 @@ int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const
   return r >= 0 ? r : kmat_general_launch(dprog, P.ndim, x1, n1, x2, n2, out, ld, s);
 }
 
+// out[i] = k(x1_i, x2_i): the evaluator of bgp_kmat_diagonal (kernel.get_value(x, diag=True))
+int kmat_diagonal_launch(const DevProgram* dprog, const double* x1, const double* x2, int64_t n, double* out,
+                         cudaStream_t s) {
+  if (n == 0) return BGP_OK;
+  const int blocks = (int)std::min<int64_t>((n + 255) / 256, 4 * num_sms());
+  kmat_diagonal_kernel<<<blocks, 256, 0, s>>>(dprog, x1, x2, n, out);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
 // upload a digested program to a fresh device buffer
 int upload_program(const DevProgram& P, DevBuf<DevProgram>& buf, cudaStream_t s) {
   BGP_TRY(buf.reserve(1, s));
@@ -473,11 +483,7 @@ static int kmat_host(const bgp_kernel_spec_t* spec, const double* x1, int64_t n1
   if (nout == 0) return BGP_OK;
   if (mode == 0) BGP_TRY(kmat_general_launch_auto(P, dprog.p, dx1.p, n1, px2, n2, dout.p, n2, s));
   else if (mode == 1) BGP_TRY(kmat_symmetric_launch_auto(P, dprog.p, dx1.p, n1, nullptr, dout.p, n1, s));
-  else {
-    const int blocks = (int)std::min<int64_t>((n1 + 255) / 256, 4 * num_sms());
-    kmat_diagonal_kernel<<<blocks, 256, 0, s>>>(dprog.p, dx1.p, px2, n1, dout.p);
-    BGP_LAUNCH_CHECK();
-  }
+  else BGP_TRY(kmat_diagonal_launch(dprog.p, dx1.p, px2, n1, dout.p, s));
   BGP_CUDA(cudaMemcpyAsync(out, dout.p, sizeof(double) * nout, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;

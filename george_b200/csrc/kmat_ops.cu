@@ -8,15 +8,19 @@
 //                             0.5 * einsum("ijk,ij", dK, alpha alpha^T - K^-1), src/george/gp.py:437-466 over
 //                             kernel_interface.cpp:109-125).  A is read once (8 n^2 bytes); the (n, n, P) tensor is never
 //                             formed.
+//   predict_var_* / predict_gemm_sub  GP.predict's variance and covariance from K(x, x*) and K^-1 K(x, x*) chunks
+//                            that the solvers stream (dense.cu, hodlr.cu; reference gp.py:534-545).
 //
 // Roofline: matvec is FP64-ALU bound (one covariance evaluation per (i, j), no HBM traffic beyond x and V);
 // the contraction reads A once -> HBM bound at 8 B per pair for cheap kernels, FP64 bound for the gradient of
 // expensive ones.  Partial sums are written per CTA and reduced by a second tiny kernel in a fixed order, so results
 // are run-to-run deterministic (no atomics).
 #include <algorithm>
+#include <cstdlib>
 #include <vector>
 
 #include "common.cuh"
+#include "gemm_dmma.cuh"
 #include "kernel_eval.cuh"
 
 namespace bgp {
@@ -270,6 +274,124 @@ __global__ void fill_identity_kernel(double* __restrict__ A, int64_t n) {
 }
 int fill_identity_launch(double* A, int64_t n, cudaStream_t s) {
   fill_identity_kernel<<<(unsigned)std::min<int64_t>((n * n + 255) / 256, 16 * (int64_t)num_sms()), 256, 0, s>>>(A, n);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Predictive variance / covariance (GP.predict with return_var / return_cov; bgp_dense_predict, bgp_hodlr_predict).
+// The solvers stream the test points in column chunks: B = K(x, x*_chunk) (N x c), W = K^-1 B (HODLR) or L^-1 B
+// (dense, W = B in place), then
+//   variance    var_j = k(x*_j, x*_j) - sum_i B_ij W_ij      (two passes: per-CTA partials, fixed-order finish)
+//   covariance  C -= W^T B  on the tensor pipe, split over K = N into zeroed slices added in a fixed order.
+// No atomics anywhere: two identical calls return bit-identical results.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int PV_THREADS = 256;
+constexpr int64_t PV_MIN_ROWS = 1024;       // rows of one column per CTA, at least
+constexpr int64_t PREDICT_BUDGET = 1 << 27; // doubles (1 GiB) of per-chunk workspace / covariance slices
+
+// Columns per chunk: as many N-row columns as fit in PREDICT_BUDGET, at least 64, a multiple of `multiple`.
+// BGP_PREDICT_CHUNK=<c> (read at every call, like BGP_DENSE_OB) forces c, rounded up to `multiple`; tests use it to run
+// many chunks with a ragged tail at small sizes.
+int64_t predict_chunk_cols(int64_t n, int64_t multiple) {
+  int64_t c = std::max<int64_t>(64, (PREDICT_BUDGET / std::max<int64_t>(n, 1)) / 64 * 64);
+  if (const char* e = getenv("BGP_PREDICT_CHUNK")) {
+    const long v = atol(e);
+    if (v >= 1) c = v;
+  }
+  return (c + multiple - 1) / multiple * multiple;
+}
+
+// partial[j * nsplit + b] = sum over the rows of split b of B[j*ld + i] * W[j*ld + i]; grid (c, nsplit)
+__global__ void __launch_bounds__(PV_THREADS) predict_var_partial_kernel(const double* __restrict__ B,
+                                                                         const double* __restrict__ W, int64_t ld,
+                                                                         int64_t n, int64_t rows_per_split,
+                                                                         double* __restrict__ partial) {
+  __shared__ double red[32];
+  const int64_t j = blockIdx.x;
+  const int64_t r0 = (int64_t)blockIdx.y * rows_per_split, r1 = min(n, r0 + rows_per_split);
+  const double* b = B + j * ld;
+  const double* w = W + j * ld;
+  double s = 0.0;
+  for (int64_t i = r0 + threadIdx.x; i < r1; i += PV_THREADS) s = fma(b[i], w[i], s);
+  s = block_sum(s, red);
+  if (threadIdx.x == 0) partial[j * gridDim.y + blockIdx.y] = s;
+}
+
+// var[j] = kdiag[j] - sum_b partial[j * nsplit + b], b ascending
+__global__ void predict_var_finish_kernel(const double* __restrict__ partial, int nsplit, const double* __restrict__ kdiag,
+                                          int64_t c, double* __restrict__ var) {
+  for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < c; j += (int64_t)gridDim.x * blockDim.x) {
+    double s = 0.0;
+    for (int b = 0; b < nsplit; ++b) s += partial[j * nsplit + b];
+    var[j] = kdiag[j] - s;
+  }
+}
+
+// var (c) = kdiag - colsum(B .* W); B, W: n x c column-major, leading dimension ld (B == W for the dense solver)
+int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
+                       double* var, DevBuf<double>& scratch, cudaStream_t s) {
+  if (c <= 0) return BGP_OK;
+  int64_t nsplit = std::max<int64_t>(1, std::min<int64_t>((4 * (int64_t)num_sms() + c - 1) / c, (n + PV_MIN_ROWS - 1) / PV_MIN_ROWS));
+  const int64_t rows = (n + nsplit - 1) / nsplit;
+  nsplit = (n + rows - 1) / rows;
+  if (c > 0x7fffffffLL || nsplit > 65535) { set_error("predict: chunk too large for one launch"); return BGP_ERR_INVALID; }
+  BGP_TRY(scratch.reserve((size_t)(c * nsplit), s));
+  predict_var_partial_kernel<<<dim3((unsigned)c, (unsigned)nsplit), PV_THREADS, 0, s>>>(B, W, ld, n, rows, scratch.p);
+  BGP_LAUNCH_CHECK();
+  predict_var_finish_kernel<<<(unsigned)std::min<int64_t>((c + 255) / 256, 4 * (int64_t)num_sms()), 256, 0, s>>>(
+      scratch.p, (int)nsplit, kdiag, c, var);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
+// C[j*ldc + i] += sum_s slices[s*m*nn + j*m + i], s ascending; `lower`: only i >= j, mirrored to C[i*ldc + j]
+__global__ void predict_slices_add_kernel(const double* __restrict__ slices, int nsplit, int64_t m, int64_t nn,
+                                          double* __restrict__ C, int64_t ldc, int lower) {
+  const int64_t total = m * nn;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t j = t / m, i = t - j * m;
+    if (lower && i < j) continue;
+    double s = 0.0;
+    for (int sp = 0; sp < nsplit; ++sp) s += slices[(int64_t)sp * total + t];
+    const double v = C[j * ldc + i] + s;
+    C[j * ldc + i] = v;
+    if (lower && i != j) C[i * ldc + j] = v;
+  }
+}
+
+// C (m x nn, column-major ldc) -= A'B' with A'(i, k) = A[i*lda + k], B'(k, j) = B[j*ldb + k], k < K: the (1, 1) DMMA
+// variant split over K into nsplit zeroed slices (each one GD_SUB target), then added into C in a fixed order.
+// `lower` (m == nn, A == B): only the lower triangle is computed and the result is mirrored, so C stays exactly symmetric.
+int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
+                     bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s) {
+  if (m <= 0 || nn <= 0) return BGP_OK;
+  if (m > 0x7fffffffLL || nn > 0x7fffffffLL || K > 0x7fffffffLL) { set_error("predict: GEMM too large"); return BGP_ERR_INVALID; }
+  const int64_t tiles = ((m + GD_BM - 1) / GD_BM) * ((nn + GD_BN - 1) / GD_BN);
+  int64_t nsplit = (2 * (int64_t)num_sms() + tiles - 1) / tiles;                   // ~2 CTAs per SM
+  nsplit = std::min<int64_t>(nsplit, std::max<int64_t>(1, (K + 255) / 256));      // >= 256 of K per split
+  nsplit = std::min<int64_t>(nsplit, std::max<int64_t>(1, PREDICT_BUDGET / (m * nn)));
+  int64_t klen = (K + nsplit - 1) / nsplit;
+  klen = (klen + GD_BK - 1) / GD_BK * GD_BK;
+  nsplit = std::max<int64_t>(1, (K + klen - 1) / klen);
+  const int64_t slice = m * nn;
+  BGP_TRY(slices.reserve((size_t)(slice * nsplit), s));
+  BGP_CUDA(cudaMemsetAsync(slices.p, 0, sizeof(double) * slice * nsplit, s));
+  std::vector<GemmDesc> hd((size_t)nsplit);
+  for (int64_t sp = 0; sp < nsplit; ++sp) {
+    const int64_t k0 = sp * klen;
+    GemmDesc& d = hd[(size_t)sp];
+    d.A = A + k0; d.lda = lda;
+    d.B = B + k0; d.ldb = ldb;
+    d.C = slices.p + sp * slice; d.ldc = m;
+    d.M = (int)m; d.N = (int)nn; d.K = (int)std::max<int64_t>(0, std::min(klen, K - k0));
+    d.mode = GD_SUB | (lower ? GD_LOWER : 0);
+  }
+  BGP_TRY(descs.reserve((size_t)nsplit, s));
+  BGP_CUDA(cudaMemcpyAsync(descs.p, hd.data(), sizeof(GemmDesc) * nsplit, cudaMemcpyHostToDevice, s));
+  BGP_TRY((gemm_dmma_launch<true, true>(descs.p, (int)nsplit, (int)m, (int)nn, nullptr, s)));
+  predict_slices_add_kernel<<<(unsigned)std::min<int64_t>((slice + 255) / 256, 8 * (int64_t)num_sms()), 256, 0, s>>>(
+      slices.p, (int)nsplit, m, nn, C, ldc, lower ? 1 : 0);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }

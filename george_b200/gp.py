@@ -331,6 +331,17 @@ class GP(ModelSet):
             # (n*, N) matrix on the host (gp.py:524-528), which stops being possible long before N = 2^18
             return kernel.matvec(xs, self._x, alpha) + self._call_mean(xs)
 
+        # variance / covariance from the stored factorisation on the device (BasicSolver, HODLRSolver): K(x*, x) and
+        # K^-1 K(x, x*) stay there, streamed in column chunks.  Solvers without `predictive`, or that return None (a
+        # pickled dense factor, a sharded tree), take the reference's host route below.
+        predictive = getattr(self.solver, "predictive", None)
+        out = predictive(kernel, xs, "var" if return_var else "cov") if predictive is not None else None
+        if out is not None:
+            return kernel.matvec(xs, self._x, alpha) + self._call_mean(xs), out
+        return self._predict_host(alpha, xs, return_var, kernel)
+
+    def _predict_host(self, alpha, xs, return_var, kernel):
+        """The reference's route (gp.py:534-545): K(x*, x) on the host, ``solver.apply_inverse`` on its transpose."""
         Kxs = kernel.get_value(xs, self._x)
         mu = np.dot(Kxs, alpha) + self._call_mean(xs)
 

@@ -47,6 +47,7 @@ class HODLRSolver(object):
             self._ptr = C.c_void_p()
             _lib.check(self._lib.bgp_hodlr_create(C.byref(self._ptr)))
         self._n = 0
+        self.shard_count = 1
         self._fresh = True  # nothing computed through THIS object yet (a parked handle still holds its previous state)
 
     def __del__(self):
@@ -103,6 +104,7 @@ class HODLRSolver(object):
         spec = flatten(kernel_spec)
         o = self._opts(min_size, tol, seed, rng_mode, rank_capacity, shard_rank, shard_count, exhaust)
         self._n = x.shape[0]
+        self.shard_count = int(shard_count)
         self._fresh = False
         _lib.check(self._lib.bgp_hodlr_compute(self._ptr, C.byref(spec), _lib.ptr(x), x.shape[0], x.shape[1],
                                                _lib.ptr(yerr), C.byref(o)))

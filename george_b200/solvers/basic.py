@@ -13,7 +13,7 @@ import ctypes as C
 import numpy as np
 
 from .. import _lib
-from .._spec import flatten
+from .._spec import DimensionMismatch, flatten
 
 __all__ = ["BasicSolver"]
 
@@ -148,6 +148,33 @@ class BasicSolver(object):
 
     def _grad_terms_call(self, which, r, alpha, g, diag):
         return self._handle.lib.bgp_dense_grad_terms(self._handle.ptr, which, r, alpha, g, diag)
+
+    def predictive(self, kernel, xs, what):
+        """The predictive variance (``what="var"``, shape ``(ns,)``) or covariance (``what="cov"``, ``(ns, ns)``) of
+        ``GP.predict`` (gp.py:534-545) at ``xs`` (``(ns, ndim)``), computed on the device from the stored factor with
+        ``kernel`` for K(x*, x) and K(x*, x*); neither K(x*, x) nor K^-1 K(x, x*) visits the host
+        (``include/bgp.h: bgp_dense_predict``).  Returns ``None`` for a solver restored from a pickle (it holds no
+        coordinates): the caller then takes the host path."""
+        self._require()
+        if not getattr(self, "_has_inputs", True):
+            return None
+        return self._predictive_call(self._handle.lib.bgp_dense_predict, self._handle.ptr, kernel, xs, what)
+
+    @staticmethod
+    def _predictive_call(fn, ptr, kernel, xs, what):
+        kinds = {"var": _lib.BGP_PREDICT_VAR, "cov": _lib.BGP_PREDICT_COV}
+        if what not in kinds:
+            raise ValueError("what must be 'var' or 'cov'")
+        xs = np.ascontiguousarray(xs, dtype=np.float64)
+        if xs.ndim == 1:
+            xs = xs[:, None]
+        spec = flatten(kernel)
+        if xs.ndim != 2 or xs.shape[1] != spec.ndim:
+            raise DimensionMismatch("dimension mismatch")  # what kernel.get_value(xs, x) raises
+        ns = xs.shape[0]
+        out = np.empty((ns,) if what == "var" else (ns, ns), dtype=np.float64)
+        _lib.check(fn(ptr, C.byref(spec), _lib.ptr(xs), ns, kinds[what], _lib.ptr(out)))
+        return out
 
     # Device handles cannot be pickled.  Like the reference (which pickles its numpy factor, tests/test_pickle.py:21-36:
     # "Unpickled GP shouldn't need to be computed") the Cholesky factor travels with the pickle and is re-uploaded.

@@ -55,6 +55,14 @@ class HODLRSolver(BasicSolver):
     def _grad_terms_call(self, which, r, alpha, g, diag):
         return self.solver._lib.bgp_hodlr_grad_terms(self.solver._ptr, which, r, alpha, g, diag)
 
+    def predictive(self, kernel, xs, what):
+        """``BasicSolver.predictive`` on the HODLR factorisation (``include/bgp.h: bgp_hodlr_predict``); ``None`` on a
+        sharded factorisation."""
+        self._require()
+        if self.solver.shard_count > 1:
+            return None
+        return self._predictive_call(self.solver._lib.bgp_hodlr_predict, self.solver._ptr, kernel, xs, what)
+
     def __getstate__(self):
         state = self.__dict__.copy()
         state["_computed"] = False

@@ -195,6 +195,33 @@ int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r,
 int bgp_dense_last_timing(const bgp_dense_t* h, double* ms2);
 
 /* ------------------------------------------------------------------------------------------
+ * Predictive variance / covariance on the stored factorisation: gp.py:534-545 (GP.predict with return_var /
+ * return_cov) without K(x*, x) or K^-1 K(x, x*) on the host.  spec = the kernel for K(x*, x) and K(x*, x*)
+ * (GP.predict's `kernel`, not necessarily the factorised one), xs (ns x ndim row-major, host).
+ *   VAR: out[ns]         = k(x*_j, x*_j) - Kxs_j . (K^-1 Kxs^T)_j
+ *   COV: out[i*ns + j]   = K**(i,j) - sum_k Kxs(i,k) (K^-1 Kxs^T)(k,j)   (row-major, the reference's orientation)
+ * K(x, x*) is built exactly as bgp_kmat_general builds K(x*, x), k(x*_j, x*_j) as bgp_kmat_diagonal and K** as
+ * bgp_kmat_symmetric.  The test points are streamed in chunks of c columns on the handle's stream; c fills a 1 GiB
+ * budget (c = max(64, 2^27 / N) rounded down to a multiple of 64; BGP_PREDICT_CHUNK overrides it, rounded up to a
+ * multiple of 64 for HODLR).  Dense: W = L^-1 K(x, x*) (forward substitution only), var = k** - ||W_j||^2,
+ * cov = K** - W^T W (lower triangle, mirrored: exactly symmetric).  HODLR: W = K_h^-1 K(x, x*) in the 64-column groups
+ * of bgp_hodlr_apply_inverse (the same W as apply_inverse), var = k** - B_j . W_j, cov = K** - B^T W.  The reductions
+ * add in a fixed order (no atomics), so identical calls return identical bits as far as the solve does: the HODLR solve
+ * accumulates a node's Gram product with atomics once a half has more than 512 rows.  Negative variances are returned
+ * as computed.
+ * Device workspace (doubles), besides the result (ns or ns^2) and xs:
+ *   dense VAR  N*c + O(c)                 dense COV  N*ns + split-K slices (ns^2 each, at most max(ns^2, 2^27) in all)
+ *   HODLR VAR  2*N*c + O(c)               HODLR COV  N*ns + N*c + split-K slices (c*ns each, at most max(c*ns, 2^27))
+ * Errors: BGP_ERR_NOT_COMPUTED before compute and on a dense handle restored by bgp_dense_import_factor (no
+ * coordinates); BGP_ERR_DIM when the spec's ndim differs from the handle's; BGP_ERR_INVALID on a sharded HODLR
+ * factorisation, an unknown `what` or ns < 0; BGP_ERR_NOMEM when the workspace cannot be allocated.  ns == 0 writes
+ * nothing.
+ * ------------------------------------------------------------------------------------------ */
+enum { BGP_PREDICT_VAR = 0, BGP_PREDICT_COV = 1 };
+int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
+                      double* out);
+
+/* ------------------------------------------------------------------------------------------
  * HODLR solver.  Replaces _hodlr.HODLRSolver (src/george/solvers/_hodlr.cpp:115-204) and the
  * hodlr::Node tree behind it (src/george/include/george/hodlr.h:13-256).
  * ------------------------------------------------------------------------------------------ */
@@ -251,6 +278,9 @@ int bgp_hodlr_get_inverse(bgp_hodlr_t* h, double* out);
  * _hodlr.cpp:193-199 does on the host).  Not available on a sharded factorisation. */
 int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
                          double* diag_out);
+/* The HODLR counterpart of bgp_dense_predict (see there for the outputs, workspace and errors). */
+int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
+                      double* out);
 
 /* Tree / index structure introspection (bit-exact parity target; hodlr.h:48-61).
  * Nodes are listed in the reference's PRE-ORDER construction order. */
