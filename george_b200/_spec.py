@@ -163,3 +163,39 @@ def flatten(kernel_spec):
 
 def num_params(spec):
     return sum(spec.nodes[i].n_params + spec.nodes[i].n_metric for i in range(spec.n_nodes))
+
+
+def parameter_slots(spec):
+    """``(node, field, index)`` of every parameter slot of ``spec``, in the order :func:`patch_specs` fills them: node
+    by node, a leaf's ``params[:n_params]`` followed by its ``metric[:n_metric]``."""
+    slots = []
+    for i in range(spec.n_nodes):
+        node = spec.nodes[i]
+        if node.op != OP_KERNEL:
+            continue
+        slots.extend((i, "params", j) for j in range(node.n_params))
+        slots.extend((i, "metric", j) for j in range(node.n_metric))
+    return slots
+
+
+def patch_specs(template, params):
+    """``B`` copies of ``template`` (a :func:`flatten` result) with their parameter slots overwritten by the rows of
+    ``params`` (``(B, num_params(template))``); returns a contiguous ``KernelSpec * B`` array.
+
+    It relies on the slot order matching the kernel's full parameter vector: for every kernel ``k``,
+    ``k.get_parameter_vector(include_frozen=True)`` is the concatenation over the leaves of ``flatten(k)``, in node
+    order, of ``params[:n_params]`` and ``metric[:n_metric]``.  So row ``b`` patched in gives, byte for byte,
+    ``flatten(k)`` after ``k.set_parameter_vector(params[b], include_frozen=True)``: everything else in the program
+    (structure, axes, blocks, constants such as a polynomial's order) does not depend on the parameter values.
+    ``bgp_dense_batch_log_likelihood`` patches the same slots in the same order."""
+    params = np.asarray(params, dtype=np.float64)
+    slots = parameter_slots(template)
+    if params.ndim != 2 or params.shape[1] != len(slots):
+        raise ValueError("params must have shape (B, {0})".format(len(slots)))
+    out = (KernelSpec * params.shape[0])()
+    for b in range(params.shape[0]):
+        C.memmove(C.byref(out[b]), C.byref(template), C.sizeof(KernelSpec))
+        row = params[b]
+        for k, (i, field, j) in enumerate(slots):
+            getattr(out[b].nodes[i], field)[j] = float(row[k])
+    return out

@@ -27,6 +27,9 @@ int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const
                              int64_t n2, double* out, int64_t ld, cudaStream_t s);
 int kmat_diagonal_launch(const DevProgram* dprog, const double* x1, const double* x2, int64_t n, double* out,
                          cudaStream_t s);
+int kmat_symmetric_batch_launch_auto(const DevProgram* P, const DevProgram* dprogs, int B, const double* x, int64_t n,
+                                     const double* diag_add, double* out, int64_t mstride, DevBuf<double>& scratch,
+                                     cudaStream_t s);
 int64_t predict_chunk_cols(int64_t n, int64_t multiple);
 int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
                        double* var, DevBuf<double>& scratch, cudaStream_t s);
@@ -42,7 +45,12 @@ constexpr int DN_OB = 2048; // outer block: trailing updates beyond it run with 
 // Right-looking, fully unrolled: at step k every thread scales its entry of column k and applies the rank-1 update to
 // its own row; the only exchanges are the pivot and the scaled column, through (double-buffered) shared memory, two
 // barriers per step.  info != 0 when a pivot is not positive (LAPACK dpotrf's info = k+1; scipy raises LinAlgError).
-__global__ void __launch_bounds__(DN_NB) potf2_kernel(double* __restrict__ A, int64_t lda, int nb, int* info, int k0) {
+// Batched factorisations (bgp_dense_batch_*) run member blockIdx.y on the slab A + blockIdx.y * mstride with its own
+// info word; a single factorisation launches one member.
+__global__ void __launch_bounds__(DN_NB) potf2_kernel(double* __restrict__ A, int64_t lda, int nb, int* info, int k0,
+                                                      int64_t mstride) {
+  A += blockIdx.y * mstride;
+  info += blockIdx.y;
   __shared__ double col[2][DN_NB];
   __shared__ double piv[2];
   const int i = threadIdx.x;
@@ -83,11 +91,13 @@ __global__ void __launch_bounds__(DN_NB) potf2_kernel(double* __restrict__ A, in
 // Column-oriented substitution (x_j = w_j / l_jj, then w_q -= x_j l_qj for q > j): the 2016 updates of a row are
 // independent FMAs instead of 64 dependent dot products; the 64 divisions are multiplications by reciprocals computed
 // once per CTA.
+// (member blockIdx.y of a batch: slab A + blockIdx.y * mstride, info word info[blockIdx.y])
 __global__ void __launch_bounds__(128, 1) trsm_panel_kernel(double* __restrict__ A, int64_t lda, int64_t rows, int nb,
-                                                         const int* info) {
+                                                         const int* info, int64_t mstride) {
   __shared__ double l[DN_NB][DN_NB + 1];
   __shared__ double rl[DN_NB];
-  if (*info != 0) return;
+  A += blockIdx.y * mstride;
+  if (info[blockIdx.y] != 0) return;
   for (int t = threadIdx.x; t < DN_NB * DN_NB; t += blockDim.x) {
     const int i = t % DN_NB, j = t / DN_NB;
     l[i][j] = (i < nb && j < nb) ? A[(int64_t)j * lda + i] : (i == j ? 1.0 : 0.0);
@@ -267,13 +277,18 @@ __device__ __forceinline__ void warp_trsv_lower_t(const double (*l)[DN_NB + 1], 
 }
 
 // step k0 of  L y = b :  Y[k0:k0+nb] = L_kk^-1 B[k0:k0+nb] ;  B[k0+nb:] -= L[k0+nb:, k0:k0+nb] Y[k0:k0+nb]
+// Member blockIdx.y of a batch solves with L + blockIdx.y * lstride on B, Y + blockIdx.y * vstride.
 template <int NR>
 __global__ void __launch_bounds__(DS_ROWS) trsv_fwd_step_kernel(const double* __restrict__ L, int64_t ld, int64_t n,
                                                                 int64_t k0, int nb, double* __restrict__ B, int64_t ldb,
-                                                                double* __restrict__ Y, int64_t ldy, int nrhs) {
+                                                                double* __restrict__ Y, int64_t ldy, int nrhs,
+                                                                int64_t lstride, int64_t vstride) {
   __shared__ double l[DN_NB][DN_NB + 1];
   __shared__ double rl[DN_NB];
   __shared__ double xs[DS_MAX_RHS][DN_NB];
+  L += blockIdx.y * lstride;
+  B += blockIdx.y * vstride;
+  Y += blockIdx.y * vstride;
   // this thread's row of the panel: the 64 loads are issued first so that they are in flight during the substitution
   const int64_t row = k0 + nb + (int64_t)blockIdx.x * DS_ROWS + threadIdx.x;
   double v[DN_NB];
@@ -312,10 +327,15 @@ __global__ void __launch_bounds__(DS_ROWS) trsv_fwd_step_kernel(const double* __
 // step k0 of  L^T x = y :  X[k0:k0+nb] = L_kk^-T Y[k0:k0+nb] ;  Y[0:k0] -= L[k0:k0+nb, 0:k0]^T X[k0:k0+nb]
 // The CTA's 64 columns of the panel (64 x 64, each column 512 contiguous bytes) are staged through shared memory with
 // all loads in flight at once; then one thread per (column, right-hand side) takes the dot product.
+// (member blockIdx.y of a batch: L + blockIdx.y * lstride, Y and X + blockIdx.y * vstride)
 template <int NR>
 __global__ void __launch_bounds__(256) trsv_bwd_step_kernel(const double* __restrict__ L, int64_t ld, int64_t k0,
                                                             int nb, double* __restrict__ Y, int64_t ldy,
-                                                            double* __restrict__ X, int64_t ldx, int nrhs) {
+                                                            double* __restrict__ X, int64_t ldx, int nrhs,
+                                                            int64_t lstride, int64_t vstride) {
+  L += blockIdx.y * lstride;
+  Y += blockIdx.y * vstride;
+  X += blockIdx.y * vstride;
   extern __shared__ __align__(16) double bwd_smem[];  // 71 KB: above the 48 KB static limit, opted in by the launcher
   double (*l)[DN_NB + 1] = reinterpret_cast<double (*)[DN_NB + 1]>(bwd_smem);
   double (*tile)[DN_NB + 1] = reinterpret_cast<double (*)[DN_NB + 1]>(bwd_smem + DN_NB * (DN_NB + 1));  // tile[c][q] = L[k0 + q, c_begin + c]
@@ -355,12 +375,14 @@ __global__ void __launch_bounds__(256) trsv_bwd_step_kernel(const double* __rest
   }
 }
 
-__global__ void logdet_diag_kernel(const double* __restrict__ A, int64_t lda, int64_t n, double* out) {
+// one CTA per matrix: member blockIdx.x of a batch reads A + blockIdx.x * mstride and writes out[blockIdx.x]
+__global__ void logdet_diag_kernel(const double* __restrict__ A, int64_t lda, int64_t n, double* out, int64_t mstride) {
   __shared__ double red[32];
+  A += blockIdx.x * mstride;
   double s = 0.0;
   for (int64_t i = threadIdx.x; i < n; i += blockDim.x) s += log(A[i * lda + i]);
   s = block_sum(s, red);
-  if (threadIdx.x == 0) *out = 2.0 * s;
+  if (threadIdx.x == 0) out[blockIdx.x] = 2.0 * s;
 }
 __global__ void dot2_kernel(const double* __restrict__ a, const double* __restrict__ b, int64_t n, double* out) {
   __shared__ double red[32];
@@ -369,6 +391,17 @@ __global__ void dot2_kernel(const double* __restrict__ a, const double* __restri
     s += a[i] * b[i];
   s = block_sum(s, red);
   if (threadIdx.x == 0) atomicAdd(out, s);
+}
+// out[b] = r_b . x_b, one CTA per member, summed in a fixed order (no atomics): repeated calls give the same bits
+__global__ void dot_rows_kernel(const double* __restrict__ r, const double* __restrict__ x, int64_t n,
+                                double* __restrict__ out) {
+  __shared__ double red[32];
+  const double* a = r + blockIdx.x * n;
+  const double* b = x + blockIdx.x * n;
+  double s = 0.0;
+  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) s = fma(a[i], b[i], s);
+  s = block_sum(s, red);
+  if (threadIdx.x == 0) out[blockIdx.x] = s;
 }
 __global__ void square2_kernel(const double* __restrict__ yerr, double* __restrict__ diag, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
@@ -432,10 +465,13 @@ static int64_t dense_mid_block(int64_t OB) {
   return (mb < OB && OB % mb == 0) ? mb : OB;
 }
 
-static int dense_potrf(bgp_dense* h) {
-  const int64_t n = h->n;
-  double* A = h->d_A.p;
-  cudaStream_t s = h->s;
+// `members` factorisations of the same order n run together: member m's matrix is A + m * mstride, its info word
+// info[m]; every step is one launch for all of them (the GEMM descriptors of a step are consecutive, one per member,
+// and go through grid.z).  gemm_info: the word the trailing updates test before running (a single factorisation
+// passes its info word so that nothing runs after a failed pivot; a batch passes nullptr, so a failed member's updates
+// run on its own slab's garbage, which no other member reads).
+static int dense_potrf_members(double* A, int64_t n, int64_t mstride, int members, int* info, const int* gemm_info,
+                               DevBuf<GemmDesc>& gdesc, cudaStream_t s) {
   // all trailing-update descriptors of the factorisation, uploaded once
   std::vector<GemmDesc> descs;
   struct Step { int64_t k0; int nb; int64_t rem; int desc[3]; };
@@ -445,13 +481,17 @@ static int dense_potrf(bgp_dense* h) {
   // C[e:n, e:cend) -= L[e:n, b:e) L[e:cend, b:e)^T   (lower part only)
   auto add_update = [&](int64_t b, int64_t e, int64_t cend) -> int {
     if (e >= n || cend <= e || e <= b) return -1;
-    GemmDesc d;
-    const double* P = A + b * n + e;          // rows e.., columns b..e of the factor
-    d.A = P; d.lda = n; d.B = P; d.ldb = n;   // B' = P^T restricted to the first (cend - e) rows of P
-    d.C = A + e * n + e; d.ldc = n;
-    d.M = (int)(n - e); d.N = (int)(cend - e); d.K = (int)(e - b); d.mode = GD_SUB | GD_LOWER;
-    descs.push_back(d);
-    return (int)descs.size() - 1;
+    const int first = (int)descs.size();
+    for (int m = 0; m < members; ++m) {
+      double* Am = A + m * mstride;
+      GemmDesc d;
+      const double* P = Am + b * n + e;         // rows e.., columns b..e of the factor
+      d.A = P; d.lda = n; d.B = P; d.ldb = n;   // B' = P^T restricted to the first (cend - e) rows of P
+      d.C = Am + e * n + e; d.ldc = n;
+      d.M = (int)(n - e); d.N = (int)(cend - e); d.K = (int)(e - b); d.mode = GD_SUB | GD_LOWER;
+      descs.push_back(d);
+    }
+    return first;
   };
   for (int64_t j0 = 0; j0 < n; j0 += DN_NB) {
     Step st;
@@ -464,54 +504,63 @@ static int dense_potrf(bgp_dense* h) {
     st.desc[2] = (e == ob1) ? add_update(ob0, e, n) : -1;
     steps.push_back(st);
   }
-  BGP_TRY(h->d_gdesc.reserve(std::max<size_t>(descs.size(), 1), s));
+  BGP_TRY(gdesc.reserve(std::max<size_t>(descs.size(), 1), s));
   if (!descs.empty())
-    BGP_CUDA(cudaMemcpyAsync(h->d_gdesc.p, descs.data(), sizeof(GemmDesc) * descs.size(), cudaMemcpyHostToDevice, s));
+    BGP_CUDA(cudaMemcpyAsync(gdesc.p, descs.data(), sizeof(GemmDesc) * descs.size(), cudaMemcpyHostToDevice, s));
   for (const Step& st : steps) {
     double* Akk = A + st.k0 * n + st.k0;
-    potf2_kernel<<<1, DN_NB, 0, s>>>(Akk, n, st.nb, h->d_info.p, (int)st.k0);
+    potf2_kernel<<<dim3(1, (unsigned)members), DN_NB, 0, s>>>(Akk, n, st.nb, info, (int)st.k0, mstride);
     BGP_LAUNCH_CHECK();
     if (st.rem <= 0) break;
-    trsm_panel_kernel<<<(unsigned)((st.rem + 127) / 128), 128, 0, s>>>(Akk, n, st.rem, st.nb, h->d_info.p);
+    trsm_panel_kernel<<<dim3((unsigned)((st.rem + 127) / 128), (unsigned)members), 128, 0, s>>>(Akk, n, st.rem, st.nb,
+                                                                                                info, mstride);
     BGP_LAUNCH_CHECK();
     for (int l = 0; l < 3; ++l)
       if (st.desc[l] >= 0)
-        BGP_TRY((gemm_dmma_launch<false, false>(h->d_gdesc.p + st.desc[l], 1, descs[st.desc[l]].M, descs[st.desc[l]].N, h->d_info.p, s)));
+        BGP_TRY((gemm_dmma_launch<false, false>(gdesc.p + st.desc[l], members, descs[st.desc[l]].M, descs[st.desc[l]].N, gemm_info, s)));
   }
   return BGP_OK;
+}
+
+static int dense_potrf(bgp_dense* h) {
+  return dense_potrf_members(h->d_A.p, h->n, 0, 1, h->d_info.p, h->d_info.p, h->d_gdesc, h->s);
 }
 
 // X (n x nrhs, column-major ldx) <- K^-1 X on the device
 constexpr size_t DS_BWD_SMEM = sizeof(double) * ((DN_NB + DS_COLS) * (DN_NB + 1) + DN_NB + DS_MAX_RHS * DN_NB);
 
-static int dense_potrs_small(bgp_dense* h, double* X, int nrhs, int64_t ldx) {
+// X <- K^-1 X for `members` factors of order n at once (member m: L + m * lstride, X and the scratch Y (n x nrhs,
+// leading dimension n) + m * vstride); a single solve passes members = 1.
+static int potrs_small_members(const double* L, int64_t n, double* X, int nrhs, int64_t ldx, double* Y, int members,
+                               int64_t lstride, int64_t vstride, cudaStream_t s) {
   // (the attribute is per device / context: set it on every call, it is cheap)
   cudaFuncSetAttribute(trsv_bwd_step_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_BWD_SMEM);
     cudaFuncSetAttribute(trsv_bwd_step_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_BWD_SMEM);
     cudaFuncSetAttribute(trsv_bwd_step_kernel<DS_MAX_RHS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_BWD_SMEM);
-  const int64_t n = h->n;
-  const double* L = h->d_A.p;
-  cudaStream_t s = h->s;
-  BGP_TRY(h->d_tmp.reserve((size_t)n * DS_MAX_RHS, s));
-  double* Y = h->d_tmp.p;
+  const unsigned mb = (unsigned)members;
   for (int64_t k0 = 0; k0 < n; k0 += DN_NB) {
     const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
     const int64_t rem = n - k0 - nb;
-    const unsigned g = (unsigned)std::max<int64_t>(1, (rem + DS_ROWS - 1) / DS_ROWS);
-    if (nrhs == 1) trsv_fwd_step_kernel<1><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nrhs);
-    else if (nrhs <= 4) trsv_fwd_step_kernel<4><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nrhs);
-    else trsv_fwd_step_kernel<DS_MAX_RHS><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nrhs);
+    const dim3 g((unsigned)std::max<int64_t>(1, (rem + DS_ROWS - 1) / DS_ROWS), mb);
+    if (nrhs == 1) trsv_fwd_step_kernel<1><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nrhs, lstride, vstride);
+    else if (nrhs <= 4) trsv_fwd_step_kernel<4><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nrhs, lstride, vstride);
+    else trsv_fwd_step_kernel<DS_MAX_RHS><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nrhs, lstride, vstride);
     BGP_LAUNCH_CHECK();
   }
   for (int64_t k0 = ((n - 1) / DN_NB) * DN_NB; k0 >= 0; k0 -= DN_NB) {
     const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
-    const unsigned g = (unsigned)std::max<int64_t>(1, (k0 + DS_COLS - 1) / DS_COLS);
-    if (nrhs == 1) trsv_bwd_step_kernel<1><<<g, 256, DS_BWD_SMEM, s>>>(L, n, k0, nb, Y, n, X, ldx, nrhs);
-    else if (nrhs <= 4) trsv_bwd_step_kernel<4><<<g, 256, DS_BWD_SMEM, s>>>(L, n, k0, nb, Y, n, X, ldx, nrhs);
-    else trsv_bwd_step_kernel<DS_MAX_RHS><<<g, 256, DS_BWD_SMEM, s>>>(L, n, k0, nb, Y, n, X, ldx, nrhs);
+    const dim3 g((unsigned)std::max<int64_t>(1, (k0 + DS_COLS - 1) / DS_COLS), mb);
+    if (nrhs == 1) trsv_bwd_step_kernel<1><<<g, 256, DS_BWD_SMEM, s>>>(L, n, k0, nb, Y, n, X, ldx, nrhs, lstride, vstride);
+    else if (nrhs <= 4) trsv_bwd_step_kernel<4><<<g, 256, DS_BWD_SMEM, s>>>(L, n, k0, nb, Y, n, X, ldx, nrhs, lstride, vstride);
+    else trsv_bwd_step_kernel<DS_MAX_RHS><<<g, 256, DS_BWD_SMEM, s>>>(L, n, k0, nb, Y, n, X, ldx, nrhs, lstride, vstride);
     BGP_LAUNCH_CHECK();
   }
   return BGP_OK;
+}
+
+static int dense_potrs_small(bgp_dense* h, double* X, int nrhs, int64_t ldx) {
+  BGP_TRY(h->d_tmp.reserve((size_t)h->n * DS_MAX_RHS, h->s));
+  return potrs_small_members(h->d_A.p, h->n, X, nrhs, ldx, h->d_tmp.p, 1, 0, 0, h->s);
 }
 
 static int dense_potrs_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
@@ -559,9 +608,9 @@ static int dense_trsm_fwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx
       const int64_t rem = n - k0 - nb;
       const unsigned g = (unsigned)std::max<int64_t>(1, (rem + DS_ROWS - 1) / DS_ROWS);
       const int nr = (int)nrhs;
-      if (nr == 1) trsv_fwd_step_kernel<1><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr);
-      else if (nr <= 4) trsv_fwd_step_kernel<4><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr);
-      else trsv_fwd_step_kernel<DS_MAX_RHS><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr);
+      if (nr == 1) trsv_fwd_step_kernel<1><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr, 0, 0);
+      else if (nr <= 4) trsv_fwd_step_kernel<4><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr, 0, 0);
+      else trsv_fwd_step_kernel<DS_MAX_RHS><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr, 0, 0);
       BGP_LAUNCH_CHECK();
     }
     BGP_CUDA(cudaMemcpy2DAsync(X, sizeof(double) * ldx, Y, sizeof(double) * n, sizeof(double) * n, nrhs,
@@ -638,7 +687,7 @@ int bgp_dense_compute(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const doubl
   BGP_TRY(kmat_symmetric_launch_auto(P, h->d_prog.p, h->d_x.p, n, h->d_diag.p, h->d_A.p, n, s));
   BGP_CUDA(cudaEventRecord(h->ev[1], s));
   BGP_TRY(dense_potrf(h));
-  logdet_diag_kernel<<<1, 1024, 0, s>>>(h->d_A.p, n, n, h->d_scalar.p);
+  logdet_diag_kernel<<<1, 1024, 0, s>>>(h->d_A.p, n, n, h->d_scalar.p, 0);
   BGP_LAUNCH_CHECK();
   BGP_CUDA(cudaEventRecord(h->ev[2], s));
   int info = 0;
@@ -844,6 +893,147 @@ int bgp_dense_import_factor(bgp_dense_t* h, const double* factor, int64_t n, dou
 int bgp_dense_last_timing(const bgp_dense_t* h, double* ms2) {
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
   ms2[0] = h->t_ms[0]; ms2[1] = h->t_ms[1];
+  return BGP_OK;
+}
+
+}  // extern "C"
+
+// ---- batched log-likelihood terms: many parameter vectors of one kernel program on the same x ----------------------
+struct bgp_dense_batch {
+  cudaStream_t s = nullptr;
+  DevBuf<DevProgram> d_prog;
+  DevBuf<double> d_x, d_yerr, d_diag, d_r, d_sol, d_tmp, d_A, d_out, d_fn;
+  DevBuf<int> d_info;
+  DevBuf<GemmDesc> d_gdesc;
+};
+
+// members per chunk: as many n x n matrices as fit in 4 GiB, at least one; BGP_BATCH_CHUNK=<members> overrides it
+// (read at every call, so that tests can force several chunks and a ragged tail at small n)
+static int64_t batch_chunk_members(int64_t n, int64_t B) {
+  int64_t c = std::max<int64_t>(1, (int64_t(4) << 30) / (n * n * (int64_t)sizeof(double)));
+  if (const char* e = getenv("BGP_BATCH_CHUNK")) {
+    const long v = atol(e);
+    if (v >= 1) c = v;
+  }
+  return std::min<int64_t>(std::min<int64_t>(c, B), 65535);  // grid.y / grid.z carry the member index
+}
+
+// member spec = template with the parameter slots of each leaf, in node order, replaced by p: the leaf's own
+// parameters (params[0 .. n_params)) followed by its metric (metric[0 .. n_metric)), at the offsets the template's
+// program assigns (DevLeaf::param_off, the order of bgp_spec_num_params)
+static void patch_member_spec(const bgp_kernel_spec_t* tmpl, const DevProgram& Pt, const double* p,
+                              bgp_kernel_spec_t* out) {
+  *out = *tmpl;
+  int l = 0;
+  for (int i = 0; i < tmpl->n_nodes; ++i) {
+    bgp_kernel_node_t& k = out->nodes[i];
+    if (k.op != BGP_OP_KERNEL) continue;
+    const DevLeaf& L = Pt.leaf[l++];
+    for (int j = 0; j < L.n_params; ++j) k.params[j] = p[L.param_off + j];
+    for (int j = 0; j < L.n_metric; ++j) k.metric[j] = p[L.param_off + L.n_params + j];
+  }
+}
+
+extern "C" {
+
+int bgp_dense_batch_create(bgp_dense_batch_t** out) {
+  *out = new (std::nothrow) bgp_dense_batch();
+  if (!*out) { set_error("out of host memory"); return BGP_ERR_NOMEM; }
+  return BGP_OK;
+}
+
+void bgp_dense_batch_destroy(bgp_dense_batch_t* h) {
+  if (!h) return;
+  if (h->s) cudaStreamSynchronize(h->s);
+  h->d_prog.release(); h->d_x.release(); h->d_yerr.release(); h->d_diag.release(); h->d_r.release();
+  h->d_sol.release(); h->d_tmp.release(); h->d_A.release(); h->d_out.release(); h->d_fn.release();
+  h->d_info.release(); h->d_gdesc.release();
+  if (h->s) {
+    cudaStreamSynchronize(h->s);
+    cudaStreamDestroy(h->s);
+  }
+  delete h;
+}
+
+int bgp_dense_batch_log_likelihood(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params,
+                                   int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
+                                   const double* yerr, const double* r,
+                                   double* log_det, double* quad, int32_t* info) {
+  if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  if (n <= 0) { set_error("invalid number of points"); return BGP_ERR_INVALID; }
+  if (B < 0) { set_error("negative number of parameter vectors"); return BGP_ERR_INVALID; }
+  DevProgram Pt;
+  BGP_TRY(build_dev_program(spec, &Pt));
+  if (P != Pt.n_params_total) {
+    set_error("the program has %d parameters, the parameter matrix %lld columns", Pt.n_params_total, (long long)P);
+    return BGP_ERR_INVALID;
+  }
+  if (Pt.ndim != ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", Pt.ndim, ndim); return BGP_ERR_DIM; }
+  if (B == 0) return BGP_OK;
+  BGP_TRY(require_device());
+  if (!h->s) BGP_CUDA(cudaStreamCreateWithFlags(&h->s, cudaStreamNonBlocking));
+  cudaStream_t s = h->s;
+
+  // one program per member, built on the host; a member whose program fails validation evaluates the template's
+  // program in its slot (reported as info = -1, its results are discarded)
+  std::vector<DevProgram> progs((size_t)B);
+  std::vector<char> valid((size_t)B, 1);
+  {
+    bgp_kernel_spec_t ms;
+    for (int64_t b = 0; b < B; ++b) {
+      patch_member_spec(spec, Pt, params + b * P, &ms);
+      if (build_dev_program(&ms, &progs[b]) != BGP_OK || progs[b].ndim != ndim) { valid[b] = 0; progs[b] = Pt; }
+    }
+  }
+  int64_t chunk = batch_chunk_members(n, B);
+  const size_t nn = (size_t)n * (size_t)n;
+  // the matrices of a chunk; a smaller chunk when they do not fit, BGP_ERR_NOMEM when one member does not
+  for (;;) {
+    const int st = h->d_A.reserve(nn * (size_t)chunk, s);
+    if (st == BGP_OK) break;
+    if (st != BGP_ERR_NOMEM || chunk == 1) return st;
+    chunk = (chunk + 1) / 2;
+  }
+  BGP_TRY(h->d_prog.reserve((size_t)B, s));
+  BGP_TRY(h->d_x.reserve((size_t)n * ndim, s));
+  BGP_TRY(h->d_yerr.reserve((size_t)n * chunk, s));
+  BGP_TRY(h->d_diag.reserve((size_t)n * chunk, s));
+  BGP_TRY(h->d_r.reserve((size_t)n * chunk, s));
+  BGP_TRY(h->d_sol.reserve((size_t)n * chunk, s));
+  BGP_TRY(h->d_tmp.reserve((size_t)n * chunk, s));
+  BGP_TRY(h->d_out.reserve((size_t)2 * chunk, s));
+  BGP_TRY(h->d_info.reserve((size_t)chunk, s));
+  BGP_CUDA(cudaMemcpyAsync(h->d_prog.p, progs.data(), sizeof(DevProgram) * B, cudaMemcpyHostToDevice, s));
+  BGP_CUDA(cudaMemcpyAsync(h->d_x.p, x, sizeof(double) * n * ndim, cudaMemcpyHostToDevice, s));
+  const int64_t mstride = (int64_t)nn;
+  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
+    const int mc = (int)std::min(chunk, B - c0);
+    const int64_t len = (int64_t)mc * n;
+    BGP_CUDA(cudaMemcpyAsync(h->d_yerr.p, yerr + c0 * n, sizeof(double) * len, cudaMemcpyHostToDevice, s));
+    BGP_CUDA(cudaMemcpyAsync(h->d_r.p, r + c0 * n, sizeof(double) * len, cudaMemcpyHostToDevice, s));
+    BGP_CUDA(cudaMemsetAsync(h->d_info.p, 0, sizeof(int) * mc, s));
+    // yerr^2 exactly as bgp_dense_compute squares it (an elementwise product: the layout does not matter)
+    square2_kernel<<<(unsigned)std::min<int64_t>((len + 255) / 256, 1184), 256, 0, s>>>(h->d_yerr.p, h->d_diag.p, len);
+    BGP_LAUNCH_CHECK();
+    BGP_TRY(kmat_symmetric_batch_launch_auto(progs.data() + c0, h->d_prog.p + c0, mc, h->d_x.p, n, h->d_diag.p,
+                                             h->d_A.p, mstride, h->d_fn, s));
+    BGP_TRY(dense_potrf_members(h->d_A.p, n, mstride, mc, h->d_info.p, nullptr, h->d_gdesc, s));
+    logdet_diag_kernel<<<(unsigned)mc, 1024, 0, s>>>(h->d_A.p, n, n, h->d_out.p, mstride);
+    BGP_LAUNCH_CHECK();
+    // quad = r^T K^-1 r: the few-right-hand-side solve of bgp_dense_dot_solve, member-indexed, then a fixed-order dot
+    BGP_CUDA(cudaMemcpyAsync(h->d_sol.p, h->d_r.p, sizeof(double) * len, cudaMemcpyDeviceToDevice, s));
+    BGP_TRY(potrs_small_members(h->d_A.p, n, h->d_sol.p, 1, n, h->d_tmp.p, mc, mstride, n, s));
+    dot_rows_kernel<<<(unsigned)mc, 256, 0, s>>>(h->d_r.p, h->d_sol.p, n, h->d_out.p + chunk);
+    BGP_LAUNCH_CHECK();
+    BGP_CUDA(cudaMemcpyAsync(log_det + c0, h->d_out.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaMemcpyAsync(quad + c0, h->d_out.p + chunk, sizeof(double) * mc, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaStreamSynchronize(s));
+  }
+  for (int64_t b = 0; b < B; ++b) {
+    if (!valid[b]) info[b] = -1;
+    if (info[b] != 0) log_det[b] = quad[b] = std::nan("");
+  }
   return BGP_OK;
 }
 

@@ -10,6 +10,7 @@
 // through a shared-memory transpose so both stores stay coalesced.
 #include <algorithm>
 #include <cstdlib>
+#include <vector>
 #include "common.cuh"
 #include "kernel_eval.cuh"
 
@@ -69,10 +70,9 @@ __global__ void __launch_bounds__(KM_THREADS) kmat_general_kernel(const DevProgr
 
 // symmetric build: out (n x n, leading dimension ld), optional diag_add on the diagonal (basic.py:64-65 fused)
 constexpr int KS_T = 64;
-__global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_kernel(const DevProgram* __restrict__ gprog,
-                                                                    const double* __restrict__ x, int64_t n,
-                                                                    const double* __restrict__ diag_add,
-                                                                    double* __restrict__ out, int64_t ld) {
+__device__ __forceinline__ void kmat_symmetric_tile(const DevProgram* __restrict__ gprog, const double* __restrict__ x,
+                                                    int64_t n, const double* __restrict__ diag_add,
+                                                    double* __restrict__ out, int64_t ld) {
   if (blockIdx.x < blockIdx.y) return;  // tiles below the diagonal are produced by the mirror store
   extern __shared__ __align__(16) unsigned char smem_raw[];
   KmatSmem* S = reinterpret_cast<KmatSmem*>(smem_raw);
@@ -125,6 +125,22 @@ __global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_kernel(const DevPro
   if (tx < ni) {
     for (int c = ty; c < nj; c += KM_THREADS / 64) out[(j0 + c) * ld + i0 + tx] = tile[tx * (KS_T + 1) + c];
   }
+}
+__global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_kernel(const DevProgram* __restrict__ gprog,
+                                                                    const double* __restrict__ x, int64_t n,
+                                                                    const double* __restrict__ diag_add,
+                                                                    double* __restrict__ out, int64_t ld) {
+  kmat_symmetric_tile(gprog, x, n, diag_add, out, ld);
+}
+// a batch of programs on the same x: member blockIdx.z builds with gprogs[z] into out + z * mstride, adding
+// diag_add[z * n ..] on its diagonal (exactly the entries the single build makes for that program)
+__global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_batch_kernel(const DevProgram* __restrict__ gprogs,
+                                                                          const double* __restrict__ x, int64_t n,
+                                                                          const double* __restrict__ diag_add,
+                                                                          double* __restrict__ out, int64_t ld,
+                                                                          int64_t mstride) {
+  const int64_t z = blockIdx.z;
+  kmat_symmetric_tile(gprogs + z, x, n, diag_add + z * n, out + z * mstride, ld);
 }
 
 __global__ void kmat_diagonal_kernel(const DevProgram* __restrict__ gprog, const double* __restrict__ x1,
@@ -250,9 +266,9 @@ __global__ void __launch_bounds__(KM_THREADS) kmat_general_fn_kernel(const Fn fn
 }
 
 template <class Fn, int ND>
-__global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_fn_kernel(const Fn fn, const double* __restrict__ x, int64_t n,
-                                                                       const double* __restrict__ diag_add,
-                                                                       double* __restrict__ out, int64_t ld) {
+__device__ __forceinline__ void kmat_symmetric_fn_tile(const Fn& fn, const double* __restrict__ x, int64_t n,
+                                                       const double* __restrict__ diag_add, double* __restrict__ out,
+                                                       int64_t ld) {
   if (blockIdx.x < blockIdx.y) return;  // tiles below the diagonal are produced by the mirror store
   __shared__ __align__(16) double sxi[KS_T * ND];
   __shared__ __align__(16) double sxj[KS_T * ND];
@@ -297,6 +313,23 @@ __global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_fn_kernel(const Fn 
   if (tx < ni) {
     for (int c = ty; c < nj; c += KM_THREADS / 64) out[(j0 + c) * ld + i0 + tx] = tile[tx * (KS_T + 1) + c];
   }
+}
+template <class Fn, int ND>
+__global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_fn_kernel(const Fn fn, const double* __restrict__ x, int64_t n,
+                                                                       const double* __restrict__ diag_add,
+                                                                       double* __restrict__ out, int64_t ld) {
+  kmat_symmetric_fn_tile<Fn, ND>(fn, x, n, diag_add, out, ld);
+}
+// batch counterpart of kmat_symmetric_batch_kernel for the specialised shapes: member z evaluates with fns[z]
+template <class Fn, int ND>
+__global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_fn_batch_kernel(const Fn* __restrict__ fns,
+                                                                             const double* __restrict__ x, int64_t n,
+                                                                             const double* __restrict__ diag_add,
+                                                                             double* __restrict__ out, int64_t ld,
+                                                                             int64_t mstride) {
+  const int64_t z = blockIdx.z;
+  const Fn fn = fns[z];
+  kmat_symmetric_fn_tile<Fn, ND>(fn, x, n, diag_add + z * n, out + z * mstride, ld);
 }
 
 // host: does the digested program have the shape  [Constant *] f(metric over all axes) ?
@@ -372,12 +405,15 @@ static int launch_fast_nd(const FastShape& F, bool symmetric, const double* x1, 
     default: return launch_fast_axis<SHAPE, 3>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, s);
   }
 }
+static bool fast_builds_disabled() {
+  static const bool disabled = getenv("BGP_KMAT_GENERIC") != nullptr;  // tuning / A-B runs
+  return disabled;
+}
 // returns -1 when the program has no specialised build (the caller then launches the interpreter kernels)
 static int try_launch_fast(const DevProgram& P, bool symmetric, const double* x1, int64_t n1, const double* x2, int64_t n2,
                            const double* diag_add, double* out, int64_t ld, cudaStream_t s) {
-  static const bool disabled = getenv("BGP_KMAT_GENERIC") != nullptr;  // tuning / A-B runs
   FastShape F;
-  if (disabled || !detect_fast_shape(P, &F)) return -1;
+  if (fast_builds_disabled() || !detect_fast_shape(P, &F)) return -1;
   switch (F.shape) {
     case BGP_SHAPE_EXPSQ: return launch_fast_nd<BGP_SHAPE_EXPSQ>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, s);
     case BGP_SHAPE_M32: return launch_fast_nd<BGP_SHAPE_M32>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, s);
@@ -430,6 +466,82 @@ int kmat_symmetric_launch_auto(const DevProgram& P, const DevProgram* dprog, con
   const int r = try_launch_fast(P, true, x, n, x, n, diag_add, out, ld, s);
   return r >= 0 ? r : kmat_symmetric_launch(dprog, P.ndim, x, n, diag_add, out, ld, s);
 }
+
+// ---- batched symmetric build (bgp_dense_batch_log_likelihood) ----------------------------------------------------
+// detect_fast_shape reads only the program's structure (node codes, kernel types, metric type, axes, blocking) to
+// decide, and the parameter values only to fill c and m; members that differ only in parameter values therefore take
+// the same evaluator.  The decision is still made for every member and checked to agree.
+template <int SHAPE, int ND, bool AXIS>
+static int launch_fast_batch(const std::vector<FastShape>& F, const double* x, int64_t n, const double* diag_add,
+                             double* out, int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
+  typedef ProfileND<SHAPE, ND, AXIS> Fn;
+  static_assert(sizeof(Fn) == sizeof(double) * (1 + ND), "ProfileND is c followed by m[ND]");
+  const int B = (int)F.size();
+  std::vector<Fn> fns(B);
+  for (int b = 0; b < B; ++b) {
+    fns[b].c = F[b].c;
+    for (int i = 0; i < ND; ++i) fns[b].m[i] = F[b].m[i];
+  }
+  BGP_TRY(scratch.reserve((size_t)B * (1 + ND), s));
+  BGP_CUDA(cudaMemcpyAsync(scratch.p, fns.data(), sizeof(Fn) * B, cudaMemcpyHostToDevice, s));
+  const unsigned nt = (unsigned)((n + KS_T - 1) / KS_T);
+  kmat_symmetric_fn_batch_kernel<Fn, ND><<<dim3(nt, nt, (unsigned)B), KM_THREADS, 0, s>>>(
+      reinterpret_cast<const Fn*>(scratch.p), x, n, diag_add, out, n, mstride);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+template <int SHAPE, int ND>
+static int launch_fast_batch_axis(const std::vector<FastShape>& F, const double* x, int64_t n, const double* diag_add,
+                                  double* out, int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
+  return F[0].axis ? launch_fast_batch<SHAPE, ND, true>(F, x, n, diag_add, out, mstride, scratch, s)
+                   : launch_fast_batch<SHAPE, ND, false>(F, x, n, diag_add, out, mstride, scratch, s);
+}
+template <int SHAPE>
+static int launch_fast_batch_nd(const std::vector<FastShape>& F, const double* x, int64_t n, const double* diag_add,
+                                double* out, int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
+  switch (F[0].nd) {
+    case 1: return launch_fast_batch_axis<SHAPE, 1>(F, x, n, diag_add, out, mstride, scratch, s);
+    case 2: return launch_fast_batch_axis<SHAPE, 2>(F, x, n, diag_add, out, mstride, scratch, s);
+    default: return launch_fast_batch_axis<SHAPE, 3>(F, x, n, diag_add, out, mstride, scratch, s);
+  }
+}
+
+// B members (host programs P[0..B), device copies dprogs[0..B)) on the same x (n points, device): member b's matrix
+// (n x n, leading dimension n) at out + b * mstride with diag_add[b * n ..] on its diagonal, in one launch.  Each
+// member gets the entries kmat_symmetric_launch_auto builds for its program.
+int kmat_symmetric_batch_launch_auto(const DevProgram* P, const DevProgram* dprogs, int B, const double* x, int64_t n,
+                                     const double* diag_add, double* out, int64_t mstride, DevBuf<double>& scratch,
+                                     cudaStream_t s) {
+  if (n == 0 || B == 0) return BGP_OK;
+  if (B > 65535) { set_error("kmat_symmetric_batch: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
+  const unsigned nt = (unsigned)((n + KS_T - 1) / KS_T);
+  if (nt > 65535) { set_error("kmat_symmetric: n too large for one launch"); return BGP_ERR_INVALID; }
+  std::vector<FastShape> F(B);
+  int n_fast = 0;
+  if (!fast_builds_disabled())
+    for (int b = 0; b < B; ++b) n_fast += detect_fast_shape(P[b], &F[b]) ? 1 : 0;
+  if (n_fast != 0 && n_fast != B) { set_error("kmat_symmetric_batch: members differ in program structure"); return BGP_ERR_INVALID; }
+  if (n_fast == B) {
+    for (int b = 1; b < B; ++b)
+      if (F[b].shape != F[0].shape || F[b].nd != F[0].nd || F[b].axis != F[0].axis) {
+        set_error("kmat_symmetric_batch: members differ in program structure");
+        return BGP_ERR_INVALID;
+      }
+    switch (F[0].shape) {
+      case BGP_SHAPE_EXPSQ: return launch_fast_batch_nd<BGP_SHAPE_EXPSQ>(F, x, n, diag_add, out, mstride, scratch, s);
+      case BGP_SHAPE_M32: return launch_fast_batch_nd<BGP_SHAPE_M32>(F, x, n, diag_add, out, mstride, scratch, s);
+      case BGP_SHAPE_M52: return launch_fast_batch_nd<BGP_SHAPE_M52>(F, x, n, diag_add, out, mstride, scratch, s);
+      case BGP_SHAPE_EXP: return launch_fast_batch_nd<BGP_SHAPE_EXP>(F, x, n, diag_add, out, mstride, scratch, s);
+    }
+  }
+  // (the attribute is per device / context: set it on every call, it is cheap)
+  cudaFuncSetAttribute(kmat_symmetric_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+  kmat_symmetric_batch_kernel<<<dim3(nt, nt, (unsigned)B), KM_THREADS, kmat_smem_sym(P[0].ndim), s>>>(
+      dprogs, x, n, diag_add, out, n, mstride);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
 int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
                              int64_t n2, double* out, int64_t ld, cudaStream_t s) {
   if (n1 == 0 || n2 == 0) return BGP_OK;

@@ -9,12 +9,14 @@ semantics) — ``compute`` hands ``(x, sqrt(yerr^2 + exp(white_noise)))`` to a f
 plugins on the H100; this file is host bookkeeping.
 """
 
+import ctypes as C
 import warnings
 
 import numpy as np
 from numpy.linalg import LinAlgError
 
-from . import kernels
+from . import _lib, kernels
+from ._spec import flatten, num_params, patch_specs
 from .modeling import ConstantModel, ModelSet
 from .solvers import BasicSolver, TrivialSolver
 from .utils import multivariate_gaussian_samples
@@ -243,6 +245,148 @@ class GP(ModelSet):
             raise
         ll = self._const - 0.5 * self.solver.dot_solve(r)
         return ll if np.isfinite(ll) else -np.inf
+
+    def batch_log_likelihood(self, vectors, y, quiet=False):
+        """:func:`log_likelihood` at many parameter vectors: entry ``b`` of the ``(B,)`` result is what
+        ``gp.set_parameter_vector(vectors[b]); gp.log_likelihood(y, quiet=quiet)`` returns on the computed ``x`` and
+        ``yerr`` (an ensemble sampler's ``vectorize=True`` step).  With ``quiet`` a failing member is ``-inf`` and the
+        others are unaffected; otherwise the exception that loop raises first is raised.  The GP is left as it was:
+        parameter vector, factorisation, cached solve and dirty flags.
+
+        Solvers with a ``batch_log_likelihood`` hook (``BasicSolver``) factorise all members in one batched pass on
+        the device; any other solver (``HODLRSolver``, ``TrivialSolver``, plug-ins) runs that loop.
+
+        :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
+        """
+        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
+            raise RuntimeError("You need to compute the model first")
+        vectors = np.asarray(vectors, dtype=np.float64)
+        if vectors.ndim != 2 or vectors.shape[1] != len(self):
+            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        if vectors.shape[0] == 0:
+            return np.empty(0, dtype=np.float64)
+        batch = getattr(self.solver_type, "batch_log_likelihood", None)
+        if batch is not None:
+            out = self._batch_device(batch, vectors, y, quiet)
+            if out is not None:
+                return out
+        return self._batch_loop(vectors, y, quiet)
+
+    def _batch_state(self):
+        return (self.get_parameter_vector(include_frozen=True), [m.dirty for m in self.models.values()],
+                dict((k, self.__dict__[k]) for k in ("_computed", "solver", "_alpha", "_y", "_const", "_x", "_yerr2")
+                     if k in self.__dict__))
+
+    def _batch_restore(self, state):
+        vector, dirty, attrs = state
+        self.set_parameter_vector(vector, include_frozen=True)
+        for m, d in zip(self.models.values(), dirty):
+            m.dirty = d
+        self.__dict__.update(attrs)
+
+    def _batch_loop(self, vectors, y, quiet):
+        state = self._batch_state()
+        try:
+            out = np.empty(len(vectors), dtype=np.float64)
+            for b, v in enumerate(vectors):
+                self.set_parameter_vector(v)
+                out[b] = self.log_likelihood(y, quiet=quiet)
+            return out
+        finally:
+            self._batch_restore(state)
+
+    def _swap_eval(self, model, vector, fn):
+        """``fn()`` with only ``model``'s full parameter vector set to ``vector``; the model is restored after."""
+        saved, dirty = model.get_parameter_vector(include_frozen=True), model.dirty
+        try:
+            model.set_parameter_vector(vector, include_frozen=True)
+            return fn()
+        finally:
+            model.set_parameter_vector(saved, include_frozen=True)
+            model.dirty = dirty
+
+    def _batch_device(self, batch, vectors, y, quiet):
+        """The batched dense path; ``None`` when the kernel has no valid device program (the loop then reproduces
+        whatever the per-vector path does with it)."""
+        try:
+            spec = flatten(self.kernel)
+        except Exception:
+            return None
+        if _lib.load().bgp_spec_validate(C.byref(spec)) != _lib.BGP_OK:
+            return None
+        nb, n = len(vectors), len(self._x)
+        full = np.tile(self.get_parameter_vector(include_frozen=True), (nb, 1))
+        full[:, self.unfrozen_mask] = vectors
+        n_mean, n_wn = self.mean.full_size, self.white_noise.full_size
+        kpar = np.ascontiguousarray(full[:, n_mean + n_wn:])
+        if kpar.shape[1] != num_params(spec):
+            return None
+        y = self._check_dimensions(y)
+
+        # per member, the exception the per-vector path meets first: while factorising (white noise, device) and
+        # then while forming the residual (mean)
+        fact_err, mean_err = [None] * nb, [None] * nb
+        sigma = np.empty((nb, n), dtype=np.float64)
+        if type(self.white_noise) is ConstantModel:
+            for b in range(nb):  # the operations of GP._sigma, member by member
+                sigma[b] = self._yerr2 + np.exp(float(full[b, n_mean]))
+            np.sqrt(sigma, out=sigma)
+        else:
+            for b in range(nb):
+                try:
+                    sigma[b] = self._swap_eval(self.white_noise, full[b, n_mean:n_mean + n_wn],
+                                               lambda: self._sigma(self._x))
+                except Exception as exc:
+                    fact_err[b] = exc
+                    sigma[b] = 1.0
+        resid = np.empty((nb, n), dtype=np.float64)
+        if type(self.mean) is ConstantModel:
+            for b in range(nb):  # the operations of GP._residual_of
+                c = float(full[b, 0])
+                if not np.isfinite(c):
+                    try:
+                        self._swap_eval(self.mean, full[b, :n_mean], lambda: self._residual_of(y))
+                    except Exception as exc:
+                        mean_err[b] = exc
+                    resid[b] = 0.0
+                else:
+                    resid[b] = y if c == 0.0 else y - c
+        else:
+            for b in range(nb):
+                try:
+                    resid[b] = self._swap_eval(self.mean, full[b, :n_mean], lambda: self._residual_of(y))
+                except Exception as exc:
+                    mean_err[b] = exc
+                    resid[b] = 0.0
+
+        log_det, quad, info = batch(spec, kpar, self._x, sigma, resid)
+        # GP.compute / GP.log_likelihood, in the same order of operations
+        const = -0.5 * (n * np.log(2 * np.pi) + log_det)
+        ll = const - 0.5 * quad
+        ll[~np.isfinite(ll)] = -np.inf
+        for b in range(nb):
+            exc = fact_err[b]
+            if exc is None and info[b] > 0:
+                exc = LinAlgError("%d-th leading minor of the array is not positive definite" % info[b])
+            elif exc is None and info[b] < 0:
+                member = patch_specs(spec, kpar[b:b + 1])[0]
+                try:
+                    _lib.check(_lib.load().bgp_spec_validate(C.byref(member)))
+                except Exception as e:
+                    exc = e
+                else:
+                    exc = ValueError("invalid kernel")
+            if exc is not None:
+                ll[b] = -np.inf
+                if not (quiet and isinstance(exc, (ValueError, LinAlgError))):
+                    raise exc
+                continue
+            exc = mean_err[b]
+            if exc is not None:
+                ll[b] = -np.inf
+                if not (quiet and isinstance(exc, ValueError) and "mean function" in str(exc)):
+                    raise exc
+        return ll
 
     def lnlikelihood(self, y, quiet=False):
         warnings.warn("'lnlikelihood' is deprecated. Use 'log_likelihood'", DeprecationWarning)

@@ -13,7 +13,7 @@ import ctypes as C
 import numpy as np
 
 from .. import _lib
-from .._spec import DimensionMismatch, flatten
+from .._spec import DimensionMismatch, flatten, num_params
 
 __all__ = ["BasicSolver"]
 
@@ -30,6 +30,35 @@ class _DenseHandle(object):
         if getattr(self, "ptr", None) is not None and self.ptr:
             self.lib.bgp_dense_destroy(self.ptr)
             self.ptr = None
+
+
+class _BatchHandle(object):
+    """Owns a ``bgp_dense_batch_t*`` (device workspace of ``BasicSolver.batch_log_likelihood``)."""
+
+    def __init__(self):
+        self.lib = _lib.load()
+        self.ptr = C.c_void_p()
+        _lib.check(self.lib.bgp_dense_batch_create(C.byref(self.ptr)))
+
+    def __del__(self):
+        if getattr(self, "ptr", None) is not None and self.ptr:
+            try:
+                self.lib.bgp_dense_batch_destroy(self.ptr)
+            except Exception:  # interpreter shutdown
+                pass
+            self.ptr = None
+
+
+# One batch handle per process, parked here rather than on a GP or solver (which therefore pickle as before): its
+# workspace is reused by the next batch of the same size.
+_batch_handle = None
+
+
+def _get_batch_handle():
+    global _batch_handle
+    if _batch_handle is None:
+        _batch_handle = _BatchHandle()
+    return _batch_handle
 
 
 class BasicSolver(object):
@@ -175,6 +204,43 @@ class BasicSolver(object):
         out = np.empty((ns,) if what == "var" else (ns, ns), dtype=np.float64)
         _lib.check(fn(ptr, C.byref(spec), _lib.ptr(xs), ns, kinds[what], _lib.ptr(out)))
         return out
+
+    @staticmethod
+    def batch_log_likelihood(spec, params, x, yerr, r):
+        """``(log_det, quad, info)``, each ``(B,)``, for ``B`` parameter vectors of one kernel program on the same
+        ``x``: member ``b`` factorises ``K(x, x; spec patched with params[b]) + diag(yerr[b]^2)`` and solves against
+        ``r[b]`` (``include/bgp.h: bgp_dense_batch_log_likelihood``).  ``info[b]`` is 0, the leading-minor index of a
+        matrix that is not positive definite, or -1 when member ``b``'s program fails validation; ``log_det`` and
+        ``quad`` are NaN there.  ``spec`` is a :func:`flatten` result, ``params`` ``(B, num_params(spec))``, ``x``
+        ``(n,)`` or ``(n, ndim)``, ``yerr`` and ``r`` ``(B, n)``.  The members run in chunks on the device; a
+        member's ``log_det`` is bit-identical to :attr:`log_determinant` after :func:`compute` with its spec and
+        yerr."""
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.ndim == 1:
+            x = x[:, None]
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
+        r = np.ascontiguousarray(r, dtype=np.float64)
+        if x.ndim != 2 or x.shape[0] == 0:
+            raise ValueError("x must have shape (n, ndim) with n > 0")
+        n, ndim = x.shape
+        if params.ndim != 2 or params.shape[1] != num_params(spec):
+            raise ValueError("params must have shape (B, {0})".format(num_params(spec)))
+        nb = params.shape[0]
+        if yerr.shape != (nb, n) or r.shape != (nb, n):
+            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
+        if ndim != spec.ndim:
+            raise DimensionMismatch("dimension mismatch")
+        log_det = np.empty(nb, dtype=np.float64)
+        quad = np.empty(nb, dtype=np.float64)
+        info = np.zeros(nb, dtype=np.int32)
+        if nb == 0:
+            return log_det, quad, info
+        h = _get_batch_handle()
+        _lib.check(h.lib.bgp_dense_batch_log_likelihood(
+            h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim, _lib.ptr(yerr),
+            _lib.ptr(r), _lib.ptr(log_det), _lib.ptr(quad), _lib.ptr(info)))
+        return log_det, quad, info
 
     # Device handles cannot be pickled.  Like the reference (which pickles its numpy factor, tests/test_pickle.py:21-36:
     # "Unpickled GP shouldn't need to be computed") the Cholesky factor travels with the pickle and is re-uploaded.

@@ -15,6 +15,9 @@ __all__ = ["HODLRSolver"]
 
 class HODLRSolver(BasicSolver):
 
+    # no batched HODLR factorisation: GP.batch_log_likelihood takes its per-vector loop
+    batch_log_likelihood = None
+
     def __init__(self, kernel, min_size=100, tol=0.1, seed=42, rng_mode=None, rank_capacity=0,
                  exhaust="dense"):
         # rng_mode=None: the reference's single shared mt19937 (bit-for-bit its pivot order) whenever the tolerance is

@@ -222,6 +222,32 @@ int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const doubl
                       double* out);
 
 /* ------------------------------------------------------------------------------------------
+ * Batched log-likelihood terms (GP.batch_log_likelihood): B parameter vectors of one kernel program on the same x,
+ * e.g. the walkers of one ensemble-sampler step.
+ * For b in [0, B): K_b = K(x, x; spec with its parameter slots replaced by params[b*P .. b*P+P)) + diag(yerr[b]^2),
+ * lower Cholesky, log_det[b] = log|K_b|, quad[b] = r_b^T K_b^-1 r_b.  info[b] = 0, or the leading-minor index k+1
+ * exactly as bgp_dense_compute reports it (log_det / quad then NaN), or -1 when member b's program fails the
+ * validation bgp_dense_compute applies.  x (n x ndim row-major), yerr and r (B x n row-major), all host memory.
+ * The parameter slots are, leaf by leaf in node order, the leaf's params[0 .. own parameter count) followed by its
+ * metric[0 .. n_metric): the order of bgp_spec_num_params, and of Kernel.get_parameter_vector(include_frozen=True).
+ * Each member's matrix, factor and log_det are bit-identical to bgp_dense_compute with the member's spec and yerr;
+ * quad is summed in a fixed order (bgp_dense_dot_solve adds per-CTA partials atomically), so a member's results do
+ * not depend on B, its position or the chunking.  Members run in chunks of as many n x n matrices as fit in 4 GiB of
+ * device memory (BGP_BATCH_CHUNK=<members> overrides it); every step of a chunk is one launch for all its members.
+ * Device workspace: chunk * (n^2 + 5 n) doubles + B programs, kept by the handle for the next call.
+ * Errors: BGP_ERR_INVALID for n <= 0, B < 0, a malformed template or P != bgp_spec_num_params(spec); BGP_ERR_DIM
+ * when the kernel's ndim differs from ndim; BGP_ERR_NOMEM when a single member does not fit.  A member that is not
+ * positive definite is not an error.  B == 0 writes nothing.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct bgp_dense_batch bgp_dense_batch_t;
+int bgp_dense_batch_create(bgp_dense_batch_t** out);
+void bgp_dense_batch_destroy(bgp_dense_batch_t* h);
+int bgp_dense_batch_log_likelihood(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params,
+                                   int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
+                                   const double* yerr, const double* r,
+                                   double* log_det, double* quad, int32_t* info);
+
+/* ------------------------------------------------------------------------------------------
  * HODLR solver.  Replaces _hodlr.HODLRSolver (src/george/solvers/_hodlr.cpp:115-204) and the
  * hodlr::Node tree behind it (src/george/include/george/hodlr.h:13-256).
  * ------------------------------------------------------------------------------------------ */
