@@ -169,6 +169,9 @@ __device__ __forceinline__ void load_coords(double* dst, const double* __restric
     }
     mbar_wait(bar, phase);
     phase ^= 1u;
+    // every thread has seen this phase complete before thread 0 may start the next one: a thread still polling this
+    // parity when the next phase completes as well would wait for the phase after it, which never comes
+    __syncthreads();
   } else {
     for (int i = threadIdx.x; i < count; i += blockDim.x) dst[i] = src[i];
     __syncthreads();

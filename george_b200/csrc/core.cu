@@ -246,7 +246,7 @@ using namespace bgp;
 extern "C" {
 
 const char* bgp_last_error(void) { return t_error; }
-int bgp_version(void) { return 1001; }
+int bgp_version(void) { return 1002; }
 
 int bgp_device_count(void) {
   int n = 0;

@@ -26,11 +26,26 @@ int fill_identity_launch(double* A, int64_t n, cudaStream_t s);
 int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
                              int64_t n2, double* out, int64_t ld, cudaStream_t s);
 int kmat_diagonal_launch(const DevProgram* dprog, const double* x1, const double* x2, int64_t n, double* out,
-                         cudaStream_t s);
+                         cudaStream_t s, int members = 1, int64_t ostride = 0);
 int kmat_symmetric_batch_launch_auto(const DevProgram* P, const DevProgram* dprogs, int B, const double* x, int64_t n,
                                      const double* diag_add, double* out, int64_t mstride, DevBuf<double>& scratch,
                                      cudaStream_t s);
+int kmat_general_batch_launch_auto(const DevProgram* P, const DevProgram* dprogs, int B, const double* x1, int64_t n1,
+                                   const double* x2, int64_t n2, double* out, int64_t ld, int64_t mstride,
+                                   DevBuf<double>& scratch, cudaStream_t s);
+int kmat_matvec_batch_launch(const DevProgram* dprogs, int nd, int members, const double* x1, int64_t n1,
+                             const double* x2, int64_t n2, const double* V, int64_t vstride, double* out,
+                             int64_t ostride, double* partial, cudaStream_t s);
+int64_t matvec_partial_size(int64_t n1, int64_t n2);
 int64_t predict_chunk_cols(int64_t n, int64_t multiple);
+int64_t predict_var_partial_size(int64_t n, int64_t c);
+int predict_var_batch_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
+                             double* var, int members, int64_t mstride, int64_t vstride, DevBuf<double>& scratch,
+                             cudaStream_t s);
+void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, int64_t* klen_out);
+int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn,
+                             int64_t K, bool lower, double* C, int64_t ldc, int members, int64_t abstride,
+                             int64_t cstride, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
 int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
                        double* var, DevBuf<double>& scratch, cudaStream_t s);
 int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
@@ -127,14 +142,19 @@ __global__ void __launch_bounds__(128, 1) trsm_panel_kernel(double* __restrict__
 //   TA == 0: A is M x K (lda), element (i,k) = A[k*lda + i];   TA == 1: A is K x M, element (i,k) = A[i*lda + k]
 //   TB == 0: B is K x N (ldb), element (k,j) = B[j*ldb + k];   TB == 1: B is N x K, element (k,j) = B[k*ldb + j]
 //   lower != 0: only tiles with i-tile >= j-tile are computed (SYRK-style trailing update)
+//   member blockIdx.z of a batch: A + z * astride, B + z * bstride, C + z * cstride
 constexpr int GM_T = 64, GM_K = 16;
 template <int TA, int TB>
 __global__ void __launch_bounds__(256) gemm_sub_kernel(int64_t M, int64_t N, int K, const double* __restrict__ A,
                                                        int64_t lda, const double* __restrict__ B, int64_t ldb,
                                                        double* __restrict__ C, int64_t ldc, int lower,
-                                                       const int* info) {
+                                                       const int* info, int64_t astride, int64_t bstride,
+                                                       int64_t cstride) {
   if (info && *info != 0) return;
   if (lower && blockIdx.x < blockIdx.y) return;
+  A += blockIdx.z * astride;
+  B += blockIdx.z * bstride;
+  C += blockIdx.z * cstride;
   __shared__ double sa[GM_K][GM_T + 4];
   __shared__ double sb[GM_K][GM_T + 4];
   const int64_t i0 = (int64_t)blockIdx.x * GM_T, j0 = (int64_t)blockIdx.y * GM_T;
@@ -187,10 +207,13 @@ __global__ void __launch_bounds__(256) gemm_sub_kernel(int64_t M, int64_t N, int
 
 // ---- triangular solves with the diagonal block for a slab of right-hand sides --------------------------------------
 // forward: X_k <- L_kk^-1 X_k ; backward: X_k <- L_kk^-T X_k.  One thread per RHS column; L_kk in shared memory.
+// (member blockIdx.y of a batch: L + y * lstride, X + y * xstride)
 __global__ void __launch_bounds__(128) trsv_block_kernel(const double* __restrict__ L, int64_t ldl, int nb,
                                                          double* __restrict__ X, int64_t ldx, int64_t nrhs,
-                                                         int backward) {
+                                                         int backward, int64_t lstride, int64_t xstride) {
   __shared__ double l[DN_NB][DN_NB + 1];
+  L += blockIdx.y * lstride;
+  X += blockIdx.y * xstride;
   for (int t = threadIdx.x; t < nb * nb; t += blockDim.x) {
     const int i = t % nb, j = t / nb;
     l[i][j] = L[(int64_t)j * ldl + i];
@@ -571,64 +594,70 @@ static int dense_potrs_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
   const unsigned cb = (unsigned)((nrhs + 127) / 128);
   for (int64_t k0 = 0; k0 < n; k0 += DN_NB) {  // forward: L y = b
     const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
-    trsv_block_kernel<<<cb, 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 0);
+    trsv_block_kernel<<<cb, 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 0, 0, 0);
     BGP_LAUNCH_CHECK();
     const int64_t rem = n - k0 - nb;
     if (rem <= 0) break;
     dim3 grid((unsigned)((rem + GM_T - 1) / GM_T), (unsigned)((nrhs + GM_T - 1) / GM_T));
-    gemm_sub_kernel<0, 0><<<grid, 256, 0, s>>>(rem, nrhs, nb, L + k0 * n + k0 + nb, n, X + k0, ldx, X + k0 + nb, ldx, 0, nullptr);
+    gemm_sub_kernel<0, 0><<<grid, 256, 0, s>>>(rem, nrhs, nb, L + k0 * n + k0 + nb, n, X + k0, ldx, X + k0 + nb, ldx, 0,
+                                               nullptr, 0, 0, 0);
     BGP_LAUNCH_CHECK();
   }
   const int64_t last = ((n - 1) / DN_NB) * DN_NB;
   for (int64_t k0 = last; k0 >= 0; k0 -= DN_NB) {  // backward: L^T x = y
     const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
-    trsv_block_kernel<<<cb, 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 1);
+    trsv_block_kernel<<<cb, 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 1, 0, 0);
     BGP_LAUNCH_CHECK();
     if (k0 == 0) break;
     // X[0:k0] -= L[k0:k0+nb, 0:k0]^T X[k0:k0+nb]
     dim3 grid((unsigned)((k0 + GM_T - 1) / GM_T), (unsigned)((nrhs + GM_T - 1) / GM_T));
-    gemm_sub_kernel<1, 0><<<grid, 256, 0, s>>>(k0, nrhs, nb, L + k0, n, X + k0, ldx, X, ldx, 0, nullptr);
+    gemm_sub_kernel<1, 0><<<grid, 256, 0, s>>>(k0, nrhs, nb, L + k0, n, X + k0, ldx, X, ldx, 0, nullptr, 0, 0, 0);
     BGP_LAUNCH_CHECK();
   }
   return BGP_OK;
 }
 
 // X (n x nrhs, column-major ldx) <- L^-1 X: the forward half of dense_potrs_dev (predictive variance / covariance need
-// only W = L^-1 K(x, x*), since K(x*, x) K^-1 K(x, x*) = W^T W).  Few right-hand sides go through the one-launch step
-// kernels, which leave the result in d_tmp; it is copied back into X.
-static int dense_trsm_fwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
-  const int64_t n = h->n;
-  const double* L = h->d_A.p;
-  cudaStream_t s = h->s;
+// only W = L^-1 K(x, x*), since K(x*, x) K^-1 K(x, x*) = W^T W).  `members` factors at once: member m solves with
+// L + m * lstride on X + m * xstride; a single solve passes one member and zero strides.  Few right-hand sides go
+// through the one-launch step kernels, which leave the result in Y; Y has X's layout (leading dimension ldy, member
+// stride xstride, so ldy >= (members - 1) * xstride + n) and is copied back into X.
+static int trsm_fwd_members(const double* L, int64_t n, int64_t lstride, double* X, int64_t nrhs, int64_t ldx,
+                            int64_t xstride, int members, double* Y, int64_t ldy, cudaStream_t s) {
+  const unsigned mb = (unsigned)members;
   if (nrhs <= DS_MAX_RHS) {
-    BGP_TRY(h->d_tmp.reserve((size_t)n * DS_MAX_RHS, s));
-    double* Y = h->d_tmp.p;
     for (int64_t k0 = 0; k0 < n; k0 += DN_NB) {
       const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
       const int64_t rem = n - k0 - nb;
-      const unsigned g = (unsigned)std::max<int64_t>(1, (rem + DS_ROWS - 1) / DS_ROWS);
+      const dim3 g((unsigned)std::max<int64_t>(1, (rem + DS_ROWS - 1) / DS_ROWS), mb);
       const int nr = (int)nrhs;
-      if (nr == 1) trsv_fwd_step_kernel<1><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr, 0, 0);
-      else if (nr <= 4) trsv_fwd_step_kernel<4><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr, 0, 0);
-      else trsv_fwd_step_kernel<DS_MAX_RHS><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, n, nr, 0, 0);
+      if (nr == 1) trsv_fwd_step_kernel<1><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, ldy, nr, lstride, xstride);
+      else if (nr <= 4) trsv_fwd_step_kernel<4><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, ldy, nr, lstride, xstride);
+      else trsv_fwd_step_kernel<DS_MAX_RHS><<<g, DS_ROWS, 0, s>>>(L, n, n, k0, nb, X, ldx, Y, ldy, nr, lstride, xstride);
       BGP_LAUNCH_CHECK();
     }
-    BGP_CUDA(cudaMemcpy2DAsync(X, sizeof(double) * ldx, Y, sizeof(double) * n, sizeof(double) * n, nrhs,
-                               cudaMemcpyDeviceToDevice, s));
+    BGP_CUDA(cudaMemcpy2DAsync(X, sizeof(double) * ldx, Y, sizeof(double) * ldy,
+                               sizeof(double) * ((int64_t)(members - 1) * xstride + n), nrhs, cudaMemcpyDeviceToDevice, s));
     return BGP_OK;
   }
   const unsigned cb = (unsigned)((nrhs + 127) / 128);
   for (int64_t k0 = 0; k0 < n; k0 += DN_NB) {
     const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
-    trsv_block_kernel<<<cb, 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 0);
+    trsv_block_kernel<<<dim3(cb, mb), 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 0, lstride, xstride);
     BGP_LAUNCH_CHECK();
     const int64_t rem = n - k0 - nb;
     if (rem <= 0) break;
-    dim3 grid((unsigned)((rem + GM_T - 1) / GM_T), (unsigned)((nrhs + GM_T - 1) / GM_T));
-    gemm_sub_kernel<0, 0><<<grid, 256, 0, s>>>(rem, nrhs, nb, L + k0 * n + k0 + nb, n, X + k0, ldx, X + k0 + nb, ldx, 0, nullptr);
+    dim3 grid((unsigned)((rem + GM_T - 1) / GM_T), (unsigned)((nrhs + GM_T - 1) / GM_T), mb);
+    gemm_sub_kernel<0, 0><<<grid, 256, 0, s>>>(rem, nrhs, nb, L + k0 * n + k0 + nb, n, X + k0, ldx, X + k0 + nb, ldx, 0,
+                                               nullptr, lstride, xstride, xstride);
     BGP_LAUNCH_CHECK();
   }
   return BGP_OK;
+}
+
+static int dense_trsm_fwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
+  if (nrhs <= DS_MAX_RHS) BGP_TRY(h->d_tmp.reserve((size_t)h->n * DS_MAX_RHS, h->s));
+  return trsm_fwd_members(h->d_A.p, h->n, 0, X, nrhs, ldx, 0, 1, h->d_tmp.p, h->n, h->s);
 }
 
 extern "C" {
@@ -898,19 +927,23 @@ int bgp_dense_last_timing(const bgp_dense_t* h, double* ms2) {
 
 }  // extern "C"
 
-// ---- batched log-likelihood terms: many parameter vectors of one kernel program on the same x ----------------------
+// ---- batched log-likelihood terms and predictions: many parameter vectors of one kernel program on the same x -------
 struct bgp_dense_batch {
   cudaStream_t s = nullptr;
   DevBuf<DevProgram> d_prog;
   DevBuf<double> d_x, d_yerr, d_diag, d_r, d_sol, d_tmp, d_A, d_out, d_fn;
   DevBuf<int> d_info;
   DevBuf<GemmDesc> d_gdesc;
+  // bgp_dense_batch_predict: test points, the member means and their matvec partials, W = L^-1 K(x, x*), k(x*, x*),
+  // variances and their partials, covariances and their split-K slices
+  DevBuf<double> d_xs, d_mean, d_mvp, d_W, d_kd, d_var, d_vp, d_C, d_slices;
+  DevBuf<GemmDesc> d_pdesc;
 };
 
-// members per chunk: as many n x n matrices as fit in 4 GiB, at least one; BGP_BATCH_CHUNK=<members> overrides it
-// (read at every call, so that tests can force several chunks and a ragged tail at small n)
-static int64_t batch_chunk_members(int64_t n, int64_t B) {
-  int64_t c = std::max<int64_t>(1, (int64_t(4) << 30) / (n * n * (int64_t)sizeof(double)));
+// members per chunk: as many members of per_member doubles as fit in 4 GiB, at least one; BGP_BATCH_CHUNK=<members>
+// overrides it (read at every call, so that tests can force several chunks and a ragged tail at small n)
+static int64_t batch_chunk_members(int64_t per_member, int64_t B) {
+  int64_t c = std::max<int64_t>(1, (int64_t(4) << 30) / (per_member * (int64_t)sizeof(double)));
   if (const char* e = getenv("BGP_BATCH_CHUNK")) {
     const long v = atol(e);
     if (v >= 1) c = v;
@@ -934,6 +967,90 @@ static void patch_member_spec(const bgp_kernel_spec_t* tmpl, const DevProgram& P
   }
 }
 
+// The start of every batched entry point: the argument checks, then (B > 0) one program per member built on the host
+// and uploaded with x.  A member whose program fails validation evaluates the template's program in its slot (reported
+// as info = -1, its results are discarded).
+struct BatchPrograms {
+  std::vector<DevProgram> progs;
+  std::vector<char> valid;
+};
+static int batch_begin(bgp_dense_batch* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B, int64_t P,
+                       const double* x, int64_t n, int32_t ndim, BatchPrograms* bp) {
+  if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  if (n <= 0) { set_error("invalid number of points"); return BGP_ERR_INVALID; }
+  if (B < 0) { set_error("negative number of parameter vectors"); return BGP_ERR_INVALID; }
+  DevProgram Pt;
+  BGP_TRY(build_dev_program(spec, &Pt));
+  if (P != Pt.n_params_total) {
+    set_error("the program has %d parameters, the parameter matrix %lld columns", Pt.n_params_total, (long long)P);
+    return BGP_ERR_INVALID;
+  }
+  if (Pt.ndim != ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", Pt.ndim, ndim); return BGP_ERR_DIM; }
+  if (B == 0) return BGP_OK;
+  BGP_TRY(require_device());
+  if (!h->s) BGP_CUDA(cudaStreamCreateWithFlags(&h->s, cudaStreamNonBlocking));
+  bp->progs.assign((size_t)B, DevProgram());
+  bp->valid.assign((size_t)B, 1);
+  bgp_kernel_spec_t ms;
+  for (int64_t b = 0; b < B; ++b) {
+    patch_member_spec(spec, Pt, params + b * P, &ms);
+    if (build_dev_program(&ms, &bp->progs[b]) != BGP_OK || bp->progs[b].ndim != ndim) { bp->valid[b] = 0; bp->progs[b] = Pt; }
+  }
+  return BGP_OK;
+}
+
+// the chunk size for the device buffers reserve(chunk) allocates: halved while they do not fit, BGP_ERR_NOMEM when one
+// member does not; release() frees what a failed attempt left allocated
+template <class Reserve, class Release>
+static int batch_reserve_chunk(int64_t* chunk, Reserve reserve, Release release) {
+  for (;;) {
+    const int st = reserve(*chunk);
+    if (st == BGP_OK) return BGP_OK;
+    if (st != BGP_ERR_NOMEM || *chunk == 1) return st;
+    release();
+    *chunk = (*chunk + 1) / 2;
+  }
+}
+
+// the shared buffers of a chunk of `chunk` members (d_A is reserved by the caller) and the programs and x of all B
+static int batch_reserve_common(bgp_dense_batch* h, const BatchPrograms& bp, const double* x, int64_t n, int32_t ndim,
+                                int64_t chunk, int64_t tmp_cols) {
+  cudaStream_t s = h->s;
+  const int64_t B = (int64_t)bp.progs.size();
+  BGP_TRY(h->d_prog.reserve((size_t)B, s));
+  BGP_TRY(h->d_x.reserve((size_t)n * ndim, s));
+  BGP_TRY(h->d_yerr.reserve((size_t)n * chunk, s));
+  BGP_TRY(h->d_diag.reserve((size_t)n * chunk, s));
+  BGP_TRY(h->d_r.reserve((size_t)n * chunk, s));
+  BGP_TRY(h->d_sol.reserve((size_t)n * chunk, s));
+  BGP_TRY(h->d_tmp.reserve((size_t)n * chunk * tmp_cols, s));
+  BGP_TRY(h->d_info.reserve((size_t)chunk, s));
+  BGP_CUDA(cudaMemcpyAsync(h->d_prog.p, bp.progs.data(), sizeof(DevProgram) * B, cudaMemcpyHostToDevice, s));
+  BGP_CUDA(cudaMemcpyAsync(h->d_x.p, x, sizeof(double) * n * ndim, cudaMemcpyHostToDevice, s));
+  return BGP_OK;
+}
+
+// members [c0, c0 + mc): K_b + diag(yerr_b^2) built and factorised in place (d_A, member stride n^2, info in d_info) and
+// alpha_b = K_b^-1 r_b in d_sol (member stride n): the steps of bgp_dense_compute and of the few-right-hand-side solve
+// of bgp_dense_apply_inverse / bgp_dense_dot_solve, member-indexed, one launch per step for the whole chunk
+static int batch_factor_chunk(bgp_dense_batch* h, const BatchPrograms& bp, int64_t c0, int mc, int64_t n,
+                              const double* yerr, const double* r) {
+  cudaStream_t s = h->s;
+  const int64_t len = (int64_t)mc * n;
+  const int64_t mstride = n * n;
+  BGP_CUDA(cudaMemcpyAsync(h->d_yerr.p, yerr + c0 * n, sizeof(double) * len, cudaMemcpyHostToDevice, s));
+  BGP_CUDA(cudaMemcpyAsync(h->d_r.p, r + c0 * n, sizeof(double) * len, cudaMemcpyHostToDevice, s));
+  BGP_CUDA(cudaMemsetAsync(h->d_info.p, 0, sizeof(int) * mc, s));
+  // yerr^2 exactly as bgp_dense_compute squares it (an elementwise product: the layout does not matter)
+  square2_kernel<<<(unsigned)std::min<int64_t>((len + 255) / 256, 1184), 256, 0, s>>>(h->d_yerr.p, h->d_diag.p, len);
+  BGP_LAUNCH_CHECK();
+  BGP_TRY(kmat_symmetric_batch_launch_auto(bp.progs.data() + c0, h->d_prog.p + c0, mc, h->d_x.p, n, h->d_diag.p,
+                                           h->d_A.p, mstride, h->d_fn, s));
+  BGP_TRY(dense_potrf_members(h->d_A.p, n, mstride, mc, h->d_info.p, nullptr, h->d_gdesc, s));
+  BGP_CUDA(cudaMemcpyAsync(h->d_sol.p, h->d_r.p, sizeof(double) * len, cudaMemcpyDeviceToDevice, s));
+  return potrs_small_members(h->d_A.p, n, h->d_sol.p, 1, n, h->d_tmp.p, mc, mstride, n, s);
+}
+
 extern "C" {
 
 int bgp_dense_batch_create(bgp_dense_batch_t** out) {
@@ -948,6 +1065,8 @@ void bgp_dense_batch_destroy(bgp_dense_batch_t* h) {
   h->d_prog.release(); h->d_x.release(); h->d_yerr.release(); h->d_diag.release(); h->d_r.release();
   h->d_sol.release(); h->d_tmp.release(); h->d_A.release(); h->d_out.release(); h->d_fn.release();
   h->d_info.release(); h->d_gdesc.release();
+  h->d_xs.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_kd.release();
+  h->d_var.release(); h->d_vp.release(); h->d_C.release(); h->d_slices.release(); h->d_pdesc.release();
   if (h->s) {
     cudaStreamSynchronize(h->s);
     cudaStreamDestroy(h->s);
@@ -959,70 +1078,23 @@ int bgp_dense_batch_log_likelihood(bgp_dense_batch_t* h, const bgp_kernel_spec_t
                                    int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
                                    const double* yerr, const double* r,
                                    double* log_det, double* quad, int32_t* info) {
-  if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
-  if (n <= 0) { set_error("invalid number of points"); return BGP_ERR_INVALID; }
-  if (B < 0) { set_error("negative number of parameter vectors"); return BGP_ERR_INVALID; }
-  DevProgram Pt;
-  BGP_TRY(build_dev_program(spec, &Pt));
-  if (P != Pt.n_params_total) {
-    set_error("the program has %d parameters, the parameter matrix %lld columns", Pt.n_params_total, (long long)P);
-    return BGP_ERR_INVALID;
-  }
-  if (Pt.ndim != ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", Pt.ndim, ndim); return BGP_ERR_DIM; }
+  BatchPrograms bp;
+  BGP_TRY(batch_begin(h, spec, params, B, P, x, n, ndim, &bp));
   if (B == 0) return BGP_OK;
-  BGP_TRY(require_device());
-  if (!h->s) BGP_CUDA(cudaStreamCreateWithFlags(&h->s, cudaStreamNonBlocking));
   cudaStream_t s = h->s;
-
-  // one program per member, built on the host; a member whose program fails validation evaluates the template's
-  // program in its slot (reported as info = -1, its results are discarded)
-  std::vector<DevProgram> progs((size_t)B);
-  std::vector<char> valid((size_t)B, 1);
-  {
-    bgp_kernel_spec_t ms;
-    for (int64_t b = 0; b < B; ++b) {
-      patch_member_spec(spec, Pt, params + b * P, &ms);
-      if (build_dev_program(&ms, &progs[b]) != BGP_OK || progs[b].ndim != ndim) { valid[b] = 0; progs[b] = Pt; }
-    }
-  }
-  int64_t chunk = batch_chunk_members(n, B);
+  int64_t chunk = batch_chunk_members(n * n, B);
   const size_t nn = (size_t)n * (size_t)n;
   // the matrices of a chunk; a smaller chunk when they do not fit, BGP_ERR_NOMEM when one member does not
-  for (;;) {
-    const int st = h->d_A.reserve(nn * (size_t)chunk, s);
-    if (st == BGP_OK) break;
-    if (st != BGP_ERR_NOMEM || chunk == 1) return st;
-    chunk = (chunk + 1) / 2;
-  }
-  BGP_TRY(h->d_prog.reserve((size_t)B, s));
-  BGP_TRY(h->d_x.reserve((size_t)n * ndim, s));
-  BGP_TRY(h->d_yerr.reserve((size_t)n * chunk, s));
-  BGP_TRY(h->d_diag.reserve((size_t)n * chunk, s));
-  BGP_TRY(h->d_r.reserve((size_t)n * chunk, s));
-  BGP_TRY(h->d_sol.reserve((size_t)n * chunk, s));
-  BGP_TRY(h->d_tmp.reserve((size_t)n * chunk, s));
+  BGP_TRY(batch_reserve_chunk(&chunk, [&](int64_t c) { return h->d_A.reserve(nn * (size_t)c, s); }, [] {}));
+  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, 1));
   BGP_TRY(h->d_out.reserve((size_t)2 * chunk, s));
-  BGP_TRY(h->d_info.reserve((size_t)chunk, s));
-  BGP_CUDA(cudaMemcpyAsync(h->d_prog.p, progs.data(), sizeof(DevProgram) * B, cudaMemcpyHostToDevice, s));
-  BGP_CUDA(cudaMemcpyAsync(h->d_x.p, x, sizeof(double) * n * ndim, cudaMemcpyHostToDevice, s));
   const int64_t mstride = (int64_t)nn;
   for (int64_t c0 = 0; c0 < B; c0 += chunk) {
     const int mc = (int)std::min(chunk, B - c0);
-    const int64_t len = (int64_t)mc * n;
-    BGP_CUDA(cudaMemcpyAsync(h->d_yerr.p, yerr + c0 * n, sizeof(double) * len, cudaMemcpyHostToDevice, s));
-    BGP_CUDA(cudaMemcpyAsync(h->d_r.p, r + c0 * n, sizeof(double) * len, cudaMemcpyHostToDevice, s));
-    BGP_CUDA(cudaMemsetAsync(h->d_info.p, 0, sizeof(int) * mc, s));
-    // yerr^2 exactly as bgp_dense_compute squares it (an elementwise product: the layout does not matter)
-    square2_kernel<<<(unsigned)std::min<int64_t>((len + 255) / 256, 1184), 256, 0, s>>>(h->d_yerr.p, h->d_diag.p, len);
-    BGP_LAUNCH_CHECK();
-    BGP_TRY(kmat_symmetric_batch_launch_auto(progs.data() + c0, h->d_prog.p + c0, mc, h->d_x.p, n, h->d_diag.p,
-                                             h->d_A.p, mstride, h->d_fn, s));
-    BGP_TRY(dense_potrf_members(h->d_A.p, n, mstride, mc, h->d_info.p, nullptr, h->d_gdesc, s));
+    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
     logdet_diag_kernel<<<(unsigned)mc, 1024, 0, s>>>(h->d_A.p, n, n, h->d_out.p, mstride);
     BGP_LAUNCH_CHECK();
-    // quad = r^T K^-1 r: the few-right-hand-side solve of bgp_dense_dot_solve, member-indexed, then a fixed-order dot
-    BGP_CUDA(cudaMemcpyAsync(h->d_sol.p, h->d_r.p, sizeof(double) * len, cudaMemcpyDeviceToDevice, s));
-    BGP_TRY(potrs_small_members(h->d_A.p, n, h->d_sol.p, 1, n, h->d_tmp.p, mc, mstride, n, s));
+    // quad = r^T K^-1 r: a fixed-order dot per member of r and the solve above
     dot_rows_kernel<<<(unsigned)mc, 256, 0, s>>>(h->d_r.p, h->d_sol.p, n, h->d_out.p + chunk);
     BGP_LAUNCH_CHECK();
     BGP_CUDA(cudaMemcpyAsync(log_det + c0, h->d_out.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, s));
@@ -1031,8 +1103,110 @@ int bgp_dense_batch_log_likelihood(bgp_dense_batch_t* h, const bgp_kernel_spec_t
     BGP_CUDA(cudaStreamSynchronize(s));
   }
   for (int64_t b = 0; b < B; ++b) {
-    if (!valid[b]) info[b] = -1;
+    if (!bp.valid[b]) info[b] = -1;
     if (info[b] != 0) log_det[b] = quad[b] = std::nan("");
+  }
+  return BGP_OK;
+}
+
+int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
+                            int64_t P, const double* x, int64_t n, int32_t ndim, const double* yerr, const double* r,
+                            const double* xs, int64_t ns, int32_t what, double* mean, double* out, int32_t* info) {
+  if (out && what != BGP_PREDICT_VAR && what != BGP_PREDICT_COV) { set_error("invalid prediction kind %d", what); return BGP_ERR_INVALID; }
+  if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
+  BatchPrograms bp;
+  BGP_TRY(batch_begin(h, spec, params, B, P, x, n, ndim, &bp));
+  if (B == 0) return BGP_OK;
+  cudaStream_t s = h->s;
+  const bool var = out && what == BGP_PREDICT_VAR, cov = out && what == BGP_PREDICT_COV;
+  const int64_t nn = n * n;
+  // test-point chunk of the W columns: the single path's (predict_chunk_cols(n, 1)), whatever the number of members
+  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
+  const int64_t tail = c > 0 ? ns - (ns - 1) / c * c : 0;
+  const int64_t mvp = matvec_partial_size(ns, n);
+  const int64_t vp = var ? std::max(predict_var_partial_size(n, c), predict_var_partial_size(n, tail)) : 0;
+  int64_t gsplit = 1, gklen = 0;
+  if (cov && ns > 0) predict_gemm_plan(ns, ns, n, &gsplit, &gklen);
+  const int64_t tmp_cols = (var || cov) ? DS_MAX_RHS : 1;
+  // doubles per member (see include/bgp.h)
+  int64_t per_member = nn + (4 + tmp_cols) * n + ns + mvp;
+  if (var) per_member += n * c + 2 * c + vp;
+  if (cov) per_member += n * ns + ns * ns * (1 + gsplit);
+  int64_t chunk = batch_chunk_members(per_member, B);
+  if (cov) chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, 65535 / gsplit));  // one DMMA launch per chunk
+  auto release = [&] {
+    h->d_A.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_kd.release();
+    h->d_var.release(); h->d_vp.release(); h->d_C.release(); h->d_slices.release(); h->d_tmp.release();
+  };
+  auto reserve = [&](int64_t m) -> int {
+    BGP_TRY(h->d_A.reserve((size_t)(nn * m), s));
+    BGP_TRY(h->d_tmp.reserve((size_t)(n * m * tmp_cols), s));
+    BGP_TRY(h->d_mean.reserve((size_t)std::max<int64_t>(1, ns * m), s));
+    BGP_TRY(h->d_mvp.reserve((size_t)std::max<int64_t>(1, mvp * m), s));
+    if (var) {
+      BGP_TRY(h->d_W.reserve((size_t)std::max<int64_t>(1, n * c * m), s));
+      BGP_TRY(h->d_kd.reserve((size_t)std::max<int64_t>(1, c * m), s));
+      BGP_TRY(h->d_var.reserve((size_t)std::max<int64_t>(1, c * m), s));
+      BGP_TRY(h->d_vp.reserve((size_t)std::max<int64_t>(1, vp * m), s));
+    }
+    if (cov) {
+      BGP_TRY(h->d_W.reserve((size_t)std::max<int64_t>(1, n * ns * m), s));
+      BGP_TRY(h->d_C.reserve((size_t)std::max<int64_t>(1, ns * ns * m), s));
+      BGP_TRY(h->d_slices.reserve((size_t)std::max<int64_t>(1, ns * ns * gsplit * m), s));
+    }
+    return BGP_OK;
+  };
+  BGP_TRY(batch_reserve_chunk(&chunk, reserve, release));
+  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, tmp_cols));
+  BGP_TRY(h->d_xs.reserve((size_t)std::max<int64_t>(1, ns * ndim), s));
+  if (ns > 0) BGP_CUDA(cudaMemcpyAsync(h->d_xs.p, xs, sizeof(double) * ns * ndim, cudaMemcpyHostToDevice, s));
+  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
+    const int mc = (int)std::min(chunk, B - c0);
+    const DevProgram* progs = bp.progs.data() + c0;
+    const DevProgram* dprogs = h->d_prog.p + c0;
+    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
+    // mean_b = K_b(x*, x) alpha_b, the matvec GP.predict computes for its mean
+    BGP_TRY(kmat_matvec_batch_launch(dprogs, ndim, mc, h->d_xs.p, ns, h->d_x.p, n, h->d_sol.p, n, h->d_mean.p, ns,
+                                     h->d_mvp.p, s));
+    if (ns > 0)
+      BGP_CUDA(cudaMemcpyAsync(mean + c0 * ns, h->d_mean.p, sizeof(double) * mc * ns, cudaMemcpyDeviceToHost, s));
+    // W columns of all members interleaved: column j of member m at W + (j * mc + m) * n, so that the columns of a
+    // test-point chunk are one contiguous block (the few-column solve copies its result back in one piece)
+    const int64_t ldw = (int64_t)mc * n;
+    if (var) {
+      // the steps of bgp_dense_predict's variance loop, member-indexed
+      for (int64_t j0 = 0; j0 < ns; j0 += c) {
+        const int64_t nc = std::min(c, ns - j0);
+        const double* xc = h->d_xs.p + j0 * ndim;
+        BGP_TRY(kmat_general_batch_launch_auto(progs, dprogs, mc, xc, nc, h->d_x.p, n, h->d_W.p, ldw, n, h->d_fn, s));
+        BGP_TRY(trsm_fwd_members(h->d_A.p, n, nn, h->d_W.p, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
+        BGP_TRY(kmat_diagonal_launch(dprogs, xc, xc, nc, h->d_kd.p, s, mc, c));
+        BGP_TRY(predict_var_batch_launch(h->d_W.p, h->d_W.p, ldw, n, nc, h->d_kd.p, h->d_var.p, mc, n, c, h->d_vp, s));
+        BGP_CUDA(cudaMemcpy2DAsync(out + c0 * ns + j0, sizeof(double) * ns, h->d_var.p, sizeof(double) * c,
+                                   sizeof(double) * nc, mc, cudaMemcpyDeviceToHost, s));
+      }
+    } else if (cov && ns > 0) {
+      // the steps of bgp_dense_predict's covariance path, member-indexed: K**, every W chunk resident, C = K** - W^T W
+      BGP_TRY(kmat_symmetric_batch_launch_auto(progs, dprogs, mc, h->d_xs.p, ns, nullptr, h->d_C.p, ns * ns, h->d_fn, s));
+      for (int64_t j0 = 0; j0 < ns; j0 += c) {
+        const int64_t nc = std::min(c, ns - j0);
+        BGP_TRY(kmat_general_batch_launch_auto(progs, dprogs, mc, h->d_xs.p + j0 * ndim, nc, h->d_x.p, n,
+                                               h->d_W.p + j0 * ldw, ldw, n, h->d_fn, s));
+        BGP_TRY(trsm_fwd_members(h->d_A.p, n, nn, h->d_W.p + j0 * ldw, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
+      }
+      BGP_TRY(predict_gemm_sub_members(h->d_W.p, ldw, h->d_W.p, ldw, ns, ns, n, true, h->d_C.p, ns, mc, n, ns * ns,
+                                       h->d_slices, h->d_pdesc, s));
+      BGP_CUDA(cudaMemcpyAsync(out + c0 * ns * ns, h->d_C.p, sizeof(double) * mc * ns * ns, cudaMemcpyDeviceToHost, s));
+    }
+    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaStreamSynchronize(s));
+  }
+  const int64_t osize = var ? ns : cov ? ns * ns : 0;
+  for (int64_t b = 0; b < B; ++b) {
+    if (!bp.valid[b]) info[b] = -1;
+    if (info[b] == 0) continue;
+    for (int64_t j = 0; j < ns; ++j) mean[b * ns + j] = std::nan("");
+    for (int64_t j = 0; j < osize; ++j) out[b * osize + j] = std::nan("");
   }
   return BGP_OK;
 }

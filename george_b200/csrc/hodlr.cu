@@ -32,7 +32,7 @@ int kmat_symmetric_launch_auto(const DevProgram& P, const DevProgram* dprog, con
 int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
                              int64_t n2, double* out, int64_t ld, cudaStream_t s);
 int kmat_diagonal_launch(const DevProgram* dprog, const double* x1, const double* x2, int64_t n, double* out,
-                         cudaStream_t s);
+                         cudaStream_t s, int members = 1, int64_t ostride = 0);
 int64_t predict_chunk_cols(int64_t n, int64_t multiple);
 int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
                        double* var, DevBuf<double>& scratch, cudaStream_t s);

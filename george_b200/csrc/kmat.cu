@@ -26,10 +26,9 @@ struct KmatSmem {
 };
 
 // out[i*ld + j] = k(x1_i, x2_j)
-__global__ void __launch_bounds__(KM_THREADS) kmat_general_kernel(const DevProgram* __restrict__ gprog,
-                                                                  const double* __restrict__ x1, int64_t n1,
-                                                                  const double* __restrict__ x2, int64_t n2,
-                                                                  double* __restrict__ out, int64_t ld) {
+__device__ __forceinline__ void kmat_general_tile(const DevProgram* __restrict__ gprog, const double* __restrict__ x1,
+                                                  int64_t n1, const double* __restrict__ x2, int64_t n2,
+                                                  double* __restrict__ out, int64_t ld) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   KmatSmem* S = reinterpret_cast<KmatSmem*>(smem_raw);
   const int nd = gprog->ndim;
@@ -66,6 +65,21 @@ __global__ void __launch_bounds__(KM_THREADS) kmat_general_kernel(const DevProgr
       }
     }
   }
+}
+__global__ void __launch_bounds__(KM_THREADS) kmat_general_kernel(const DevProgram* __restrict__ gprog,
+                                                                  const double* __restrict__ x1, int64_t n1,
+                                                                  const double* __restrict__ x2, int64_t n2,
+                                                                  double* __restrict__ out, int64_t ld) {
+  kmat_general_tile(gprog, x1, n1, x2, n2, out, ld);
+}
+// a batch of programs on the same x1, x2: member blockIdx.z evaluates gprogs[z] into out + z * mstride
+__global__ void __launch_bounds__(KM_THREADS) kmat_general_batch_kernel(const DevProgram* __restrict__ gprogs,
+                                                                        const double* __restrict__ x1, int64_t n1,
+                                                                        const double* __restrict__ x2, int64_t n2,
+                                                                        double* __restrict__ out, int64_t ld,
+                                                                        int64_t mstride) {
+  const int64_t z = blockIdx.z;
+  kmat_general_tile(gprogs + z, x1, n1, x2, n2, out + z * mstride, ld);
 }
 
 // symmetric build: out (n x n, leading dimension ld), optional diag_add on the diagonal (basic.py:64-65 fused)
@@ -133,20 +147,23 @@ __global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_kernel(const DevPro
   kmat_symmetric_tile(gprog, x, n, diag_add, out, ld);
 }
 // a batch of programs on the same x: member blockIdx.z builds with gprogs[z] into out + z * mstride, adding
-// diag_add[z * n ..] on its diagonal (exactly the entries the single build makes for that program)
+// diag_add[z * n ..] on its diagonal when diag_add is given (exactly the entries the single build makes for that program)
 __global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_batch_kernel(const DevProgram* __restrict__ gprogs,
                                                                           const double* __restrict__ x, int64_t n,
                                                                           const double* __restrict__ diag_add,
                                                                           double* __restrict__ out, int64_t ld,
                                                                           int64_t mstride) {
   const int64_t z = blockIdx.z;
-  kmat_symmetric_tile(gprogs + z, x, n, diag_add + z * n, out + z * mstride, ld);
+  kmat_symmetric_tile(gprogs + z, x, n, diag_add ? diag_add + z * n : nullptr, out + z * mstride, ld);
 }
 
+// (member blockIdx.y of a batch: program gprog[blockIdx.y], output out + blockIdx.y * ostride)
 __global__ void kmat_diagonal_kernel(const DevProgram* __restrict__ gprog, const double* __restrict__ x1,
-                                     const double* __restrict__ x2, int64_t n, double* __restrict__ out) {
+                                     const double* __restrict__ x2, int64_t n, double* __restrict__ out,
+                                     int64_t ostride) {
   __shared__ DevProgram P;
-  stage_program(&P, gprog);
+  out += blockIdx.y * ostride;
+  stage_program(&P, gprog + blockIdx.y);
   __syncthreads();
   const int nd = P.ndim;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
@@ -229,9 +246,9 @@ struct ProfileND {
 };
 
 template <class Fn, int ND>
-__global__ void __launch_bounds__(KM_THREADS) kmat_general_fn_kernel(const Fn fn, const double* __restrict__ x1,
-                                                                     int64_t n1, const double* __restrict__ x2,
-                                                                     int64_t n2, double* __restrict__ out, int64_t ld) {
+__device__ __forceinline__ void kmat_general_fn_tile(const Fn& fn, const double* __restrict__ x1, int64_t n1,
+                                                     const double* __restrict__ x2, int64_t n2,
+                                                     double* __restrict__ out, int64_t ld) {
   __shared__ __align__(16) double sx1[KM_TI * ND];
   __shared__ __align__(16) double sx2[KM_TJ * ND];
   __shared__ uint64_t bar;
@@ -263,6 +280,23 @@ __global__ void __launch_bounds__(KM_THREADS) kmat_general_fn_kernel(const Fn fn
       }
     }
   }
+}
+template <class Fn, int ND>
+__global__ void __launch_bounds__(KM_THREADS) kmat_general_fn_kernel(const Fn fn, const double* __restrict__ x1,
+                                                                     int64_t n1, const double* __restrict__ x2,
+                                                                     int64_t n2, double* __restrict__ out, int64_t ld) {
+  kmat_general_fn_tile<Fn, ND>(fn, x1, n1, x2, n2, out, ld);
+}
+// batch counterpart of kmat_general_batch_kernel for the specialised shapes: member z evaluates with fns[z]
+template <class Fn, int ND>
+__global__ void __launch_bounds__(KM_THREADS) kmat_general_fn_batch_kernel(const Fn* __restrict__ fns,
+                                                                           const double* __restrict__ x1, int64_t n1,
+                                                                           const double* __restrict__ x2, int64_t n2,
+                                                                           double* __restrict__ out, int64_t ld,
+                                                                           int64_t mstride) {
+  const int64_t z = blockIdx.z;
+  const Fn fn = fns[z];
+  kmat_general_fn_tile<Fn, ND>(fn, x1, n1, x2, n2, out + z * mstride, ld);
 }
 
 template <class Fn, int ND>
@@ -329,7 +363,7 @@ __global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_fn_batch_kernel(con
                                                                              int64_t mstride) {
   const int64_t z = blockIdx.z;
   const Fn fn = fns[z];
-  kmat_symmetric_fn_tile<Fn, ND>(fn, x, n, diag_add + z * n, out + z * mstride, ld);
+  kmat_symmetric_fn_tile<Fn, ND>(fn, x, n, diag_add ? diag_add + z * n : nullptr, out + z * mstride, ld);
 }
 
 // host: does the digested program have the shape  [Constant *] f(metric over all axes) ?
@@ -467,13 +501,14 @@ int kmat_symmetric_launch_auto(const DevProgram& P, const DevProgram* dprog, con
   return r >= 0 ? r : kmat_symmetric_launch(dprog, P.ndim, x, n, diag_add, out, ld, s);
 }
 
-// ---- batched symmetric build (bgp_dense_batch_log_likelihood) ----------------------------------------------------
+// ---- batched builds (bgp_dense_batch_log_likelihood, bgp_dense_batch_predict) ----------------------------------
 // detect_fast_shape reads only the program's structure (node codes, kernel types, metric type, axes, blocking) to
 // decide, and the parameter values only to fill c and m; members that differ only in parameter values therefore take
 // the same evaluator.  The decision is still made for every member and checked to agree.
 template <int SHAPE, int ND, bool AXIS>
-static int launch_fast_batch(const std::vector<FastShape>& F, const double* x, int64_t n, const double* diag_add,
-                             double* out, int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
+static int launch_fast_batch(const std::vector<FastShape>& F, bool symmetric, const double* x1, int64_t n1,
+                             const double* x2, int64_t n2, const double* diag_add, double* out, int64_t ld,
+                             int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
   typedef ProfileND<SHAPE, ND, AXIS> Fn;
   static_assert(sizeof(Fn) == sizeof(double) * (1 + ND), "ProfileND is c followed by m[ND]");
   const int B = (int)F.size();
@@ -484,31 +519,65 @@ static int launch_fast_batch(const std::vector<FastShape>& F, const double* x, i
   }
   BGP_TRY(scratch.reserve((size_t)B * (1 + ND), s));
   BGP_CUDA(cudaMemcpyAsync(scratch.p, fns.data(), sizeof(Fn) * B, cudaMemcpyHostToDevice, s));
-  const unsigned nt = (unsigned)((n + KS_T - 1) / KS_T);
-  kmat_symmetric_fn_batch_kernel<Fn, ND><<<dim3(nt, nt, (unsigned)B), KM_THREADS, 0, s>>>(
-      reinterpret_cast<const Fn*>(scratch.p), x, n, diag_add, out, n, mstride);
+  const Fn* dfns = reinterpret_cast<const Fn*>(scratch.p);
+  if (symmetric) {
+    const unsigned nt = (unsigned)((n1 + KS_T - 1) / KS_T);
+    kmat_symmetric_fn_batch_kernel<Fn, ND><<<dim3(nt, nt, (unsigned)B), KM_THREADS, 0, s>>>(dfns, x1, n1, diag_add, out,
+                                                                                             ld, mstride);
+  } else {
+    const dim3 grid((unsigned)((n2 + KM_TJ - 1) / KM_TJ), (unsigned)((n1 + KM_TI - 1) / KM_TI), (unsigned)B);
+    kmat_general_fn_batch_kernel<Fn, ND><<<grid, KM_THREADS, 0, s>>>(dfns, x1, n1, x2, n2, out, ld, mstride);
+  }
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
 template <int SHAPE, int ND>
-static int launch_fast_batch_axis(const std::vector<FastShape>& F, const double* x, int64_t n, const double* diag_add,
-                                  double* out, int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
-  return F[0].axis ? launch_fast_batch<SHAPE, ND, true>(F, x, n, diag_add, out, mstride, scratch, s)
-                   : launch_fast_batch<SHAPE, ND, false>(F, x, n, diag_add, out, mstride, scratch, s);
+static int launch_fast_batch_axis(const std::vector<FastShape>& F, bool symmetric, const double* x1, int64_t n1,
+                                  const double* x2, int64_t n2, const double* diag_add, double* out, int64_t ld,
+                                  int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
+  return F[0].axis ? launch_fast_batch<SHAPE, ND, true>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, mstride, scratch, s)
+                   : launch_fast_batch<SHAPE, ND, false>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, mstride, scratch, s);
 }
 template <int SHAPE>
-static int launch_fast_batch_nd(const std::vector<FastShape>& F, const double* x, int64_t n, const double* diag_add,
-                                double* out, int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
+static int launch_fast_batch_nd(const std::vector<FastShape>& F, bool symmetric, const double* x1, int64_t n1,
+                                const double* x2, int64_t n2, const double* diag_add, double* out, int64_t ld,
+                                int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
   switch (F[0].nd) {
-    case 1: return launch_fast_batch_axis<SHAPE, 1>(F, x, n, diag_add, out, mstride, scratch, s);
-    case 2: return launch_fast_batch_axis<SHAPE, 2>(F, x, n, diag_add, out, mstride, scratch, s);
-    default: return launch_fast_batch_axis<SHAPE, 3>(F, x, n, diag_add, out, mstride, scratch, s);
+    case 1: return launch_fast_batch_axis<SHAPE, 1>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, mstride, scratch, s);
+    case 2: return launch_fast_batch_axis<SHAPE, 2>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, mstride, scratch, s);
+    default: return launch_fast_batch_axis<SHAPE, 3>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, mstride, scratch, s);
   }
+}
+// the specialised build of a batch: -1 when no member has one (the caller launches the interpreter kernels), an error
+// when the members disagree, otherwise the status of the one launch
+static int try_launch_fast_batch(const DevProgram* P, int B, bool symmetric, const double* x1, int64_t n1,
+                                 const double* x2, int64_t n2, const double* diag_add, double* out, int64_t ld,
+                                 int64_t mstride, DevBuf<double>& scratch, cudaStream_t s) {
+  std::vector<FastShape> F(B);
+  int n_fast = 0;
+  if (!fast_builds_disabled())
+    for (int b = 0; b < B; ++b) n_fast += detect_fast_shape(P[b], &F[b]) ? 1 : 0;
+  if (n_fast == 0) return -1;
+  const char* what = symmetric ? "kmat_symmetric_batch" : "kmat_general_batch";
+  if (n_fast != B) { set_error("%s: members differ in program structure", what); return BGP_ERR_INVALID; }
+  for (int b = 1; b < B; ++b)
+    if (F[b].shape != F[0].shape || F[b].nd != F[0].nd || F[b].axis != F[0].axis) {
+      set_error("%s: members differ in program structure", what);
+      return BGP_ERR_INVALID;
+    }
+  switch (F[0].shape) {
+    case BGP_SHAPE_EXPSQ: return launch_fast_batch_nd<BGP_SHAPE_EXPSQ>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, mstride, scratch, s);
+    case BGP_SHAPE_M32: return launch_fast_batch_nd<BGP_SHAPE_M32>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, mstride, scratch, s);
+    case BGP_SHAPE_M52: return launch_fast_batch_nd<BGP_SHAPE_M52>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, mstride, scratch, s);
+    case BGP_SHAPE_EXP: return launch_fast_batch_nd<BGP_SHAPE_EXP>(F, symmetric, x1, n1, x2, n2, diag_add, out, ld, mstride, scratch, s);
+  }
+  set_error("%s: unknown specialised shape", what);
+  return BGP_ERR_INVALID;
 }
 
 // B members (host programs P[0..B), device copies dprogs[0..B)) on the same x (n points, device): member b's matrix
-// (n x n, leading dimension n) at out + b * mstride with diag_add[b * n ..] on its diagonal, in one launch.  Each
-// member gets the entries kmat_symmetric_launch_auto builds for its program.
+// (n x n, leading dimension n) at out + b * mstride with diag_add[b * n ..] on its diagonal (none when diag_add is
+// null), in one launch.  Each member gets the entries kmat_symmetric_launch_auto builds for its program.
 int kmat_symmetric_batch_launch_auto(const DevProgram* P, const DevProgram* dprogs, int B, const double* x, int64_t n,
                                      const double* diag_add, double* out, int64_t mstride, DevBuf<double>& scratch,
                                      cudaStream_t s) {
@@ -516,28 +585,31 @@ int kmat_symmetric_batch_launch_auto(const DevProgram* P, const DevProgram* dpro
   if (B > 65535) { set_error("kmat_symmetric_batch: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
   const unsigned nt = (unsigned)((n + KS_T - 1) / KS_T);
   if (nt > 65535) { set_error("kmat_symmetric: n too large for one launch"); return BGP_ERR_INVALID; }
-  std::vector<FastShape> F(B);
-  int n_fast = 0;
-  if (!fast_builds_disabled())
-    for (int b = 0; b < B; ++b) n_fast += detect_fast_shape(P[b], &F[b]) ? 1 : 0;
-  if (n_fast != 0 && n_fast != B) { set_error("kmat_symmetric_batch: members differ in program structure"); return BGP_ERR_INVALID; }
-  if (n_fast == B) {
-    for (int b = 1; b < B; ++b)
-      if (F[b].shape != F[0].shape || F[b].nd != F[0].nd || F[b].axis != F[0].axis) {
-        set_error("kmat_symmetric_batch: members differ in program structure");
-        return BGP_ERR_INVALID;
-      }
-    switch (F[0].shape) {
-      case BGP_SHAPE_EXPSQ: return launch_fast_batch_nd<BGP_SHAPE_EXPSQ>(F, x, n, diag_add, out, mstride, scratch, s);
-      case BGP_SHAPE_M32: return launch_fast_batch_nd<BGP_SHAPE_M32>(F, x, n, diag_add, out, mstride, scratch, s);
-      case BGP_SHAPE_M52: return launch_fast_batch_nd<BGP_SHAPE_M52>(F, x, n, diag_add, out, mstride, scratch, s);
-      case BGP_SHAPE_EXP: return launch_fast_batch_nd<BGP_SHAPE_EXP>(F, x, n, diag_add, out, mstride, scratch, s);
-    }
-  }
+  const int r = try_launch_fast_batch(P, B, true, x, n, x, n, diag_add, out, n, mstride, scratch, s);
+  if (r >= 0) return r;
   // (the attribute is per device / context: set it on every call, it is cheap)
   cudaFuncSetAttribute(kmat_symmetric_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
   kmat_symmetric_batch_kernel<<<dim3(nt, nt, (unsigned)B), KM_THREADS, kmat_smem_sym(P[0].ndim), s>>>(
       dprogs, x, n, diag_add, out, n, mstride);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
+// B members on the same x1 (n1 points) and x2 (n2 points): member b's K(x1, x2) at out + b * mstride (element (i, j)
+// at [i * ld + j]), in one launch; each member gets the entries kmat_general_launch_auto builds for its program
+int kmat_general_batch_launch_auto(const DevProgram* P, const DevProgram* dprogs, int B, const double* x1, int64_t n1,
+                                   const double* x2, int64_t n2, double* out, int64_t ld, int64_t mstride,
+                                   DevBuf<double>& scratch, cudaStream_t s) {
+  if (n1 == 0 || n2 == 0 || B == 0) return BGP_OK;
+  if (B > 65535) { set_error("kmat_general_batch: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
+  const dim3 grid((unsigned)((n2 + KM_TJ - 1) / KM_TJ), (unsigned)((n1 + KM_TI - 1) / KM_TI), (unsigned)B);
+  if ((n1 + KM_TI - 1) / KM_TI > 65535) { set_error("kmat_general: n1 too large for one launch"); return BGP_ERR_INVALID; }
+  const int r = try_launch_fast_batch(P, B, false, x1, n1, x2, n2, nullptr, out, ld, mstride, scratch, s);
+  if (r >= 0) return r;
+  // (the attribute is per device / context: set it on every call, it is cheap)
+  cudaFuncSetAttribute(kmat_general_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+  kmat_general_batch_kernel<<<grid, KM_THREADS, kmat_smem_general(P[0].ndim), s>>>(dprogs, x1, n1, x2, n2, out, ld,
+                                                                                   mstride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
@@ -550,11 +622,13 @@ int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const
 }
 
 // out[i] = k(x1_i, x2_i): the evaluator of bgp_kmat_diagonal (kernel.get_value(x, diag=True))
+// (members > 1: member b evaluates dprog[b] into out + b * ostride, in the same launch)
 int kmat_diagonal_launch(const DevProgram* dprog, const double* x1, const double* x2, int64_t n, double* out,
-                         cudaStream_t s) {
-  if (n == 0) return BGP_OK;
+                         cudaStream_t s, int members = 1, int64_t ostride = 0) {
+  if (n == 0 || members == 0) return BGP_OK;
+  if (members > 65535) { set_error("kmat_diagonal: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
   const int blocks = (int)std::min<int64_t>((n + 255) / 256, 4 * num_sms());
-  kmat_diagonal_kernel<<<blocks, 256, 0, s>>>(dprog, x1, x2, n, out);
+  kmat_diagonal_kernel<<<dim3(blocks, members), 256, 0, s>>>(dprog, x1, x2, n, out, ostride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }

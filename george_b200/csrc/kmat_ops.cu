@@ -53,9 +53,13 @@ __global__ void __launch_bounds__(MV_THREADS) kmat_matvec_kernel(const DevProgra
                                                                  const double* __restrict__ x1, int64_t n1,
                                                                  const double* __restrict__ x2, int64_t n2,
                                                                  const double* __restrict__ V, int64_t ldv, int nrhs,
-                                                                 double* __restrict__ partial, int chunks_per_split) {
+                                                                 double* __restrict__ partial, int chunks_per_split,
+                                                                 int64_t vstride, int64_t pstride) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   MvSmem* S = reinterpret_cast<MvSmem*>(smem_raw);
+  gprog += blockIdx.z;  // member blockIdx.z of a batch: its program, V + z * vstride, partial + z * pstride
+  V += blockIdx.z * vstride;
+  partial += blockIdx.z * pstride;
   const int nd = gprog->ndim;
   double* sx1 = reinterpret_cast<double*>(smem_raw + ((sizeof(MvSmem) + 15) & ~size_t(15)));
   double* sx2 = sx1 + MV_TI * nd + ((MV_TI * nd) & 1);
@@ -106,9 +110,14 @@ __global__ void __launch_bounds__(MV_THREADS) kmat_matvec_kernel(const DevProgra
 }
 
 // out[i + c*ldo] = sum_s partial[(s*n1 + i)*MV_NR + c]  (+ diag[i] * V[i + c*ldv])
+// (member blockIdx.y of a batch: partial + y * pstride, V + y * vstride, out + y * ostride)
 __global__ void kmat_matvec_reduce_kernel(const double* __restrict__ partial, int64_t n1, int nsplit, int nrhs,
                                           const double* __restrict__ diag, const double* __restrict__ V, int64_t ldv,
-                                          double* __restrict__ out, int64_t ldo) {
+                                          double* __restrict__ out, int64_t ldo, int64_t pstride, int64_t vstride,
+                                          int64_t ostride) {
+  partial += blockIdx.y * pstride;
+  V += blockIdx.y * vstride;
+  out += blockIdx.y * ostride;
   const int64_t total = n1 * nrhs;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t c = t / n1, i = t - c * n1;
@@ -124,6 +133,27 @@ static size_t matvec_smem(int nd) {
          sizeof(double) * ((size_t)MV_TI * nd + 1 + (size_t)MV_TJ * nd + (size_t)MV_NR * MV_TJ + (size_t)MV_THREADS * MV_NR);
 }
 
+// The column split of K(x1, x2) V (n1 x n2): nsplit groups of cps 512-column chunks, one partial per (split, row).
+// Enough CTAs for ~8 per SM; when there are few row tiles (predict at a handful of points) split the columns instead.
+int matvec_plan(int64_t n1, int64_t n2, int64_t* nsplit_out, int* cps_out) {
+  const int64_t row_tiles = (n1 + MV_TI - 1) / MV_TI;
+  const int64_t nchunks = (n2 + MV_TJ - 1) / MV_TJ;
+  int64_t nsplit = std::max<int64_t>(1, std::min<int64_t>(nchunks, (8 * (int64_t)num_sms() + row_tiles - 1) / row_tiles));
+  const int cps = (int)((nchunks + nsplit - 1) / nsplit);
+  nsplit = (nchunks + cps - 1) / cps;
+  if (row_tiles > 0x7fffffffLL || nsplit > 65535) { set_error("kmat_matvec: problem too large for one launch"); return BGP_ERR_INVALID; }
+  *nsplit_out = nsplit;
+  *cps_out = cps;
+  return BGP_OK;
+}
+// doubles of matvec partials per member (one right-hand side group)
+int64_t matvec_partial_size(int64_t n1, int64_t n2) {
+  int64_t nsplit = 1;
+  int cps = 1;
+  if (n1 <= 0 || n2 <= 0 || matvec_plan(n1, n2, &nsplit, &cps) != BGP_OK) return 0;
+  return nsplit * n1 * MV_NR;
+}
+
 // out (n1 x nrhs, column-major ldo) = K(x1, x2) V (n2 x nrhs, column-major ldv) [+ diag .* V, only when n1 == n2]
 int kmat_matvec_launch(const DevProgram* dprog, int nd, const double* x1, int64_t n1, const double* x2, int64_t n2,
                        const double* diag, const double* V, int64_t ldv, int64_t nrhs, double* out, int64_t ldo,
@@ -137,23 +167,48 @@ int kmat_matvec_launch(const DevProgram* dprog, int nd, const double* x1, int64_
   cudaFuncSetAttribute(kmat_matvec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   const size_t smem = matvec_smem(nd);
   const int64_t row_tiles = (n1 + MV_TI - 1) / MV_TI;
-  const int64_t nchunks = (n2 + MV_TJ - 1) / MV_TJ;
-  // enough CTAs for ~8 per SM; when there are few row tiles (predict at a handful of points) split the columns instead
-  int64_t nsplit = std::max<int64_t>(1, std::min<int64_t>(nchunks, (8 * (int64_t)num_sms() + row_tiles - 1) / row_tiles));
-  const int cps = (int)((nchunks + nsplit - 1) / nsplit);
-  nsplit = (nchunks + cps - 1) / cps;
-  if (row_tiles > 0x7fffffffLL || nsplit > 65535) { set_error("kmat_matvec: problem too large for one launch"); return BGP_ERR_INVALID; }
+  int64_t nsplit;
+  int cps;
+  BGP_TRY(matvec_plan(n1, n2, &nsplit, &cps));
   BGP_TRY(scratch.reserve((size_t)nsplit * (size_t)n1 * MV_NR, s));
   for (int64_t c0 = 0; c0 < nrhs; c0 += MV_NR) {
     const int nc = (int)std::min<int64_t>(MV_NR, nrhs - c0);
     dim3 grid((unsigned)row_tiles, (unsigned)nsplit);
-    kmat_matvec_kernel<<<grid, MV_THREADS, smem, s>>>(dprog, x1, n1, x2, n2, V + c0 * ldv, ldv, nc, scratch.p, cps);
+    kmat_matvec_kernel<<<grid, MV_THREADS, smem, s>>>(dprog, x1, n1, x2, n2, V + c0 * ldv, ldv, nc, scratch.p, cps, 0, 0);
     BGP_LAUNCH_CHECK();
     const int blocks = (int)std::min<int64_t>((n1 * nc + 255) / 256, 8 * (int64_t)num_sms());
     kmat_matvec_reduce_kernel<<<blocks, 256, 0, s>>>(scratch.p, n1, (int)nsplit, nc, diag, V + c0 * ldv, ldv,
-                                                     out + c0 * ldo, ldo);
+                                                     out + c0 * ldo, ldo, 0, 0, 0);
     BGP_LAUNCH_CHECK();
   }
+  return BGP_OK;
+}
+
+// `members` products of one right-hand side on the same x1, x2 in one launch each: member b computes
+// out + b * ostride (n1) = K_b(x1, x2) (V + b * vstride) with program dprogs[b], exactly as kmat_matvec_launch computes
+// it for that program (the same split plan, the same per-row order).  partial: members * matvec_partial_size(n1, n2).
+int kmat_matvec_batch_launch(const DevProgram* dprogs, int nd, int members, const double* x1, int64_t n1,
+                             const double* x2, int64_t n2, const double* V, int64_t vstride, double* out,
+                             int64_t ostride, double* partial, cudaStream_t s) {
+  if (n1 <= 0 || members <= 0) return BGP_OK;
+  if (members > 65535) { set_error("kmat_matvec: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
+  if (n2 <= 0) {
+    BGP_CUDA(cudaMemset2DAsync(out, sizeof(double) * ostride, 0, sizeof(double) * n1, members, s));
+    return BGP_OK;
+  }
+  cudaFuncSetAttribute(kmat_matvec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+  const int64_t row_tiles = (n1 + MV_TI - 1) / MV_TI;
+  int64_t nsplit;
+  int cps;
+  BGP_TRY(matvec_plan(n1, n2, &nsplit, &cps));
+  const int64_t pstride = nsplit * n1 * MV_NR;
+  kmat_matvec_kernel<<<dim3((unsigned)row_tiles, (unsigned)nsplit, (unsigned)members), MV_THREADS, matvec_smem(nd), s>>>(
+      dprogs, x1, n1, x2, n2, V, n2, 1, partial, cps, vstride, pstride);
+  BGP_LAUNCH_CHECK();
+  const int blocks = (int)std::min<int64_t>((n1 + 255) / 256, 8 * (int64_t)num_sms());
+  kmat_matvec_reduce_kernel<<<dim3(blocks, members), 256, 0, s>>>(partial, n1, (int)nsplit, 1, nullptr, V, n2, out, n1,
+                                                                  pstride, vstride, ostride);
+  BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
 
@@ -302,12 +357,16 @@ int64_t predict_chunk_cols(int64_t n, int64_t multiple) {
   return (c + multiple - 1) / multiple * multiple;
 }
 
-// partial[j * nsplit + b] = sum over the rows of split b of B[j*ld + i] * W[j*ld + i]; grid (c, nsplit)
+// partial[j * nsplit + b] = sum over the rows of split b of B[j*ld + i] * W[j*ld + i]; grid (c, nsplit, members):
+// member z reads B and W + z * mstride and writes partial + z * c * nsplit
 __global__ void __launch_bounds__(PV_THREADS) predict_var_partial_kernel(const double* __restrict__ B,
                                                                          const double* __restrict__ W, int64_t ld,
                                                                          int64_t n, int64_t rows_per_split,
-                                                                         double* __restrict__ partial) {
+                                                                         double* __restrict__ partial, int64_t mstride) {
   __shared__ double red[32];
+  B += blockIdx.z * mstride;
+  W += blockIdx.z * mstride;
+  partial += (int64_t)blockIdx.z * gridDim.x * gridDim.y;
   const int64_t j = blockIdx.x;
   const int64_t r0 = (int64_t)blockIdx.y * rows_per_split, r1 = min(n, r0 + rows_per_split);
   const double* b = B + j * ld;
@@ -318,9 +377,13 @@ __global__ void __launch_bounds__(PV_THREADS) predict_var_partial_kernel(const d
   if (threadIdx.x == 0) partial[j * gridDim.y + blockIdx.y] = s;
 }
 
-// var[j] = kdiag[j] - sum_b partial[j * nsplit + b], b ascending
+// var[j] = kdiag[j] - sum_b partial[j * nsplit + b], b ascending (member blockIdx.y of a batch: partial + y * c * nsplit,
+// kdiag and var + y * vstride)
 __global__ void predict_var_finish_kernel(const double* __restrict__ partial, int nsplit, const double* __restrict__ kdiag,
-                                          int64_t c, double* __restrict__ var) {
+                                          int64_t c, double* __restrict__ var, int64_t vstride) {
+  partial += blockIdx.y * c * nsplit;
+  kdiag += blockIdx.y * vstride;
+  var += blockIdx.y * vstride;
   for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < c; j += (int64_t)gridDim.x * blockDim.x) {
     double s = 0.0;
     for (int b = 0; b < nsplit; ++b) s += partial[j * nsplit + b];
@@ -328,27 +391,52 @@ __global__ void predict_var_finish_kernel(const double* __restrict__ partial, in
   }
 }
 
-// var (c) = kdiag - colsum(B .* W); B, W: n x c column-major, leading dimension ld (B == W for the dense solver)
-int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
-                       double* var, DevBuf<double>& scratch, cudaStream_t s) {
-  if (c <= 0) return BGP_OK;
+// the row split of a variance chunk of c columns of n rows: nsplit groups of `rows` rows, one partial per (column, group)
+static void predict_var_plan(int64_t n, int64_t c, int64_t* nsplit_out, int64_t* rows_out) {
   int64_t nsplit = std::max<int64_t>(1, std::min<int64_t>((4 * (int64_t)num_sms() + c - 1) / c, (n + PV_MIN_ROWS - 1) / PV_MIN_ROWS));
   const int64_t rows = (n + nsplit - 1) / nsplit;
-  nsplit = (n + rows - 1) / rows;
-  if (c > 0x7fffffffLL || nsplit > 65535) { set_error("predict: chunk too large for one launch"); return BGP_ERR_INVALID; }
-  BGP_TRY(scratch.reserve((size_t)(c * nsplit), s));
-  predict_var_partial_kernel<<<dim3((unsigned)c, (unsigned)nsplit), PV_THREADS, 0, s>>>(B, W, ld, n, rows, scratch.p);
+  *nsplit_out = (n + rows - 1) / rows;
+  *rows_out = rows;
+}
+// doubles of variance partials per member for a chunk of c columns
+int64_t predict_var_partial_size(int64_t n, int64_t c) {
+  if (c <= 0) return 0;
+  int64_t nsplit, rows;
+  predict_var_plan(n, c, &nsplit, &rows);
+  return c * nsplit;
+}
+
+// var (c) = kdiag - colsum(B .* W); B, W: n x c column-major, leading dimension ld (B == W for the dense solver).
+// `members` > 1: member b reads B and W + b * mstride and writes var + b * vstride from kdiag + b * vstride, in the
+// same two launches; scratch holds members * predict_var_partial_size(n, c).
+int predict_var_batch_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
+                             double* var, int members, int64_t mstride, int64_t vstride, DevBuf<double>& scratch,
+                             cudaStream_t s) {
+  if (c <= 0 || members <= 0) return BGP_OK;
+  int64_t nsplit, rows;
+  predict_var_plan(n, c, &nsplit, &rows);
+  if (c > 0x7fffffffLL || nsplit > 65535 || members > 65535) { set_error("predict: chunk too large for one launch"); return BGP_ERR_INVALID; }
+  BGP_TRY(scratch.reserve((size_t)(c * nsplit * members), s));
+  predict_var_partial_kernel<<<dim3((unsigned)c, (unsigned)nsplit, (unsigned)members), PV_THREADS, 0, s>>>(
+      B, W, ld, n, rows, scratch.p, mstride);
   BGP_LAUNCH_CHECK();
-  predict_var_finish_kernel<<<(unsigned)std::min<int64_t>((c + 255) / 256, 4 * (int64_t)num_sms()), 256, 0, s>>>(
-      scratch.p, (int)nsplit, kdiag, c, var);
+  predict_var_finish_kernel<<<dim3((unsigned)std::min<int64_t>((c + 255) / 256, 4 * (int64_t)num_sms()), (unsigned)members),
+                              256, 0, s>>>(scratch.p, (int)nsplit, kdiag, c, var, vstride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
+int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
+                       double* var, DevBuf<double>& scratch, cudaStream_t s) {
+  return predict_var_batch_launch(B, W, ld, n, c, kdiag, var, 1, 0, 0, scratch, s);
+}
 
 // C[j*ldc + i] += sum_s slices[s*m*nn + j*m + i], s ascending; `lower`: only i >= j, mirrored to C[i*ldc + j]
+// (member blockIdx.y of a batch: slices + y * nsplit * m * nn, C + y * cstride)
 __global__ void predict_slices_add_kernel(const double* __restrict__ slices, int nsplit, int64_t m, int64_t nn,
-                                          double* __restrict__ C, int64_t ldc, int lower) {
+                                          double* __restrict__ C, int64_t ldc, int lower, int64_t cstride) {
   const int64_t total = m * nn;
+  slices += blockIdx.y * nsplit * total;
+  C += blockIdx.y * cstride;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t j = t / m, i = t - j * m;
     if (lower && i < j) continue;
@@ -360,40 +448,58 @@ __global__ void predict_slices_add_kernel(const double* __restrict__ slices, int
   }
 }
 
-// C (m x nn, column-major ldc) -= A'B' with A'(i, k) = A[i*lda + k], B'(k, j) = B[j*ldb + k], k < K: the (1, 1) DMMA
-// variant split over K into nsplit zeroed slices (each one GD_SUB target), then added into C in a fixed order.
-// `lower` (m == nn, A == B): only the lower triangle is computed and the result is mirrored, so C stays exactly symmetric.
-int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
-                     bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s) {
-  if (m <= 0 || nn <= 0) return BGP_OK;
-  if (m > 0x7fffffffLL || nn > 0x7fffffffLL || K > 0x7fffffffLL) { set_error("predict: GEMM too large"); return BGP_ERR_INVALID; }
+// The split-K plan of the covariance product (m x nn, K deep): nsplit slices of klen (a multiple of GD_BK) each
+void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, int64_t* klen_out) {
   const int64_t tiles = ((m + GD_BM - 1) / GD_BM) * ((nn + GD_BN - 1) / GD_BN);
   int64_t nsplit = (2 * (int64_t)num_sms() + tiles - 1) / tiles;                   // ~2 CTAs per SM
   nsplit = std::min<int64_t>(nsplit, std::max<int64_t>(1, (K + 255) / 256));      // >= 256 of K per split
   nsplit = std::min<int64_t>(nsplit, std::max<int64_t>(1, PREDICT_BUDGET / (m * nn)));
   int64_t klen = (K + nsplit - 1) / nsplit;
   klen = (klen + GD_BK - 1) / GD_BK * GD_BK;
-  nsplit = std::max<int64_t>(1, (K + klen - 1) / klen);
+  *nsplit_out = std::max<int64_t>(1, (K + klen - 1) / klen);
+  *klen_out = klen;
+}
+
+// C (m x nn, column-major ldc) -= A'B' with A'(i, k) = A[i*lda + k], B'(k, j) = B[j*ldb + k], k < K: the (1, 1) DMMA
+// variant split over K into nsplit zeroed slices (each one GD_SUB target), then added into C in a fixed order.
+// `lower` (m == nn, A == B): only the lower triangle is computed and the result is mirrored, so C stays exactly symmetric.
+// `members` > 1: member b uses A and B + b * abstride and C + b * cstride; all members' slices go through one DMMA
+// launch (nsplit * members descriptors, member-major) and one add, so the launch count does not depend on members
+// while nsplit * members <= 65535.
+int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn,
+                             int64_t K, bool lower, double* C, int64_t ldc, int members, int64_t abstride,
+                             int64_t cstride, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s) {
+  if (m <= 0 || nn <= 0 || members <= 0) return BGP_OK;
+  if (m > 0x7fffffffLL || nn > 0x7fffffffLL || K > 0x7fffffffLL) { set_error("predict: GEMM too large"); return BGP_ERR_INVALID; }
+  if (members > 65535) { set_error("predict: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
+  int64_t nsplit, klen;
+  predict_gemm_plan(m, nn, K, &nsplit, &klen);
   const int64_t slice = m * nn;
-  BGP_TRY(slices.reserve((size_t)(slice * nsplit), s));
-  BGP_CUDA(cudaMemsetAsync(slices.p, 0, sizeof(double) * slice * nsplit, s));
-  std::vector<GemmDesc> hd((size_t)nsplit);
-  for (int64_t sp = 0; sp < nsplit; ++sp) {
-    const int64_t k0 = sp * klen;
-    GemmDesc& d = hd[(size_t)sp];
-    d.A = A + k0; d.lda = lda;
-    d.B = B + k0; d.ldb = ldb;
-    d.C = slices.p + sp * slice; d.ldc = m;
-    d.M = (int)m; d.N = (int)nn; d.K = (int)std::max<int64_t>(0, std::min(klen, K - k0));
-    d.mode = GD_SUB | (lower ? GD_LOWER : 0);
-  }
-  BGP_TRY(descs.reserve((size_t)nsplit, s));
-  BGP_CUDA(cudaMemcpyAsync(descs.p, hd.data(), sizeof(GemmDesc) * nsplit, cudaMemcpyHostToDevice, s));
-  BGP_TRY((gemm_dmma_launch<true, true>(descs.p, (int)nsplit, (int)m, (int)nn, nullptr, s)));
-  predict_slices_add_kernel<<<(unsigned)std::min<int64_t>((slice + 255) / 256, 8 * (int64_t)num_sms()), 256, 0, s>>>(
-      slices.p, (int)nsplit, m, nn, C, ldc, lower ? 1 : 0);
+  const int64_t nslices = nsplit * members;
+  BGP_TRY(slices.reserve((size_t)(slice * nslices), s));
+  BGP_CUDA(cudaMemsetAsync(slices.p, 0, sizeof(double) * slice * nslices, s));
+  std::vector<GemmDesc> hd((size_t)nslices);
+  for (int64_t mb = 0; mb < members; ++mb)
+    for (int64_t sp = 0; sp < nsplit; ++sp) {
+      const int64_t k0 = sp * klen;
+      GemmDesc& d = hd[(size_t)(mb * nsplit + sp)];
+      d.A = A + mb * abstride + k0; d.lda = lda;
+      d.B = B + mb * abstride + k0; d.ldb = ldb;
+      d.C = slices.p + (mb * nsplit + sp) * slice; d.ldc = m;
+      d.M = (int)m; d.N = (int)nn; d.K = (int)std::max<int64_t>(0, std::min(klen, K - k0));
+      d.mode = GD_SUB | (lower ? GD_LOWER : 0);
+    }
+  BGP_TRY(descs.reserve((size_t)nslices, s));
+  BGP_CUDA(cudaMemcpyAsync(descs.p, hd.data(), sizeof(GemmDesc) * nslices, cudaMemcpyHostToDevice, s));
+  BGP_TRY((gemm_dmma_launch<true, true>(descs.p, (int)nslices, (int)m, (int)nn, nullptr, s)));
+  predict_slices_add_kernel<<<dim3((unsigned)std::min<int64_t>((slice + 255) / 256, 8 * (int64_t)num_sms()), (unsigned)members),
+                              256, 0, s>>>(slices.p, (int)nsplit, m, nn, C, ldc, lower ? 1 : 0, cstride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
+}
+int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
+                     bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s) {
+  return predict_gemm_sub_members(A, lda, B, ldb, m, nn, K, lower, C, ldc, 1, 0, 0, slices, descs, s);
 }
 
 }  // namespace bgp

@@ -305,9 +305,14 @@ class GP(ModelSet):
             model.set_parameter_vector(saved, include_frozen=True)
             model.dirty = dirty
 
-    def _batch_device(self, batch, vectors, y, quiet):
-        """The batched dense path; ``None`` when the kernel has no valid device program (the loop then reproduces
-        whatever the per-vector path does with it)."""
+    def _batch_members(self, vectors, y, residual, const_residual):
+        """The per-member host inputs of the batched dense paths: ``(spec, full, kpar, sigma, resid, fact_err,
+        mean_err)``, or ``None`` when the kernel has no valid device program (the loop then reproduces whatever the
+        per-vector path does with it).  ``full`` holds the members' full parameter vectors, ``kpar`` their kernel part;
+        ``sigma`` and ``resid`` (``(B, n)``) are built with the elementwise operations of :func:`_sigma` and of
+        ``residual`` (the method the single path forms its residual with), ``const_residual(c)`` being that residual
+        for a constant mean ``c``.  ``fact_err[b]`` / ``mean_err[b]`` is the exception the per-vector path meets while
+        factorising (white noise) and while forming the residual (mean), or ``None``."""
         try:
             spec = flatten(self.kernel)
         except Exception:
@@ -323,8 +328,6 @@ class GP(ModelSet):
             return None
         y = self._check_dimensions(y)
 
-        # per member, the exception the per-vector path meets first: while factorising (white noise, device) and
-        # then while forming the residual (mean)
         fact_err, mean_err = [None] * nb, [None] * nb
         sigma = np.empty((nb, n), dtype=np.float64)
         if type(self.white_noise) is ConstantModel:
@@ -341,41 +344,56 @@ class GP(ModelSet):
                     sigma[b] = 1.0
         resid = np.empty((nb, n), dtype=np.float64)
         if type(self.mean) is ConstantModel:
-            for b in range(nb):  # the operations of GP._residual_of
+            for b in range(nb):
                 c = float(full[b, 0])
                 if not np.isfinite(c):
                     try:
-                        self._swap_eval(self.mean, full[b, :n_mean], lambda: self._residual_of(y))
+                        self._swap_eval(self.mean, full[b, :n_mean], lambda: residual(y))
                     except Exception as exc:
                         mean_err[b] = exc
                     resid[b] = 0.0
                 else:
-                    resid[b] = y if c == 0.0 else y - c
+                    resid[b] = const_residual(y, c)
         else:
             for b in range(nb):
                 try:
-                    resid[b] = self._swap_eval(self.mean, full[b, :n_mean], lambda: self._residual_of(y))
+                    resid[b] = self._swap_eval(self.mean, full[b, :n_mean], lambda: residual(y))
                 except Exception as exc:
                     mean_err[b] = exc
                     resid[b] = 0.0
+        return spec, full, kpar, sigma, resid, fact_err, mean_err
 
+    @staticmethod
+    def _batch_factor_error(spec, kpar, b, err, info):
+        """The exception member ``b``'s factorisation raises on the per-vector path (``err``: the white-noise one),
+        from the batch's ``info``; ``None`` when it succeeds."""
+        if err is not None or info == 0:
+            return err
+        if info > 0:
+            return LinAlgError("%d-th leading minor of the array is not positive definite" % info)
+        member = patch_specs(spec, kpar[b:b + 1])[0]
+        try:
+            _lib.check(_lib.load().bgp_spec_validate(C.byref(member)))
+        except Exception as e:
+            return e
+        return ValueError("invalid kernel")
+
+    def _batch_device(self, batch, vectors, y, quiet):
+        """The batched dense path of :func:`batch_log_likelihood`; ``None`` when the kernel has no valid device
+        program."""
+        members = self._batch_members(vectors, y, self._residual_of,
+                                      lambda y, c: y if c == 0.0 else y - c)  # the operations of GP._residual_of
+        if members is None:
+            return None
+        spec, _, kpar, sigma, resid, fact_err, mean_err = members
+        n = len(self._x)
         log_det, quad, info = batch(spec, kpar, self._x, sigma, resid)
         # GP.compute / GP.log_likelihood, in the same order of operations
         const = -0.5 * (n * np.log(2 * np.pi) + log_det)
         ll = const - 0.5 * quad
         ll[~np.isfinite(ll)] = -np.inf
-        for b in range(nb):
-            exc = fact_err[b]
-            if exc is None and info[b] > 0:
-                exc = LinAlgError("%d-th leading minor of the array is not positive definite" % info[b])
-            elif exc is None and info[b] < 0:
-                member = patch_specs(spec, kpar[b:b + 1])[0]
-                try:
-                    _lib.check(_lib.load().bgp_spec_validate(C.byref(member)))
-                except Exception as e:
-                    exc = e
-                else:
-                    exc = ValueError("invalid kernel")
+        for b in range(len(vectors)):
+            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
             if exc is not None:
                 ll[b] = -np.inf
                 if not (quiet and isinstance(exc, (ValueError, LinAlgError))):
@@ -387,6 +405,85 @@ class GP(ModelSet):
                 if not (quiet and isinstance(exc, ValueError) and "mean function" in str(exc)):
                     raise exc
         return ll
+
+    def batch_predict(self, vectors, y, t, return_cov=True, return_var=False, kernel=None):
+        """:func:`predict` at many parameter vectors: ``mu`` (``(B, ns)``), ``(mu, var)`` or ``(mu, cov)`` (``var``
+        ``(B, ns)``, ``cov`` ``(B, ns, ns)``; ``return_var`` wins, as in :func:`predict`).  Entry ``b`` is bit for bit
+        what ``gp.set_parameter_vector(vectors[b]); gp.predict(y, t, return_cov=..., return_var=...)`` returns on the
+        computed ``x`` and ``yerr``: the posterior predictive of a sampler's chain in one call.  The GP is left as it
+        was: parameter vector, factorisation, cached solve and dirty flags.
+
+        The call raises the exception that loop would raise first, with its type and message, with one difference:
+        the checks that do not depend on the member (the shape of ``vectors``, ``y``'s length, ``t``'s dimension)
+        come first, so when member 0 would also fail to factorise the loop raises that error instead.  With no
+        members or no test points nothing is computed and the empty results are returned.
+
+        Solvers with a ``batch_predict`` hook (``BasicSolver``) factorise and predict all members in one batched pass
+        on the device; any other solver (``HODLRSolver``, ``TrivialSolver``, plug-ins), and an explicit ``kernel``,
+        take that loop.
+
+        :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
+        """
+        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
+            raise RuntimeError("You need to compute the model first")
+        vectors = np.asarray(vectors, dtype=np.float64)
+        if vectors.ndim != 2 or vectors.shape[1] != len(self):
+            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        self._check_dimensions(y)
+        xs = self.parse_samples(t)
+        what = "var" if return_var else ("cov" if return_cov else None)
+        nb, ns = len(vectors), len(xs)
+        if nb == 0 or ns == 0:
+            mu = np.empty((nb, ns), dtype=np.float64)
+            if what is None:
+                return mu
+            return mu, np.empty((nb, ns) if what == "var" else (nb, ns, ns), dtype=np.float64)
+        batch = getattr(self.solver_type, "batch_predict", None)
+        if batch is not None and kernel is None:
+            out = self._batch_predict_device(batch, vectors, y, xs, what)
+            if out is not None:
+                return out
+        return self._batch_predict_loop(vectors, y, t, return_cov, return_var, kernel)
+
+    def _batch_predict_loop(self, vectors, y, t, return_cov, return_var, kernel):
+        state = self._batch_state()
+        try:
+            res = []
+            for v in vectors:
+                self.set_parameter_vector(v)
+                res.append(self.predict(y, t, return_cov=return_cov, return_var=return_var, kernel=kernel))
+        finally:
+            self._batch_restore(state)
+        if not (return_var or return_cov):
+            return np.stack(res)
+        return np.stack([r[0] for r in res]), np.stack([r[1] for r in res])
+
+    def _batch_predict_device(self, batch, vectors, y, xs, what):
+        """The batched dense path of :func:`batch_predict`; ``None`` when the kernel has no valid device program."""
+        members = self._batch_members(vectors, y, self._residual,
+                                      lambda y, c: y - (c + np.zeros(len(y))))  # GP._residual of a ConstantModel
+        if members is None:
+            return None
+        spec, full, kpar, sigma, resid, fact_err, mean_err = members
+        nb, ns, n_mean = len(vectors), len(xs), self.mean.full_size
+        # the mean model at x*, what GP.predict adds last (a non-finite constant already failed in the residual)
+        mean_xs, xs_err = np.zeros((nb, ns), dtype=np.float64), [None] * nb
+        for b in range(nb):
+            if type(self.mean) is ConstantModel:
+                mean_xs[b] = float(full[b, 0]) + np.zeros(ns)
+                continue
+            try:
+                mean_xs[b] = self._swap_eval(self.mean, full[b, :n_mean], lambda: self._call_mean(xs))
+            except Exception as exc:
+                xs_err[b] = exc
+        mu, out, info = batch(spec, kpar, self._x, sigma, resid, xs, what)
+        for b in range(nb):  # the loop's order: white noise, factorisation, residual, mean at x*
+            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
+            exc = exc if exc is not None else (mean_err[b] if mean_err[b] is not None else xs_err[b])
+            if exc is not None:
+                raise exc
+        mu += mean_xs
+        return mu if what is None else (mu, out)
 
     def lnlikelihood(self, y, quiet=False):
         warnings.warn("'lnlikelihood' is deprecated. Use 'log_likelihood'", DeprecationWarning)

@@ -33,7 +33,7 @@ class _DenseHandle(object):
 
 
 class _BatchHandle(object):
-    """Owns a ``bgp_dense_batch_t*`` (device workspace of ``BasicSolver.batch_log_likelihood``)."""
+    """Owns a ``bgp_dense_batch_t*`` (device workspace of ``BasicSolver.batch_log_likelihood`` / ``batch_predict``)."""
 
     def __init__(self):
         self.lib = _lib.load()
@@ -241,6 +241,54 @@ class BasicSolver(object):
             h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim, _lib.ptr(yerr),
             _lib.ptr(r), _lib.ptr(log_det), _lib.ptr(quad), _lib.ptr(info)))
         return log_det, quad, info
+
+    @staticmethod
+    def batch_predict(spec, params, x, yerr, r, xs, what):
+        """``(mean, out, info)`` for ``B`` parameter vectors of one kernel program on the same ``x``: member ``b``
+        factorises as in :func:`batch_log_likelihood`, ``mean[b] = K_b(xs, x) K_b^-1 r[b]`` (``(B, ns)``, the kernel
+        part of ``GP.predict``'s mean), ``out`` is ``None`` (``what=None``), the variances (``"var"``, ``(B, ns)``) or
+        the covariances (``"cov"``, ``(B, ns, ns)``) of :func:`predictive` (``include/bgp.h: bgp_dense_batch_predict``).
+        ``info`` is that of :func:`batch_log_likelihood`; a failed member's rows are NaN.  Every entry is bit-identical
+        to :func:`compute` with member ``b``'s spec and yerr followed by ``apply_inverse(r[b])``, ``kernel.matvec`` and
+        :func:`predictive`.  ``xs``: ``(ns,)`` or ``(ns, ndim)``."""
+        kinds = {None: 0, "var": _lib.BGP_PREDICT_VAR, "cov": _lib.BGP_PREDICT_COV}
+        if what not in kinds:
+            raise ValueError("what must be None, 'var' or 'cov'")
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.ndim == 1:
+            x = x[:, None]
+        xs = np.ascontiguousarray(xs, dtype=np.float64)
+        if xs.ndim == 1:
+            xs = xs[:, None]
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
+        r = np.ascontiguousarray(r, dtype=np.float64)
+        if x.ndim != 2 or x.shape[0] == 0:
+            raise ValueError("x must have shape (n, ndim) with n > 0")
+        n, ndim = x.shape
+        if params.ndim != 2 or params.shape[1] != num_params(spec):
+            raise ValueError("params must have shape (B, {0})".format(num_params(spec)))
+        nb = params.shape[0]
+        if yerr.shape != (nb, n) or r.shape != (nb, n):
+            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
+        if ndim != spec.ndim or xs.ndim != 2 or xs.shape[1] != ndim:
+            raise DimensionMismatch("dimension mismatch")
+        ns = xs.shape[0]
+        mean = np.empty((nb, ns), dtype=np.float64)
+        out = None
+        if what == "var":
+            out = np.empty((nb, ns), dtype=np.float64)
+        elif what == "cov":
+            out = np.empty((nb, ns, ns), dtype=np.float64)
+        info = np.zeros(nb, dtype=np.int32)
+        if nb == 0:
+            return mean, out, info
+        h = _get_batch_handle()
+        _lib.check(h.lib.bgp_dense_batch_predict(
+            h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim, _lib.ptr(yerr),
+            _lib.ptr(r), _lib.ptr(xs), ns, kinds[what], _lib.ptr(mean), _lib.ptr(out) if out is not None else None,
+            _lib.ptr(info)))
+        return mean, out, info
 
     # Device handles cannot be pickled.  Like the reference (which pickles its numpy factor, tests/test_pickle.py:21-36:
     # "Unpickled GP shouldn't need to be computed") the Cholesky factor travels with the pickle and is re-uploaded.

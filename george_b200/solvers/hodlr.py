@@ -15,8 +15,9 @@ __all__ = ["HODLRSolver"]
 
 class HODLRSolver(BasicSolver):
 
-    # no batched HODLR factorisation: GP.batch_log_likelihood takes its per-vector loop
+    # no batched HODLR factorisation: GP.batch_log_likelihood and GP.batch_predict take their per-vector loops
     batch_log_likelihood = None
+    batch_predict = None
 
     def __init__(self, kernel, min_size=100, tol=0.1, seed=42, rng_mode=None, rank_capacity=0,
                  exhaust="dense"):

@@ -246,6 +246,34 @@ int bgp_dense_batch_log_likelihood(bgp_dense_batch_t* h, const bgp_kernel_spec_t
                                    int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
                                    const double* yerr, const double* r,
                                    double* log_det, double* quad, int32_t* info);
+/* Batched predictions (GP.batch_predict): for the same B members as bgp_dense_batch_log_likelihood (spec, params, x,
+ * yerr; r = y - mean(x) per member, B x n row-major) and the test points xs (ns x ndim row-major, host):
+ *   mean[b*ns + j]        = (K_b(x*, x) K_b^-1 r_b)_j            (the kernel part of GP.predict's mean)
+ *   out == NULL           mean only
+ *   what == BGP_PREDICT_VAR   out[b*ns + j]        = k_b(x*_j, x*_j) - K_b(x*_j, x) K_b^-1 K_b(x, x*_j)
+ *   what == BGP_PREDICT_COV   out[(b*ns + i)*ns + j] = K_b**(i, j) - K_b(x*_i, x) K_b^-1 K_b(x, x*_j)
+ * Every entry is bit-identical to the single path on member b's spec and yerr: alpha = bgp_dense_apply_inverse of r_b
+ * (one right-hand side), the mean = bgp_kmat_matvec(xs, x, alpha), VAR / COV = bgp_dense_predict after
+ * bgp_dense_compute.  Each step runs the single path's kernels with a member index, with its split and chunk decisions
+ * (test-point chunks of predict_chunk_cols(n) columns, BGP_PREDICT_CHUNK applies alike); a member's results therefore
+ * do not depend on B, its position or the chunking.  info[b] as in bgp_dense_batch_log_likelihood; a failed member's
+ * rows of mean and out are NaN and do not disturb the other members.
+ * Members run in chunks that fit in 4 GiB of device memory (BGP_BATCH_CHUNK=<members> overrides it; a covariance chunk
+ * also keeps its split-K product to one launch); every step of a chunk is one launch for all its members, so the launch
+ * count depends on n, ns and the number of chunks, never on B within a chunk.
+ * Device workspace per member (doubles): n^2 + (4 + t) n + ns + P_mv, t = 8 with out (the few-column solve), 1 without,
+ * P_mv = nsplit_mv * ns * 4 matvec partials (nsplit_mv <= ceil(n / 512)); VAR adds n c + 2 c + P_var (c the test-point
+ * chunk, P_var <= c * ceil(n / 1024) partials); COV adds n ns + ns^2 (1 + nsplit) (K** and the split-K slices,
+ * nsplit * ns^2 <= max(ns^2, 2^27)).  Shared: B programs, x, xs.  The handle keeps it for the next call.
+ * Errors: those of bgp_dense_batch_log_likelihood; BGP_ERR_INVALID for ns < 0 or an unknown `what` with out != NULL.
+ * B == 0 writes nothing. */
+int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params,
+                            int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
+                            const double* yerr, const double* r,            /* B x n, row-major            */
+                            const double* xs, int64_t ns, int32_t what,      /* BGP_PREDICT_VAR / _COV       */
+                            double* mean,                                    /* B x ns                       */
+                            double* out,                                     /* B x ns, B x ns x ns, or NULL */
+                            int32_t* info);
 
 /* ------------------------------------------------------------------------------------------
  * HODLR solver.  Replaces _hodlr.HODLRSolver (src/george/solvers/_hodlr.cpp:115-204) and the
