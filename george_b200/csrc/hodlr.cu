@@ -114,6 +114,9 @@ struct bgp_hodlr {
   DevBuf<AcaDesc> d_aca;
   DevBuf<AcaOut> d_aca_out;
   DevBuf<NodeDesc> d_nodes;
+  DevBuf<PanelTile> d_ptiles;                // finalize_panels_kernel's row tiles (top set first)
+  int small_limit = SS_MAX_N;                // 2r above which a level takes launch_level_big (BGP_SMALL_RANK_LIMIT)
+  bool leaf_cols_wide = false;               // BGP_LEAF_COLS=32
   DevBuf<int> d_idx, d_piv_rows, d_piv_cols, d_ticket, d_chain_done, d_ncols_by_depth;
   DevBuf<uint32_t> d_chain_state;
   DevBuf<A2Node> d_a2nodes;
@@ -175,14 +178,31 @@ constexpr int LS_MAX_LEAF = (int)(LS_SMEM_MAX / sizeof(double));  // 25600 rows:
 
 static bool leaf_solve_fits(int max_leaf, int cols) { return sizeof(double) * (size_t)max_leaf * cols <= LS_SMEM_MAX; }
 
+// cudaFuncSetAttribute applies to the current device: the sweep kernels that take more than the default 48 KB of dynamic
+// shared memory get their limits once per device, not at every level of every call.
+static void set_sweep_func_attrs() {
+  static std::atomic<uint64_t> done{0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const uint64_t bit = dev < 64 ? (1ull << dev) : 0;
+  if (bit && (done.load(std::memory_order_relaxed) & bit)) return;
+  cudaFuncSetAttribute(leaf_solve_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
+  cudaFuncSetAttribute(leaf_solve_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
+  cudaFuncSetAttribute(leaf_solve_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
+  cudaFuncSetAttribute(leaf_solve_kernel<LS_COLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
+  cudaFuncSetAttribute(leaf_solve_kernel<LS_COLS_WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
+  cudaFuncSetAttribute(small_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+  done.fetch_or(bit, std::memory_order_relaxed);
+}
+
 template <int COLS>
 static int leaf_solve_launch(bgp_hodlr* h, double* X, int64_t ldx, const int* ncols_by_depth, int ncols_fixed,
                              int max_cols, cudaStream_t s) {
-  const dim3 grid((unsigned)h->leaves.size(), (unsigned)((max_cols + COLS - 1) / COLS));
+  const int ngroups = (max_cols + COLS - 1) / COLS;
+  const dim3 grid((unsigned)(h->leaves.size() * (size_t)ngroups));
   const size_t smem = sizeof(double) * (size_t)h->max_leaf * COLS;
-  // (the attribute is per device / context: set it on every call, it is cheap)
-  cudaFuncSetAttribute(leaf_solve_kernel<COLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
-  leaf_solve_kernel<COLS><<<grid, LS_THREADS, smem, s>>>(h->d_leaves.p, h->d_L.p, X, ldx, ncols_by_depth, ncols_fixed, h->max_leaf);
+  leaf_solve_kernel<COLS><<<grid, LS_THREADS, smem, s>>>(h->d_leaves.p, h->d_L.p, X, ldx, ncols_by_depth, ncols_fixed,
+                                                         h->max_leaf, ngroups);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
@@ -191,20 +211,27 @@ static int launch_leaf_solve(bgp_hodlr* h, double* X, int64_t ldx, const int* nc
                              int max_cols, cudaStream_t s) {
   const int nl = (int)h->leaves.size();
   if (nl == 0 || max_cols == 0) return BGP_OK;
-  // only leaves handled locally are in d_leaves.  Column groups of 8 by default.  BGP_LEAF_COLS=32 selects the 32-column
-  // instantiation for calls with more than 8 columns (the up-sweep): it streams the leaf factor once per 32 columns
-  // instead of once per 8, but at four times the serial work per CTA it measured slower on H100 (up-sweep 3.42 vs 3.36 ms,
-  // Matern32 N = 262144) — kept as an experiment.
+  // only leaves handled locally are in d_leaves.  The narrowest instantiation that covers the call (1, 2, 4 or 8
+  // columns; a one-column solve carries no 8-wide registers), wider calls in groups of 8.  BGP_LEAF_COLS=32 selects the
+  // 32-column instantiation for calls with more than 8 columns (the up-sweep): it streams the leaf factor once per 32
+  // columns instead of once per 8, but at four times the serial work per CTA it measured slower on H100 (up-sweep 3.42
+  // vs 3.36 ms, Matern32 N = 262144, before the groups of a leaf were scheduled together) — kept as an experiment.
+  // Leaves too large for the group in shared memory take the widest narrower one that fits.
   const int m = h->max_leaf;
-  if (const char* e = getenv("BGP_LEAF_COLS"))
-    if (atoi(e) > LS_COLS && max_cols > LS_COLS && leaf_solve_fits(m, LS_COLS_WIDE))
-      return leaf_solve_launch<LS_COLS_WIDE>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
-  if (leaf_solve_fits(m, LS_COLS)) return leaf_solve_launch<LS_COLS>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
-  if (leaf_solve_fits(m, 4)) return leaf_solve_launch<4>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
-  if (leaf_solve_fits(m, 2)) return leaf_solve_launch<2>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
-  if (leaf_solve_fits(m, 1)) return leaf_solve_launch<1>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
-  set_error("leaf size %d too large for the leaf solve kernel (at most %d rows)", m, LS_MAX_LEAF);  // compute() rejects it first
-  return BGP_ERR_INVALID;
+  if (h->leaf_cols_wide && max_cols > LS_COLS && leaf_solve_fits(m, LS_COLS_WIDE))
+    return leaf_solve_launch<LS_COLS_WIDE>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+  int cols = max_cols <= 1 ? 1 : max_cols <= 2 ? 2 : max_cols <= 4 ? 4 : LS_COLS;
+  while (cols > 1 && !leaf_solve_fits(m, cols)) cols /= 2;
+  if (!leaf_solve_fits(m, cols)) {
+    set_error("leaf size %d too large for the leaf solve kernel (at most %d rows)", m, LS_MAX_LEAF);  // compute() rejects it first
+    return BGP_ERR_INVALID;
+  }
+  switch (cols) {
+    case LS_COLS: return leaf_solve_launch<LS_COLS>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+    case 4: return leaf_solve_launch<4>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+    case 2: return leaf_solve_launch<2>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+    default: return leaf_solve_launch<1>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+  }
 }
 
 // one internal level: W = V^T X (both halves), small solve, X -= U T.   factor: up-sweep (X = U panel) vs plain solve
@@ -224,21 +251,26 @@ static int launch_level(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t ldx
   const size_t need = (size_t)nn * stride;
   if (need > h->w_cap) { set_error("internal: W workspace too small (%zu > %zu)", need, h->w_cap); return BGP_ERR_CUDA; }
   BGP_CUDA(cudaMemsetAsync(h->d_W.p, 0, sizeof(double) * need, s));
-  // diagnostics: BGP_SMALL_RANK_LIMIT=<2r> lowers the switch-over so the tests can drive every level through the big path
-  int small_limit = SS_MAX_N;
-  if (const char* e = getenv("BGP_SMALL_RANK_LIMIT")) small_limit = std::min(SS_MAX_N, atoi(e));
-  if (2 * r > small_limit) return launch_level_big(h, L, X, ldx, ncolsW, own_off, factor, col_lo, col_hi, s);
+  // h->small_limit: BGP_SMALL_RANK_LIMIT=<2r> (read at compute()) lowers the switch-over so the tests can drive every
+  // level through the big path
+  if (2 * r > h->small_limit) return launch_level_big(h, L, X, ldx, ncolsW, own_off, factor, col_lo, col_hi, s);
   const NodeDesc* nd = h->d_nodes.p + L.desc_off;
   const int max_nh = L.max_half + 1;
-  {
+  if (r <= GTS_MAX_R) {
+    dim3 grid((max_nh + GTS_ROWS - 1) / GTS_ROWS, nn * 2, (ncolsW + GTS_TC - 1) / GTS_TC);
+    const double* vb = h->pset(L).vbase();
+    const int64_t ldv = h->pset(L).ld;
+    if (r <= 2) gram_tn_small_kernel<2><<<grid, GTS_THREADS, 0, s>>>(nd, vb, ldv, X, ldx, ncolsW, h->d_W.p, stride);
+    else if (r <= 4) gram_tn_small_kernel<4><<<grid, GTS_THREADS, 0, s>>>(nd, vb, ldv, X, ldx, ncolsW, h->d_W.p, stride);
+    else gram_tn_small_kernel<GTS_MAX_R><<<grid, GTS_THREADS, 0, s>>>(nd, vb, ldv, X, ldx, ncolsW, h->d_W.p, stride);
+    BGP_LAUNCH_CHECK();
+  } else {
     dim3 grid((max_nh + GT_CHUNK - 1) / GT_CHUNK, nn * 2, (ncolsW + GT_TC - 1) / GT_TC);
     gram_tn_kernel<<<grid, GT_THREADS, 0, s>>>(nd, h->pset(L).vbase(), h->pset(L).ld, X, ldx, ncolsW, h->d_W.p, stride);
     BGP_LAUNCH_CHECK();
   }
   {
     const size_t sbytes = sizeof(double) * (size_t)(2 * r) * (2 * r);
-    // (the attribute is per device / context: set it on every call, it is cheap)
-    cudaFuncSetAttribute(small_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
     small_solve_kernel<<<nn, SS_THREADS, sbytes, s>>>(nd, h->d_W.p, stride, ncolsW, own_off, factor, h->d_S.p,
                                                       h->d_node_logdet.p, L.desc_off);
     BGP_LAUNCH_CHECK();
@@ -556,6 +588,12 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
   h->n = n;
   h->ndim = ndim;
   cudaStream_t sA = h->sA, sB = h->sB;
+  set_sweep_func_attrs();
+  // diagnostic switches of the sweeps, fixed for this factorisation and the solves that use it
+  h->small_limit = SS_MAX_N;
+  if (const char* e = getenv("BGP_SMALL_RANK_LIMIT")) h->small_limit = std::min(SS_MAX_N, atoi(e));
+  h->leaf_cols_wide = false;
+  if (const char* e = getenv("BGP_LEAF_COLS")) h->leaf_cols_wide = atoi(e) > LS_COLS;
 
   // ---- tree geometry ----
   h->nodes.clear(); h->leaves.clear(); h->levels.clear();
@@ -826,16 +864,29 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
     BGP_CUDA(cudaMemcpyAsync(h->d_nodes.p, hnd.data(), sizeof(NodeDesc) * ndesc, cudaMemcpyHostToDevice, sA));
     h->h_nodes = hnd;
     BGP_CUDA(cudaMemsetAsync(h->d_node_logdet.p, 0, sizeof(double) * ndesc, sA));
-    // the levels above the cut come first in the descriptor list: one launch per panel set
-    int rmax_set[2] = {0, 0};
-    for (auto& L : h->levels) rmax_set[L.set] = std::max(rmax_set[L.set], L.r);
-    if (ndesc_top > 0 && rmax_set[0] > 0) {
-      finalize_panels_kernel<<<dim3(ndesc_top, rmax_set[0]), 256, 0, sA>>>(h->d_nodes.p, h->top.vbase(), h->top.ld, h->top.ubase(), h->top.ld);
+    // the levels above the cut come first in the descriptor list: one launch per panel set, over FP_ROWS-row tiles of
+    // the nodes of rank > 0
+    std::vector<PanelTile> tiles;
+    int ntiles_top = 0;
+    for (int i = 0; i < ndesc; ++i) {
+      if (i == ndesc_top) ntiles_top = (int)tiles.size();
+      if (hnd[i].r == 0) continue;
+      for (int r0 = 0; r0 < hnd[i].size; r0 += FP_ROWS) tiles.push_back(PanelTile{i, r0});
+    }
+    if (ndesc_top == ndesc) ntiles_top = (int)tiles.size();
+    const int ntiles = (int)tiles.size();
+    if (ntiles > 0) {
+      BGP_TRY(h->d_ptiles.reserve(ntiles, sA));
+      BGP_CUDA(cudaMemcpyAsync(h->d_ptiles.p, tiles.data(), sizeof(PanelTile) * ntiles, cudaMemcpyHostToDevice, sA));
+    }
+    if (ntiles_top > 0) {
+      finalize_panels_kernel<<<ntiles_top, FP_THREADS, 0, sA>>>(h->d_nodes.p, h->d_ptiles.p, h->top.vbase(), h->top.ld,
+                                                                h->top.ubase(), h->top.ld);
       BGP_LAUNCH_CHECK();
     }
-    if (ndesc > ndesc_top && rmax_set[1] > 0) {
-      finalize_panels_kernel<<<dim3(ndesc - ndesc_top, rmax_set[1]), 256, 0, sA>>>(h->d_nodes.p + ndesc_top, h->loc.vbase(), h->loc.ld,
-                                                                                  h->loc.ubase(), h->loc.ld);
+    if (ntiles > ntiles_top) {
+      finalize_panels_kernel<<<ntiles - ntiles_top, FP_THREADS, 0, sA>>>(h->d_nodes.p, h->d_ptiles.p + ntiles_top,
+                                                                         h->loc.vbase(), h->loc.ld, h->loc.ubase(), h->loc.ld);
       BGP_LAUNCH_CHECK();
     }
   }
@@ -1018,7 +1069,7 @@ void bgp_hodlr_destroy(bgp_hodlr_t* h) {
   h->d_prog.release(); h->d_x.release(); h->d_yerr.release(); h->d_diag.release(); h->d_L.release();
   h->d_leaf_logdet.release(); h->d_node_logdet.release(); h->top.V.release(); h->top.U.release(); h->loc.V.release(); h->loc.U.release(); h->d_S.release();
   h->d_W.release(); h->d_scalar.release(); h->d_rhs.release(); h->d_leaves.release(); h->d_aca.release();
-  h->d_aca_out.release(); h->d_nodes.release(); h->d_idx.release(); h->d_piv_rows.release(); h->d_piv_cols.release();
+  h->d_aca_out.release(); h->d_nodes.release(); h->d_ptiles.release(); h->d_idx.release(); h->d_piv_rows.release(); h->d_piv_cols.release();
   h->lu_ws.d_nodes.release(); h->lu_ws.d_trsm.release(); h->lu_ws.d_gemm.release(); h->d_gram_desc.release(); h->d_upd_desc.release();
   h->d_ticket.release(); h->d_chain_done.release(); h->d_ncols_by_depth.release(); h->d_chain_state.release();
   h->d_a2nodes.release(); h->d_a2states.release(); h->d_a2rngs.release(); h->d_epart.release(); h->d_cand.release(); h->d_cand_k.release();

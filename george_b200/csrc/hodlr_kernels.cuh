@@ -205,29 +205,31 @@ __global__ void __launch_bounds__(LEAF_THREADS) leaf_build_factor_kernel(const D
 // ---------------------------------------------------------------------------------------------------------------
 // Leaf solve: X <- A^-1 X for the rows of each leaf and `ncols(depth)` columns of a column-major matrix
 // (hodlr.h:242 ldlt_.solve, applied to the ancestors' U in the up-sweep :95-102 and to the right-hand side in
-// solve :107-114).  grid = (leaf, column chunk); each thread owns one column of the chunk... the chunk of columns is
-// staged in shared memory and all threads cooperate on the substitutions.
+// solve :107-114).  One CTA per (leaf, group of COLS columns): the group is staged in shared memory and all threads
+// cooperate on the substitutions.  grid.x = leaf * ngroups + group, so the groups of one leaf are dispatched next to
+// each other and read the leaf's factor from L2 instead of once each from HBM.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int LS_THREADS = 256;
 constexpr int LS_COLS = 8;        // right-hand sides per CTA of the narrow instantiation (a solve: 1 .. 8 columns)
 constexpr int LS_COLS_WIDE = 32;  // ... of the wide one (BGP_LEAF_COLS=32; measured slower than four narrow groups, see hodlr.cu)
 constexpr int LS_NB = 32;         // diagonal block
+constexpr int LS_BATCH = 4;       // rows per lane loaded together in the backward column dots
 
 // Blocked substitution: per 32-column block of L, (a) the 32 x 32 diagonal block is staged in shared memory and each
 // warp solves it for its right-hand sides (columns w, w + 8, ...) with shuffles (no block barrier inside), (b) the rows
 // below (forward) / the columns of the block against the rows below (backward) are updated by the whole CTA with
 // coalesced, independent loads.  m / 32 block steps with two barriers each instead of m dependent steps.
 template <int COLS>
-__global__ void __launch_bounds__(LS_THREADS) leaf_solve_kernel(const LeafDesc* __restrict__ leaves,
+__global__ void __launch_bounds__(LS_THREADS, COLS <= LS_COLS ? 3 : 1) leaf_solve_kernel(const LeafDesc* __restrict__ leaves,
                                                                 const double* __restrict__ Lbuf,
                                                                 double* __restrict__ X, int64_t ldx,
                                                                 const int* __restrict__ ncols_by_depth, int ncols_fixed,
-                                                                int max_m) {
+                                                                int max_m, int ngroups) {
   extern __shared__ double xs[];  // max_m x COLS, column-major with leading dimension max_m
   __shared__ double sL[LS_NB][LS_NB + 1];
-  const LeafDesc lf = leaves[blockIdx.x];
+  const LeafDesc lf = leaves[blockIdx.x / ngroups];
   const int ncols = ncols_by_depth ? ncols_by_depth[lf.depth] : ncols_fixed;
-  const int c0 = blockIdx.y * COLS;
+  const int c0 = (blockIdx.x % ngroups) * COLS;
   if (c0 >= ncols) return;
   const int nc = min(COLS, ncols - c0);
   const int m = lf.size;
@@ -262,7 +264,7 @@ __global__ void __launch_bounds__(LS_THREADS) leaf_solve_kernel(const LeafDesc* 
 #pragma unroll
       for (int c = 0; c < COLS; ++c) acc[c] = 0.0;
       const double* Li = A + (int64_t)kb * m + i;
-#pragma unroll 4
+#pragma unroll 8
       for (int k = 0; k < nb; ++k) {
         const double l = Li[(int64_t)k * m];
 #pragma unroll
@@ -294,10 +296,20 @@ __global__ void __launch_bounds__(LS_THREADS) leaf_solve_kernel(const LeafDesc* 
 #pragma unroll
       for (int c = 0; c < COLS; ++c) acc[c] = 0.0;
       const double* Lk = A + (int64_t)(kb + k) * m;
-      for (int i = r0 + lane; i < m; i += 32) {
-        const double l = Lk[i];
+      // LS_BATCH rows per lane are loaded before they are used: one load latency per batch instead of one per row
+      // (the sums run over the rows in the same order either way)
+      for (int i0 = r0 + lane; i0 < m; i0 += 32 * LS_BATCH) {
+        double l[LS_BATCH];
 #pragma unroll
-        for (int c = 0; c < COLS; ++c) acc[c] += l * xs[c * max_m + i];
+        for (int j = 0; j < LS_BATCH; ++j) l[j] = (i0 + 32 * j < m) ? Lk[i0 + 32 * j] : 0.0;
+#pragma unroll
+        for (int j = 0; j < LS_BATCH; ++j) {
+          const int i = i0 + 32 * j;
+          if (i < m) {
+#pragma unroll
+            for (int c = 0; c < COLS; ++c) acc[c] += l[j] * xs[c * max_m + i];
+          }
+        }
       }
 #pragma unroll
       for (int c = 0; c < COLS; ++c) {
@@ -579,7 +591,9 @@ __global__ void __launch_bounds__(ACA_THREADS) aca_kernel(const DevProgram* __re
 
 // ---------------------------------------------------------------------------------------------------------------
 // Panel finalisation: U <- V for the used columns, zero padding up to the level's common rank (both panels).
-// One CTA per (node, column): rows of the node only.
+// One CTA per tile of FP_ROWS rows of one node (a host-built list, PanelTile), all r columns of the node's level: the
+// root's 2^k rows are spread over many CTAs instead of one CTA walking each column.  A copy and a zero fill, so the
+// panels do not depend on the tiling.
 // ---------------------------------------------------------------------------------------------------------------
 struct NodeDesc {
   int start, size, half, depth;
@@ -590,18 +604,34 @@ struct NodeDesc {
   int64_t s_off;  // offset of the node's (2r x 2r LU | 2r pivots) block in the S buffer
 };
 
-__global__ void finalize_panels_kernel(const NodeDesc* __restrict__ nodes, double* __restrict__ Vp, int64_t ldv,
-                                       double* __restrict__ Up, int64_t ldu) {
-  const NodeDesc nd = nodes[blockIdx.x];
-  const int k = blockIdx.y;
-  if (k >= nd.r) return;
-  double* v = Vp + (int64_t)(nd.vcol + k) * ldv + nd.start;
-  double* u = Up + (int64_t)(nd.ucol + k) * ldu + nd.start;
-  const bool used = k < nd.rank;
-  for (int i = threadIdx.x; i < nd.size; i += blockDim.x) {
-    double val = 0.0;
-    if (used) val = v[i]; else v[i] = 0.0;
-    u[i] = val;
+struct PanelTile {
+  int node;  // index into the NodeDesc array
+  int row0;  // first row of the tile, relative to the node's start
+};
+
+constexpr int FP_THREADS = 256;
+constexpr int FP_ROWS = 1024;  // rows per tile: 4 independent loads per thread and column
+
+__global__ void __launch_bounds__(FP_THREADS) finalize_panels_kernel(const NodeDesc* __restrict__ nodes,
+                                                                     const PanelTile* __restrict__ tiles,
+                                                                     double* __restrict__ Vp, int64_t ldv,
+                                                                     double* __restrict__ Up, int64_t ldu) {
+  const PanelTile t = tiles[blockIdx.x];
+  const NodeDesc nd = nodes[t.node];
+  const int row_hi = min(nd.size, t.row0 + FP_ROWS);
+  for (int k = 0; k < nd.r; ++k) {
+    double* v = Vp + (int64_t)(nd.vcol + k) * ldv + nd.start;
+    double* u = Up + (int64_t)(nd.ucol + k) * ldu + nd.start;
+    const bool used = k < nd.rank;
+#pragma unroll
+    for (int e = 0; e < FP_ROWS / FP_THREADS; ++e) {
+      const int i = t.row0 + e * FP_THREADS + threadIdx.x;
+      if (i < row_hi) {
+        double val = 0.0;
+        if (used) val = v[i]; else v[i] = 0.0;
+        u[i] = val;
+      }
+    }
   }
 }
 
@@ -670,6 +700,76 @@ __global__ void __launch_bounds__(GT_THREADS) gram_tn_kernel(const NodeDesc* __r
         if (c < nc) atomicAdd(Wh + (int64_t)(c0 + c) * ldw + q0 + tq, acc[e]);
       }
     }
+  }
+}
+
+// The same product for small ranks (r <= RQ <= GTS_MAX_R), where most of gram_tn_kernel's 32 q-lanes would stage and
+// multiply zeros: threads own rows (loads coalesced along the rows, V and X read once), each thread keeps all
+// r x GTS_TC products of its rows in registers, then a warp-shuffle + shared-memory reduction and one atomicAdd per
+// (q, c) per CTA.  grid = (row chunk of GTS_ROWS, node*2 + h, column tile of GTS_TC)
+constexpr int GTS_THREADS = 256;
+constexpr int GTS_ROWS = 1024;  // rows per CTA (4 per thread)
+constexpr int GTS_TC = 8;       // W cols (X columns) per CTA
+constexpr int GTS_MAX_R = 8;    // levels with 2r <= 16 take this kernel
+
+template <int RQ>
+__global__ void __launch_bounds__(GTS_THREADS) gram_tn_small_kernel(const NodeDesc* __restrict__ nodes,
+                                                                    const double* __restrict__ Vp, int64_t ldv,
+                                                                    const double* __restrict__ X, int64_t ldx, int ncols,
+                                                                    double* __restrict__ W, int64_t w_stride_node) {
+  constexpr int NW = GTS_THREADS / 32;
+  __shared__ double red[NW][RQ * GTS_TC];
+  const NodeDesc nd = nodes[blockIdx.y >> 1];
+  const int h = blockIdx.y & 1;
+  const int rs = nd.start + (h ? nd.half : 0), nh = h ? (nd.size - nd.half) : nd.half;
+  const int row_lo = blockIdx.x * GTS_ROWS;
+  if (row_lo >= nh) return;
+  const int row_hi = min(nh, row_lo + GTS_ROWS);
+  const int c0 = blockIdx.z * GTS_TC;
+  if (c0 >= ncols) return;
+  const int nc = min(GTS_TC, ncols - c0);
+  const int r = nd.r;
+  double* Wh = W + (int64_t)(blockIdx.y >> 1) * w_stride_node + (h ? 0 : r);  // as in gram_tn_kernel
+  const int ldw = 2 * r;
+  const double* v = Vp + (int64_t)nd.vcol * ldv + rs;
+  const double* xc = X + (int64_t)c0 * ldx + rs;
+
+  double acc[RQ][GTS_TC];
+#pragma unroll
+  for (int q = 0; q < RQ; ++q)
+#pragma unroll
+    for (int c = 0; c < GTS_TC; ++c) acc[q][c] = 0.0;
+#pragma unroll
+  for (int e = 0; e < GTS_ROWS / GTS_THREADS; ++e) {
+    const int i = row_lo + e * GTS_THREADS + threadIdx.x;
+    if (i < row_hi) {
+      double a[RQ], b[GTS_TC];
+#pragma unroll
+      for (int q = 0; q < RQ; ++q) a[q] = (q < r) ? v[(int64_t)q * ldv + i] : 0.0;
+#pragma unroll
+      for (int c = 0; c < GTS_TC; ++c) b[c] = (c < nc) ? xc[(int64_t)c * ldx + i] : 0.0;
+#pragma unroll
+      for (int q = 0; q < RQ; ++q)
+#pragma unroll
+        for (int c = 0; c < GTS_TC; ++c) acc[q][c] += a[q] * b[c];
+    }
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int q = 0; q < RQ; ++q)
+#pragma unroll
+    for (int c = 0; c < GTS_TC; ++c)
+      if (q < r && c < nc) {  // uniform over the CTA
+        const double s = warp_sum(acc[q][c]);
+        if (lane == 0) red[warp][q * GTS_TC + c] = s;
+      }
+  __syncthreads();
+  for (int t = threadIdx.x; t < r * nc; t += GTS_THREADS) {
+    const int q = t / nc, c = t % nc;
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < NW; ++w) s += red[w][q * GTS_TC + c];
+    atomicAdd(Wh + (int64_t)(c0 + c) * ldw + q, s);
   }
 }
 
