@@ -688,13 +688,9 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
     // BGP_LEAF_FACTOR=generic: the CUDA-core kernel at any leaf size (tests compare the two LDL^T implementations)
     const char* lf_env = getenv("BGP_LEAF_FACTOR");
     const bool generic = lf_env && strcmp(lf_env, "generic") == 0;
-    if (h->max_leaf <= 768 && !generic) {
-      const int ldp = lf_panel_ld(h->max_leaf);
-      const size_t smem = sizeof(double) * (size_t)LF_NB * ldp;
-      // (the attribute is per device / context: set it on every call, it is cheap)
-      cudaFuncSetAttribute(leaf_factor_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      leaf_factor_dmma_kernel<<<nl, LF_THREADS, smem, sA>>>(h->d_prog.p, h->d_x.p, h->d_diag.p, h->d_leaves.p, h->d_L.p,
-                                                            h->d_leaf_logdet.p, ldp);
+    if (h->max_leaf <= LF_MAX_LEAF && !generic) {
+      leaf_factor_launch(h->prog.shape, nl, h->max_leaf, sA, h->d_prog.p, h->d_x.p, h->d_diag.p, h->d_leaves.p, h->d_L.p,
+                         h->d_leaf_logdet.p);
     } else {
       leaf_build_factor_kernel<<<nl, LEAF_THREADS, 0, sA>>>(h->d_prog.p, h->d_x.p, h->d_diag.p, h->d_leaves.p, h->d_L.p,
                                                             h->d_leaf_logdet.p);
@@ -703,13 +699,16 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
   }
   BGP_CUDA(cudaEventRecord(h->ev[1], sA));  // leaves done
 
-  // ---- ACA (stream B, concurrent with the leaves) ----
+  // ---- ACA (stream B, after the leaves: DESIGN.md §6) ----
   std::vector<AcaDesc> hdesc;
   std::vector<int> desc_node;  // pre-order id per descriptor
   std::vector<AcaOut> houts;
   int64_t idx_total = 0, piv_total = 0;
   int nint = 0;
-  BGP_CUDA(cudaStreamWaitEvent(sB, h->ev[0], 0));
+  // The ACA's per-node kernels take a whole SM per CTA and can only start on an SM the leaf kernel has left, so starting
+  // them beside the leaves overlaps little; after the leaves, the step measured as fast at 256-row leaves and faster at
+  // 128-row ones.  The host still prepares the ACA while the leaves run.
+  BGP_CUDA(cudaStreamWaitEvent(sB, h->ev[1], 0));
   for (int attempt = 0;; ++attempt) {
     int vcols_set[2] = {0, 0};
     for (auto& L : h->levels) { L.vcol = vcols_set[L.set]; vcols_set[L.set] += L.cap; }

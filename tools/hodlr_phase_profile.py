@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""Per-kernel device time of the HODLR up-sweep and solve of the bench workload, from torch.profiler.
+"""Per-kernel device time of the HODLR factorisation, up-sweep and solve of the bench workload, from torch.profiler.
 
     python tools/hodlr_phase_profile.py --out DIR [--root TREE] [--workload cfg3] [--n N] [--steps 3] [--warmup 2]
 
@@ -7,7 +7,12 @@ Runs ``--warmup`` + ``--steps`` x (``compute`` + ``dot_solve``) of ``bench.py``'
 ``tools/profile_step.py``) and profiles the last ``--steps`` with CUDA activities, in a run of its own.  ``--root``
 imports ``bench`` and ``george_b200`` from another checkout, so that two builds can be compared in one session.
 
-The GPU timeline of each step is cut into two windows:
+The GPU timeline of each step is cut into three windows:
+  * factor: from the start of the leaf factorisation (``leaf_factor*`` or ``leaf_build_factor``) to the end of the last
+    ``a2_tick`` of the ACA loop that runs beside it on a second stream.  Besides the common fields below it reports
+    ``leaf_ms`` (span of the leaf kernel), ``a2_init_start_ms`` (start of ``a2_init`` after the first leaf activity)
+    and ``aca_busy_ms`` (union of the ``a2_*`` kernels): an ``a2_init`` that starts only near the end of ``leaf_ms``
+    means the ACA waited for the leaves;
   * up-sweep: from the start of ``finalize_panels_kernel`` to the end of the last activity before ``compute``'s
     device-to-host copy of the log-determinants (panel finalisation, leaf solve, level sweeps);
   * solve: from ``dot_solve``'s device-to-device copy of the right-hand side to the end of ``dot_kernel``.
@@ -52,13 +57,40 @@ def gpu_activities(trace):
     return out
 
 
+def is_leaf_factor(key):
+    return key.startswith("leaf_factor") or key == "leaf_build_factor"
+
+
+def union_ms(acts):
+    """Time covered by at least one of the activities, in ms."""
+    busy, cur0, cur1 = 0.0, None, None
+    for a0, a1, _ in sorted(acts):
+        if cur1 is None or a0 > cur1:
+            if cur1 is not None:
+                busy += cur1 - cur0
+            cur0, cur1 = a0, a1
+        else:
+            cur1 = max(cur1, a1)
+    if cur1 is not None:
+        busy += cur1 - cur0
+    return busy * 1e-3
+
+
 def windows(acts):
-    """Cut the sorted activities into per-step (kind, [activities]) windows, kind "upsweep" or "solve"."""
+    """Cut the sorted activities into per-step (kind, [activities]) windows, kind "factor", "upsweep" or "solve"."""
     res = []
     i, n = 0, len(acts)
     dtod = None  # the latest device-to-device copy since the last up-sweep: where a solve starts
     while i < n:
         k = acts[i][2]
+        if is_leaf_factor(k):
+            j = i
+            while j < n and acts[j][2] != "finalize_panels":
+                j += 1
+            ticks = [t for t in range(i, j) if acts[t][2] == "a2_tick"]
+            res.append(("factor", acts[i:ticks[-1] + 1] if ticks else acts[i:j]))
+            i, dtod = j, None
+            continue
         if k == "finalize_panels":
             j = i
             while j < n and acts[j][2] != "memcpy_DtoH":
@@ -84,24 +116,25 @@ def summarise(acts):
         if not w:
             continue
         t0, t1 = w[0][0], max(a[1] for a in w)
-        busy, cur0, cur1 = 0.0, None, None
         for a0, a1, key in w:
             kk = s["kernels"].setdefault(key, {"ms": 0.0, "launches": 0})
             kk["ms"] += (a1 - a0) * 1e-3
             kk["launches"] += 1
-            if cur1 is None or a0 > cur1:
-                if cur1 is not None:
-                    busy += cur1 - cur0
-                cur0, cur1 = a0, a1
-            else:
-                cur1 = max(cur1, a1)
-        busy += cur1 - cur0
+        busy = union_ms(w)
         s["span_ms"] += (t1 - t0) * 1e-3
-        s["busy_ms"] += busy * 1e-3
-        s["idle_ms"] += (t1 - t0 - busy) * 1e-3
+        s["busy_ms"] += busy
+        s["idle_ms"] += (t1 - t0) * 1e-3 - busy
+        if kind == "factor":
+            leaf = [a for a in w if is_leaf_factor(a[2])]
+            init = [a[0] for a in w if a[2] == "a2_init"]
+            s["leaf_ms"] = s.get("leaf_ms", 0.0) + (max(a[1] for a in leaf) - leaf[0][0]) * 1e-3
+            s["a2_init_start_ms"] = s.get("a2_init_start_ms", 0.0) + ((init[0] - leaf[0][0]) * 1e-3 if init else 0.0)
+            s["aca_busy_ms"] = s.get("aca_busy_ms", 0.0) + union_ms([a for a in w if a[2].startswith("a2_")])
     for s in out.values():
         k = max(s["steps"], 1)
-        for f in ("span_ms", "busy_ms", "idle_ms"):
+        for f in ("span_ms", "busy_ms", "idle_ms", "leaf_ms", "a2_init_start_ms", "aca_busy_ms"):
+            if f not in s:
+                continue
             s[f] /= k
         for v in s["kernels"].values():
             v["ms"] /= k
@@ -112,13 +145,18 @@ def summarise(acts):
 
 def format_summary(summary, header=""):
     lines = [header] if header else []
-    for kind in ("upsweep", "solve"):
+    for kind in ("factor", "upsweep", "solve"):
         s = summary.get(kind)
+        if not s and kind == "factor":  # a trace without the factorisation (older callers cut only the sweeps)
+            continue
         if not s:
             lines.append("{0}: not found in the trace".format(kind))
             continue
         lines.append("{0}: span {1:.3f} ms/step = busy {2:.3f} + idle {3:.3f} (mean of {4} steps)".format(
             kind, s["span_ms"], s["busy_ms"], s["idle_ms"], s["steps"]))
+        if kind == "factor":
+            lines.append("  leaf kernel span {0:.3f} ms, a2_init starts at +{1:.3f} ms, ACA kernels busy {2:.3f} ms".format(
+                s["leaf_ms"], s["a2_init_start_ms"], s["aca_busy_ms"]))
         for name, v in s["kernels"].items():
             lines.append("  {0:<28s} {1:8.3f} ms  {2:6.1f} launches".format(name, v["ms"], v["launches"]))
     return "\n".join(lines) + "\n"
