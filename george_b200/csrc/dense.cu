@@ -815,6 +815,7 @@ int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r,
   if (!h->has_inputs) { set_error("the factor was imported: the handle holds no kernel/coordinates"); return BGP_ERR_NOT_COMPUTED; }
   const int64_t n = h->n;
   const int np = h->n_params;
+  if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
   cudaStream_t s = h->s;
   BGP_TRY(h->d_rhs.reserve((size_t)n * 2 + 64, s));
   double* alpha = h->d_rhs.p;
@@ -823,7 +824,6 @@ int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r,
   BGP_CUDA(cudaMemcpyAsync(alpha, r, sizeof(double) * n, cudaMemcpyHostToDevice, s));
   BGP_TRY(dense_potrs_dev(h, alpha, 1, n));
   if (alpha_out) BGP_CUDA(cudaMemcpyAsync(alpha_out, alpha, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
-  if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
   BGP_TRY(h->d_inv.reserve((size_t)n * n, s));
   BGP_TRY(fill_identity_launch(h->d_inv.p, n, s));
   BGP_TRY(dense_potrs_dev(h, h->d_inv.p, n, n));

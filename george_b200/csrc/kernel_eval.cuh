@@ -45,6 +45,22 @@ __host__ __device__ inline size_t program_bytes(int n_leaves) {
 // host: digest + validate a bgp_kernel_spec_t (replaces parser.h:14-509 + update_reparams())
 int build_dev_program(const bgp_kernel_spec_t* spec, DevProgram* out);
 
+// The tile kernels (the kernel-matrix builds of kmat.cu, the matvec of kmat_ops.cu) stage a tile's coordinates in
+// dynamic shared memory next to the program, a block that grows with ndim.  Each comes in two instantiations: `staged`
+// (footprint staged_bytes) and one that reads the coordinates from global memory (unstaged_bytes), with the same
+// evaluation order and results.  The staged one runs whenever it fits under the kernel's cap, so no input dimension is
+// too wide for these paths.  Returns the instantiation to launch, with its attribute set and *smem its footprint.
+template <class Kernel>
+Kernel tile_kernel_for(Kernel staged, Kernel unstaged, size_t staged_bytes, size_t unstaged_bytes, size_t cap,
+                       size_t* smem) {
+  const bool fits = staged_bytes <= cap;
+  *smem = fits ? staged_bytes : unstaged_bytes;
+  const Kernel k = fits ? staged : unstaged;
+  // (the attribute is per device / context: set it on every call, it is cheap)
+  cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+  return k;
+}
+
 #ifdef __CUDACC__
 
 // cooperative copy of the live part of the program into shared memory (all threads of the CTA must call)

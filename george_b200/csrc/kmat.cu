@@ -25,7 +25,9 @@ struct KmatSmem {
   uint64_t bar;
 };
 
-// out[i*ld + j] = k(x1_i, x2_j)
+// out[i*ld + j] = k(x1_i, x2_j).  STAGED: the tile's coordinates are staged in shared memory; otherwise (inputs too
+// wide for the cap, tile_kernel_for) they are read from global memory, with the same evaluation order.
+template <bool STAGED>
 __device__ __forceinline__ void kmat_general_tile(const DevProgram* __restrict__ gprog, const double* __restrict__ x1,
                                                   int64_t n1, const double* __restrict__ x2, int64_t n2,
                                                   double* __restrict__ out, int64_t ld) {
@@ -36,24 +38,30 @@ __device__ __forceinline__ void kmat_general_tile(const DevProgram* __restrict__
   double* sx2 = sx1 + KM_TI * nd + ((KM_TI * nd) & 1);
 
   stage_program(&S->prog, gprog);
-  if (threadIdx.x == 0) { mbar_init(&S->bar, 1); mbar_fence_init(); }
+  if (STAGED && threadIdx.x == 0) { mbar_init(&S->bar, 1); mbar_fence_init(); }
   __syncthreads();
   uint32_t phase = 0;
 
   const int64_t i0 = (int64_t)blockIdx.y * KM_TI, j0 = (int64_t)blockIdx.x * KM_TJ;
   const int ni = (int)min((int64_t)KM_TI, n1 - i0), nj = (int)min((int64_t)KM_TJ, n2 - j0);
-  load_coords(sx1, x1 + i0 * nd, ni * nd, &S->bar, phase);
-  load_coords(sx2, x2 + j0 * nd, nj * nd, &S->bar, phase);
+  const double* X1 = x1 + i0 * nd;
+  const double* X2 = x2 + j0 * nd;
+  if (STAGED) {
+    load_coords(sx1, X1, ni * nd, &S->bar, phase);
+    load_coords(sx2, X2, nj * nd, &S->bar, phase);
+    X1 = sx1;
+    X2 = sx2;
+  }
   __syncthreads();
 
   const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;
   const int ja = 2 * tx, jb = 2 * tx + 1;
   const bool vec = ((ld & 1) == 0) && ((reinterpret_cast<uintptr_t>(out) & 15u) == 0) && ((j0 & 1) == 0);
   if (ja < nj) {
-    const double* xa = sx2 + ja * nd;
-    const double* xb = sx2 + (jb < nj ? jb : ja) * nd;
+    const double* xa = X2 + ja * nd;
+    const double* xb = X2 + (jb < nj ? jb : ja) * nd;
     for (int i = ty; i < ni; i += KM_THREADS / 64) {
-      const double* xi = sx1 + i * nd;
+      const double* xi = X1 + i * nd;
       const double va = kernel_value(S->prog, xi, xa);
       const double vb = (jb < nj) ? kernel_value(S->prog, xi, xb) : 0.0;
       double* o = out + (i0 + i) * ld + j0 + ja;
@@ -66,24 +74,27 @@ __device__ __forceinline__ void kmat_general_tile(const DevProgram* __restrict__
     }
   }
 }
+template <bool STAGED>
 __global__ void __launch_bounds__(KM_THREADS) kmat_general_kernel(const DevProgram* __restrict__ gprog,
                                                                   const double* __restrict__ x1, int64_t n1,
                                                                   const double* __restrict__ x2, int64_t n2,
                                                                   double* __restrict__ out, int64_t ld) {
-  kmat_general_tile(gprog, x1, n1, x2, n2, out, ld);
+  kmat_general_tile<STAGED>(gprog, x1, n1, x2, n2, out, ld);
 }
 // a batch of programs on the same x1, x2: member blockIdx.z evaluates gprogs[z] into out + z * mstride
+template <bool STAGED>
 __global__ void __launch_bounds__(KM_THREADS) kmat_general_batch_kernel(const DevProgram* __restrict__ gprogs,
                                                                         const double* __restrict__ x1, int64_t n1,
                                                                         const double* __restrict__ x2, int64_t n2,
                                                                         double* __restrict__ out, int64_t ld,
                                                                         int64_t mstride) {
   const int64_t z = blockIdx.z;
-  kmat_general_tile(gprogs + z, x1, n1, x2, n2, out + z * mstride, ld);
+  kmat_general_tile<STAGED>(gprogs + z, x1, n1, x2, n2, out + z * mstride, ld);
 }
 
 // symmetric build: out (n x n, leading dimension ld), optional diag_add on the diagonal (basic.py:64-65 fused)
 constexpr int KS_T = 64;
+template <bool STAGED>
 __device__ __forceinline__ void kmat_symmetric_tile(const DevProgram* __restrict__ gprog, const double* __restrict__ x,
                                                     int64_t n, const double* __restrict__ diag_add,
                                                     double* __restrict__ out, int64_t ld) {
@@ -91,20 +102,27 @@ __device__ __forceinline__ void kmat_symmetric_tile(const DevProgram* __restrict
   extern __shared__ __align__(16) unsigned char smem_raw[];
   KmatSmem* S = reinterpret_cast<KmatSmem*>(smem_raw);
   const int nd = gprog->ndim;
+  const int snd = STAGED ? nd : 0;  // doubles per staged point
   double* sxi = reinterpret_cast<double*>(smem_raw + ((sizeof(KmatSmem) + 15) & ~size_t(15)));
-  double* sxj = sxi + KS_T * nd + ((KS_T * nd) & 1);
-  double* tile = sxj + KS_T * nd + ((KS_T * nd) & 1);  // KS_T x (KS_T+1)
+  double* sxj = sxi + KS_T * snd + ((KS_T * snd) & 1);
+  double* tile = sxj + KS_T * snd + ((KS_T * snd) & 1);  // KS_T x (KS_T+1)
 
   stage_program(&S->prog, gprog);
-  if (threadIdx.x == 0) { mbar_init(&S->bar, 1); mbar_fence_init(); }
+  if (STAGED && threadIdx.x == 0) { mbar_init(&S->bar, 1); mbar_fence_init(); }
   __syncthreads();
   uint32_t phase = 0;
 
   const int64_t i0 = (int64_t)blockIdx.y * KS_T, j0 = (int64_t)blockIdx.x * KS_T;
   const int ni = (int)min((int64_t)KS_T, n - i0), nj = (int)min((int64_t)KS_T, n - j0);
   const bool on_diag = (blockIdx.x == blockIdx.y);
-  load_coords(sxi, x + i0 * nd, ni * nd, &S->bar, phase);
-  load_coords(sxj, x + j0 * nd, nj * nd, &S->bar, phase);
+  const double* Xi = x + i0 * nd;
+  const double* Xj = x + j0 * nd;
+  if (STAGED) {
+    load_coords(sxi, Xi, ni * nd, &S->bar, phase);
+    load_coords(sxj, Xj, nj * nd, &S->bar, phase);
+    Xi = sxi;
+    Xj = sxj;
+  }
   __syncthreads();
 
   const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;  // one column per thread, 16 rows
@@ -112,9 +130,9 @@ __device__ __forceinline__ void kmat_symmetric_tile(const DevProgram* __restrict
     // evaluate k(x_i, x_j) for j >= i only and mirror, exactly like the reference loop (kernel_interface.cpp:69-75):
     // FMA contraction makes k(a, b) and k(b, a) differ in the last bit for some kernels.
     if (tx < nj) {
-      const double* xj = sxj + tx * nd;
+      const double* xj = Xj + tx * nd;
       for (int i = ty; i < ni && i <= tx; i += KM_THREADS / 64) {
-        double v = kernel_value(S->prog, sxi + i * nd, xj);
+        double v = kernel_value(S->prog, Xi + i * nd, xj);
         if (i == tx && diag_add) v += diag_add[i0 + i];
         tile[i * (KS_T + 1) + tx] = v;
       }
@@ -127,9 +145,9 @@ __device__ __forceinline__ void kmat_symmetric_tile(const DevProgram* __restrict
     return;
   }
   if (tx < nj) {
-    const double* xj = sxj + tx * nd;
+    const double* xj = Xj + tx * nd;
     for (int i = ty; i < ni; i += KM_THREADS / 64) {
-      const double v = kernel_value(S->prog, sxi + i * nd, xj);
+      const double v = kernel_value(S->prog, Xi + i * nd, xj);
       out[(i0 + i) * ld + j0 + tx] = v;
       tile[i * (KS_T + 1) + tx] = v;
     }
@@ -140,21 +158,23 @@ __device__ __forceinline__ void kmat_symmetric_tile(const DevProgram* __restrict
     for (int c = ty; c < nj; c += KM_THREADS / 64) out[(j0 + c) * ld + i0 + tx] = tile[tx * (KS_T + 1) + c];
   }
 }
+template <bool STAGED>
 __global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_kernel(const DevProgram* __restrict__ gprog,
                                                                     const double* __restrict__ x, int64_t n,
                                                                     const double* __restrict__ diag_add,
                                                                     double* __restrict__ out, int64_t ld) {
-  kmat_symmetric_tile(gprog, x, n, diag_add, out, ld);
+  kmat_symmetric_tile<STAGED>(gprog, x, n, diag_add, out, ld);
 }
 // a batch of programs on the same x: member blockIdx.z builds with gprogs[z] into out + z * mstride, adding
 // diag_add[z * n ..] on its diagonal when diag_add is given (exactly the entries the single build makes for that program)
+template <bool STAGED>
 __global__ void __launch_bounds__(KM_THREADS) kmat_symmetric_batch_kernel(const DevProgram* __restrict__ gprogs,
                                                                           const double* __restrict__ x, int64_t n,
                                                                           const double* __restrict__ diag_add,
                                                                           double* __restrict__ out, int64_t ld,
                                                                           int64_t mstride) {
   const int64_t z = blockIdx.z;
-  kmat_symmetric_tile(gprogs + z, x, n, diag_add ? diag_add + z * n : nullptr, out + z * mstride, ld);
+  kmat_symmetric_tile<STAGED>(gprogs + z, x, n, diag_add ? diag_add + z * n : nullptr, out + z * mstride, ld);
 }
 
 // (member blockIdx.y of a batch: program gprog[blockIdx.y], output out + blockIdx.y * ostride)
@@ -457,6 +477,9 @@ static int try_launch_fast(const DevProgram& P, bool symmetric, const double* x1
   return -1;
 }
 
+// dynamic shared memory of the interpreter builds staging the coordinates of nd-dimensional points (nd = 0: none);
+// the caps are the most the staged builds may take
+constexpr size_t KM_SMEM_CAP = 96 * 1024;
 static size_t kmat_smem_general(int nd) {
   return ((sizeof(KmatSmem) + 15) & ~size_t(15)) + sizeof(double) * ((size_t)KM_TI * nd + 1 + (size_t)KM_TJ * nd + 1);
 }
@@ -469,12 +492,12 @@ static size_t kmat_smem_sym(int nd) {
 int kmat_general_launch(const DevProgram* dprog, int nd, const double* x1, int64_t n1, const double* x2, int64_t n2,
                         double* out, int64_t ld, cudaStream_t s) {
   if (n1 == 0 || n2 == 0) return BGP_OK;
-  const size_t smem = kmat_smem_general(nd);
-  // (the attribute is per device / context: set it on every call, it is cheap)
-  cudaFuncSetAttribute(kmat_general_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
   dim3 grid((unsigned)((n2 + KM_TJ - 1) / KM_TJ), (unsigned)((n1 + KM_TI - 1) / KM_TI));
   if (grid.y > 65535) { set_error("kmat_general: n1 too large for one launch"); return BGP_ERR_INVALID; }
-  kmat_general_kernel<<<grid, KM_THREADS, smem, s>>>(dprog, x1, n1, x2, n2, out, ld);
+  size_t smem;
+  const auto kern = tile_kernel_for(kmat_general_kernel<true>, kmat_general_kernel<false>, kmat_smem_general(nd),
+                                    kmat_smem_general(0), KM_SMEM_CAP, &smem);
+  kern<<<grid, KM_THREADS, smem, s>>>(dprog, x1, n1, x2, n2, out, ld);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
@@ -482,13 +505,13 @@ int kmat_general_launch(const DevProgram* dprog, int nd, const double* x1, int64
 int kmat_symmetric_launch(const DevProgram* dprog, int nd, const double* x, int64_t n, const double* diag_add,
                           double* out, int64_t ld, cudaStream_t s) {
   if (n == 0) return BGP_OK;
-  const size_t smem = kmat_smem_sym(nd);
-  // (the attribute is per device / context: set it on every call, it is cheap)
-  cudaFuncSetAttribute(kmat_symmetric_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
   const unsigned nt = (unsigned)((n + KS_T - 1) / KS_T);
   if (nt > 65535) { set_error("kmat_symmetric: n too large for one launch"); return BGP_ERR_INVALID; }
   dim3 grid(nt, nt);
-  kmat_symmetric_kernel<<<grid, KM_THREADS, smem, s>>>(dprog, x, n, diag_add, out, ld);
+  size_t smem;
+  const auto kern = tile_kernel_for(kmat_symmetric_kernel<true>, kmat_symmetric_kernel<false>, kmat_smem_sym(nd),
+                                    kmat_smem_sym(0), KM_SMEM_CAP, &smem);
+  kern<<<grid, KM_THREADS, smem, s>>>(dprog, x, n, diag_add, out, ld);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
@@ -587,10 +610,10 @@ int kmat_symmetric_batch_launch_auto(const DevProgram* P, const DevProgram* dpro
   if (nt > 65535) { set_error("kmat_symmetric: n too large for one launch"); return BGP_ERR_INVALID; }
   const int r = try_launch_fast_batch(P, B, true, x, n, x, n, diag_add, out, n, mstride, scratch, s);
   if (r >= 0) return r;
-  // (the attribute is per device / context: set it on every call, it is cheap)
-  cudaFuncSetAttribute(kmat_symmetric_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-  kmat_symmetric_batch_kernel<<<dim3(nt, nt, (unsigned)B), KM_THREADS, kmat_smem_sym(P[0].ndim), s>>>(
-      dprogs, x, n, diag_add, out, n, mstride);
+  size_t smem;
+  const auto kern = tile_kernel_for(kmat_symmetric_batch_kernel<true>, kmat_symmetric_batch_kernel<false>,
+                                    kmat_smem_sym(P[0].ndim), kmat_smem_sym(0), KM_SMEM_CAP, &smem);
+  kern<<<dim3(nt, nt, (unsigned)B), KM_THREADS, smem, s>>>(dprogs, x, n, diag_add, out, n, mstride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
@@ -606,10 +629,10 @@ int kmat_general_batch_launch_auto(const DevProgram* P, const DevProgram* dprogs
   if ((n1 + KM_TI - 1) / KM_TI > 65535) { set_error("kmat_general: n1 too large for one launch"); return BGP_ERR_INVALID; }
   const int r = try_launch_fast_batch(P, B, false, x1, n1, x2, n2, nullptr, out, ld, mstride, scratch, s);
   if (r >= 0) return r;
-  // (the attribute is per device / context: set it on every call, it is cheap)
-  cudaFuncSetAttribute(kmat_general_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-  kmat_general_batch_kernel<<<grid, KM_THREADS, kmat_smem_general(P[0].ndim), s>>>(dprogs, x1, n1, x2, n2, out, ld,
-                                                                                   mstride);
+  size_t smem;
+  const auto kern = tile_kernel_for(kmat_general_batch_kernel<true>, kmat_general_batch_kernel<false>,
+                                    kmat_smem_general(P[0].ndim), kmat_smem_general(0), KM_SMEM_CAP, &smem);
+  kern<<<grid, KM_THREADS, smem, s>>>(dprogs, x1, n1, x2, n2, out, ld, mstride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }

@@ -49,6 +49,9 @@ __device__ __forceinline__ void matvec_tile(const Fn& fn, int nd, const double* 
   }
 }
 
+// STAGED: the coordinates are staged in shared memory; otherwise (inputs too wide for the cap, tile_kernel_for) they
+// are read from global memory, with the same evaluation order
+template <bool STAGED>
 __global__ void __launch_bounds__(MV_THREADS) kmat_matvec_kernel(const DevProgram* __restrict__ gprog,
                                                                  const double* __restrict__ x1, int64_t n1,
                                                                  const double* __restrict__ x2, int64_t n2,
@@ -61,19 +64,24 @@ __global__ void __launch_bounds__(MV_THREADS) kmat_matvec_kernel(const DevProgra
   V += blockIdx.z * vstride;
   partial += blockIdx.z * pstride;
   const int nd = gprog->ndim;
+  const int snd = STAGED ? nd : 0;  // doubles per staged point
   double* sx1 = reinterpret_cast<double*>(smem_raw + ((sizeof(MvSmem) + 15) & ~size_t(15)));
-  double* sx2 = sx1 + MV_TI * nd + ((MV_TI * nd) & 1);
-  double* sv = sx2 + MV_TJ * nd;           // MV_NR x MV_TJ
+  double* sx2 = sx1 + MV_TI * snd + ((MV_TI * snd) & 1);
+  double* sv = sx2 + MV_TJ * snd;          // MV_NR x MV_TJ
   double* red = sv + MV_NR * MV_TJ;         // MV_THREADS x MV_NR
 
   stage_program(&S->prog, gprog);
-  if (threadIdx.x == 0) { mbar_init(&S->bar, 1); mbar_fence_init(); }
+  if (STAGED && threadIdx.x == 0) { mbar_init(&S->bar, 1); mbar_fence_init(); }
   __syncthreads();
   uint32_t phase = 0;
 
   const int64_t i0 = (int64_t)blockIdx.x * MV_TI;
   const int ni = (int)min((int64_t)MV_TI, n1 - i0);
-  load_coords(sx1, x1 + i0 * nd, ni * nd, &S->bar, phase);
+  const double* X1 = x1 + i0 * nd;
+  if (STAGED) {
+    load_coords(sx1, X1, ni * nd, &S->bar, phase);
+    X1 = sx1;
+  }
 
   const int row = threadIdx.x & (MV_TI - 1), lane4 = threadIdx.x / MV_TI;
   double acc[MV_NR];
@@ -87,13 +95,17 @@ __global__ void __launch_bounds__(MV_THREADS) kmat_matvec_kernel(const DevProgra
     const int64_t j0 = ch * MV_TJ;
     const int nj = (int)min((int64_t)MV_TJ, n2 - j0);
     __syncthreads();  // previous iteration's readers are done with sx2 / sv
-    load_coords(sx2, x2 + j0 * nd, nj * nd, &S->bar, phase);
+    const double* X2 = x2 + j0 * nd;
+    if (STAGED) {
+      load_coords(sx2, X2, nj * nd, &S->bar, phase);
+      X2 = sx2;
+    }
     for (int t = threadIdx.x; t < MV_NR * MV_TJ; t += MV_THREADS) {
       const int c = t / MV_TJ, j = t - c * MV_TJ;
       sv[t] = (c < nrhs && j < nj) ? V[(int64_t)c * ldv + j0 + j] : 0.0;
     }
     __syncthreads();
-    BGP_DISPATCH_SHAPE(S->prog, matvec_tile(fn, nd, sx1, sx2, sv, ni, nj, row, lane4, acc));
+    BGP_DISPATCH_SHAPE(S->prog, matvec_tile(fn, nd, X1, X2, sv, ni, nj, row, lane4, acc));
   }
   // combine the 4 column lanes of each row (fixed order), one partial per (split, row, rhs)
 #pragma unroll
@@ -128,6 +140,9 @@ __global__ void kmat_matvec_reduce_kernel(const double* __restrict__ partial, in
   }
 }
 
+// dynamic shared memory of the matvec staging the coordinates of nd-dimensional points (nd = 0: none); the cap is the
+// most the staged matvec may take
+constexpr size_t MV_SMEM_CAP = 160 * 1024;
 static size_t matvec_smem(int nd) {
   return ((sizeof(MvSmem) + 15) & ~size_t(15)) +
          sizeof(double) * ((size_t)MV_TI * nd + 1 + (size_t)MV_TJ * nd + (size_t)MV_NR * MV_TJ + (size_t)MV_THREADS * MV_NR);
@@ -163,9 +178,9 @@ int kmat_matvec_launch(const DevProgram* dprog, int nd, const double* x1, int64_
     for (int64_t c = 0; c < nrhs; ++c) BGP_CUDA(cudaMemsetAsync(out + c * ldo, 0, sizeof(double) * n1, s));
     return BGP_OK;
   }
-  // (the attribute is per device / context: set it on every call, it is cheap)
-  cudaFuncSetAttribute(kmat_matvec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-  const size_t smem = matvec_smem(nd);
+  size_t smem;
+  const auto kern = tile_kernel_for(kmat_matvec_kernel<true>, kmat_matvec_kernel<false>, matvec_smem(nd), matvec_smem(0),
+                                    MV_SMEM_CAP, &smem);
   const int64_t row_tiles = (n1 + MV_TI - 1) / MV_TI;
   int64_t nsplit;
   int cps;
@@ -174,7 +189,7 @@ int kmat_matvec_launch(const DevProgram* dprog, int nd, const double* x1, int64_
   for (int64_t c0 = 0; c0 < nrhs; c0 += MV_NR) {
     const int nc = (int)std::min<int64_t>(MV_NR, nrhs - c0);
     dim3 grid((unsigned)row_tiles, (unsigned)nsplit);
-    kmat_matvec_kernel<<<grid, MV_THREADS, smem, s>>>(dprog, x1, n1, x2, n2, V + c0 * ldv, ldv, nc, scratch.p, cps, 0, 0);
+    kern<<<grid, MV_THREADS, smem, s>>>(dprog, x1, n1, x2, n2, V + c0 * ldv, ldv, nc, scratch.p, cps, 0, 0);
     BGP_LAUNCH_CHECK();
     const int blocks = (int)std::min<int64_t>((n1 * nc + 255) / 256, 8 * (int64_t)num_sms());
     kmat_matvec_reduce_kernel<<<blocks, 256, 0, s>>>(scratch.p, n1, (int)nsplit, nc, diag, V + c0 * ldv, ldv,
@@ -196,13 +211,15 @@ int kmat_matvec_batch_launch(const DevProgram* dprogs, int nd, int members, cons
     BGP_CUDA(cudaMemset2DAsync(out, sizeof(double) * ostride, 0, sizeof(double) * n1, members, s));
     return BGP_OK;
   }
-  cudaFuncSetAttribute(kmat_matvec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   const int64_t row_tiles = (n1 + MV_TI - 1) / MV_TI;
   int64_t nsplit;
   int cps;
   BGP_TRY(matvec_plan(n1, n2, &nsplit, &cps));
   const int64_t pstride = nsplit * n1 * MV_NR;
-  kmat_matvec_kernel<<<dim3((unsigned)row_tiles, (unsigned)nsplit, (unsigned)members), MV_THREADS, matvec_smem(nd), s>>>(
+  size_t smem;
+  const auto kern = tile_kernel_for(kmat_matvec_kernel<true>, kmat_matvec_kernel<false>, matvec_smem(nd), matvec_smem(0),
+                                    MV_SMEM_CAP, &smem);
+  kern<<<dim3((unsigned)row_tiles, (unsigned)nsplit, (unsigned)members), MV_THREADS, smem, s>>>(
       dprogs, x1, n1, x2, n2, V, n2, 1, partial, cps, vstride, pstride);
   BGP_LAUNCH_CHECK();
   const int blocks = (int)std::min<int64_t>((n1 + 255) / 256, 8 * (int64_t)num_sms());

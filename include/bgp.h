@@ -65,6 +65,16 @@ uint64_t bgp_launch_count(void);
 #define BGP_MAX_DIM 8      /* max axes a kernel leaf may act on                                  */
 #define BGP_MAX_METRIC 36  /* BGP_MAX_DIM*(BGP_MAX_DIM+1)/2 packed-Cholesky entries (metrics.h:166-168) */
 #define BGP_MAX_NODES 32   /* max nodes (leaves + operators) of one program                       */
+/* Limits of a kernel program on the device (BGP_ERR_INVALID past them; the Python layer raises ValueError):
+ *   - at most 16 leaves (hence at most 31 nodes in use);
+ *   - an expression depth of at most 8: the operand stack of the postfix program, e.g. 8 leaves nested to the right,
+ *     k1 + (k2 + (... + k8)), while any number of left-nested operators keep it at 2;
+ *   - hyper-parameter gradients (bgp_kmat_gradient_*, bgp_kmat_gradient_contract, bgp_dense_grad_terms,
+ *     bgp_hodlr_grad_terms) take at most 64 hyper-parameters, checked before anything is solved;
+ *   - input-coordinate gradients (bgp_kmat_x1/x2_gradient_general) take at most BGP_MAX_DIM = 8 input dimensions;
+ *   - the HODLR solver takes at most 32 input dimensions.
+ * The kernel-matrix builds, the matvec, the dense solver, the batched paths and predictions have no input-dimension
+ * limit: a leaf acts on at most BGP_MAX_DIM axes, but a program's leaves may read any columns of a wider x. */
 
 enum { BGP_OP_KERNEL = 0, BGP_OP_SUM = 1, BGP_OP_PRODUCT = 2 }; /* kernels.py:234-247 operator_type+1 */
 

@@ -2,8 +2,9 @@
 """
 Generates tests/golden/reference_kernel_interface.json: SHA-256 digests (golden_digest below) of what the reference's OWN
 compiled kernel_interface.cpp (oracle/_ref, built by `make -C oracle ref` from the reference sources) returns for every
-kernel of the zoo in tests/conftest.py (make_kernels) and of the reference's own kernel suite (reference_kernel_list),
-on the inputs that tests/test_oracle_kernels.py and tests/test_reference_kernel_list.py draw.  Those tests compare the
+kernel of the zoo in tests/conftest.py (make_kernels), of the reference's own kernel suite (reference_kernel_list) and
+of the size-limit programs of tests/test_gpu_program_limits.py (limit_programs), on the inputs that
+tests/test_oracle_kernels.py, tests/test_reference_kernel_list.py and tests/test_gpu_program_limits.py draw.  Those tests compare the
 CPU oracle with the reference bit for bit through these digests, so they run wherever the repository is checked out.
 (Digests rather than the arrays: the outputs are ~0.9 MB of incompressible doubles.)
 
@@ -58,6 +59,8 @@ def main():
             out[p + "gradient_general"] = r.gradient_general(np.ones(kernel.full_size, dtype=np.uint32), t1, t1[:3])
         out[p + "x1_gradient_general"] = r.x1_gradient_general(t1, t1[:3])
         out[p + "x2_gradient_general"] = r.x2_gradient_general(t1[:3], t1)
+    from test_gpu_program_limits import reference_outputs  # tests/test_gpu_program_limits.py: the size limits
+    out.update(reference_outputs(ref))
     with open(PATH, "w") as fh:
         json.dump({k: golden_digest(v) for k, v in out.items()}, fh, indent=0, sort_keys=True)
         fh.write("\n")
