@@ -96,6 +96,7 @@ struct bgp_hodlr {
   int max_leaf = 0, rtot = 0, vcols = 0, cut_depth = 0;
   int64_t row0 = 0, nloc = 0;
   std::vector<int64_t> shard_row0, shard_rows;
+  bool top_pending = false;  // sharded compute without a communicator done, the host has not called finish_top yet
 
   DevBuf<DevProgram> d_prog;
   DevBuf<double> d_x, d_yerr, d_diag, d_L, d_leaf_logdet, d_node_logdet, d_S, d_W, d_scalar, d_rhs;
@@ -169,6 +170,22 @@ static void build_tree(bgp_hodlr* h, int start, int size, int dir, int parent, i
 
 static int hodlr_solve_dev(bgp_hodlr* h, double* b, int64_t nrhs, int64_t ldb, cudaStream_t s, int part);
 static int hodlr_exchange_finish(bgp_hodlr* h);
+
+// A sharded factorisation exchanges rows through the library's communicator when it spans exactly the shards and this
+// process is the handle's shard; otherwise the host runs the exchange (export/import_top, solve_local/top_dev).
+static bool host_exchange(const bgp_hodlr* h) {
+  return h->opts.shard_count > 1 &&
+         !(comm_ready() && comm_world() == h->opts.shard_count && comm_rank() == h->opts.shard_rank);
+}
+
+// The full solves need every shard's rows: on a host-exchange shard they would apply the top levels to a vector whose
+// other rows were never solved.
+static int reject_host_exchange(const bgp_hodlr* h, const char* what) {
+  if (!host_exchange(h)) return BGP_OK;
+  set_error("%s is not available on a host-exchange shard (shard %d of %d without a matching communicator): use "
+            "bgp_hodlr_solve_local_dev / bgp_hodlr_solve_top_dev", what, h->opts.shard_rank, h->opts.shard_count);
+  return BGP_ERR_INVALID;
+}
 static int hodlr_finish_top_impl(bgp_hodlr* h, bool allreduce);
 
 // The leaf solve stages a (max_leaf x cols) column group in shared memory: leaves of up to 3200 rows take the default
@@ -571,6 +588,8 @@ static int run_aca2(bgp_hodlr* h, const std::vector<AcaDesc>& descs, std::vector
 static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, const double* x_dev, int64_t n,
                                   int32_t ndim, const double* yerr_dev, const bgp_hodlr_opts_t* opts_in) {
   h->computed = false;
+  h->top_pending = false;
+  h->shard_row0.clear(); h->shard_rows.clear();  // only a sharded compute that cuts the tree reports ranges
   BGP_TRY(require_device());
   BGP_TRY(ensure_streams(h));
   BGP_TRY(build_dev_program(spec, &h->prog));
@@ -609,7 +628,6 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
   h->row0 = 0; h->nloc = n;
   if (o.shard_count > 1) {
     int seen = 0; bool found = false;
-    h->shard_row0.clear(); h->shard_rows.clear();
     for (size_t i = 0; i < h->nodes.size(); ++i) {
       HNode& nd = h->nodes[i];
       if (nd.depth == cut) {
@@ -618,7 +636,11 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
         seen++;
       }
     }
-    if (!found || seen != o.shard_count) { set_error("tree too shallow to shard %d ways (N=%lld, min_size=%d)", o.shard_count, (long long)n, o.min_size); return BGP_ERR_INVALID; }
+    if (!found || seen != o.shard_count) {
+      h->shard_row0.clear(); h->shard_rows.clear();
+      set_error("tree too shallow to shard %d ways (N=%lld, min_size=%d)", o.shard_count, (long long)n, o.min_size);
+      return BGP_ERR_INVALID;
+    }
     for (auto& nd : h->nodes) {
       nd.top = nd.depth < cut;
       nd.owned = !nd.top && nd.start >= h->row0 && nd.start + nd.size <= h->row0 + h->nloc;
@@ -903,9 +925,10 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
   if (o.shard_count > 1 && h->top.ucols > 0) BGP_TRY(hodlr_solve_dev(h, h->top.U.p, h->top.ucols, n, sA, 1));
   BGP_CUDA(cudaEventRecord(h->ev[3], sA));
   if (o.shard_count > 1) {
-    if (comm_ready() && comm_world() == o.shard_count && comm_rank() == o.shard_rank) return hodlr_exchange_finish(h);
+    if (!host_exchange(h)) return hodlr_exchange_finish(h);
     // no communicator: the caller exchanges the top panel rows itself and calls bgp_hodlr_finish_top()
     BGP_CUDA(cudaStreamSynchronize(sA));
+    h->top_pending = true;
     return BGP_OK;
   }
 
@@ -973,7 +996,7 @@ static int exchange_rows(bgp_hodlr* h, double* P, int64_t ld, int64_t cols, cuda
 static int hodlr_solve_dev(bgp_hodlr* h, double* b, int64_t nrhs, int64_t ldb, cudaStream_t s, int part) {
   const int nlev = (int)h->levels.size();
   const int cut = h->opts.shard_count > 1 ? h->cut_depth : 0;
-  const bool native_x = part == 0 && h->opts.shard_count > 1 && comm_ready() && comm_world() == h->opts.shard_count;
+  const bool native_x = part == 0 && h->opts.shard_count > 1 && !host_exchange(h);
   for (int64_t c0 = 0; c0 < nrhs; c0 += 64) {
     const int nc = (int)std::min<int64_t>(64, nrhs - c0);
     double* X = b + c0 * ldb;
@@ -1098,6 +1121,8 @@ int bgp_hodlr_compute(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
                       const double* yerr, const bgp_hodlr_opts_t* opts) {
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
   h->computed = false;
+  h->top_pending = false;  // (hodlr_compute_dev_impl resets these too; this covers the returns before it)
+  h->shard_row0.clear(); h->shard_rows.clear();
   BGP_TRY(require_device());
   BGP_TRY(ensure_streams(h));
   if (n <= 0 || ndim <= 0) { set_error("invalid input shape (%lld, %d)", (long long)n, ndim); return BGP_ERR_INVALID; }
@@ -1118,6 +1143,7 @@ int bgp_hodlr_log_determinant(const bgp_hodlr_t* h, double* out) {
 
 int bgp_hodlr_apply_inverse(bgp_hodlr_t* h, double* b, int64_t nrhs, int64_t ldb) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  BGP_TRY(reject_host_exchange(h, "apply_inverse"));
   if (nrhs <= 0) return BGP_OK;
   if (ldb < h->n) { set_error("dimension mismatch: ldb < n"); return BGP_ERR_DIM; }
   cudaStream_t s = h->sA;
@@ -1140,6 +1166,7 @@ int bgp_hodlr_apply_inverse(bgp_hodlr_t* h, double* b, int64_t nrhs, int64_t ldb
 
 int bgp_hodlr_dot_solve_dev(bgp_hodlr_t* h, const double* y_dev, double* out) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  BGP_TRY(reject_host_exchange(h, "dot_solve"));
   cudaStream_t s = h->sA;
   const int64_t n = h->n;
   BGP_TRY(h->d_rhs.reserve((size_t)n, s));
@@ -1158,6 +1185,7 @@ int bgp_hodlr_dot_solve_dev(bgp_hodlr_t* h, const double* y_dev, double* out) {
 
 int bgp_hodlr_dot_solve(bgp_hodlr_t* h, const double* y, double* out) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  BGP_TRY(reject_host_exchange(h, "dot_solve"));
   cudaStream_t s = h->sA;
   BGP_TRY(h->d_yerr.reserve((size_t)h->n, s));  // reuse as staging for y
   BGP_CUDA(cudaMemcpyAsync(h->d_yerr.p, y, sizeof(double) * h->n, cudaMemcpyHostToDevice, s));
@@ -1166,6 +1194,7 @@ int bgp_hodlr_dot_solve(bgp_hodlr_t* h, const double* y, double* out) {
 
 int bgp_hodlr_get_inverse(bgp_hodlr_t* h, double* out) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  BGP_TRY(reject_host_exchange(h, "get_inverse"));
   const int64_t n = h->n;
   for (int64_t j = 0; j < n; ++j) {
     double* c = out + j * n;
@@ -1403,11 +1432,27 @@ int bgp_hodlr_shard_rows(const bgp_hodlr_t* h, int32_t s, int64_t* row0, int64_t
   return BGP_OK;
 }
 
+// export / import / finish_top belong between a host-exchange compute and its (one) finish_top: finish_top updates the
+// top panel in place, so a second one, or an import after it, would work on rows that were already finished.
+static int require_top_pending(const bgp_hodlr* h, const char* what) {
+  if (h->top_pending) return BGP_OK;
+  if (!h->computed) {
+    set_error("%s: no sharded factorisation is waiting for its top levels (the solver has not been computed)", what);
+    return BGP_ERR_NOT_COMPUTED;
+  }
+  set_error("%s: the factorisation is complete (unsharded, or finish_top was already called)", what);
+  return BGP_ERR_INVALID;
+}
+
 int bgp_hodlr_export_top(bgp_hodlr_t* h, double* buf_dev, int64_t rows_pad) {
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  BGP_TRY(require_top_pending(h, "export_top"));
+  if (rows_pad < h->nloc) {  // checked even when there is nothing to pack, as import_top does
+    set_error("rows_pad %lld smaller than this shard (%lld rows)", (long long)rows_pad, (long long)h->nloc);
+    return BGP_ERR_INVALID;
+  }
   const int64_t cols = top_cols(h);
   if (cols == 0 || h->nloc == 0) return BGP_OK;
-  if (rows_pad < h->nloc) { set_error("rows_pad too small"); return BGP_ERR_INVALID; }
   pack_rows_kernel<<<1184, 256, 0, h->sA>>>(h->top.U.p, h->n, h->row0, h->nloc, cols, buf_dev, rows_pad);
   BGP_LAUNCH_CHECK();
   BGP_CUDA(cudaStreamSynchronize(h->sA));
@@ -1416,6 +1461,13 @@ int bgp_hodlr_export_top(bgp_hodlr_t* h, double* buf_dev, int64_t rows_pad) {
 
 int bgp_hodlr_import_top(bgp_hodlr_t* h, const double* all_buf_dev, int64_t rows_pad) {
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  BGP_TRY(require_top_pending(h, "import_top"));
+  int64_t max_rows = 0;
+  for (int64_t r : h->shard_rows) max_rows = std::max(max_rows, r);
+  if (rows_pad < max_rows) {  // the slices would be read at the wrong offsets
+    set_error("rows_pad %lld smaller than the largest shard (%lld rows)", (long long)rows_pad, (long long)max_rows);
+    return BGP_ERR_INVALID;
+  }
   const int64_t cols = top_cols(h);
   if (cols == 0) return BGP_OK;
   for (size_t s = 0; s < h->shard_rows.size(); ++s) {
@@ -1430,6 +1482,8 @@ int bgp_hodlr_import_top(bgp_hodlr_t* h, const double* all_buf_dev, int64_t rows
 
 int bgp_hodlr_finish_top(bgp_hodlr_t* h) {
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  BGP_TRY(require_top_pending(h, "finish_top"));
+  h->top_pending = false;
   return hodlr_finish_top_impl(h, false);
 }
 

@@ -404,17 +404,38 @@ int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n
  * opts.shard_rank, bgp_hodlr_compute[_dev] is COLLECTIVE and complete: local sub-tree, all-gather of the rows this shard
  * owns of the top-level factor panel (pack kernel -> ncclAllGather -> unpack kernels on the solver's stream), the nodes
  * above the cut, log-det all-reduce; apply_inverse / dot_solve are collective too (replicated right-hand side, one
- * all-gather of the locally solved slices).  WITHOUT a communicator the same steps are exposed one by one so that a host
- * can run the exchange itself: the rows are exported, all-gathered by the host, imported, and the top nodes finished.
- *   bgp_hodlr_top_panel(h, &ptr_dev, &rows, &cols, &ld): device pointer to the (N x cols) column-major panel
- *   bgp_hodlr_finish_top(h): Gram/LU/log-det/update of the nodes above the shard cut.               */
+ * all-gather of the locally solved slices).  WITHOUT a communicator (a "host-exchange shard": no communicator, or one
+ * whose size or rank does not match) the same steps are exposed one by one so that a host can run the exchange itself.
+ * The P shards may be P processes or P handles in one process, on any devices.  The call order is:
+ *   1. bgp_hodlr_compute[_dev] on every shard (opts.shard_rank = s, opts.shard_count = P, rng_mode = per-node).  It
+ *      returns with the local sub-tree factored and applied to this shard's rows of the top panel; the handle is not
+ *      computed yet (bgp_hodlr_computed = 0, solves return BGP_ERR_NOT_COMPUTED).
+ *   2. bgp_hodlr_export_top on every shard into its slot of a (P, cols, rows_pad) buffer, rows_pad >= the largest
+ *      bgp_hodlr_shard_rows; the host all-gathers the buffer (every device stream involved must have finished).
+ *   3. bgp_hodlr_import_top on every shard; the top panels of all shards are then identical.
+ *   4. bgp_hodlr_finish_top on every shard, exactly once.
+ *   5. solves: bgp_hodlr_solve_local_dev on every shard with the same right-hand side, the host assembles rows
+ *      [row0_s, row0_s + rows_s) from shard s and copies the assembled block to every shard, then
+ *      bgp_hodlr_solve_top_dev on every shard; every shard then holds the whole solution.
+ * The full solves (bgp_hodlr_apply_inverse, bgp_hodlr_dot_solve[_dev], bgp_hodlr_get_inverse), like grad_terms,
+ * predict and node_factors, return BGP_ERR_INVALID on a host-exchange shard: they need the other shards' rows.
+ * bgp_hodlr_log_determinant on a host-exchange shard returns that shard's PARTIAL log-determinant: its own leaves and
+ * sub-tree nodes, plus the nodes above the cut on shard 0 only, so the sum over the P shards is log det K.
+ *   bgp_hodlr_top_panel(h, &ptr_dev, &row0, &rows, &cols, &ld): device pointer to the (N x cols) column-major panel of
+ *     the levels above the cut (ld = N), and this shard's rows [row0, row0 + rows).                               */
 int bgp_hodlr_top_panel(bgp_hodlr_t* h, double** ptr_dev, int64_t* row0, int64_t* rows, int64_t* cols, int64_t* ld);
 /* pack this shard's rows of the top panel into a contiguous (cols x rows_pad) device buffer (column c at c*rows_pad),
- * and scatter the all-gathered buffers (shard s at s*cols*rows_pad) of all shards back into the panel. */
+ * and scatter the all-gathered buffers (shard s at s*cols*rows_pad) of all shards back into the panel.  Both are valid
+ * only between step 1 and step 4: BGP_ERR_NOT_COMPUTED before any compute, BGP_ERR_INVALID on an unsharded or already
+ * finished factorisation.  BGP_ERR_INVALID also when rows_pad is smaller than this shard's rows (export) or than the
+ * largest shard's rows (import), also when the panel has no columns (a rank-0 top: nothing is copied). */
 int bgp_hodlr_export_top(bgp_hodlr_t* h, double* buf_dev, int64_t rows_pad);
 int bgp_hodlr_import_top(bgp_hodlr_t* h, const double* all_buf_dev, int64_t rows_pad);
-/* row range [row0, row0+rows) owned by shard `s` (same on every shard; -1 rows if the tree cannot be cut) */
+/* row range [row0, row0+rows) owned by shard `s` (same on every shard).  BGP_ERR_INDEX if `s` is out of range, and for
+ * every `s` when the last compute was unsharded or failed because the tree cannot be cut shard_count ways. */
 int bgp_hodlr_shard_rows(const bgp_hodlr_t* h, int32_t s, int64_t* row0, int64_t* rows);
+/* Gram/LU/log-det/update of the nodes above the shard cut, on the imported top panel; marks the handle computed.  Once
+ * per compute: BGP_ERR_NOT_COMPUTED before any compute, BGP_ERR_INVALID on an unsharded factorisation or a second call. */
 int bgp_hodlr_finish_top(bgp_hodlr_t* h);
 /* The library's NCCL communicator (one per process).  Rank 0 makes a unique id (128 bytes), the host broadcasts it over
  * whatever it has (torch.distributed, MPI, a file), every rank calls bgp_comm_init.  `nccl_path` may be NULL: the library
@@ -423,7 +444,8 @@ int bgp_comm_unique_id(void* out128, const char* nccl_path);
 int bgp_comm_init(const void* id128, int rank, int world, const char* nccl_path);
 int bgp_comm_destroy(void);
 int bgp_comm_size(void);
-/* sharded solve: local part, then (host all-gathers the vector), then top part. */
+/* sharded solve (step 5 above): local part, then (host all-gathers the vector), then top part, in place on an
+ * (N x nrhs) column-major device block with ldb >= N.  BGP_ERR_NOT_COMPUTED before finish_top. */
 int bgp_hodlr_solve_local_dev(bgp_hodlr_t* h, double* b_dev, int64_t nrhs, int64_t ldb);
 int bgp_hodlr_solve_top_dev(bgp_hodlr_t* h, double* b_dev, int64_t nrhs, int64_t ldb);
 
