@@ -22,7 +22,12 @@ int kmat_symmetric_launch_auto(const DevProgram& P, const DevProgram* dprog, con
 int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const unsigned* which_dev, const double* x,
                               int64_t n, const double* M, int64_t ldm, const double* alpha, double ca, double cm,
                               double* g_dev, double* diag_dev, DevBuf<double>& scratch, cudaStream_t s);
+int kmat_grad_contract_members(const DevProgram* dprogs, int np, const unsigned* which_dev, const double* x, int64_t n,
+                               const double* M, int64_t ldm, int64_t mstride, const double* alpha, int64_t astride,
+                               double ca, double cm, double* g_dev, int64_t gstride, double* diag_dev, int64_t dstride,
+                               int members, DevBuf<double>& scratch, cudaStream_t s);
 int fill_identity_launch(double* A, int64_t n, cudaStream_t s);
+int fill_identity_members(double* A, int64_t n, int members, cudaStream_t s);
 int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
                              int64_t n2, double* out, int64_t ld, cudaStream_t s);
 int kmat_diagonal_launch(const DevProgram* dprog, const double* x1, const double* x2, int64_t n, double* out,
@@ -581,42 +586,6 @@ static int potrs_small_members(const double* L, int64_t n, double* X, int nrhs, 
   return BGP_OK;
 }
 
-static int dense_potrs_small(bgp_dense* h, double* X, int nrhs, int64_t ldx) {
-  BGP_TRY(h->d_tmp.reserve((size_t)h->n * DS_MAX_RHS, h->s));
-  return potrs_small_members(h->d_A.p, h->n, X, nrhs, ldx, h->d_tmp.p, 1, 0, 0, h->s);
-}
-
-static int dense_potrs_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
-  if (nrhs <= DS_MAX_RHS) return dense_potrs_small(h, X, (int)nrhs, ldx);
-  const int64_t n = h->n;
-  const double* L = h->d_A.p;
-  cudaStream_t s = h->s;
-  const unsigned cb = (unsigned)((nrhs + 127) / 128);
-  for (int64_t k0 = 0; k0 < n; k0 += DN_NB) {  // forward: L y = b
-    const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
-    trsv_block_kernel<<<cb, 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 0, 0, 0);
-    BGP_LAUNCH_CHECK();
-    const int64_t rem = n - k0 - nb;
-    if (rem <= 0) break;
-    dim3 grid((unsigned)((rem + GM_T - 1) / GM_T), (unsigned)((nrhs + GM_T - 1) / GM_T));
-    gemm_sub_kernel<0, 0><<<grid, 256, 0, s>>>(rem, nrhs, nb, L + k0 * n + k0 + nb, n, X + k0, ldx, X + k0 + nb, ldx, 0,
-                                               nullptr, 0, 0, 0);
-    BGP_LAUNCH_CHECK();
-  }
-  const int64_t last = ((n - 1) / DN_NB) * DN_NB;
-  for (int64_t k0 = last; k0 >= 0; k0 -= DN_NB) {  // backward: L^T x = y
-    const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
-    trsv_block_kernel<<<cb, 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 1, 0, 0);
-    BGP_LAUNCH_CHECK();
-    if (k0 == 0) break;
-    // X[0:k0] -= L[k0:k0+nb, 0:k0]^T X[k0:k0+nb]
-    dim3 grid((unsigned)((k0 + GM_T - 1) / GM_T), (unsigned)((nrhs + GM_T - 1) / GM_T));
-    gemm_sub_kernel<1, 0><<<grid, 256, 0, s>>>(k0, nrhs, nb, L + k0, n, X + k0, ldx, X, ldx, 0, nullptr, 0, 0, 0);
-    BGP_LAUNCH_CHECK();
-  }
-  return BGP_OK;
-}
-
 // X (n x nrhs, column-major ldx) <- L^-1 X: the forward half of dense_potrs_dev (predictive variance / covariance need
 // only W = L^-1 K(x, x*), since K(x*, x) K^-1 K(x, x*) = W^T W).  `members` factors at once: member m solves with
 // L + m * lstride on X + m * xstride; a single solve passes one member and zero strides.  Few right-hand sides go
@@ -653,6 +622,36 @@ static int trsm_fwd_members(const double* L, int64_t n, int64_t lstride, double*
     BGP_LAUNCH_CHECK();
   }
   return BGP_OK;
+}
+
+// X <- K^-1 X for `members` factors of order n (member m: L + m * lstride, X + m * xstride); a single solve passes one
+// member and zero strides.  Up to DS_MAX_RHS right-hand sides go through the one-launch step kernels with the scratch Y
+// (members blocks of xstride >= n * nrhs doubles); more through the forward sweep of trsm_fwd_members and the
+// backward sweep below.
+static int potrs_members(const double* L, int64_t n, int64_t lstride, double* X, int64_t nrhs, int64_t ldx,
+                         int64_t xstride, int members, double* Y, cudaStream_t s) {
+  if (nrhs <= DS_MAX_RHS) return potrs_small_members(L, n, X, (int)nrhs, ldx, Y, members, lstride, xstride, s);
+  BGP_TRY(trsm_fwd_members(L, n, lstride, X, nrhs, ldx, xstride, members, nullptr, 0, s));  // forward: L y = b
+  const unsigned mb = (unsigned)members;
+  const unsigned cb = (unsigned)((nrhs + 127) / 128);
+  const int64_t last = ((n - 1) / DN_NB) * DN_NB;
+  for (int64_t k0 = last; k0 >= 0; k0 -= DN_NB) {  // backward: L^T x = y
+    const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
+    trsv_block_kernel<<<dim3(cb, mb), 128, 0, s>>>(L + k0 * n + k0, n, nb, X + k0, ldx, nrhs, 1, lstride, xstride);
+    BGP_LAUNCH_CHECK();
+    if (k0 == 0) break;
+    // X[0:k0] -= L[k0:k0+nb, 0:k0]^T X[k0:k0+nb]
+    dim3 grid((unsigned)((k0 + GM_T - 1) / GM_T), (unsigned)((nrhs + GM_T - 1) / GM_T), mb);
+    gemm_sub_kernel<1, 0><<<grid, 256, 0, s>>>(k0, nrhs, nb, L + k0, n, X + k0, ldx, X, ldx, 0, nullptr, lstride, xstride,
+                                               xstride);
+    BGP_LAUNCH_CHECK();
+  }
+  return BGP_OK;
+}
+
+static int dense_potrs_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
+  if (nrhs <= DS_MAX_RHS) BGP_TRY(h->d_tmp.reserve((size_t)h->n * DS_MAX_RHS, h->s));
+  return potrs_members(h->d_A.p, h->n, 0, X, nrhs, ldx, 0, 1, h->d_tmp.p, h->s);
 }
 
 static int dense_trsm_fwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
@@ -938,6 +937,9 @@ struct bgp_dense_batch {
   // variances and their partials, covariances and their split-K slices
   DevBuf<double> d_xs, d_mean, d_mvp, d_W, d_kd, d_var, d_vp, d_C, d_slices;
   DevBuf<GemmDesc> d_pdesc;
+  // bgp_dense_batch_grad_terms: K_b^-1, the contraction partials and g
+  DevBuf<double> d_inv, d_gp, d_g;
+  DevBuf<unsigned> d_which;
 };
 
 // members per chunk: as many members of per_member doubles as fit in 4 GiB, at least one; BGP_BATCH_CHUNK=<members>
@@ -1067,6 +1069,7 @@ void bgp_dense_batch_destroy(bgp_dense_batch_t* h) {
   h->d_info.release(); h->d_gdesc.release();
   h->d_xs.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_kd.release();
   h->d_var.release(); h->d_vp.release(); h->d_C.release(); h->d_slices.release(); h->d_pdesc.release();
+  h->d_inv.release(); h->d_gp.release(); h->d_g.release(); h->d_which.release();
   if (h->s) {
     cudaStreamSynchronize(h->s);
     cudaStreamDestroy(h->s);
@@ -1105,6 +1108,74 @@ int bgp_dense_batch_log_likelihood(bgp_dense_batch_t* h, const bgp_kernel_spec_t
   for (int64_t b = 0; b < B; ++b) {
     if (!bp.valid[b]) info[b] = -1;
     if (info[b] != 0) log_det[b] = quad[b] = std::nan("");
+  }
+  return BGP_OK;
+}
+
+int bgp_dense_batch_grad_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
+                               int64_t P, const double* x, int64_t n, int32_t ndim, const double* yerr, const double* r,
+                               const uint32_t* which, double* log_det, double* quad, double* alpha, double* diag,
+                               double* g, int32_t* info) {
+  if (P > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  BatchPrograms bp;
+  BGP_TRY(batch_begin(h, spec, params, B, P, x, n, ndim, &bp));
+  if (B == 0) return BGP_OK;
+  cudaStream_t s = h->s;
+  const int64_t nn = n * n;
+  // n <= DS_MAX_RHS: K^-1 goes through the few-column solve, as bgp_dense_grad_terms sends it, with n x n of scratch
+  const int64_t tmp_cols = n <= DS_MAX_RHS ? n : 1;
+  const int64_t nt = (n + 31) / 32;  // the contraction's 32 x 32 tiles
+  // doubles per member (see include/bgp.h): factor, K^-1, the vectors of batch_reserve_common, partials, g
+  const int64_t per_member = 2 * nn + (4 + tmp_cols) * n + nt * nt * P + P;
+  int64_t chunk = batch_chunk_members(per_member, B);
+  auto release = [&] { h->d_A.release(); h->d_inv.release(); h->d_gp.release(); h->d_g.release(); };
+  auto reserve = [&](int64_t m) -> int {
+    BGP_TRY(h->d_A.reserve((size_t)(nn * m), s));
+    BGP_TRY(h->d_inv.reserve((size_t)(nn * m), s));
+    BGP_TRY(h->d_gp.reserve((size_t)std::max<int64_t>(1, nt * nt * P * m), s));
+    BGP_TRY(h->d_g.reserve((size_t)std::max<int64_t>(1, P * m), s));
+    return BGP_OK;
+  };
+  BGP_TRY(batch_reserve_chunk(&chunk, reserve, release));
+  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, tmp_cols));
+  BGP_TRY(h->d_out.reserve((size_t)2 * chunk, s));
+  BGP_TRY(h->d_which.reserve((size_t)std::max<int64_t>(1, P), s));
+  if (P > 0) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * P, cudaMemcpyHostToDevice, s));
+  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
+    const int mc = (int)std::min(chunk, B - c0);
+    // the steps of bgp_dense_compute and bgp_dense_grad_terms, member-indexed: factor and alpha (d_sol), log_det and
+    // quad as bgp_dense_batch_log_likelihood computes them
+    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
+    logdet_diag_kernel<<<(unsigned)mc, 1024, 0, s>>>(h->d_A.p, n, n, h->d_out.p, nn);
+    BGP_LAUNCH_CHECK();
+    dot_rows_kernel<<<(unsigned)mc, 256, 0, s>>>(h->d_r.p, h->d_sol.p, n, h->d_out.p + chunk);
+    BGP_LAUNCH_CHECK();
+    // K_b^-1 by solving against the identity
+    BGP_TRY(fill_identity_members(h->d_inv.p, n, mc, s));
+    BGP_TRY(potrs_members(h->d_A.p, n, nn, h->d_inv.p, n, n, nn, mc, h->d_tmp.p, s));
+    // g_b and diag(alpha_b alpha_b^T - K_b^-1); the diagonal goes to d_diag, whose yerr^2 the build above consumed
+    BGP_TRY(kmat_grad_contract_members(h->d_prog.p + c0, (int)P, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, nn,
+                                       h->d_sol.p, n, 1.0, -1.0, h->d_g.p, P, diag ? h->d_diag.p : nullptr, n, mc,
+                                       h->d_gp, s));
+    if (log_det) BGP_CUDA(cudaMemcpyAsync(log_det + c0, h->d_out.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, s));
+    if (quad) BGP_CUDA(cudaMemcpyAsync(quad + c0, h->d_out.p + chunk, sizeof(double) * mc, cudaMemcpyDeviceToHost, s));
+    if (alpha) BGP_CUDA(cudaMemcpyAsync(alpha + c0 * n, h->d_sol.p, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
+    if (diag) BGP_CUDA(cudaMemcpyAsync(diag + c0 * n, h->d_diag.p, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
+    if (g && P > 0) BGP_CUDA(cudaMemcpyAsync(g + c0 * P, h->d_g.p, sizeof(double) * mc * P, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaStreamSynchronize(s));
+  }
+  const double nan = std::nan("");
+  for (int64_t b = 0; b < B; ++b) {
+    if (!bp.valid[b]) info[b] = -1;
+    if (info[b] == 0) continue;
+    if (log_det) log_det[b] = nan;
+    if (quad) quad[b] = nan;
+    for (int64_t i = 0; i < n; ++i) {
+      if (alpha) alpha[b * n + i] = nan;
+      if (diag) diag[b * n + i] = nan;
+    }
+    if (g) for (int64_t q = 0; q < P; ++q) g[b * P + q] = nan;
   }
   return BGP_OK;
 }

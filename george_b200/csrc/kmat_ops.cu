@@ -235,6 +235,8 @@ int kmat_matvec_batch_launch(const DevProgram* dprogs, int nd, int members, cons
 //     A_ij = ca * alpha_i * alpha_j + cm * M_ij          (grad_log_likelihood: ca = 1, cm = -1, M = K^-1).
 // Tiles of 32 x 32 pairs; M's tile and its transposed partner are staged through shared memory so both reads are
 // coalesced.  NPMAX is the register budget for the per-parameter accumulators.
+// Member blockIdx.z of a batch (bgp_dense_batch_grad_terms) contracts with its own program gprog[z], M + z * mstride,
+// alpha + z * astride and writes partial + z * pstride; a single contraction launches one member with zero strides.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int GC_T = 32;
 constexpr int GC_THREADS = 256;
@@ -245,7 +247,13 @@ __global__ void __launch_bounds__(GC_THREADS) kmat_grad_contract_kernel(const De
                                                                         const double* __restrict__ x, int64_t n,
                                                                         const double* __restrict__ M, int64_t ldm,
                                                                         const double* __restrict__ alpha, double ca,
-                                                                        double cm, double* __restrict__ partial) {
+                                                                        double cm, double* __restrict__ partial,
+                                                                        int64_t mstride, int64_t astride,
+                                                                        int64_t pstride) {
+  gprog += blockIdx.z;
+  M += blockIdx.z * mstride;
+  if (alpha) alpha += blockIdx.z * astride;
+  partial += blockIdx.z * pstride;
   __shared__ DevProgram P;
   __shared__ unsigned sw[BGP_MAX_LEAVES * (4 + BGP_MAX_METRIC)];
   __shared__ double tA[GC_T][GC_T + 1], tB[GC_T][GC_T + 1];
@@ -295,9 +303,12 @@ __global__ void __launch_bounds__(GC_THREADS) kmat_grad_contract_kernel(const De
   }
 }
 
+// (member blockIdx.y of a batch: partial + y * pstride, out + y * ostride)
 __global__ void grad_contract_reduce_kernel(const double* __restrict__ partial, int64_t nctas, int np,
-                                            double* __restrict__ out) {
+                                            double* __restrict__ out, int64_t pstride, int64_t ostride) {
   __shared__ double red[32];
+  partial += blockIdx.y * pstride;
+  out += blockIdx.y * ostride;
   const int q = blockIdx.x;
   double s = 0.0;
   for (int64_t c = threadIdx.x; c < nctas; c += blockDim.x) s += partial[c * np + q];
@@ -305,50 +316,78 @@ __global__ void grad_contract_reduce_kernel(const double* __restrict__ partial, 
   if (threadIdx.x == 0) out[q] = s;
 }
 
-// diagA[i] = ca * alpha_i^2 + cm * M_ii
+// diagA[i] = ca * alpha_i^2 + cm * M_ii  (member blockIdx.y of a batch: M + y * mstride, alpha + y * astride,
+// out + y * ostride)
 __global__ void grad_diag_kernel(const double* __restrict__ M, int64_t ldm, const double* __restrict__ alpha, double ca,
-                                 double cm, int64_t n, double* __restrict__ out) {
+                                 double cm, int64_t n, double* __restrict__ out, int64_t mstride, int64_t astride,
+                                 int64_t ostride) {
+  M += blockIdx.y * mstride;
+  if (alpha) alpha += blockIdx.y * astride;
+  out += blockIdx.y * ostride;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     out[i] = cm * M[i * ldm + i] + (alpha ? ca * alpha[i] * alpha[i] : 0.0);
 }
 
-// g_dev[np] = sum_ij (ca alpha_i alpha_j + cm M_ij) dK_ij/dtheta ; diag_dev[n] (may be null) = diag of that weight matrix
-int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const unsigned* which_dev, const double* x,
-                              int64_t n, const double* M, int64_t ldm, const double* alpha, double ca, double cm,
-                              double* g_dev, double* diag_dev, DevBuf<double>& scratch, cudaStream_t s) {
-  (void)nd;
-  if (n <= 0) return BGP_OK;
+// g_dev[np] = sum_ij (ca alpha_i alpha_j + cm M_ij) dK_ij/dtheta ; diag_dev[n] (may be null) = diag of that weight matrix.
+// `members` contractions of one x in the same three launches: member b uses dprogs[b], M + b * mstride and
+// alpha + b * astride, and writes g_dev + b * gstride and diag_dev + b * dstride, exactly as a one-member call computes
+// it (the same tiles, NPMAX and reduction order).  All members share np and which_dev; scratch holds
+// members * ceil(n / 32)^2 * np partials.
+int kmat_grad_contract_members(const DevProgram* dprogs, int np, const unsigned* which_dev, const double* x, int64_t n,
+                               const double* M, int64_t ldm, int64_t mstride, const double* alpha, int64_t astride,
+                               double ca, double cm, double* g_dev, int64_t gstride, double* diag_dev, int64_t dstride,
+                               int members, DevBuf<double>& scratch, cudaStream_t s) {
+  if (n <= 0 || members <= 0) return BGP_OK;
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  if (members > 65535) { set_error("kmat_grad_contract: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
+  const unsigned mb = (unsigned)members;
   if (np > 0) {
     const int64_t nt = (n + GC_T - 1) / GC_T;
     if (nt > 65535) { set_error("kmat_grad_contract: n too large for one launch"); return BGP_ERR_INVALID; }
     const int64_t nctas = nt * nt;
-    BGP_TRY(scratch.reserve((size_t)nctas * np, s));
-    dim3 grid((unsigned)nt, (unsigned)nt);
-    if (np <= 8) kmat_grad_contract_kernel<8><<<grid, GC_THREADS, 0, s>>>(dprog, which_dev, x, n, M, ldm, alpha, ca, cm, scratch.p);
-    else kmat_grad_contract_kernel<64><<<grid, GC_THREADS, 0, s>>>(dprog, which_dev, x, n, M, ldm, alpha, ca, cm, scratch.p);
+    const int64_t pstride = nctas * np;
+    BGP_TRY(scratch.reserve((size_t)(pstride * members), s));
+    dim3 grid((unsigned)nt, (unsigned)nt, mb);
+    if (np <= 8)
+      kmat_grad_contract_kernel<8><<<grid, GC_THREADS, 0, s>>>(dprogs, which_dev, x, n, M, ldm, alpha, ca, cm, scratch.p,
+                                                               mstride, astride, pstride);
+    else
+      kmat_grad_contract_kernel<64><<<grid, GC_THREADS, 0, s>>>(dprogs, which_dev, x, n, M, ldm, alpha, ca, cm, scratch.p,
+                                                                mstride, astride, pstride);
     BGP_LAUNCH_CHECK();
-    grad_contract_reduce_kernel<<<np, 256, 0, s>>>(scratch.p, nctas, np, g_dev);
+    grad_contract_reduce_kernel<<<dim3((unsigned)np, mb), 256, 0, s>>>(scratch.p, nctas, np, g_dev, pstride, gstride);
     BGP_LAUNCH_CHECK();
   }
   if (diag_dev) {
-    grad_diag_kernel<<<(unsigned)std::min<int64_t>((n + 255) / 256, 1184), 256, 0, s>>>(M, ldm, alpha, ca, cm, n, diag_dev);
+    grad_diag_kernel<<<dim3((unsigned)std::min<int64_t>((n + 255) / 256, 1184), mb), 256, 0, s>>>(
+        M, ldm, alpha, ca, cm, n, diag_dev, mstride, astride, dstride);
     BGP_LAUNCH_CHECK();
   }
   return BGP_OK;
 }
-
-// I (n x n, column-major == row-major) on the device
-__global__ void fill_identity_kernel(double* __restrict__ A, int64_t n) {
-  const int64_t total = n * n;
-  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x)
-    A[t] = (t / n == t % n) ? 1.0 : 0.0;
+int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const unsigned* which_dev, const double* x,
+                              int64_t n, const double* M, int64_t ldm, const double* alpha, double ca, double cm,
+                              double* g_dev, double* diag_dev, DevBuf<double>& scratch, cudaStream_t s) {
+  (void)nd;
+  return kmat_grad_contract_members(dprog, np, which_dev, x, n, M, ldm, 0, alpha, 0, ca, cm, g_dev, 0, diag_dev, 0, 1,
+                                    scratch, s);
 }
-int fill_identity_launch(double* A, int64_t n, cudaStream_t s) {
-  fill_identity_kernel<<<(unsigned)std::min<int64_t>((n * n + 255) / 256, 16 * (int64_t)num_sms()), 256, 0, s>>>(A, n);
+
+// `members` identity matrices of order n, back to back (member stride n^2; column-major == row-major)
+__global__ void fill_identity_kernel(double* __restrict__ A, int64_t n, int64_t total) {
+  const int64_t nn = n * n;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t u = t % nn;
+    A[t] = (u / n == u % n) ? 1.0 : 0.0;
+  }
+}
+int fill_identity_members(double* A, int64_t n, int members, cudaStream_t s) {
+  const int64_t total = n * n * members;
+  fill_identity_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 16 * (int64_t)num_sms()), 256, 0, s>>>(A, n, total);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
+int fill_identity_launch(double* A, int64_t n, cudaStream_t s) { return fill_identity_members(A, n, 1, s); }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Predictive variance / covariance (GP.predict with return_var / return_cov; bgp_dense_predict, bgp_hodlr_predict).

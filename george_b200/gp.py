@@ -25,6 +25,8 @@ __all__ = ["GP"]
 
 # jitter added to the diagonal when no observational uncertainty is given (reference gp.py:19)
 TINY = 1.25e-12
+# most kernel parameters the device gradient contraction takes (include/bgp.h)
+_MAX_GRAD_PARAMS = 64
 
 
 def _as_model(obj):
@@ -542,6 +544,111 @@ class GP(ModelSet):
                 mask = self.kernel.unfrozen_mask
                 grad[pos:pos + n_k] = 0.5 * self.kernel.kernel.gradient_contract(mask.astype(np.uint32), self._x, A)[mask]
         return grad
+
+    def batch_grad_log_likelihood(self, vectors, y, quiet=False, return_log_likelihood=False):
+        """:func:`grad_log_likelihood` at many parameter vectors: row ``b`` of the ``(B, len(gp))`` result is bit for
+        bit what ``gp.set_parameter_vector(vectors[b]); gp.grad_log_likelihood(y, quiet=quiet)`` returns on the
+        computed ``x`` and ``yerr`` (chains of a gradient-based sampler in lock-step, the starts of a multi-start fit).
+        With ``return_log_likelihood`` the result is ``(ll, grad)``: ``ll[b]`` is what :func:`log_likelihood` returns
+        when that loop calls it before the gradient, bit for bit :func:`batch_log_likelihood`'s, and value and
+        gradient come from one factorisation.
+
+        With ``quiet`` a failing member gets the loop's ``-inf`` and zero gradient and the others are unaffected;
+        otherwise the exception that loop raises first is raised, with its type and message, with one difference: the
+        checks that do not depend on the member (the shape of ``vectors``, ``y``'s length) come first.  The GP is left
+        as it was: parameter vector, factorisation, cached solve and dirty flags.
+
+        Solvers with a ``batch_grad_terms`` hook (``BasicSolver``) factorise all members, form their ``K^-1`` and
+        contract the kernel gradients in one batched pass on the device.  Any other solver (``HODLRSolver``,
+        ``TrivialSolver``, plug-ins) takes that loop, and so do a kernel without a valid device program, one with more
+        than 64 parameters (the device contraction's limit: every member's gradient then fails as it does in the
+        loop) and a GP whose only active parameters are the mean's.
+
+        :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
+        """
+        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
+            raise RuntimeError("You need to compute the model first")
+        vectors = np.asarray(vectors, dtype=np.float64)
+        if vectors.ndim != 2 or vectors.shape[1] != len(self):
+            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        self._check_dimensions(y)
+        out = None
+        if len(vectors) == 0:
+            out = np.empty(0, dtype=np.float64), np.empty((0, len(self)), dtype=np.float64)
+        batch = getattr(self.solver_type, "batch_grad_terms", None)
+        if out is None and batch is not None and (len(self.white_noise) or len(self.kernel)):
+            out = self._batch_grad_device(batch, vectors, y, quiet, return_log_likelihood)
+        if out is None:
+            out = self._batch_grad_loop(vectors, y, quiet, return_log_likelihood)
+        return out if return_log_likelihood else out[1]
+
+    def _batch_grad_loop(self, vectors, y, quiet, return_ll):
+        state = self._batch_state()
+        try:
+            ll = np.empty(len(vectors), dtype=np.float64)
+            grad = np.empty((len(vectors), len(self)), dtype=np.float64)
+            for b, v in enumerate(vectors):
+                self.set_parameter_vector(v)
+                if return_ll:
+                    ll[b] = self.log_likelihood(y, quiet=quiet)
+                grad[b] = self.grad_log_likelihood(y, quiet=quiet)
+            return ll, grad
+        finally:
+            self._batch_restore(state)
+
+    def _batch_grad_device(self, batch, vectors, y, quiet, return_ll):
+        """The batched dense path of :func:`batch_grad_log_likelihood`: ``(ll, grad)``, or ``None`` when the kernel
+        has no valid device program or more than ``_MAX_GRAD_PARAMS`` parameters."""
+        # one residual serves both terms: GP._residual (the gradient's) and GP._residual_of (the value's) round alike
+        members = self._batch_members(vectors, y, self._residual,
+                                      lambda y, c: y - (c + np.zeros(len(y))))  # GP._residual of a ConstantModel
+        if members is None or members[2].shape[1] > _MAX_GRAD_PARAMS:
+            return None
+        spec, full, kpar, sigma, resid, fact_err, mean_err = members
+        nb, n = len(vectors), len(self._x)
+        mask = self.kernel.unfrozen_mask
+        log_det, quad, alpha, g, diag, info = batch(spec, kpar, self._x, sigma, resid, mask.astype(np.uint32))
+        # GP.compute / GP.log_likelihood, in the same order of operations
+        const = -0.5 * (n * np.log(2 * np.pi) + log_det)
+        ll = const - 0.5 * quad
+        ll[~np.isfinite(ll)] = -np.inf
+        # GP.grad_log_likelihood member by member, with its operations
+        n_mean, n_wn, n_k = len(self.mean), len(self.white_noise), len(self.kernel)
+        full_mean, full_wn = self.mean.full_size, self.white_noise.full_size
+        grad = np.zeros((nb, len(self)), dtype=np.float64)
+        for b in range(nb):  # the loop's order: factorisation (white noise included), residual, mean gradient
+            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
+            if exc is not None:
+                if not (quiet and isinstance(exc, (ValueError, LinAlgError))):
+                    raise exc
+                ll[b] = -np.inf
+                continue
+            exc = mean_err[b]
+            if exc is not None:
+                # log_likelihood swallows only the mean's own ValueError under quiet, grad_log_likelihood any ValueError
+                if not (quiet and isinstance(exc, ValueError) and (not return_ll or "mean function" in str(exc))):
+                    raise exc
+                ll[b] = -np.inf
+                continue
+            pos = 0
+            if n_mean:
+                try:
+                    dmu = self._swap_eval(self.mean, full[b, :full_mean], lambda: self._call_mean_gradient(self._x))
+                except ValueError:
+                    if quiet:
+                        continue
+                    raise
+                grad[b, pos:pos + n_mean] = np.dot(dmu, alpha[b])
+                pos += n_mean
+            if n_wn:
+                wn, dwn = self._swap_eval(self.white_noise, full[b, full_mean:full_mean + full_wn],
+                                          lambda: (self._call_white_noise(self._x),
+                                                   self._call_white_noise_gradient(self._x)))
+                grad[b, pos:pos + n_wn] = 0.5 * np.sum((np.exp(wn) * diag[b])[None, :] * dwn, axis=1)
+                pos += n_wn
+            if n_k:
+                grad[b, pos:pos + n_k] = 0.5 * g[b][mask]
+        return ll, grad
 
     def grad_lnlikelihood(self, y, quiet=False):
         warnings.warn("'grad_lnlikelihood' is deprecated. Use 'grad_log_likelihood'", DeprecationWarning)

@@ -243,6 +243,50 @@ class BasicSolver(object):
         return log_det, quad, info
 
     @staticmethod
+    def batch_grad_terms(spec, params, x, yerr, r, which):
+        """``(log_det, quad, alpha, g, diag, info)`` for ``B`` parameter vectors of one kernel program on the same
+        ``x``: member ``b`` factorises as in :func:`batch_log_likelihood` and returns what :func:`grad_terms` returns
+        for it, ``alpha`` ``(B, n)``, ``g`` ``(B, P)`` and ``diag`` ``(B, n)``, with ``which`` (``(P,)``) shared by all
+        members (``include/bgp.h: bgp_dense_batch_grad_terms``).  ``log_det``, ``quad`` and ``info`` are those of
+        :func:`batch_log_likelihood`; a failed member's rows are NaN.  A member's ``alpha``, ``g``, ``diag`` and
+        ``log_det`` are bit-identical to :func:`compute` with its spec and yerr followed by :func:`grad_terms`.  More
+        than 64 kernel parameters raise ``ValueError`` before anything is solved."""
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.ndim == 1:
+            x = x[:, None]
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
+        r = np.ascontiguousarray(r, dtype=np.float64)
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        if x.ndim != 2 or x.shape[0] == 0:
+            raise ValueError("x must have shape (n, ndim) with n > 0")
+        n, ndim = x.shape
+        npar = num_params(spec)
+        if params.ndim != 2 or params.shape[1] != npar:
+            raise ValueError("params must have shape (B, {0})".format(npar))
+        nb = params.shape[0]
+        if yerr.shape != (nb, n) or r.shape != (nb, n):
+            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
+        if which.shape != (npar,):
+            raise ValueError("which must have shape ({0},)".format(npar))
+        if ndim != spec.ndim:
+            raise DimensionMismatch("dimension mismatch")
+        log_det = np.empty(nb, dtype=np.float64)
+        quad = np.empty(nb, dtype=np.float64)
+        alpha = np.empty((nb, n), dtype=np.float64)
+        g = np.empty((nb, npar), dtype=np.float64)
+        diag = np.empty((nb, n), dtype=np.float64)
+        info = np.zeros(nb, dtype=np.int32)
+        if nb == 0:
+            return log_det, quad, alpha, g, diag, info
+        h = _get_batch_handle()
+        _lib.check(h.lib.bgp_dense_batch_grad_terms(
+            h.ptr, C.byref(spec), _lib.ptr(params), nb, npar, _lib.ptr(x), n, ndim, _lib.ptr(yerr), _lib.ptr(r),
+            _lib.ptr(which), _lib.ptr(log_det), _lib.ptr(quad), _lib.ptr(alpha), _lib.ptr(diag), _lib.ptr(g),
+            _lib.ptr(info)))
+        return log_det, quad, alpha, g, diag, info
+
+    @staticmethod
     def batch_predict(spec, params, x, yerr, r, xs, what):
         """``(mean, out, info)`` for ``B`` parameter vectors of one kernel program on the same ``x``: member ``b``
         factorises as in :func:`batch_log_likelihood`, ``mean[b] = K_b(xs, x) K_b^-1 r[b]`` (``(B, ns)``, the kernel

@@ -15,9 +15,11 @@ __all__ = ["HODLRSolver"]
 
 class HODLRSolver(BasicSolver):
 
-    # no batched HODLR factorisation: GP.batch_log_likelihood and GP.batch_predict take their per-vector loops
+    # no batched HODLR factorisation: GP.batch_log_likelihood, GP.batch_predict and GP.batch_grad_log_likelihood take
+    # their per-vector loops
     batch_log_likelihood = None
     batch_predict = None
+    batch_grad_terms = None
 
     def __init__(self, kernel, min_size=100, tol=0.1, seed=42, rng_mode=None, rank_capacity=0,
                  exhaust="dense"):

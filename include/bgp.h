@@ -70,7 +70,8 @@ uint64_t bgp_launch_count(void);
  *   - an expression depth of at most 8: the operand stack of the postfix program, e.g. 8 leaves nested to the right,
  *     k1 + (k2 + (... + k8)), while any number of left-nested operators keep it at 2;
  *   - hyper-parameter gradients (bgp_kmat_gradient_*, bgp_kmat_gradient_contract, bgp_dense_grad_terms,
- *     bgp_hodlr_grad_terms) take at most 64 hyper-parameters, checked before anything is solved;
+ *     bgp_dense_batch_grad_terms, bgp_hodlr_grad_terms) take at most 64 hyper-parameters, checked before anything
+ *     is solved;
  *   - input-coordinate gradients (bgp_kmat_x1/x2_gradient_general) take at most BGP_MAX_DIM = 8 input dimensions;
  *   - the HODLR solver takes at most 32 input dimensions.
  * The kernel-matrix builds, the matvec, the dense solver, the batched paths and predictions have no input-dimension
@@ -256,6 +257,33 @@ int bgp_dense_batch_log_likelihood(bgp_dense_batch_t* h, const bgp_kernel_spec_t
                                    int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
                                    const double* yerr, const double* r,
                                    double* log_det, double* quad, int32_t* info);
+/* Batched gradient terms (GP.batch_grad_log_likelihood): for the same B members as bgp_dense_batch_log_likelihood
+ * (spec, params, x, yerr; r = y - mean(x) per member, B x n row-major) and one selection `which` (P entries, shared by
+ * all members), what bgp_dense_grad_terms returns for each member plus its log-likelihood terms:
+ *   log_det[b], quad[b]    as bgp_dense_batch_log_likelihood computes them (bit-identical to it)
+ *   alpha[b*n + i]         (K_b^-1 r_b)_i
+ *   g[b*P + p]             sum_ij (alpha_b alpha_b^T - K_b^-1)_ij dK_b,ij/dtheta_p   (zeros where which[p] == 0)
+ *   diag[b*n + i]          (alpha_b alpha_b^T - K_b^-1)_ii
+ * Any output but info may be NULL.  Each member's alpha, g, diag and log_det are bit-identical to bgp_dense_compute
+ * followed by bgp_dense_grad_terms on member b's spec and yerr: the same kernels run with a member index (K_b^-1 by
+ * solving against the identity, through the few-column solve when n <= 8, and the same contraction tiles and fixed
+ * reduction order), so a member's results do not depend on B, its position or the chunking.  info[b] as in
+ * bgp_dense_batch_log_likelihood (0, the leading-minor index, or -1 for an invalid member program); a failed member's
+ * outputs are NaN and do not disturb the other members.
+ * Members run in chunks that fit in 4 GiB of device memory (BGP_BATCH_CHUNK=<members> overrides it); every step of a
+ * chunk is one launch for all its members.  Device workspace per member (doubles): 2 n^2 (factor and K^-1) +
+ * (4 + t) n (t = n for n <= 8, else 1) + ceil(n / 32)^2 P contraction partials + P.  Shared: B programs, x, which.
+ * Forming K_b^-1 costs about 2 n^3 flops per member on the CUDA cores, against n^3 / 3 for the factorisation.
+ * Errors: those of bgp_dense_batch_log_likelihood; BGP_ERR_INVALID for P > 64, before anything is solved.  B == 0
+ * writes nothing. */
+int bgp_dense_batch_grad_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params,
+                               int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
+                               const double* yerr, const double* r,      /* B x n row-major          */
+                               const uint32_t* which,                    /* P, shared by all members */
+                               double* log_det, double* quad,            /* B, may be NULL           */
+                               double* alpha, double* diag,              /* B x n, may be NULL       */
+                               double* g,                                /* B x P, may be NULL       */
+                               int32_t* info);                           /* B                        */
 /* Batched predictions (GP.batch_predict): for the same B members as bgp_dense_batch_log_likelihood (spec, params, x,
  * yerr; r = y - mean(x) per member, B x n row-major) and the test points xs (ns x ndim row-major, host):
  *   mean[b*ns + j]        = (K_b(x*, x) K_b^-1 r_b)_j            (the kernel part of GP.predict's mean)
