@@ -101,6 +101,7 @@ SIGNATURES = {
     "bgp_hodlr_node_pivots": (C.c_int, [_p, _i64, _p, _p]),
     "bgp_hodlr_node_factors": (C.c_int, [_p, _i64, _p]),
     "bgp_hodlr_last_timing": (C.c_int, [_p, _dp]),
+    "bgp_hodlr_last_grad_timing": (C.c_int, [_p, _dp]),
     "bgp_hodlr_last_work": (C.c_int, [_p, _dp]),
     "bgp_hodlr_set_profiling": (C.c_int, [_p, C.c_int]),
     "bgp_hodlr_last_aca_profile": (C.c_int, [_p, _dp]),

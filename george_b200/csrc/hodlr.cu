@@ -27,6 +27,12 @@ int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const uns
                               int64_t n, const double* M, int64_t ldm, const double* alpha, double ca, double cm,
                               double* g_dev, double* diag_dev, DevBuf<double>& scratch, cudaStream_t s);
 int fill_identity_launch(double* A, int64_t n, cudaStream_t s);
+int64_t grad_slab_partial_size(int64_t n, int64_t c, int np);
+int64_t grad_slab_tile_size(int64_t n, int np);
+int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigned* which_dev, const double* x, int64_t n,
+                          const double* W, int64_t j0, int64_t nc, const double* alpha, double* partial,
+                          double* tile_part, double* diag_dev, cudaStream_t s);
+int kmat_grad_slab_finish(int np, int64_t n, const double* tile_part, double* g_dev, cudaStream_t s);
 int kmat_symmetric_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x, int64_t n,
                                const double* diag_add, double* out, int64_t ld, cudaStream_t s);
 int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
@@ -142,6 +148,7 @@ struct bgp_hodlr {
   size_t w_cap = 0;
 
   double t_ms[5] = {0, 0, 0, 0, 0};
+  double grad_t[4] = {0, 0, 0, 0};  // see bgp_hodlr_last_grad_timing
   double work[6] = {0, 0, 0, 0, 0, 0};
 };
 
@@ -168,7 +175,8 @@ static void build_tree(bgp_hodlr* h, int start, int size, int dir, int parent, i
   }
 }
 
-static int hodlr_solve_dev(bgp_hodlr* h, double* b, int64_t nrhs, int64_t ldb, cudaStream_t s, int part);
+static int hodlr_solve_dev(bgp_hodlr* h, double* b, int64_t nrhs, int64_t ldb, cudaStream_t s, int part,
+                           int64_t eye_row0 = -1);
 static int hodlr_exchange_finish(bgp_hodlr* h);
 
 // A sharded factorisation exchanges rows through the library's communicator when it spans exactly the shards and this
@@ -212,22 +220,25 @@ static void set_sweep_func_attrs() {
   done.fetch_or(bit, std::memory_order_relaxed);
 }
 
+// Leaves [l0, l1) of h->leaves (l1 < 0: all of them).
 template <int COLS>
 static int leaf_solve_launch(bgp_hodlr* h, double* X, int64_t ldx, const int* ncols_by_depth, int ncols_fixed,
-                             int max_cols, cudaStream_t s) {
+                             int max_cols, cudaStream_t s, int l0, int l1) {
   const int ngroups = (max_cols + COLS - 1) / COLS;
-  const dim3 grid((unsigned)(h->leaves.size() * (size_t)ngroups));
+  const dim3 grid((unsigned)((size_t)(l1 - l0) * (size_t)ngroups));
   const size_t smem = sizeof(double) * (size_t)h->max_leaf * COLS;
-  leaf_solve_kernel<COLS><<<grid, LS_THREADS, smem, s>>>(h->d_leaves.p, h->d_L.p, X, ldx, ncols_by_depth, ncols_fixed,
-                                                         h->max_leaf, ngroups);
+  leaf_solve_kernel<COLS><<<grid, LS_THREADS, smem, s>>>(h->d_leaves.p + l0, h->d_L.p, X, ldx, ncols_by_depth,
+                                                         ncols_fixed, h->max_leaf, ngroups);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
 
+// l0, l1: only leaves [l0, l1) of h->leaves (a row-restricted solve, hodlr_solve_dev); l1 < 0 runs every leaf
 static int launch_leaf_solve(bgp_hodlr* h, double* X, int64_t ldx, const int* ncols_by_depth, int ncols_fixed,
-                             int max_cols, cudaStream_t s) {
-  const int nl = (int)h->leaves.size();
-  if (nl == 0 || max_cols == 0) return BGP_OK;
+                             int max_cols, cudaStream_t s, int l0 = 0, int l1 = -1) {
+  if (l1 < 0) l1 = (int)h->leaves.size();
+  const int nl = l1 - l0;
+  if (nl <= 0 || max_cols == 0) return BGP_OK;
   // only leaves handled locally are in d_leaves.  The narrowest instantiation that covers the call (1, 2, 4 or 8
   // columns; a one-column solve carries no 8-wide registers), wider calls in groups of 8.  BGP_LEAF_COLS=32 selects the
   // 32-column instantiation for calls with more than 8 columns (the up-sweep): it streams the leaf factor once per 32
@@ -236,7 +247,7 @@ static int launch_leaf_solve(bgp_hodlr* h, double* X, int64_t ldx, const int* nc
   // Leaves too large for the group in shared memory take the widest narrower one that fits.
   const int m = h->max_leaf;
   if (h->leaf_cols_wide && max_cols > LS_COLS && leaf_solve_fits(m, LS_COLS_WIDE))
-    return leaf_solve_launch<LS_COLS_WIDE>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+    return leaf_solve_launch<LS_COLS_WIDE>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s, l0, l1);
   int cols = max_cols <= 1 ? 1 : max_cols <= 2 ? 2 : max_cols <= 4 ? 4 : LS_COLS;
   while (cols > 1 && !leaf_solve_fits(m, cols)) cols /= 2;
   if (!leaf_solve_fits(m, cols)) {
@@ -244,23 +255,26 @@ static int launch_leaf_solve(bgp_hodlr* h, double* X, int64_t ldx, const int* nc
     return BGP_ERR_INVALID;
   }
   switch (cols) {
-    case LS_COLS: return leaf_solve_launch<LS_COLS>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
-    case 4: return leaf_solve_launch<4>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
-    case 2: return leaf_solve_launch<2>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
-    default: return leaf_solve_launch<1>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s);
+    case LS_COLS: return leaf_solve_launch<LS_COLS>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s, l0, l1);
+    case 4: return leaf_solve_launch<4>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s, l0, l1);
+    case 2: return leaf_solve_launch<2>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s, l0, l1);
+    default: return leaf_solve_launch<1>(h, X, ldx, ncols_by_depth, ncols_fixed, max_cols, s, l0, l1);
   }
 }
 
 // one internal level: W = V^T X (both halves), small solve, X -= U T.   factor: up-sweep (X = U panel) vs plain solve
 // Two paths: ranks whose 2r x 2r Woodbury matrix fits one CTA's shared memory (the common case) run three batched
 // kernels; larger ranks run the Gram / update products on DMMA and the blocked LU of hodlr_lu.cuh.
+// b0, b1: only nodes [b0, b1) of L.nodes (a row-restricted solve, hodlr_solve_dev); b1 < 0 runs the whole level.  Node
+// b's W block is then block b - b0.
 static int launch_level_big(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t ldx, int ncolsW, int own_off, int factor,
-                            int col_lo, int col_hi, cudaStream_t s);
+                            int col_lo, int col_hi, cudaStream_t s, int b0, int b1);
 
 static int launch_level(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t ldx, int ncolsW, int own_off, int factor,
-                        int col_lo, int col_hi, cudaStream_t s) {
-  const int nn = (int)L.nodes.size();
-  if (nn == 0 || L.r == 0) {
+                        int col_lo, int col_hi, cudaStream_t s, int b0 = 0, int b1 = -1) {
+  if (b1 < 0) b1 = (int)L.nodes.size();
+  const int nn = b1 - b0;
+  if (nn <= 0 || L.r == 0) {
     return BGP_OK;
   }
   const int r = L.r;
@@ -270,8 +284,8 @@ static int launch_level(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t ldx
   BGP_CUDA(cudaMemsetAsync(h->d_W.p, 0, sizeof(double) * need, s));
   // h->small_limit: BGP_SMALL_RANK_LIMIT=<2r> (read at compute()) lowers the switch-over so the tests can drive every
   // level through the big path
-  if (2 * r > h->small_limit) return launch_level_big(h, L, X, ldx, ncolsW, own_off, factor, col_lo, col_hi, s);
-  const NodeDesc* nd = h->d_nodes.p + L.desc_off;
+  if (2 * r > h->small_limit) return launch_level_big(h, L, X, ldx, ncolsW, own_off, factor, col_lo, col_hi, s, b0, b1);
+  const NodeDesc* nd = h->d_nodes.p + L.desc_off + b0;
   const int max_nh = L.max_half + 1;
   if (r <= GTS_MAX_R) {
     dim3 grid((max_nh + GTS_ROWS - 1) / GTS_ROWS, nn * 2, (ncolsW + GTS_TC - 1) / GTS_TC);
@@ -289,7 +303,7 @@ static int launch_level(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t ldx
   {
     const size_t sbytes = sizeof(double) * (size_t)(2 * r) * (2 * r);
     small_solve_kernel<<<nn, SS_THREADS, sbytes, s>>>(nd, h->d_W.p, stride, ncolsW, own_off, factor, h->d_S.p,
-                                                      h->d_node_logdet.p, L.desc_off);
+                                                      h->d_node_logdet.p, L.desc_off + b0);
     BGP_LAUNCH_CHECK();
   }
   if (col_hi > col_lo) {
@@ -301,8 +315,8 @@ static int launch_level(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t ldx
 }
 
 static int launch_level_big(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t ldx, int ncolsW, int own_off, int factor,
-                            int col_lo, int col_hi, cudaStream_t s) {
-  const int nn = (int)L.nodes.size();
+                            int col_lo, int col_hi, cudaStream_t s, int b0, int b1) {
+  const int nn = b1 - b0;
   const int r = L.r, n2 = 2 * r;
   const int64_t stride = (int64_t)n2 * ncolsW;
   const int64_t ldv = h->pset(L).ld, ldu = h->pset(L).ld;
@@ -311,13 +325,14 @@ static int launch_level_big(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t
   std::vector<LuNode> lun(nn);
   std::vector<GemmDesc> gram, upd;
   int max_nh = 0;
-  for (int b = 0; b < nn; ++b) {
+  for (int k = 0; k < nn; ++k) {
+    const int b = b0 + k;
     const HNode& nd = h->nodes[L.nodes[b]];
     const int64_t s_off = h->h_nodes[L.desc_off + b].s_off;
-    lun[b].S = h->d_S.p + s_off;
-    lun[b].piv = reinterpret_cast<int*>(lun[b].S + (int64_t)n2 * n2);
-    lun[b].logdet = h->d_node_logdet.p + L.desc_off + b;
-    double* Wn = W + (int64_t)b * stride;
+    lun[k].S = h->d_S.p + s_off;
+    lun[k].piv = reinterpret_cast<int*>(lun[k].S + (int64_t)n2 * n2);
+    lun[k].logdet = h->d_node_logdet.p + L.desc_off + b;
+    double* Wn = W + (int64_t)k * stride;
     for (int hh = 0; hh < 2; ++hh) {
       const int rs = nd.start + (hh ? nd.half : 0), nh = hh ? (nd.size - nd.half) : nd.half;
       max_nh = std::max(max_nh, nh);
@@ -992,14 +1007,76 @@ static int exchange_rows(bgp_hodlr* h, double* P, int64_t ld, int64_t cols, cuda
   return BGP_OK;
 }
 
+// [*first, *last): the items 0 .. count-1, whose row intervals [start(k), start(k) + size(k)) are disjoint and ordered
+// by start, that meet rows [lo, hi)
+template <class StartSize>
+static void rows_meeting(int count, const StartSize& start_size, int64_t lo, int64_t hi, int* first, int* last) {
+  int a = 0, b = count;  // first item ending after lo
+  while (a < b) {
+    const int m = (a + b) / 2;
+    int st, sz;
+    start_size(m, &st, &sz);
+    if ((int64_t)st + sz <= lo) a = m + 1; else b = m;
+  }
+  *first = a;
+  b = count;  // first item starting at or after hi
+  while (a < b) {
+    const int m = (a + b) / 2;
+    int st, sz;
+    start_size(m, &st, &sz);
+    if (st < hi) a = m + 1; else b = m;
+  }
+  *last = a;
+}
+
+// Leaves (h->leaves) and each level's nodes (L.nodes, and so its NodeDesc block) are in pre-order, which lists the
+// disjoint row intervals of one depth, and the leaves, from left to right: rows_meeting's precondition.
+static bool rows_ordered(const bgp_hodlr* h) {
+  auto ordered = [&](const std::vector<int>& ids) {
+    for (size_t k = 1; k < ids.size(); ++k) {
+      const HNode& a = h->nodes[ids[k - 1]];
+      if (a.start + a.size > h->nodes[ids[k]].start) return false;
+    }
+    return true;
+  };
+  if (!ordered(h->leaves)) return false;
+  for (const LevelInfo& L : h->levels)
+    if (!ordered(L.nodes)) return false;
+  return true;
+}
+
 // part: 0 = everything, 1 = local (leaves + levels >= cut), 2 = top (levels < cut)
-static int hodlr_solve_dev(bgp_hodlr* h, double* b, int64_t nrhs, int64_t ldb, cudaStream_t s, int part) {
+// eye_row0 >= 0 restricts the solve by rows: the caller guarantees that columns [c0, c0 + 64) of b are zero outside rows
+// [eye_row0 + c0, eye_row0 + c0 + 64) (identity columns e_j, j = eye_row0 + column: grad_terms' K^-1 slabs).  Every step
+// of the solve is block diagonal and maps zero rows to zero rows, so only the leaves and, per level, the nodes that meet
+// those rows run; the result is bit for bit the unrestricted one.  Single-GPU factorisations only (part 0).
+static int hodlr_solve_dev(bgp_hodlr* h, double* b, int64_t nrhs, int64_t ldb, cudaStream_t s, int part,
+                           int64_t eye_row0) {
   const int nlev = (int)h->levels.size();
   const int cut = h->opts.shard_count > 1 ? h->cut_depth : 0;
   const bool native_x = part == 0 && h->opts.shard_count > 1 && !host_exchange(h);
+  if (eye_row0 >= 0 && (part != 0 || h->opts.shard_count > 1)) {
+    set_error("internal: a row-restricted solve needs a single-GPU factorisation");
+    return BGP_ERR_INVALID;
+  }
   for (int64_t c0 = 0; c0 < nrhs; c0 += 64) {
     const int nc = (int)std::min<int64_t>(64, nrhs - c0);
     double* X = b + c0 * ldb;
+    if (eye_row0 >= 0) {
+      const int64_t lo = eye_row0 + c0, hi = lo + nc;
+      int l0, l1;
+      rows_meeting((int)h->leaves.size(), [&](int k, int* st, int* sz) {
+        const HNode& nd = h->nodes[h->leaves[k]]; *st = nd.start; *sz = nd.size; }, lo, hi, &l0, &l1);
+      BGP_TRY(launch_leaf_solve(h, X, ldb, nullptr, nc, nc, s, l0, l1));
+      for (int l = nlev - 1; l >= 0; --l) {
+        const LevelInfo& L = h->levels[l];
+        int b0, b1;
+        rows_meeting((int)L.nodes.size(), [&](int k, int* st, int* sz) {
+          const HNode& nd = h->nodes[L.nodes[k]]; *st = nd.start; *sz = nd.size; }, lo, hi, &b0, &b1);
+        BGP_TRY(launch_level(h, L, X, ldb, nc, 0, 0, 0, nc, s, b0, b1));
+      }
+      continue;
+    }
     if (part != 2) {
       BGP_TRY(launch_leaf_solve(h, X, ldb, nullptr, nc, nc, s));
       for (int l = nlev - 1; l >= cut; --l) BGP_TRY(launch_level(h, h->levels[l], X, ldb, nc, 0, 0, 0, nc, s));
@@ -1204,9 +1281,41 @@ int bgp_hodlr_get_inverse(bgp_hodlr_t* h, double* out) {
   return bgp_hodlr_apply_inverse(h, out, n, n);  // COLUMN-major K^-1 (symmetric only to tol: the host transposes)
 }
 
+// E_J: columns j0 .. j0 + nc of the identity, n rows (the slab W is zeroed before)
+__global__ void eye_slab_kernel(double* __restrict__ W, int64_t n, int64_t j0, int64_t nc) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nc; k += (int64_t)gridDim.x * blockDim.x)
+    W[k * n + j0 + k] = 1.0;
+}
+
+// K^-1 resident (n x n) up to this many doubles (n <= 65536); larger n streams it in column slabs
+constexpr int64_t GRAD_RESIDENT_MAX = (int64_t)1 << 32;
+constexpr int64_t GRAD_SLAB_BUDGET = (int64_t)1 << 27;  // doubles (1 GiB) per K^-1 slab
+
+// Columns per K^-1 slab: as many n-row columns as fit in GRAD_SLAB_BUDGET, at least 64, a multiple of 64 (the
+// predict_chunk_cols rule).  BGP_GRAD_CHUNK=<c> (read at every call, like BGP_PREDICT_CHUNK) forces the streamed path at
+// any n with c columns, rounded up to 64; tests use it to run many slabs with a ragged tail at small sizes.
+static int64_t grad_slab_cols(int64_t n, bool* forced) {
+  int64_t c = std::max<int64_t>(64, (GRAD_SLAB_BUDGET / std::max<int64_t>(n, 1)) / 64 * 64);
+  *forced = false;
+  if (const char* e = getenv("BGP_GRAD_CHUNK")) {
+    const long v = atol(e);
+    if (v >= 1) { c = (v + 63) / 64 * 64; *forced = true; }
+  }
+  return std::min(c, (n + 63) / 64 * 64);
+}
+
+static float event_ms(cudaEvent_t a, cudaEvent_t b) {
+  float ms = 0;
+  cudaEventElapsedTime(&ms, a, b);
+  return ms;
+}
+
 // alpha = K^-1 r, g_p = sum_ij (alpha alpha^T - K^-1)_ij dK_ij/dtheta_p, diag(alpha alpha^T - K^-1): everything
 // GP.grad_log_likelihood (gp.py:406-468) needs from the solver, with K^-1 (solve against the identity, _hodlr.cpp:193-199)
 // and the gradient contraction staying on the device.
+// Two regimes (include/bgp.h): up to n = 65536 K^-1 is formed whole and contracted by kmat_grad_contract_kernel; above,
+// or with BGP_GRAD_CHUNK set, it is streamed in column slabs W = K^-1 E_J, each solved with the row-restricted solve
+// and contracted by kmat_grad_slab_kernel, so K^-1 is never resident.
 int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
                          double* diag_out) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
@@ -1215,23 +1324,81 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
   const int np = h->prog.n_params_total;
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
   cudaStream_t s = h->sA;
+  bool forced = false;
+  const int64_t c = grad_slab_cols(n, &forced);
+  const bool resident = !forced && n * n <= GRAD_RESIDENT_MAX;
+  const bool prof = h->profile;
+  double t_solve = 0, t_contract = 0;
+  for (double& t : h->grad_t) t = 0;
   BGP_TRY(h->d_rhs.reserve((size_t)n * 2 + 64, s));
   double* alpha = h->d_rhs.p;
   double* dg = h->d_rhs.p + n;
   double* ddiag = h->d_rhs.p + n + 64;
   BGP_CUDA(cudaMemcpyAsync(alpha, r, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+  if (prof) BGP_CUDA(cudaEventRecord(h->ev[4], s));
   BGP_TRY(hodlr_solve_dev(h, alpha, 1, n, s, 0));
+  if (prof) { BGP_CUDA(cudaEventRecord(h->ev[5], s)); BGP_CUDA(cudaEventSynchronize(h->ev[5])); t_solve += event_ms(h->ev[4], h->ev[5]); }
   if (alpha_out) BGP_CUDA(cudaMemcpyAsync(alpha_out, alpha, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
-  BGP_TRY(h->d_inv.reserve((size_t)n * n, s));
-  BGP_TRY(fill_identity_launch(h->d_inv.p, n, s));
-  BGP_TRY(hodlr_solve_dev(h, h->d_inv.p, n, n, s, 0));
-  BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
-  if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
-  BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, alpha, 1.0, -1.0, dg,
-                                    diag_out ? ddiag : nullptr, h->d_gscratch, s));
+  if (resident) {
+    if (prof) BGP_CUDA(cudaEventRecord(h->ev[4], s));
+    BGP_TRY(h->d_inv.reserve((size_t)n * n, s));
+    BGP_TRY(fill_identity_launch(h->d_inv.p, n, s));
+    BGP_TRY(hodlr_solve_dev(h, h->d_inv.p, n, n, s, 0));
+    if (prof) BGP_CUDA(cudaEventRecord(h->ev[5], s));
+    BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
+    if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
+    BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, alpha, 1.0, -1.0, dg,
+                                      diag_out ? ddiag : nullptr, h->d_gscratch, s));
+    if (prof) {
+      BGP_CUDA(cudaEventRecord(h->ev[7], s));
+      BGP_CUDA(cudaEventSynchronize(h->ev[7]));
+      t_solve += event_ms(h->ev[4], h->ev[5]);
+      t_contract += event_ms(h->ev[5], h->ev[7]);
+    }
+  } else {
+    // streamed: slab W (n x c), then the per-tile partials and one slab's per-split partials in d_gscratch
+    if (!rows_ordered(h)) { set_error("internal: HODLR rows are not ordered by level"); return BGP_ERR_CUDA; }
+    const int64_t tsize = grad_slab_tile_size(n, np), psize = grad_slab_partial_size(n, c, np);
+    BGP_TRY(h->d_inv.reserve((size_t)n * c, s));
+    BGP_TRY(h->d_gscratch.reserve((size_t)(tsize + psize), s));
+    BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
+    if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
+    double* W = h->d_inv.p;
+    double* tile_part = h->d_gscratch.p;
+    double* partial = h->d_gscratch.p + tsize;
+    int64_t slabs = 0;
+    for (int64_t j0 = 0; j0 < n; j0 += c, ++slabs) {
+      const int64_t nc = std::min(c, n - j0);
+      if (prof) BGP_CUDA(cudaEventRecord(h->ev[4], s));
+      BGP_CUDA(cudaMemsetAsync(W, 0, sizeof(double) * n * nc, s));
+      eye_slab_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, n, j0, nc);
+      BGP_LAUNCH_CHECK();
+      BGP_TRY(hodlr_solve_dev(h, W, nc, n, s, 0, j0));
+      if (prof) BGP_CUDA(cudaEventRecord(h->ev[5], s));
+      BGP_TRY(kmat_grad_slab_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, W, j0, nc, alpha, partial,
+                                    tile_part, diag_out ? ddiag : nullptr, s));
+      if (prof) {
+        BGP_CUDA(cudaEventRecord(h->ev[7], s));
+        BGP_CUDA(cudaEventSynchronize(h->ev[7]));
+        t_solve += event_ms(h->ev[4], h->ev[5]);
+        t_contract += event_ms(h->ev[5], h->ev[7]);
+      }
+    }
+    if (prof) BGP_CUDA(cudaEventRecord(h->ev[4], s));
+    BGP_TRY(kmat_grad_slab_finish(np, n, tile_part, dg, s));
+    if (prof) {
+      BGP_CUDA(cudaEventRecord(h->ev[5], s));
+      BGP_CUDA(cudaEventSynchronize(h->ev[5]));
+      t_contract += event_ms(h->ev[4], h->ev[5]);
+    }
+    h->grad_t[2] = (double)slabs;
+    h->grad_t[3] = (double)c;
+  }
   if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
   if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));
+  h->grad_t[0] = t_solve;
+  h->grad_t[1] = t_contract;
   return BGP_OK;
 }
 
@@ -1347,6 +1514,11 @@ int bgp_hodlr_node_factors(const bgp_hodlr_t* h, int64_t node, double* out) {
 int bgp_hodlr_last_timing(const bgp_hodlr_t* h, double* ms5) {
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
   for (int i = 0; i < 5; ++i) ms5[i] = h->t_ms[i];
+  return BGP_OK;
+}
+int bgp_hodlr_last_grad_timing(const bgp_hodlr_t* h, double* out4) {
+  if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  for (int i = 0; i < 4; ++i) out4[i] = h->grad_t[i];
   return BGP_OK;
 }
 int bgp_hodlr_set_profiling(bgp_hodlr_t* h, int on) {

@@ -373,6 +373,141 @@ int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const uns
                                     scratch, s);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Slab gradient contraction (bgp_hodlr_grad_terms at large n, which never holds all of K^-1): for a slab
+// W = K^-1 E_J of columns J = [j0, j0 + nc) (n x nc, column-major, W[(j - j0) n + i] = (K^-1)_ij),
+//     g_p += sum_{i, j in J} (alpha_i alpha_j - W_ij) dK_ij/dtheta_p.
+// Every ordered pair is evaluated (george's einsum over all (i, j)): the symmetric weighting of
+// kmat_grad_contract_kernel would need rows of K^-1 from two slabs.  One thread per row i; the coordinates and alpha of
+// a 32-column j-tile are staged in shared memory and W is read coalesced along i.  CTA (tile t, split s) covers rows
+// [s GS_ROWS, (s + 1) GS_ROWS) of tile t and writes one partial per parameter; grad_slab_reduce_kernel sums the splits
+// in order into the tile's slot of a (ceil(n / 32) x P) array, and grad_contract_reduce_kernel sums the tiles in order
+// once every slab is done.  The split plan and the tile boundaries depend only on n (slabs start at multiples of 64),
+// so g does not depend on the slab width, and no atomics: two identical calls return the same bits.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int GS_TJ = 32;          // columns per j-tile
+constexpr int GS_THREADS = 256;
+constexpr int64_t GS_ROWS = 1024;  // rows per i-split
+// x_j staging (inputs of up to 128 dimensions): with the ~12 KB of static shared memory it stays under the default
+// 48 KB per CTA; wider inputs read x_j from global memory
+constexpr size_t GS_SMEM_CAP = 32 * 1024;
+
+template <int NPMAX>
+__global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevProgram* __restrict__ gprog,
+                                                                    const unsigned* __restrict__ which,
+                                                                    const double* __restrict__ x, int64_t n,
+                                                                    const double* __restrict__ W, int64_t j0,
+                                                                    int64_t nc, const double* __restrict__ alpha,
+                                                                    int stage_x, double* __restrict__ partial) {
+  extern __shared__ double sxj[];  // GS_TJ x nd coordinates of the tile's columns (stage_x)
+  __shared__ DevProgram P;
+  __shared__ unsigned sw[BGP_MAX_LEAVES * (4 + BGP_MAX_METRIC)];
+  __shared__ double saj[GS_TJ];
+  __shared__ double red[32];
+  const int np = gprog->n_params_total, nd = gprog->ndim;
+  const int64_t jt = j0 + (int64_t)blockIdx.x * GS_TJ;  // first column of the tile
+  const int nj = (int)min((int64_t)GS_TJ, j0 + nc - jt);
+  const int64_t r0 = (int64_t)blockIdx.y * GS_ROWS, r1 = min(n, r0 + GS_ROWS);
+  stage_program(&P, gprog);
+  for (int q = threadIdx.x; q < np; q += blockDim.x) sw[q] = which[q];
+  if (threadIdx.x < nj) saj[threadIdx.x] = alpha[jt + threadIdx.x];
+  if (stage_x)
+    for (int t = threadIdx.x; t < nj * nd; t += GS_THREADS) sxj[t] = x[jt * nd + t];
+  __syncthreads();
+  const double* Wt = W + (jt - j0) * n;
+  double acc[NPMAX], g[NPMAX];
+#pragma unroll
+  for (int q = 0; q < NPMAX; ++q) acc[q] = 0.0;
+  for (int64_t i = r0 + threadIdx.x; i < r1; i += GS_THREADS) {
+    const double ai = alpha[i];
+    const double* xi = x + i * nd;
+    for (int c = 0; c < nj; ++c) {
+      const double w = ai * saj[c] - Wt[(int64_t)c * n + i];
+      kernel_value_grad(P, xi, stage_x ? sxj + c * nd : x + (jt + c) * nd, sw, g);
+#pragma unroll
+      for (int q = 0; q < NPMAX; ++q)
+        if (q < np) acc[q] = fma(w, g[q], acc[q]);
+    }
+  }
+  // one partial per (tile, split, parameter)
+#pragma unroll
+  for (int q = 0; q < NPMAX; ++q) {
+    if (q < np) {  // uniform across the CTA
+      const double s = block_sum(acc[q], red);
+      if (threadIdx.x == 0) partial[((int64_t)blockIdx.x * gridDim.y + blockIdx.y) * np + q] = s;
+    }
+  }
+}
+
+// tile_part[t * np + q] = sum_s partial[(t * nsplit + s) * np + q], s ascending, for the ntile tiles of one slab
+__global__ void grad_slab_reduce_kernel(const double* __restrict__ partial, int64_t nsplit, int64_t ntile, int np,
+                                        double* __restrict__ tile_part) {
+  const int64_t total = ntile * np;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t tile = t / np, q = t - tile * np;
+    double s = 0.0;
+    for (int64_t sp = 0; sp < nsplit; ++sp) s += partial[(tile * nsplit + sp) * np + q];
+    tile_part[t] = s;
+  }
+}
+
+// diag[j] = alpha_j^2 - W_jj for j in [j0, j0 + nc): the square and the difference rounded separately (no contraction
+// into an FMA), as alpha**2 - diag(K^-1) is on the host
+__global__ void grad_slab_diag_kernel(const double* __restrict__ W, int64_t n, int64_t j0, int64_t nc,
+                                      const double* __restrict__ alpha, double* __restrict__ diag) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nc; k += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t j = j0 + k;
+    diag[j] = __dsub_rn(__dmul_rn(alpha[j], alpha[j]), W[k * n + j]);
+  }
+}
+
+// doubles of per-slab partials for slabs of up to c columns of an n-row K^-1
+int64_t grad_slab_partial_size(int64_t n, int64_t c, int np) {
+  return ((n + GS_ROWS - 1) / GS_ROWS) * ((c + GS_TJ - 1) / GS_TJ) * std::max(np, 1);
+}
+// doubles of per-tile partials (all slabs) for an n-row K^-1
+int64_t grad_slab_tile_size(int64_t n, int np) { return ((n + GS_TJ - 1) / GS_TJ) * std::max(np, 1); }
+
+// One slab (j0 a multiple of 32): its tiles' partials into tile_part + (j0 / 32) * np, and diag[j0 .. j0 + nc) when
+// diag_dev is set.  partial: grad_slab_partial_size(n, nc, np) doubles.
+int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigned* which_dev, const double* x, int64_t n,
+                          const double* W, int64_t j0, int64_t nc, const double* alpha, double* partial,
+                          double* tile_part, double* diag_dev, cudaStream_t s) {
+  if (nc <= 0) return BGP_OK;
+  if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  if (j0 % GS_TJ) { set_error("internal: slab start %lld is not a multiple of %d", (long long)j0, GS_TJ); return BGP_ERR_INVALID; }
+  if (np > 0) {
+    const int64_t nsplit = (n + GS_ROWS - 1) / GS_ROWS, ntile = (nc + GS_TJ - 1) / GS_TJ;
+    if (nsplit > 65535 || ntile > 0x7fffffffLL) { set_error("kmat_grad_slab: n too large for one launch"); return BGP_ERR_INVALID; }
+    const size_t sbytes = sizeof(double) * (size_t)GS_TJ * nd;
+    const int stage_x = sbytes <= GS_SMEM_CAP ? 1 : 0;
+    const size_t smem = stage_x ? sbytes : 0;
+    const dim3 grid((unsigned)ntile, (unsigned)nsplit);
+    if (np <= 8)
+      kmat_grad_slab_kernel<8><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, alpha, stage_x, partial);
+    else
+      kmat_grad_slab_kernel<64><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, alpha, stage_x, partial);
+    BGP_LAUNCH_CHECK();
+    const int64_t total = ntile * np;
+    grad_slab_reduce_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 8 * (int64_t)num_sms()), 256, 0, s>>>(
+        partial, nsplit, ntile, np, tile_part + (j0 / GS_TJ) * np);
+    BGP_LAUNCH_CHECK();
+  }
+  if (diag_dev) {
+    grad_slab_diag_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, n, j0, nc, alpha, diag_dev);
+    BGP_LAUNCH_CHECK();
+  }
+  return BGP_OK;
+}
+
+// g_dev[q] = sum_t tile_part[t * np + q] over the ceil(n / 32) tiles, in a fixed order
+int kmat_grad_slab_finish(int np, int64_t n, const double* tile_part, double* g_dev, cudaStream_t s) {
+  if (np <= 0) return BGP_OK;
+  grad_contract_reduce_kernel<<<dim3((unsigned)np, 1), 256, 0, s>>>(tile_part, (n + GS_TJ - 1) / GS_TJ, np, g_dev, 0, 0);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
 // `members` identity matrices of order n, back to back (member stride n^2; column-major == row-major)
 __global__ void fill_identity_kernel(double* __restrict__ A, int64_t n, int64_t total) {
   const int64_t nn = n * n;

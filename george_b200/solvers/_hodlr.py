@@ -179,6 +179,16 @@ class HODLRSolver(object):
         _lib.check(self._lib.bgp_hodlr_last_timing(self._ptr, t))
         return dict(zip(("leaves_ms", "aca_ms", "upsweep_ms", "compute_ms", "solve_ms"), list(t)))
 
+    def grad_timing(self):
+        """The last ``grad_terms`` call (``include/bgp.h: bgp_hodlr_last_grad_timing``): ``solve_ms`` and
+        ``contract_ms`` (measured with profiling on, 0 otherwise), ``slabs`` and ``slab_cols`` (0 on the resident
+        path)."""
+        t = (C.c_double * 4)()
+        _lib.check(self._lib.bgp_hodlr_last_grad_timing(self._ptr, t))
+        out = dict(zip(("solve_ms", "contract_ms", "slabs", "slab_cols"), list(t)))
+        out["slabs"], out["slab_cols"] = int(out["slabs"]), int(out["slab_cols"])
+        return out
+
     def set_profiling(self, on=True):
         _lib.check(self._lib.bgp_hodlr_set_profiling(self._ptr, 1 if on else 0))
 
