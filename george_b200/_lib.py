@@ -100,6 +100,7 @@ SIGNATURES = {
     "bgp_hodlr_node_info": (C.c_int, [_p, C.POINTER(HodlrNodeInfo)]),
     "bgp_hodlr_node_pivots": (C.c_int, [_p, _i64, _p, _p]),
     "bgp_hodlr_node_factors": (C.c_int, [_p, _i64, _p]),
+    "bgp_hodlr_last_draw_paths": (C.c_int, [_p, C.POINTER(C.c_uint64)]),
     "bgp_hodlr_last_timing": (C.c_int, [_p, _dp]),
     "bgp_hodlr_last_grad_timing": (C.c_int, [_p, _dp]),
     "bgp_hodlr_last_work": (C.c_int, [_p, _dp]),

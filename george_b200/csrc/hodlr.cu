@@ -143,6 +143,7 @@ struct bgp_hodlr {
   bool profile = false;
   std::vector<cudaEvent_t> prof_events;
   double prof[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};  // see bgp_hodlr_last_aca_profile
+  uint64_t draw_paths[4] = {0, 0, 0, 0};  // see bgp_hodlr_last_draw_paths
   DevBuf<double> d_vpart, d_upart, d_vmax;
   int aca_iters = 0;
   size_t w_cap = 0;
@@ -433,7 +434,7 @@ static int run_aca2(bgp_hodlr* h, const std::vector<AcaDesc>& descs, std::vector
   BGP_TRY(h->d_nactive.reserve(2, s));
   int n_top = 0;
   for (int i = 0; i < nn; ++i) n_top += hn[i].is_top;
-  BGP_TRY(h->d_stats.reserve(4, s));
+  BGP_TRY(h->d_stats.reserve(A2_NSTATS, s));
   int64_t work_cap = 0;
   // items per chunk: batches of up to 256 live candidates are cut into blocks of A2_CG, larger ones into A2_CG * A2_ITEM_CB
   for (int i = 0; i < nn; ++i) {
@@ -446,7 +447,7 @@ static int run_aca2(bgp_hodlr* h, const std::vector<AcaDesc>& descs, std::vector
   BGP_TRY(h->d_iter.reserve(1, s));
   BGP_CUDA(cudaMemsetAsync(h->d_iter.p, 0, sizeof(int), s));
   BGP_CUDA(cudaMemsetAsync(h->d_work_count.p, 0, sizeof(int) * 4, s));
-  BGP_CUDA(cudaMemsetAsync(h->d_stats.p, 0, sizeof(unsigned long long) * 4, s));
+  BGP_CUDA(cudaMemsetAsync(h->d_stats.p, 0, sizeof(unsigned long long) * A2_NSTATS, s));
   BGP_CUDA(cudaMemcpyAsync(h->d_a2nodes.p, hn.data(), sizeof(A2Node) * nn, cudaMemcpyHostToDevice, s));
   BGP_CUDA(cudaMemcpyAsync(h->d_cchunk_node.p, cchunk_node.data(), sizeof(int) * ncc, cudaMemcpyHostToDevice, s));
   BGP_CUDA(cudaMemcpyAsync(h->d_rchunk_node.p, rchunk_node.data(), sizeof(int) * nrc, cudaMemcpyHostToDevice, s));
@@ -566,9 +567,10 @@ static int run_aca2(bgp_hodlr* h, const std::vector<AcaDesc>& descs, std::vector
   }
   h->aca_iters = iters;
   {
-    unsigned long long st4[4] = {0, 0, 0, 0};
+    unsigned long long st4[A2_NSTATS] = {0};
     BGP_CUDA(cudaMemcpyAsync(st4, h->d_stats.p, sizeof(st4), cudaMemcpyDeviceToHost, s));
     BGP_CUDA(cudaStreamSynchronize(s));
+    for (int k = 0; k < 4; ++k) h->draw_paths[k] = st4[A2_PATH_REDO + k];
     h->prof[1] = iters; h->prof[2] = (double)st4[0]; h->prof[3] = (double)st4[1]; h->prof[4] = (double)st4[2];
     h->prof[5] = (double)st4[3];
     if (h->profile) {
@@ -604,6 +606,7 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
                                   int32_t ndim, const double* yerr_dev, const bgp_hodlr_opts_t* opts_in) {
   h->computed = false;
   h->top_pending = false;
+  for (uint64_t& c : h->draw_paths) c = 0;  // (rng_mode = reference never runs the speculative draws)
   h->shard_row0.clear(); h->shard_rows.clear();  // only a sharded compute that cuts the tree reports ranges
   BGP_TRY(require_device());
   BGP_TRY(ensure_streams(h));
@@ -1508,6 +1511,13 @@ int bgp_hodlr_node_factors(const bgp_hodlr_t* h, int64_t node, double* out) {
   const double* src = ps.vbase() + (int64_t)L.vcol * ps.ld + nd.start;
   BGP_CUDA(cudaMemcpy2D(out, sizeof(double) * nd.size, src, sizeof(double) * ps.ld, sizeof(double) * nd.size, nd.rank,
                         cudaMemcpyDeviceToHost));
+  return BGP_OK;
+}
+
+int bgp_hodlr_last_draw_paths(const bgp_hodlr_t* h, uint64_t* out4) {
+  if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  if (!h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  for (int i = 0; i < 4; ++i) out4[i] = h->draw_paths[i];
   return BGP_OK;
 }
 

@@ -179,6 +179,15 @@ struct A2Args {
   int shard_rank, shard_count;  // multi-GPU: top nodes' column chunks are dealt round-robin to the ranks
   unsigned long long* stats;  // [0] candidate-row entries verified (pairs), [1] residual-update FMAs executed, [2] candidates,
                               // [3] entries actually evaluated by a2_eval (the rest were bounded < 1e-14 without evaluation)
+                              // [4..7] rare paths of the speculative draws, see A2_PATH_* (bgp_hodlr_last_draw_paths)
+};
+// stats slots counting how often a2_generate / a2_decide left the common path
+enum {
+  A2_PATH_REDO = 4,        // Lemire rejections redone inside a batch (one pass of a2_generate's redo loop each)
+  A2_PATH_TRUNCATED = 5,   // batches cut short before a rejecting draw whose next words were not generated yet
+  A2_PATH_SEQUENTIAL = 6,  // rejecting draws at position 0 of such a batch, drawn alone by mt_uniform
+  A2_PATH_PARTIAL = 7,     // commits that replayed the stream to the winning draw instead of copying the end-of-batch state
+  A2_NSTATS = 8
 };
 
 // shared-memory workspace of the per-node kernels (dynamic shared memory)
@@ -287,6 +296,7 @@ __device__ inline void a2_generate(const A2Args& a, A2State& st, A2NodeSmem& S, 
     __syncthreads();  // every thread has read S.flag before thread 0 rewrites it below
     // redo draw c0: words raw[c0 + extra + 1], ... until one is accepted (they were already generated for later draws)
     if (threadIdx.x == 0) {
+      atomicAdd(a.stats + A2_PATH_REDO, 1ull);
       const uint32_t srange = (uint32_t)(n_index - c0);
       const uint32_t thr = (0u - srange) % srange;
       int e = extra;
@@ -300,13 +310,22 @@ __device__ inline void a2_generate(const A2Args& a, A2State& st, A2NodeSmem& S, 
       else S.flag = -1 - c0;  // ran out of generated words / budget: truncate the batch before this draw
     }
     __syncthreads();
-    if (S.flag < 0) {  // (practically unreachable) keep the draws before c0; with none left, draw c0 alone, sequentially
+    // The LAST draw of the batch rejected (about one rejection in B; every rejection of a one-candidate batch, the steady
+    // state of a high-rank node): its next word is not in raw[].  Keep the draws before c0 and let the next batch start
+    // with c0; with none left (B = 1), draw c0 alone, sequentially.  Running out of the A2_XWORDS budget lands here too.
+    if (S.flag < 0) {
       const int c0t = -1 - S.flag;
       __syncthreads();
-      if (c0t > 0) { B = c0t; truncated = true; break; }
+      if (c0t > 0) {
+        if (threadIdx.x == 0) atomicAdd(a.stats + A2_PATH_TRUNCATED, 1ull);
+        B = c0t; truncated = true; break;
+      }
       mt_copy(&S.rng, rng_commit);
       __syncthreads();
-      if (threadIdx.x == 0) { int w = 0; S.k[0] = mt_uniform(S.rng, (uint32_t)n_index, &w); words[0] = w; cmax[0] = 0ull; S.extra = -1; }
+      if (threadIdx.x == 0) {
+        atomicAdd(a.stats + A2_PATH_SEQUENTIAL, 1ull);
+        int w = 0; S.k[0] = mt_uniform(S.rng, (uint32_t)n_index, &w); words[0] = w; cmax[0] = 0ull; S.extra = -1;
+      }
       __syncthreads();
       B = 1;
       break;
@@ -680,6 +699,7 @@ __global__ void __launch_bounds__(A2_NODE_THREADS) a2_decide_kernel(A2Args a) {
     if (w == st.end_words) {
       mt_copy(&S.rng, rng_commit + 1);
     } else {
+      if (threadIdx.x == 0) atomicAdd(a.stats + A2_PATH_PARTIAL, 1ull);
       mt_copy(&S.rng, rng_commit);
       __syncthreads();
       mt_skip_coop(S.rng, w);

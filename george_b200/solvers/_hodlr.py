@@ -174,6 +174,14 @@ class HODLRSolver(object):
         _lib.check(self._lib.bgp_hodlr_node_factors(self._ptr, node, _lib.ptr(out)))
         return out[:nd["half"]], out[nd["half"]:]
 
+    def draw_paths(self):
+        """How often the last compute's speculative row draws left the common path
+        (``include/bgp.h: bgp_hodlr_last_draw_paths``)."""
+        self._require_computed()
+        c = (C.c_uint64 * 4)()
+        _lib.check(self._lib.bgp_hodlr_last_draw_paths(self._ptr, c))
+        return dict(zip(("lemire_redos", "truncated_batches", "sequential_draws", "partial_commits"), (int(v) for v in c)))
+
     def timing(self):
         t = (C.c_double * 5)()
         _lib.check(self._lib.bgp_hodlr_last_timing(self._ptr, t))

@@ -408,6 +408,12 @@ int bgp_hodlr_node_pivots(const bgp_hodlr_t* h, int64_t node, int32_t* rows, int
  * BGP_ERR_INVALID on a sharded factorisation; BGP_ERR_INDEX for a leaf or an out-of-range node; BGP_ERR_NOT_COMPUTED
  * before compute. */
 int bgp_hodlr_node_factors(const bgp_hodlr_t* h, int64_t node, double* out);
+/* Diagnostics: how often the per-node-stream ACA of the last compute left the common path of its speculative row draws
+ * (csrc/hodlr_aca2.cuh).  out4 = [0] Lemire rejections redone inside a batch, [1] batches truncated before a rejecting
+ * last draw, [2] rejecting draws of one-candidate batches drawn sequentially, [3] commits that replayed the mt19937
+ * stream to the winning draw instead of taking the saved end-of-batch state.  All zero for rng_mode = REFERENCE, which
+ * draws one row at a time.  BGP_ERR_NOT_COMPUTED before compute. */
+int bgp_hodlr_last_draw_paths(const bgp_hodlr_t* h, uint64_t* out4);
 /* Device-event timings of the last compute, ms: [0] leaves (build+factor; stream A, CONCURRENT with [1]),
  * [1] ACA (stream B, from the start of compute), [2] up-sweep (panel finalisation + leaf solves + level sweeps, from the
  * moment both streams have drained), [3] total compute, [4] last solve.  [3] ~ max([0], [1]) + host gap + [2]. */
