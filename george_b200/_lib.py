@@ -64,6 +64,7 @@ SIGNATURES = {
     "bgp_kmat_gradient_contract": (C.c_int, [_specp, _p, _p, _i64, _p, _p]),
     "bgp_dense_grad_terms": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_grad_terms": (C.c_int, [_p, _p, _p, _p, _p, _p]),
+    "bgp_hodlr_grad_terms_local_dev": (C.c_int, [_p, _p, _p, _p, _p]),
     "bgp_dense_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
     "bgp_hodlr_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
     "bgp_dense_batch_create": (C.c_int, [C.POINTER(_p)]),

@@ -286,7 +286,14 @@ int bgp_dev_alloc(void** p, size_t bytes) {
   return BGP_OK;
 }
 int bgp_dev_free(void* p) { BGP_CUDA(cudaFree(p)); return BGP_OK; }
-int bgp_dev_upload(void* dst, const void* src, size_t bytes) { BGP_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice)); return BGP_OK; }
+// From pageable host memory cudaMemcpy may return once the source is staged, before the DMA has reached dst, and the
+// library's streams are non-blocking (they do not order after the legacy stream that carries the copy): wait for the
+// copy, so a library call made right after the upload reads the uploaded data.
+int bgp_dev_upload(void* dst, const void* src, size_t bytes) {
+  BGP_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+  BGP_CUDA(cudaStreamSynchronize(cudaStreamLegacy));
+  return BGP_OK;
+}
 int bgp_dev_download(void* dst, const void* src, size_t bytes) { BGP_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost)); return BGP_OK; }
 int bgp_dev_synchronize(void) { BGP_CUDA(cudaDeviceSynchronize()); return BGP_OK; }
 int bgp_host_alloc_pinned(void** p, size_t bytes) { BGP_CUDA(cudaMallocHost(p, bytes)); return BGP_OK; }

@@ -30,9 +30,9 @@ int fill_identity_launch(double* A, int64_t n, cudaStream_t s);
 int64_t grad_slab_partial_size(int64_t n, int64_t c, int np);
 int64_t grad_slab_tile_size(int64_t n, int np);
 int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigned* which_dev, const double* x, int64_t n,
-                          const double* W, int64_t j0, int64_t nc, const double* alpha, double* partial,
-                          double* tile_part, double* diag_dev, cudaStream_t s);
-int kmat_grad_slab_finish(int np, int64_t n, const double* tile_part, double* g_dev, cudaStream_t s);
+                          const double* W, int64_t j0, int64_t nc, int64_t jlo, int64_t jhi, const double* alpha,
+                          double* partial, double* tile_part, double* diag_dev, cudaStream_t s);
+int kmat_grad_slab_finish(int np, int64_t jlo, int64_t jhi, const double* tile_part, double* g_dev, cudaStream_t s);
 int kmat_symmetric_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x, int64_t n,
                                const double* diag_add, double* out, int64_t ld, cudaStream_t s);
 int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
@@ -1052,21 +1052,27 @@ static bool rows_ordered(const bgp_hodlr* h) {
 // eye_row0 >= 0 restricts the solve by rows: the caller guarantees that columns [c0, c0 + 64) of b are zero outside rows
 // [eye_row0 + c0, eye_row0 + c0 + 64) (identity columns e_j, j = eye_row0 + column: grad_terms' K^-1 slabs).  Every step
 // of the solve is block diagonal and maps zero rows to zero rows, so only the leaves and, per level, the nodes that meet
-// those rows run; the result is bit for bit the unrestricted one.  Single-GPU factorisations only (part 0).
+// those rows run; the result is bit for bit the unrestricted one.  Part 0 only.
+// On a shard the caller also guarantees that b is zero outside the shard's rows [row0, row0 + nloc), so the identity
+// rows are clamped to them: the other shards' sub-tree solves of such columns are zero.  The owned leaves and levels then
+// run through the local panel set, the levels above the cut through the top panels (all N rows, identical on every shard
+// after finish_top), and no rows are exchanged: a restricted solve issues no collective, so shards that run different
+// numbers of slabs cannot block each other.
 static int hodlr_solve_dev(bgp_hodlr* h, double* b, int64_t nrhs, int64_t ldb, cudaStream_t s, int part,
                            int64_t eye_row0) {
   const int nlev = (int)h->levels.size();
   const int cut = h->opts.shard_count > 1 ? h->cut_depth : 0;
   const bool native_x = part == 0 && h->opts.shard_count > 1 && !host_exchange(h);
-  if (eye_row0 >= 0 && (part != 0 || h->opts.shard_count > 1)) {
-    set_error("internal: a row-restricted solve needs a single-GPU factorisation");
+  if (eye_row0 >= 0 && part != 0) {
+    set_error("internal: a row-restricted solve runs every part of the solve");
     return BGP_ERR_INVALID;
   }
   for (int64_t c0 = 0; c0 < nrhs; c0 += 64) {
     const int nc = (int)std::min<int64_t>(64, nrhs - c0);
     double* X = b + c0 * ldb;
     if (eye_row0 >= 0) {
-      const int64_t lo = eye_row0 + c0, hi = lo + nc;
+      const int64_t lo = std::max(eye_row0 + c0, h->row0), hi = std::min(eye_row0 + c0 + nc, h->row0 + h->nloc);
+      if (lo >= hi) continue;  // no identity row of this handle's: the group stays zero
       int l0, l1;
       rows_meeting((int)h->leaves.size(), [&](int k, int* st, int* sz) {
         const HNode& nd = h->nodes[h->leaves[k]]; *st = nd.start; *sz = nd.size; }, lo, hi, &l0, &l1);
@@ -1284,10 +1290,11 @@ int bgp_hodlr_get_inverse(bgp_hodlr_t* h, double* out) {
   return bgp_hodlr_apply_inverse(h, out, n, n);  // COLUMN-major K^-1 (symmetric only to tol: the host transposes)
 }
 
-// E_J: columns j0 .. j0 + nc of the identity, n rows (the slab W is zeroed before)
-__global__ void eye_slab_kernel(double* __restrict__ W, int64_t n, int64_t j0, int64_t nc) {
+// E_J: columns j0 .. j0 + nc of the identity, n rows, where j0 + k lies in [jlo, jhi); the other columns stay zero (the
+// slab W is zeroed before)
+__global__ void eye_slab_kernel(double* __restrict__ W, int64_t n, int64_t j0, int64_t nc, int64_t jlo, int64_t jhi) {
   for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nc; k += (int64_t)gridDim.x * blockDim.x)
-    W[k * n + j0 + k] = 1.0;
+    if (j0 + k >= jlo && j0 + k < jhi) W[k * n + j0 + k] = 1.0;
 }
 
 // K^-1 resident (n x n) up to this many doubles (n <= 65536); larger n streams it in column slabs
@@ -1313,23 +1320,75 @@ static float event_ms(cudaEvent_t a, cudaEvent_t b) {
   return ms;
 }
 
+// The streamed gradient over this handle's own columns J = [row0, row0 + nloc) ([0, n) unsharded, a shard's rows):
+//     dg_p = sum_{i, j in J} (alpha_i alpha_j - K^-1_ij) dK_ij/dtheta_p,   ddiag_j = alpha_j^2 - K^-1_jj (j in J only).
+// Slabs of c columns start at the global multiple of 64 at or below row0; the identity is placed in J only, each slab is
+// solved with the row-restricted solve and contracted over the window J, and the per-tile partials of the tiles meeting
+// J are summed in order.  alpha: the full n-vector K^-1 r; d_which holds which[0 .. np).  Issues no collective.
+static int grad_stream_own_columns(bgp_hodlr* h, int np, const double* alpha, int64_t c, double* dg, double* ddiag,
+                                   double* t_solve, double* t_contract) {
+  cudaStream_t s = h->sA;
+  const int64_t n = h->n, jlo = h->row0, jhi = h->row0 + h->nloc;
+  const bool prof = h->profile;
+  // slab W (n x c), then the per-tile partials and one slab's per-split partials in d_gscratch
+  const int64_t tsize = grad_slab_tile_size(n, np), psize = grad_slab_partial_size(n, c, np);
+  BGP_TRY(h->d_inv.reserve((size_t)n * c, s));
+  BGP_TRY(h->d_gscratch.reserve((size_t)(tsize + psize), s));
+  double* W = h->d_inv.p;
+  double* tile_part = h->d_gscratch.p;
+  double* partial = h->d_gscratch.p + tsize;
+  int64_t slabs = 0;
+  for (int64_t j0 = jlo / 64 * 64; j0 < jhi; j0 += c, ++slabs) {
+    const int64_t nc = std::min(c, jhi - j0);
+    if (prof) BGP_CUDA(cudaEventRecord(h->ev[4], s));
+    BGP_CUDA(cudaMemsetAsync(W, 0, sizeof(double) * n * nc, s));
+    eye_slab_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, n, j0, nc, jlo, jhi);
+    BGP_LAUNCH_CHECK();
+    BGP_TRY(hodlr_solve_dev(h, W, nc, n, s, 0, j0));
+    if (prof) BGP_CUDA(cudaEventRecord(h->ev[5], s));
+    BGP_TRY(kmat_grad_slab_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, W, j0, nc, jlo, jhi, alpha,
+                                  partial, tile_part, ddiag, s));
+    if (prof) {
+      BGP_CUDA(cudaEventRecord(h->ev[7], s));
+      BGP_CUDA(cudaEventSynchronize(h->ev[7]));
+      *t_solve += event_ms(h->ev[4], h->ev[5]);
+      *t_contract += event_ms(h->ev[5], h->ev[7]);
+    }
+  }
+  if (prof) BGP_CUDA(cudaEventRecord(h->ev[4], s));
+  BGP_TRY(kmat_grad_slab_finish(np, jlo, jhi, tile_part, dg, s));
+  if (prof) {
+    BGP_CUDA(cudaEventRecord(h->ev[5], s));
+    BGP_CUDA(cudaEventSynchronize(h->ev[5]));
+    *t_contract += event_ms(h->ev[4], h->ev[5]);
+  }
+  h->grad_t[2] = (double)slabs;
+  h->grad_t[3] = (double)c;
+  return BGP_OK;
+}
+
 // alpha = K^-1 r, g_p = sum_ij (alpha alpha^T - K^-1)_ij dK_ij/dtheta_p, diag(alpha alpha^T - K^-1): everything
 // GP.grad_log_likelihood (gp.py:406-468) needs from the solver, with K^-1 (solve against the identity, _hodlr.cpp:193-199)
 // and the gradient contraction staying on the device.
 // Two regimes (include/bgp.h): up to n = 65536 K^-1 is formed whole and contracted by kmat_grad_contract_kernel; above,
 // or with BGP_GRAD_CHUNK set, it is streamed in column slabs W = K^-1 E_J, each solved with the row-restricted solve
 // and contracted by kmat_grad_slab_kernel, so K^-1 is never resident.
+// On a shard with a matching communicator the call is collective and always streamed, composed of the existing pieces:
+// alpha by the collective solve, grad_stream_own_columns on this shard's columns, an all-reduce of g and an all-gather
+// of the diag slices.  Every rank issues the same collectives in the same order; none sits inside the slab loop.
 int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
                          double* diag_out) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
-  if (h->opts.shard_count > 1) { set_error("grad_terms is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  if (host_exchange(h)) { set_error("grad_terms is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
   const int64_t n = h->n;
   const int np = h->prog.n_params_total;
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  const bool sharded = h->opts.shard_count > 1;
+  if (sharded && !rows_ordered(h)) { set_error("internal: HODLR rows are not ordered by level"); return BGP_ERR_CUDA; }
   cudaStream_t s = h->sA;
   bool forced = false;
   const int64_t c = grad_slab_cols(n, &forced);
-  const bool resident = !forced && n * n <= GRAD_RESIDENT_MAX;
+  const bool resident = !sharded && !forced && n * n <= GRAD_RESIDENT_MAX;
   const bool prof = h->profile;
   double t_solve = 0, t_contract = 0;
   for (double& t : h->grad_t) t = 0;
@@ -1359,46 +1418,42 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
       t_contract += event_ms(h->ev[5], h->ev[7]);
     }
   } else {
-    // streamed: slab W (n x c), then the per-tile partials and one slab's per-split partials in d_gscratch
     if (!rows_ordered(h)) { set_error("internal: HODLR rows are not ordered by level"); return BGP_ERR_CUDA; }
-    const int64_t tsize = grad_slab_tile_size(n, np), psize = grad_slab_partial_size(n, c, np);
-    BGP_TRY(h->d_inv.reserve((size_t)n * c, s));
-    BGP_TRY(h->d_gscratch.reserve((size_t)(tsize + psize), s));
     BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
     if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
-    double* W = h->d_inv.p;
-    double* tile_part = h->d_gscratch.p;
-    double* partial = h->d_gscratch.p + tsize;
-    int64_t slabs = 0;
-    for (int64_t j0 = 0; j0 < n; j0 += c, ++slabs) {
-      const int64_t nc = std::min(c, n - j0);
-      if (prof) BGP_CUDA(cudaEventRecord(h->ev[4], s));
-      BGP_CUDA(cudaMemsetAsync(W, 0, sizeof(double) * n * nc, s));
-      eye_slab_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, n, j0, nc);
-      BGP_LAUNCH_CHECK();
-      BGP_TRY(hodlr_solve_dev(h, W, nc, n, s, 0, j0));
-      if (prof) BGP_CUDA(cudaEventRecord(h->ev[5], s));
-      BGP_TRY(kmat_grad_slab_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, W, j0, nc, alpha, partial,
-                                    tile_part, diag_out ? ddiag : nullptr, s));
-      if (prof) {
-        BGP_CUDA(cudaEventRecord(h->ev[7], s));
-        BGP_CUDA(cudaEventSynchronize(h->ev[7]));
-        t_solve += event_ms(h->ev[4], h->ev[5]);
-        t_contract += event_ms(h->ev[5], h->ev[7]);
-      }
+    BGP_TRY(grad_stream_own_columns(h, np, alpha, c, dg, diag_out ? ddiag : nullptr, &t_solve, &t_contract));
+    if (sharded) {  // every shard's partial g, and its rows of diag to every shard
+      if (np) BGP_TRY(comm_allreduce_sum_f64(dg, (size_t)np, s));
+      if (diag_out) BGP_TRY(exchange_rows(h, ddiag, n, 1, s));
     }
-    if (prof) BGP_CUDA(cudaEventRecord(h->ev[4], s));
-    BGP_TRY(kmat_grad_slab_finish(np, n, tile_part, dg, s));
-    if (prof) {
-      BGP_CUDA(cudaEventRecord(h->ev[5], s));
-      BGP_CUDA(cudaEventSynchronize(h->ev[5]));
-      t_contract += event_ms(h->ev[4], h->ev[5]);
-    }
-    h->grad_t[2] = (double)slabs;
-    h->grad_t[3] = (double)c;
   }
   if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
   if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  h->grad_t[0] = t_solve;
+  h->grad_t[1] = t_contract;
+  return BGP_OK;
+}
+
+// One shard's part of the streamed gradient (include/bgp.h): grad_stream_own_columns with the caller's alpha and diag.
+int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const double* alpha_dev, double* g_part_out,
+                                   double* diag_dev) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  const int np = h->prog.n_params_total;
+  if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  if (!alpha_dev) { set_error("grad_terms_local: alpha_dev is null"); return BGP_ERR_INVALID; }
+  if (!rows_ordered(h)) { set_error("internal: HODLR rows are not ordered by level"); return BGP_ERR_CUDA; }
+  cudaStream_t s = h->sA;
+  bool forced = false;
+  const int64_t c = grad_slab_cols(h->n, &forced);
+  double t_solve = 0, t_contract = 0;
+  for (double& t : h->grad_t) t = 0;
+  BGP_TRY(h->d_rhs.reserve(64, s));
+  double* dg = h->d_rhs.p;
+  BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
+  if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
+  BGP_TRY(grad_stream_own_columns(h, np, alpha_dev, c, dg, diag_dev, &t_solve, &t_contract));
+  if (np && g_part_out) BGP_CUDA(cudaMemcpyAsync(g_part_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));
   h->grad_t[0] = t_solve;
   h->grad_t[1] = t_contract;

@@ -384,6 +384,11 @@ int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const uns
 // in order into the tile's slot of a (ceil(n / 32) x P) array, and grad_contract_reduce_kernel sums the tiles in order
 // once every slab is done.  The split plan and the tile boundaries depend only on n (slabs start at multiples of 64),
 // so g does not depend on the slab width, and no atomics: two identical calls return the same bits.
+// A column window [jlo, jhi) restricts the sum to j in the window (a shard of a sharded factorisation owns the columns
+// of its rows, bgp_hodlr_grad_terms_local_dev): a tile that straddles a window edge contributes only its columns inside
+// it (the others carry weight 0, set where alpha_j is staged, so the inner loop and its registers are those of the
+// unrestricted kernel), the tile boundaries stay global multiples of 32, and the window [0, n) is the unrestricted sum,
+// bit for bit.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int GS_TJ = 32;          // columns per j-tile
 constexpr int GS_THREADS = 256;
@@ -397,8 +402,9 @@ __global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevPro
                                                                     const unsigned* __restrict__ which,
                                                                     const double* __restrict__ x, int64_t n,
                                                                     const double* __restrict__ W, int64_t j0,
-                                                                    int64_t nc, const double* __restrict__ alpha,
-                                                                    int stage_x, double* __restrict__ partial) {
+                                                                    int64_t nc, int64_t jlo, int64_t jhi,
+                                                                    const double* __restrict__ alpha, int stage_x,
+                                                                    double* __restrict__ partial) {
   extern __shared__ double sxj[];  // GS_TJ x nd coordinates of the tile's columns (stage_x)
   __shared__ DevProgram P;
   __shared__ unsigned sw[BGP_MAX_LEAVES * (4 + BGP_MAX_METRIC)];
@@ -410,7 +416,12 @@ __global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevPro
   const int64_t r0 = (int64_t)blockIdx.y * GS_ROWS, r1 = min(n, r0 + GS_ROWS);
   stage_program(&P, gprog);
   for (int q = threadIdx.x; q < np; q += blockDim.x) sw[q] = which[q];
-  if (threadIdx.x < nj) saj[threadIdx.x] = alpha[jt + threadIdx.x];
+  // a column outside the window gets weight 0 (alpha_j staged as 0, and its W column is zero: the identity is placed in
+  // the window only), so it adds exactly nothing, and the loop below carries no window bounds
+  if (threadIdx.x < nj) {
+    const int64_t j = jt + threadIdx.x;
+    saj[threadIdx.x] = (j >= jlo && j < jhi) ? alpha[j] : 0.0;
+  }
   if (stage_x)
     for (int t = threadIdx.x; t < nj * nd; t += GS_THREADS) sxj[t] = x[jt * nd + t];
   __syncthreads();
@@ -451,13 +462,13 @@ __global__ void grad_slab_reduce_kernel(const double* __restrict__ partial, int6
   }
 }
 
-// diag[j] = alpha_j^2 - W_jj for j in [j0, j0 + nc): the square and the difference rounded separately (no contraction
-// into an FMA), as alpha**2 - diag(K^-1) is on the host
-__global__ void grad_slab_diag_kernel(const double* __restrict__ W, int64_t n, int64_t j0, int64_t nc,
-                                      const double* __restrict__ alpha, double* __restrict__ diag) {
+// diag[j] = alpha_j^2 - W_jj for j in [j0, j0 + nc) inside the window [jlo, jhi) (no other entry is written): the
+// square and the difference rounded separately (no contraction into an FMA), as alpha**2 - diag(K^-1) is on the host
+__global__ void grad_slab_diag_kernel(const double* __restrict__ W, int64_t n, int64_t j0, int64_t nc, int64_t jlo,
+                                      int64_t jhi, const double* __restrict__ alpha, double* __restrict__ diag) {
   for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nc; k += (int64_t)gridDim.x * blockDim.x) {
     const int64_t j = j0 + k;
-    diag[j] = __dsub_rn(__dmul_rn(alpha[j], alpha[j]), W[k * n + j]);
+    if (j >= jlo && j < jhi) diag[j] = __dsub_rn(__dmul_rn(alpha[j], alpha[j]), W[k * n + j]);
   }
 }
 
@@ -468,11 +479,12 @@ int64_t grad_slab_partial_size(int64_t n, int64_t c, int np) {
 // doubles of per-tile partials (all slabs) for an n-row K^-1
 int64_t grad_slab_tile_size(int64_t n, int np) { return ((n + GS_TJ - 1) / GS_TJ) * std::max(np, 1); }
 
-// One slab (j0 a multiple of 32): its tiles' partials into tile_part + (j0 / 32) * np, and diag[j0 .. j0 + nc) when
-// diag_dev is set.  partial: grad_slab_partial_size(n, nc, np) doubles.
+// One slab (j0 a multiple of 32) restricted to the columns [jlo, jhi): its tiles' partials into
+// tile_part + (j0 / 32) * np, and diag[j] for j in [j0, j0 + nc) and in the window when diag_dev is set.
+// partial: grad_slab_partial_size(n, nc, np) doubles.
 int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigned* which_dev, const double* x, int64_t n,
-                          const double* W, int64_t j0, int64_t nc, const double* alpha, double* partial,
-                          double* tile_part, double* diag_dev, cudaStream_t s) {
+                          const double* W, int64_t j0, int64_t nc, int64_t jlo, int64_t jhi, const double* alpha,
+                          double* partial, double* tile_part, double* diag_dev, cudaStream_t s) {
   if (nc <= 0) return BGP_OK;
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
   if (j0 % GS_TJ) { set_error("internal: slab start %lld is not a multiple of %d", (long long)j0, GS_TJ); return BGP_ERR_INVALID; }
@@ -484,9 +496,11 @@ int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigne
     const size_t smem = stage_x ? sbytes : 0;
     const dim3 grid((unsigned)ntile, (unsigned)nsplit);
     if (np <= 8)
-      kmat_grad_slab_kernel<8><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, alpha, stage_x, partial);
+      kmat_grad_slab_kernel<8><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, jlo, jhi, alpha,
+                                                               stage_x, partial);
     else
-      kmat_grad_slab_kernel<64><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, alpha, stage_x, partial);
+      kmat_grad_slab_kernel<64><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, jlo, jhi, alpha,
+                                                                stage_x, partial);
     BGP_LAUNCH_CHECK();
     const int64_t total = ntile * np;
     grad_slab_reduce_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 8 * (int64_t)num_sms()), 256, 0, s>>>(
@@ -494,16 +508,19 @@ int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigne
     BGP_LAUNCH_CHECK();
   }
   if (diag_dev) {
-    grad_slab_diag_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, n, j0, nc, alpha, diag_dev);
+    grad_slab_diag_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, n, j0, nc, jlo, jhi,
+                                                                                              alpha, diag_dev);
     BGP_LAUNCH_CHECK();
   }
   return BGP_OK;
 }
 
-// g_dev[q] = sum_t tile_part[t * np + q] over the ceil(n / 32) tiles, in a fixed order
-int kmat_grad_slab_finish(int np, int64_t n, const double* tile_part, double* g_dev, cudaStream_t s) {
+// g_dev[q] = sum_t tile_part[t * np + q] over the tiles that meet the columns [jlo, jhi) (all ceil(n / 32) tiles for
+// [0, n)), in a fixed order that depends only on the window
+int kmat_grad_slab_finish(int np, int64_t jlo, int64_t jhi, const double* tile_part, double* g_dev, cudaStream_t s) {
   if (np <= 0) return BGP_OK;
-  grad_contract_reduce_kernel<<<dim3((unsigned)np, 1), 256, 0, s>>>(tile_part, (n + GS_TJ - 1) / GS_TJ, np, g_dev, 0, 0);
+  const int64_t t0 = jlo / GS_TJ, t1 = (jhi + GS_TJ - 1) / GS_TJ;
+  grad_contract_reduce_kernel<<<dim3((unsigned)np, 1), 256, 0, s>>>(tile_part + t0 * np, t1 - t0, np, g_dev, 0, 0);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }

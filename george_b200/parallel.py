@@ -14,7 +14,9 @@ The reference has no distributed code; what shards is the algorithmic independen
 3. finishes the ``P - 1`` top nodes redundantly (Gram, 2r x 2r LU, log-det, update).
 
 ``log|K|`` is an all-reduce of one double; a solve is: local sub-tree solve on the owned slice, one all-gather of the
-vector, top nodes redundantly.  ``torch.distributed`` is plumbing only: it broadcasts the 128-byte NCCL unique id with
+vector, top nodes redundantly.  The log-likelihood gradient (``grad_terms``) is that solve for alpha, each rank
+streaming K^-1 over the columns of its own rows, an all-reduce of ``g`` and an all-gather of the diagonal.
+``torch.distributed`` is plumbing only: it broadcasts the 128-byte NCCL unique id with
 which every rank initialises the library's communicator (``ensure_device_comm``).  All arithmetic and all data-path
 collectives are in ``csrc/hodlr.cu`` / ``csrc/comm.cu``.
 
@@ -153,6 +155,25 @@ class ShardedHODLRSolver(object):
     def dot_solve(self, y):
         """Collective; ``y`` replicated on every rank."""
         return self.solver.dot_solve(y)
+
+    def grad_terms(self, r, which):
+        """``(alpha, g, diagA)`` for ``GP.grad_log_likelihood``, as ``BasicSolver.grad_terms`` returns them.
+        Collective; ``r`` replicated on every rank.  Each rank streams K^-1 over the columns of its own rows; the only
+        collectives are the solve for alpha, an all-reduce of ``g`` and an all-gather of the diagonal
+        (``include/bgp.h: bgp_hodlr_grad_terms``).  K^-1 is never formed."""
+        if self.solver is None or not self._computed:
+            raise RuntimeError("you must call 'compute' first")
+        r = np.ascontiguousarray(r, dtype=np.float64)
+        if r.shape != (self._n,):
+            raise ValueError("dimension mismatch")
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        alpha = np.empty(self._n, dtype=np.float64)
+        g = np.zeros(max(which.size, 1), dtype=np.float64)
+        diag = np.empty(self._n, dtype=np.float64)
+        lib = self.solver._lib
+        _lib.check(lib.bgp_hodlr_grad_terms(self.solver._ptr, _lib.ptr(which), _lib.ptr(r), _lib.ptr(alpha),
+                                            _lib.ptr(g), _lib.ptr(diag)))
+        return alpha, g[:which.size], diag
 
     def apply_sqrt(self, r):
         raise NotImplementedError("apply_sqrt is not implemented for the HODLRSolver")

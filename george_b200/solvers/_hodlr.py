@@ -197,6 +197,18 @@ class HODLRSolver(object):
         out["slabs"], out["slab_cols"] = int(out["slabs"]), int(out["slab_cols"])
         return out
 
+    def grad_terms_local(self, alpha_dev, which, diag_dev=None):
+        """This handle's part of the streamed gradient (``include/bgp.h: bgp_hodlr_grad_terms_local_dev``): the partial
+        ``g`` (``(len(which),)``) over the columns of its own rows, from ``alpha_dev``, a device pointer to the full
+        ``K^-1 r``.  ``diag_dev`` (a device pointer to ``n`` doubles, or ``None``) receives ``alpha_j^2 - K^-1_jj`` for
+        those rows only.  Issues no collective."""
+        self._require_computed()
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        g = np.zeros(max(which.size, 1), dtype=np.float64)
+        _lib.check(self._lib.bgp_hodlr_grad_terms_local_dev(self._ptr, _lib.ptr(which), alpha_dev, _lib.ptr(g),
+                                                            diag_dev))
+        return g[:which.size]
+
     def set_profiling(self, on=True):
         _lib.check(self._lib.bgp_hodlr_set_profiling(self._ptr, 1 if on else 0))
 

@@ -376,10 +376,32 @@ int bgp_hodlr_get_inverse(bgp_hodlr_t* h, double* out);
  *     never resident.  Device workspace (doubles): n c + ceil(n / 32) P + ceil(n / 1024) (c / 32) P, plus 2 n + 64.
  *     The sum order depends only on n: g does not depend on c, and two identical calls return the same bits.
  * BGP_GRAD_CHUNK=<c> (environment, read at every call; rounded up to a multiple of 64) forces the streamed path at any n
- * with c-column slabs, a diagnostic switch like BGP_PREDICT_CHUNK.  Errors: BGP_ERR_NOT_COMPUTED before compute,
- * BGP_ERR_INVALID on a sharded factorisation and for more than 64 kernel parameters (before anything is solved). */
+ * with c-column slabs, a diagnostic switch like BGP_PREDICT_CHUNK.
+ * On a sharded factorisation with a matching communicator (see the multi-GPU block below) the call is COLLECTIVE, with r
+ * replicated, and always streamed: alpha by the collective solve, each shard's slabs of its own columns
+ * (bgp_hodlr_grad_terms_local_dev), one all-reduce of the P doubles of g and one all-gather of the diag slices; every
+ * rank returns the whole alpha, g and diag.  diag_out must be NULL on every rank or on none (it decides whether the
+ * diag all-gather is issued); alpha_out and g_out only affect this rank's copies.  Errors: BGP_ERR_NOT_COMPUTED before
+ * compute, BGP_ERR_INVALID for more than 64 kernel parameters (before anything is solved or exchanged) and on a
+ * host-exchange shard, which computes its part with bgp_hodlr_grad_terms_local_dev instead. */
 int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
                          double* diag_out);
+/* One shard's part of the streamed gradient: with J = this handle's own rows [row0, row0 + rows) ([0, n) unsharded),
+ *   g_part_out[p] = sum_{i in [0, n), j in J} (alpha_i alpha_j - K^-1_ij) dK_ij/dtheta_p   (host, P doubles; 0 where
+ *                   which[p] = 0),
+ *   diag_dev[j]   = alpha_j^2 - K^-1_jj for j in J only (device, n rows; no other row is written; may be NULL),
+ * from alpha_dev, the full replicated n-vector K^-1 r on the device (on a host-exchange shard: solve_local_dev, the host's
+ * all-gather, solve_top_dev).  K^-1 E_J is streamed in slabs of the bgp_hodlr_grad_terms width that start at the
+ * multiple of 64 at or below row0, with the identity placed in J only; each slab is solved with the row-restricted solve
+ * (this shard's leaves and owned levels, then the top levels on the top panels) and contracted over J.  Issues no
+ * collective, so shards may call it independently; summing the P shards' g_part_out and assembling their diag slices
+ * gives the gradient.  On an unsharded handle it returns bit for bit what bgp_hodlr_grad_terms returns on the streamed
+ * path with the same slab width.  g does not depend on the slab width, and two identical calls return the same bits.
+ * bgp_hodlr_last_grad_timing reports this call's slabs, slab width and (profiling on) its solve and contraction times.
+ * Errors: BGP_ERR_NOT_COMPUTED before compute and on a shard whose top levels are not finished; BGP_ERR_INVALID for more
+ * than 64 kernel parameters and for a NULL alpha_dev (both before anything is launched). */
+int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const double* alpha_dev, double* g_part_out,
+                                   double* diag_dev);
 /* The HODLR counterpart of bgp_dense_predict (see there for the outputs, workspace and errors). */
 int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
                       double* out);
@@ -418,7 +440,7 @@ int bgp_hodlr_last_draw_paths(const bgp_hodlr_t* h, uint64_t* out4);
  * [1] ACA (stream B, from the start of compute), [2] up-sweep (panel finalisation + leaf solves + level sweeps, from the
  * moment both streams have drained), [3] total compute, [4] last solve.  [3] ~ max([0], [1]) + host gap + [2]. */
 int bgp_hodlr_last_timing(const bgp_hodlr_t* h, double* ms5);
-/* The last bgp_hodlr_grad_terms: out4 = [0] ms in the solves (alpha and K^-1), [1] ms in the contraction (with the
+/* The last bgp_hodlr_grad_terms[_local_dev]: out4 = [0] ms in the solves (alpha and K^-1), [1] ms in the contraction (with the
  * diagonal and the reductions), both measured with CUDA events only while profiling is on (bgp_hodlr_set_profiling;
  * every K^-1 slab then waits for its events) and 0 otherwise, [2] number of K^-1 slabs, [3] columns per slab ([2] and
  * [3] are 0 on the resident path). */
@@ -467,7 +489,9 @@ int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n
  *      [row0_s, row0_s + rows_s) from shard s and copies the assembled block to every shard, then
  *      bgp_hodlr_solve_top_dev on every shard; every shard then holds the whole solution.
  * The full solves (bgp_hodlr_apply_inverse, bgp_hodlr_dot_solve[_dev], bgp_hodlr_get_inverse), like grad_terms,
- * predict and node_factors, return BGP_ERR_INVALID on a host-exchange shard: they need the other shards' rows.
+ * predict and node_factors, return BGP_ERR_INVALID on a host-exchange shard: they need the other shards' rows.  The
+ * gradient runs there as bgp_hodlr_grad_terms_local_dev on every shard with the solved alpha, the host summing g and
+ * assembling the diag slices; with a matching communicator bgp_hodlr_grad_terms does all of it collectively.
  * bgp_hodlr_log_determinant on a host-exchange shard returns that shard's PARTIAL log-determinant: its own leaves and
  * sub-tree nodes, plus the nodes above the cut on shard 0 only, so the sum over the P shards is log det K.
  *   bgp_hodlr_top_panel(h, &ptr_dev, &row0, &rows, &cols, &ld): device pointer to the (N x cols) column-major panel of
@@ -503,6 +527,8 @@ int bgp_hodlr_solve_top_dev(bgp_hodlr_t* h, double* b_dev, int64_t nrhs, int64_t
  * ------------------------------------------------------------------------------------------ */
 int bgp_dev_alloc(void** ptr_dev, size_t bytes);
 int bgp_dev_free(void* ptr_dev);
+/* bgp_dev_upload returns once the data is on the device (also from pageable host memory), so any library call made
+ * after it, on whichever of the library's streams, reads the uploaded bytes. */
 int bgp_dev_upload(void* dst_dev, const void* src_host, size_t bytes);
 int bgp_dev_download(void* dst_host, const void* src_dev, size_t bytes);
 int bgp_dev_synchronize(void);

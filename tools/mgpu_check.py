@@ -1,6 +1,8 @@
 # -*- coding: utf-8 -*-
 """Multi-GPU parity probe (run under torchrun): sharded HODLR (sub-tree per rank + one all-gather) must reproduce the
-single-GPU factorisation — same per-node RNG streams, so log-det / solve agree to rounding."""
+single-GPU factorisation — same per-node RNG streams, so log-det / solve / gradient terms agree to rounding.  The
+gradient leg runs the collective grad_terms (each rank streams K^-1 over its own columns; all-reduce of g, all-gather of
+the diagonal) against the single-GPU grad_terms on rank 0."""
 import os, sys, json
 import numpy as np
 import torch
@@ -29,14 +31,22 @@ for name, kernel, n, ms, exhaust in [
     sh.compute(x[:, None], yerr)
     ld, ds = sh.log_determinant, sh.dot_solve(y)
     a = sh.apply_inverse(y)[:, 0]
+    which = np.ones(len(kernel.get_parameter_vector(include_frozen=True)), dtype=np.uint32)
+    ga, gg, gd = sh.grad_terms(y, which)  # collective
     if rank == 0:
         s = HODLRSolver(); s.compute(kernel, x[:, None], yerr, min_size=ms, tol=1e-10, seed=42, exhaust=exhaust)
         ld1, ds1 = s.log_determinant, s.dot_solve(y)
         a1 = s.apply_inverse(y)[:, 0]
+        ga1, gg1, gd1 = np.empty(n), np.zeros(which.size), np.empty(n)
+        _lib.check(s._lib.bgp_hodlr_grad_terms(s._ptr, _lib.ptr(which), _lib.ptr(y), _lib.ptr(ga1), _lib.ptr(gg1), _lib.ptr(gd1)))
+        g_rel = float(np.max(np.abs(gg - gg1) / np.maximum(1.0, np.abs(gg1))))
+        d_rel = float(np.linalg.norm(gd - gd1) / np.linalg.norm(gd1))
         good = abs(ld - ld1) <= 1e-10 * abs(ld1) and abs(ds - ds1) <= 1e-9 * abs(ds1) and np.linalg.norm(a - a1) <= 1e-9 * np.linalg.norm(a1)
+        good = good and g_rel <= 1e-9 and d_rel <= 1e-9 and np.linalg.norm(ga - ga1) <= 1e-9 * np.linalg.norm(ga1)
         ok = ok and good
         print(json.dumps({"case": name, "world": world, "logdet_sharded": ld, "logdet_single": ld1, "dot_sharded": ds, "dot_single": ds1,
-                          "solve_relerr": float(np.linalg.norm(a - a1) / np.linalg.norm(a1)), "ok": bool(good)}))
+                          "solve_relerr": float(np.linalg.norm(a - a1) / np.linalg.norm(a1)), "grad_relerr": g_rel,
+                          "grad_diag_relerr": d_rel, "ok": bool(good)}))
 dist.barrier()
 if rank == 0:
     print("MGPU_CHECK", "PASS" if ok else "FAIL")
