@@ -105,6 +105,9 @@ __device__ __forceinline__ double warp_max(double v) {
 __device__ __forceinline__ void argmax_combine(double& v, int& i, double ov, int oi) {
   if (ov > v || (ov == v && oi < i)) { v = ov; i = oi; }
 }
+// arg-max key of the ACA pivot searches (every route and the oracle): |v| with a NaN counted as +inf, so that the first
+// NaN (or infinity) in column order wins and a NaN row still has a pivot column (DESIGN.md §2)
+__device__ __forceinline__ double aca_pivot_key(double v) { return (v != v) ? __longlong_as_double(0x7ff0000000000000ll) : fabs(v); }
 __device__ __forceinline__ void warp_argmax(double& v, int& i) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {

@@ -232,15 +232,16 @@ __device__ __forceinline__ int a2_next_writer(const A2NodeSmem& S, int pos, int 
   return best;
 }
 
-// upper bound of |k| at distance >= gap for the program's shape (+inf when the program has no decreasing bound)
-__device__ __forceinline__ double program_bound(const DevProgram* g, double gap) {
+// upper bound of |k| at a distance in [gap, far] for the program's shape (+inf when the program has no decreasing bound;
+// NaN when a pair in that range may evaluate to NaN)
+__device__ __forceinline__ double program_bound(const DevProgram* g, double gap, double far) {
   switch (g->shape) {
-    case BGP_SHAPE_EXPSQ: return ScaledProfile1D<BGP_SHAPE_EXPSQ>(*g).bound(gap);
-    case BGP_SHAPE_M32: return ScaledProfile1D<BGP_SHAPE_M32>(*g).bound(gap);
-    case BGP_SHAPE_M52: return ScaledProfile1D<BGP_SHAPE_M52>(*g).bound(gap);
-    case BGP_SHAPE_EXP: return ScaledProfile1D<BGP_SHAPE_EXP>(*g).bound(gap);
-    case BGP_SHAPE_PROD_EXPSQ_ES2: return ScaledProfile1D<BGP_SHAPE_PROD_EXPSQ_ES2>(*g).bound(gap);
-    case BGP_SHAPE_PROD_M32_ES2: return ScaledProfile1D<BGP_SHAPE_PROD_M32_ES2>(*g).bound(gap);
+    case BGP_SHAPE_EXPSQ: return ScaledProfile1D<BGP_SHAPE_EXPSQ>(*g).bound(gap, far);
+    case BGP_SHAPE_M32: return ScaledProfile1D<BGP_SHAPE_M32>(*g).bound(gap, far);
+    case BGP_SHAPE_M52: return ScaledProfile1D<BGP_SHAPE_M52>(*g).bound(gap, far);
+    case BGP_SHAPE_EXP: return ScaledProfile1D<BGP_SHAPE_EXP>(*g).bound(gap, far);
+    case BGP_SHAPE_PROD_EXPSQ_ES2: return ScaledProfile1D<BGP_SHAPE_PROD_EXPSQ_ES2>(*g).bound(gap, far);
+    case BGP_SHAPE_PROD_M32_ES2: return ScaledProfile1D<BGP_SHAPE_PROD_M32_ES2>(*g).bound(gap, far);
     default: return __longlong_as_double(0x7ff0000000000000ll);
   }
 }
@@ -402,7 +403,8 @@ __device__ inline void a2_generate(const A2Args& a, A2State& st, A2NodeSmem& S, 
       for (int j = 0; j < G; ++j) {
         const int c = c0 + j * blockDim.x;
         if (c < B) {
-          const double bb = b[j] + program_bound(a.prog, fmax(0.0, fmax(clo - xi[j], xi[j] - chi)));
+          // (a NaN box, one NaN column, makes far NaN; a non-finite x_i makes it NaN or inf: the bound keeps the row)
+          const double bb = b[j] + program_bound(a.prog, fmax(0.0, fmax(clo - xi[j], xi[j] - chi)), fmax(xi[j] - clo, chi - xi[j]));
           if (!(bb * 1.000001 < 1e-14)) {  // NaN keeps the candidate
             live[atomicAdd(&S.n_live, 1)] = c;
             a.cand_xu[nd.cand_off + c] = make_double2(xi[j], b[j]);
@@ -468,9 +470,11 @@ __global__ void __launch_bounds__(A2_NODE_THREADS) a2_init_kernel(A2Args a) {
   // bounding interval of the node's columns (candidate-level bound culling; 1-D programs with a distance bound only)
   if (a.vmax) {
     double lo = __longlong_as_double(0x7ff0000000000000ll), hi = -lo;
-    for (int n = threadIdx.x; n < nd.n_cols; n += blockDim.x) { const double xv = a.x[nd.col0 + n]; lo = fmin(lo, xv); hi = fmax(hi, xv); }
+    bool has_nan = false;  // fmin / fmax drop NaN: a NaN column is carried as a NaN box, which culls nothing
+    for (int n = threadIdx.x; n < nd.n_cols; n += blockDim.x) { const double xv = a.x[nd.col0 + n]; lo = fmin(lo, xv); hi = fmax(hi, xv); has_nan |= (xv != xv); }
     lo = -block_max_signed(-lo, S.red);
     hi = block_max_signed(hi, S.red);
+    if (__syncthreads_or(has_nan)) lo = hi = __longlong_as_double(0x7ff8000000000000ll);
     if (threadIdx.x == 0) { a.node_box[2 * nid] = lo; a.node_box[2 * nid + 1] = hi; }
     __syncthreads();
   }
@@ -515,13 +519,16 @@ __device__ __forceinline__ void a2_eval_body(const A2Args& a, const A2Node& nd, 
   double vg = 0.0;
   if constexpr (CULL) if (cull) {
     glo = __longlong_as_double(0x7ff0000000000000ll); ghi = -glo;
+    bool gnan = false;
 #pragma unroll
-    for (int e = 0; e < A2_EPT; ++e) { const double xv = xc[ncol[e]]; glo = fmin(glo, xv); ghi = fmax(ghi, xv); }
+    for (int e = 0; e < A2_EPT; ++e) { const double xv = xc[ncol[e]]; glo = fmin(glo, xv); ghi = fmax(ghi, xv); gnan |= (xv != xv); }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       glo = fmin(glo, __shfl_xor_sync(0xffffffffu, glo, o));
       ghi = fmax(ghi, __shfl_xor_sync(0xffffffffu, ghi, o));
     }
+    // fmin / fmax drop NaN: a group with a NaN column gets a NaN range, whose bound is NaN and keeps every candidate
+    if (__any_sync(0xffffffffu, gnan)) glo = ghi = __longlong_as_double(0x7ff8000000000000ll);
     vmaxg = a.vmax + ((int64_t)chunk * A2_NGROUP + warp);
     vg = __ldcg(vmaxg);
   }
@@ -537,7 +544,7 @@ __device__ __forceinline__ void a2_eval_body(const A2Args& a, const A2Node& nd, 
       if (valid) {
         const double2 xu = __ldcg(a.cand_xu + nd.cand_off + myc);  // (x_i, sum_q |U(i, q)|) from a2_generate
         const double gap = fmax(0.0, fmax(glo - xu.x, xu.x - ghi));
-        const double b = fn.bound(gap) + xu.y * vg;
+        const double b = fn.bound(gap, fmax(xu.x - glo, ghi - xu.x)) + xu.y * vg;
         keep = !(b * 1.000001 < 1e-14);  // NaN keeps the candidate
       }
       live = __ballot_sync(0xffffffffu, keep);
@@ -780,6 +787,13 @@ __device__ __forceinline__ double a2_resid_entry(const KFn& fn, const double* xa
 
 // ---- vrow: residual of the winning row over one column sub-chunk, stored UN-normalised in panel column `rank`, plus
 //      the sub-chunk's arg-max (hodlr.h:186-189).  Same evaluator as a2_eval (one shape, one arithmetic).
+// (value v, column i) beats the running (bv, bi): larger aca_pivot_key, lowest column on ties, so a reduction in any
+// order names the first NaN (or the first maximum) of the row
+__device__ __forceinline__ bool a2_pivot_better(double v, int i, double bv, int bi) {
+  const double k = aca_pivot_key(v), bk = aca_pivot_key(bv);
+  return bi == 0x7fffffff || k > bk || (k == bk && i < bi);
+}
+
 template <int SHAPE>
 __global__ void __launch_bounds__(A2_THREADS) a2_vrow_kernel(A2Args a) {
   __shared__ DevProgram P;
@@ -813,8 +827,7 @@ __global__ void __launch_bounds__(A2_THREADS) a2_vrow_kernel(A2Args a) {
   int bidx = 0x7fffffff;
   if (act) {
     Vcols[(int64_t)rank * nd.ld + nd.col0 + c_lo + n] = val;
-    best = fabs(val); bidx = c_lo + n; bval = val;
-    if (val != val) best = __longlong_as_double(0x7ff0000000000000ll);  // a NaN wins the arg-max (it ends the reference's loop)
+    best = aca_pivot_key(val); bidx = c_lo + n; bval = val;  // a NaN wins the arg-max (it ends the reference's loop)
   }
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
@@ -831,7 +844,7 @@ __global__ void __launch_bounds__(A2_THREADS) a2_vrow_kernel(A2Args a) {
       const double ov = s_red[w];
       const int oi = s_redi[w];
       if (oi == 0x7fffffff) continue;
-      if (bidx == 0x7fffffff || fabs(ov) > fabs(bval) || (fabs(ov) == fabs(bval) && oi < bidx) || (ov != ov && !(bval != bval))) { bval = ov; bidx = oi; }
+      if (a2_pivot_better(ov, oi, bval, bidx)) { bval = ov; bidx = oi; }
     }
     A2EPart p;
     p.val = bval; p.idx = bidx; p._pad = 0;
@@ -852,17 +865,20 @@ __global__ void __launch_bounds__(32) a2_pivot_kernel(A2Args a) {
   for (int ch = lane; ch < nsub; ch += 32) {
     const A2EPart q = a.epart[(int64_t)nd.cchunk0 * A2_NSUB + ch];
     if (q.idx == 0x7fffffff) continue;
-    if (bidx == 0x7fffffff || fabs(q.val) > fabs(bval) || (fabs(q.val) == fabs(bval) && q.idx < bidx) || (q.val != q.val && !(bval != bval))) { bval = q.val; bidx = q.idx; }
+    if (a2_pivot_better(q.val, q.idx, bval, bidx)) { bval = q.val; bidx = q.idx; }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const double ov = __shfl_xor_sync(0xffffffffu, bval, o);
     const int oi = __shfl_xor_sync(0xffffffffu, bidx, o);
     if (oi == 0x7fffffff) continue;
-    if (bidx == 0x7fffffff || fabs(ov) > fabs(bval) || (fabs(ov) == fabs(bval) && oi < bidx) || (ov != ov && !(bval != bval))) { bval = ov; bidx = oi; }
+    if (a2_pivot_better(ov, oi, bval, bidx)) { bval = ov; bidx = oi; }
   }
   if (lane == 0) {
     st.piv_j = bidx; st.pivot = bval;
+    // a non-finite pivot (always accepted) leaves NaN in the normalised row, so |V| <= 1 no longer bounds the factors'
+    // term of a2_generate's cull; a NaN box keeps every later candidate of the node
+    if (a.vmax && !(fabs(bval) <= DBL_MAX)) a.node_box[2 * nid] = a.node_box[2 * nid + 1] = __longlong_as_double(0x7ff8000000000000ll);
     if (st.deferred && fabs(bval) < 1e-14) st.phase = A2_LATE_REJECT;  // hodlr.h:191 (a NaN pivot leaves the loop: accepted)
   }
 }

@@ -487,7 +487,7 @@ __global__ void __launch_bounds__(ACA_THREADS) aca_kernel(const DevProgram* __re
         }
         for (; k < rank; ++k) val -= rowbuf[k] * vk[(int64_t)k * ld];
         vnew[n] = val;
-        const double a = fabs(val);
+        const double a = aca_pivot_key(val);  // a NaN counts as +inf: an all-NaN row still names a column
         if (a > best) { best = a; bidx = n; }
       }
       block_argmax(best, bidx, S->red, S->redi);

@@ -8,6 +8,8 @@
 // constants and differs from the CPU path by the <=2 ulp of CUDA's exp/sin/cos/pow.
 #pragma once
 
+#include <cfloat>
+
 #include "common.cuh"
 #include "user_kernels.cuh"  // generated from kernels/*.yml (tools/generate_kernels.py)
 
@@ -257,17 +259,18 @@ __host__ __device__ constexpr bool shape_has_bound(int shape) { return shape != 
 
 // radial profile f(r2) of the specialised evaluators.  exp(-t) rounds to exactly 0 in double for t > 745.14: far-apart
 // pairs (the bulk of every large off-diagonal block) skip the software exp/sqrt; the branch is warp-uniform because a
-// warp sweeps 32 neighbouring points.  Same expressions, same order, as leaf_value_1d / radial_value.
+// warp sweeps 32 neighbouring points.  Same expressions, same order, as leaf_value_1d / radial_value.  At r2 = +inf
+// the Matern forms are (1 + inf) * exp(-inf) = NaN there, so their cutoffs stop at DBL_MAX; EXPSQ and EXP give 0.
 template <int PROFILE>
 __device__ __forceinline__ double profile_value(double r2) {
   if (PROFILE == BGP_SHAPE_EXPSQ) return (r2 > 1490.4) ? 0.0 : exp(-0.5 * r2);
   if (PROFILE == BGP_SHAPE_M32) {
-    if (r2 > 185200.0) return 0.0;  // sqrt(3 r2) > 745.3
+    if (r2 > 185200.0 && r2 <= DBL_MAX) return 0.0;  // sqrt(3 r2) > 745.3
     const double r = sqrt(3.0 * r2);
     return (1.0 + r) * exp(-r);
   }
   if (PROFILE == BGP_SHAPE_M52) {
-    if (r2 > 111100.0) return 0.0;  // sqrt(5 r2) > 745.3
+    if (r2 > 111100.0 && r2 <= DBL_MAX) return 0.0;  // sqrt(5 r2) > 745.3
     const double r = sqrt(5.0 * r2);
     return (1 + r + 5.0 * r2 / 3.0) * exp(-r);
   }
@@ -293,9 +296,12 @@ struct ScaledProfile1D {
     if (shape_is_sum(SHAPE)) return __dadd_rn(a, __dmul_rn(c2, e));
     return __dmul_rn(a, e);
   }
-  // upper bound of |k(x1, x2)| over all pairs at distance >= gap (monotone profiles; the periodic factor is <= 1).
-  // Only meaningful when shape_has_bound(SHAPE).
-  __device__ __forceinline__ double bound(double gap) const {
+  // upper bound of |k(x1, x2)| over all pairs at a distance in [gap, far] (monotone profiles; the periodic factor is
+  // <= 1).  NaN, which keeps every candidate, when some such pair may evaluate to NaN: far not finite (a non-finite
+  // coordinate), or r2 / the periodic phase overflowing to inf at distance far.  Only meaningful when shape_has_bound(SHAPE).
+  __device__ __forceinline__ double bound(double gap, double far) const {
+    if (!(far * far * m <= DBL_MAX) || (shape_is_prod(SHAPE) && !(fabs(far * w) <= DBL_MAX)))
+      return __longlong_as_double(0x7ff8000000000000ll);
     double b = fabs(c) * profile_value<shape_profile(SHAPE)>(gap * gap * m);
     if (shape_is_prod(SHAPE) && g < 0.0) b *= exp(-g);  // exp(-Gamma sin^2) <= 1 only for Gamma >= 0
     return b;

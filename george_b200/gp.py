@@ -19,6 +19,7 @@ from . import _lib, kernels
 from ._spec import flatten, num_params, patch_specs
 from .modeling import ConstantModel, ModelSet
 from .solvers import BasicSolver, TrivialSolver
+from .solvers.basic import NONFINITE_RHS
 from .utils import multivariate_gaussian_samples
 
 __all__ = ["GP"]
@@ -363,6 +364,10 @@ class GP(ModelSet):
                 except Exception as exc:
                     mean_err[b] = exc
                     resid[b] = 0.0
+        for b in range(nb):  # the per-vector solve rejects a non-finite right-hand side (BasicSolver, as scipy does)
+            if mean_err[b] is None and not np.all(np.isfinite(resid[b])):
+                mean_err[b] = ValueError(NONFINITE_RHS)
+                resid[b] = 0.0
         return spec, full, kpar, sigma, resid, fact_err, mean_err
 
     @staticmethod

@@ -15,6 +15,15 @@ import numpy as np
 from .. import _lib
 from .._spec import DimensionMismatch, flatten, num_params
 
+NONFINITE_RHS = "array must not contain infs or NaNs"
+
+
+def _check_finite(b):
+    """The right-hand side check of scipy's ``cho_solve`` (``check_finite=True``), which the reference's solves go
+    through: a NaN or infinite entry raises ``ValueError`` instead of returning a NaN solve."""
+    if not np.all(np.isfinite(b)):
+        raise ValueError(NONFINITE_RHS)
+
 __all__ = ["BasicSolver"]
 
 
@@ -122,6 +131,7 @@ class BasicSolver(object):
             b = np.array(y, dtype=np.float64, order="F")
         if b.shape[0] != self._n:
             raise ValueError("dimension mismatch")
+        _check_finite(b)
         nrhs = 1 if b.ndim == 1 else int(np.prod(b.shape[1:]))
         _lib.check(self._handle.lib.bgp_dense_apply_inverse(self._handle.ptr, _lib.ptr(b), nrhs, self._n))
         if in_place and b is not y:
@@ -135,6 +145,7 @@ class BasicSolver(object):
         y = np.ascontiguousarray(y, dtype=np.float64)
         if y.shape != (self._n,):
             raise ValueError("dimension mismatch")
+        _check_finite(y)
         out = C.c_double()
         _lib.check(self._handle.lib.bgp_dense_dot_solve(self._handle.ptr, _lib.ptr(y), C.byref(out)))
         return out.value
@@ -168,6 +179,7 @@ class BasicSolver(object):
         r = np.ascontiguousarray(r, dtype=np.float64)
         if r.shape != (self._n,):
             raise ValueError("dimension mismatch")
+        _check_finite(r)
         which = np.ascontiguousarray(which, dtype=np.uint32)
         alpha = np.empty(self._n, dtype=np.float64)
         g = np.zeros(max(which.size, 1), dtype=np.float64)

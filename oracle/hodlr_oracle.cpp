@@ -223,9 +223,14 @@ static int low_rank_approx(Solver* S, Node* nd, int start_row, int n_rows, int s
 
       for (int n = 0; n < n_cols; ++n) v[n] = S->K(start_row + i, start_col + n);
       for (int q = 0; q < rank; ++q) { const double uiq = U[q][i]; const double* vq = V[q].data(); for (int n = 0; n < n_cols; ++n) v[n] -= uiq * vq[n]; }
+      // first max, as Eigen's maxCoeff, with a NaN counted as +inf (NOT the reference, DESIGN.md §2: Eigen only lets a
+      // NaN at column 0 win): the first NaN wins and an all-NaN row pivots on column 0 instead of a stale j
       double best = -1.0;
-      for (int n = 0; n < n_cols; ++n) if (std::abs(v[n]) > best) { best = std::abs(v[n]); j = n; }  // first max, as Eigen's maxCoeff
-    } while (std::abs(v[j]) < 1e-14);
+      for (int n = 0; n < n_cols; ++n) {
+        const double a = std::isnan(v[n]) ? HUGE_VAL : std::abs(v[n]);
+        if (a > best) { best = a; j = n; }
+      }
+    } while (std::abs(v[j]) < 1e-14);  // a NaN pivot is accepted
 
     const double pivot = v[j];
     for (int n = 0; n < n_cols; ++n) v[n] /= pivot;
