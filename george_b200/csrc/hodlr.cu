@@ -132,7 +132,7 @@ struct bgp_hodlr {
   DevBuf<A2EPart> d_epart;
   DevBuf<int> d_cand, d_cand_k, d_cand_words, d_cand_L, d_cand_next, d_cand_live, d_cchunk_node, d_rchunk_node, d_nactive;
   DevBuf<double> d_node_box;
-  DevBuf<double2> d_cand_xu;
+  DevBuf<double2> d_cand_xu, d_gbox, d_cbox;
   DevBuf<unsigned long long> d_cmax, d_stats;
   DevBuf<int4> d_work;
   DevBuf<int> d_work_count, d_iter;
@@ -144,6 +144,7 @@ struct bgp_hodlr {
   std::vector<cudaEvent_t> prof_events;
   double prof[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};  // see bgp_hodlr_last_aca_profile
   uint64_t draw_paths[4] = {0, 0, 0, 0};  // see bgp_hodlr_last_draw_paths
+  uint64_t eval_units[2] = {0, 0};  // see bgp_hodlr_last_eval_units
   DevBuf<double> d_vpart, d_upart, d_vmax;
   int aca_iters = 0;
   size_t w_cap = 0;
@@ -430,6 +431,8 @@ static int run_aca2(bgp_hodlr* h, const std::vector<AcaDesc>& descs, std::vector
   if (cull) {
     BGP_TRY(h->d_vmax.reserve((size_t)ncc * A2_NGROUP, s));
     BGP_TRY(h->d_cand_xu.reserve((size_t)cand_total, s));
+    BGP_TRY(h->d_gbox.reserve((size_t)ncc * A2_NGROUP, s));
+    BGP_TRY(h->d_cbox.reserve((size_t)ncc, s));
   }
   BGP_TRY(h->d_nactive.reserve(2, s));
   int n_top = 0;
@@ -461,6 +464,8 @@ static int run_aca2(bgp_hodlr* h, const std::vector<AcaDesc>& descs, std::vector
   a.cchunk_node = h->d_cchunk_node.p; a.rchunk_node = h->d_rchunk_node.p; a.vpart = h->d_vpart.p; a.upart = h->d_upart.p;
   a.vmax = cull ? h->d_vmax.p : nullptr;
   a.cand_xu = cull ? h->d_cand_xu.p : nullptr;
+  a.gbox = cull ? h->d_gbox.p : nullptr;
+  a.cbox = cull ? h->d_cbox.p : nullptr;
   a.cand_L = h->d_cand_L.p; a.cand_next = h->d_cand_next.p; a.cand_live = h->d_cand_live.p; a.node_box = h->d_node_box.p;
   a.capmax = capmax; a.n_active = h->d_nactive.p; a.stats = h->d_stats.p;
   a.work = h->d_work.p; a.work_count = h->d_work_count.p; a.work_cursor = h->d_work_count.p + 2; a.work_cap = (int)work_cap; a.iter_ptr = h->d_iter.p;
@@ -571,6 +576,7 @@ static int run_aca2(bgp_hodlr* h, const std::vector<AcaDesc>& descs, std::vector
     BGP_CUDA(cudaMemcpyAsync(st4, h->d_stats.p, sizeof(st4), cudaMemcpyDeviceToHost, s));
     BGP_CUDA(cudaStreamSynchronize(s));
     for (int k = 0; k < 4; ++k) h->draw_paths[k] = st4[A2_PATH_REDO + k];
+    h->eval_units[0] = st4[A2_UNITS_PULLED]; h->eval_units[1] = st4[A2_UNITS_LIVE];
     h->prof[1] = iters; h->prof[2] = (double)st4[0]; h->prof[3] = (double)st4[1]; h->prof[4] = (double)st4[2];
     h->prof[5] = (double)st4[3];
     if (h->profile) {
@@ -607,6 +613,7 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
   h->computed = false;
   h->top_pending = false;
   for (uint64_t& c : h->draw_paths) c = 0;  // (rng_mode = reference never runs the speculative draws)
+  for (uint64_t& c : h->eval_units) c = 0;
   h->shard_row0.clear(); h->shard_rows.clear();  // only a sharded compute that cuts the tree reports ranges
   BGP_TRY(require_device());
   BGP_TRY(ensure_streams(h));
@@ -1181,7 +1188,7 @@ void bgp_hodlr_destroy(bgp_hodlr_t* h) {
   h->lu_ws.d_nodes.release(); h->lu_ws.d_trsm.release(); h->lu_ws.d_gemm.release(); h->d_gram_desc.release(); h->d_upd_desc.release();
   h->d_ticket.release(); h->d_chain_done.release(); h->d_ncols_by_depth.release(); h->d_chain_state.release();
   h->d_a2nodes.release(); h->d_a2states.release(); h->d_a2rngs.release(); h->d_epart.release(); h->d_cand.release(); h->d_cand_k.release();
-  h->d_cand_words.release(); h->d_cand_L.release(); h->d_cand_next.release(); h->d_cand_live.release(); h->d_node_box.release(); h->d_cand_xu.release(); h->d_cchunk_node.release(); h->d_rchunk_node.release(); h->d_nactive.release();
+  h->d_cand_words.release(); h->d_cand_L.release(); h->d_cand_next.release(); h->d_cand_live.release(); h->d_node_box.release(); h->d_cand_xu.release(); h->d_gbox.release(); h->d_cbox.release(); h->d_cchunk_node.release(); h->d_rchunk_node.release(); h->d_nactive.release();
   h->d_inv.release(); h->d_gscratch.release(); h->d_which.release(); h->d_xsend.release(); h->d_xrecv.release();
   h->d_vpart.release(); h->d_upart.release(); h->d_vmax.release(); h->d_cmax.release(); h->d_stats.release(); h->d_work.release(); h->d_work_count.release();
   for (cudaEvent_t e : h->prof_events) cudaEventDestroy(e);
@@ -1573,6 +1580,13 @@ int bgp_hodlr_last_draw_paths(const bgp_hodlr_t* h, uint64_t* out4) {
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
   if (!h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
   for (int i = 0; i < 4; ++i) out4[i] = h->draw_paths[i];
+  return BGP_OK;
+}
+
+int bgp_hodlr_last_eval_units(const bgp_hodlr_t* h, uint64_t* out2) {
+  if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  if (!h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  for (int i = 0; i < 2; ++i) out2[i] = h->eval_units[i];
   return BGP_OK;
 }
 

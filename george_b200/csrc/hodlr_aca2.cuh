@@ -39,6 +39,8 @@ static_assert(A2_NSUB * A2_THREADS == A2_CHUNK, "sub-chunks tile a chunk");
 constexpr int A2_HASH = 16384;    // open-addressing slots of the swap-pop multimap (>= 2 * A2_BMAX)
 static_assert(A2_BMAX <= 65536, "multimap values are 16-bit draw numbers");
 constexpr int A2_XWORDS = 64;     // room for the extra words consumed by Lemire rejections inside one batch
+constexpr int A2_PUB_BLOCKS = A2_BMAX / (A2_CG * A2_ITEM_CB);  // most candidate blocks a batch publishes per chunk
+static_assert(256 / A2_CG <= A2_PUB_BLOCKS, "blocks of A2_CG candidates (batches of up to 256 live ones) fit too");
 
 struct A2Node {  // static description
   int row0, n_rows, col0, n_cols;
@@ -169,6 +171,8 @@ struct A2Args {
   double* vmax;    // per (column chunk, 128-column group): max over the factors q and the group's columns j of |V(j, q)|
                    // [chunk * 8 + g]  (bound culling of a2_eval; nullptr when the program has no distance bound)
   double2* cand_xu;  // per candidate: (coordinate of its row, sum_q |U(row, q)|), written by a2_generate for a2_eval
+  double2* gbox;     // per (column chunk, 128-column group): (min, max) coordinate of its columns [chunk * 8 + g], and
+  double2* cbox;     // per column chunk; both written once per compute by a2_init_kernel (NaN: the range has a NaN column)
   int capmax;
   int* n_active;
   int4* work;          // eval work items (chunk, first candidate, #candidates, node), two buffers of work_cap
@@ -180,6 +184,7 @@ struct A2Args {
   unsigned long long* stats;  // [0] candidate-row entries verified (pairs), [1] residual-update FMAs executed, [2] candidates,
                               // [3] entries actually evaluated by a2_eval (the rest were bounded < 1e-14 without evaluation)
                               // [4..7] rare paths of the speculative draws, see A2_PATH_* (bgp_hodlr_last_draw_paths)
+                              // [8..9] eval work units pulled / live (A2_UNITS_*)
 };
 // stats slots counting how often a2_generate / a2_decide left the common path
 enum {
@@ -187,7 +192,9 @@ enum {
   A2_PATH_TRUNCATED = 5,   // batches cut short before a rejecting draw whose next words were not generated yet
   A2_PATH_SEQUENTIAL = 6,  // rejecting draws at position 0 of such a batch, drawn alone by mt_uniform
   A2_PATH_PARTIAL = 7,     // commits that replayed the stream to the winning draw instead of copying the end-of-batch state
-  A2_NSTATS = 8
+  A2_UNITS_PULLED = 8,     // a2_eval work units (item, 128-column group) pulled from the cursor (bgp_hodlr_last_eval_units)
+  A2_UNITS_LIVE = 9,       // ... of which at least one candidate survived the group bound and was evaluated
+  A2_NSTATS = 10
 };
 
 // shared-memory workspace of the per-node kernels (dynamic shared memory)
@@ -205,6 +212,7 @@ struct A2NodeSmem {
   int n_live;
   int extra;
 };
+static_assert(sizeof(int) * A2_HASH >= sizeof(double) * (3 * A2_PUB_BLOCKS + 1), "a2_generate's per-block ranges fit in hkey");
 
 __device__ __forceinline__ unsigned a2_hash(int pos) { return ((unsigned)pos * 2654435761u) & (A2_HASH - 1); }
 // most recent draw before `c` that wrote position `pos` (-1: none)
@@ -244,6 +252,29 @@ __device__ __forceinline__ double program_bound(const DevProgram* g, double gap,
     case BGP_SHAPE_PROD_M32_ES2: return ScaledProfile1D<BGP_SHAPE_PROD_M32_ES2>(*g).bound(gap, far);
     default: return __longlong_as_double(0x7ff0000000000000ll);
   }
+}
+
+// exclusive prefix sum of `v` over the CTA in thread order, and the CTA's total.  Every thread calls it; s_warp holds
+// blockDim.x / 32 ints.
+__device__ __forceinline__ int a2_block_scan(int v, int* s_warp, int& total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  int inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  __syncthreads();  // s_warp may still be read by the previous call
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  int before = 0;
+  total = 0;
+  for (int w = 0; w < nw; ++w) {
+    const int t = s_warp[w];
+    before += (w < warp) ? t : 0;
+    total += t;
+  }
+  return before + inc - v;
 }
 
 // Draw the next min(B, bmax, n_index) candidate rows speculatively: k_c = uniform(0, n_index-1-c) from `S.rng`
@@ -383,11 +414,14 @@ __device__ inline void a2_generate(const A2Args& a, A2State& st, A2NodeSmem& S, 
     const double* Ucol = nd.vbase + nd.row0;
     const double* xr = a.x + nd.row0;
     constexpr int G = 4;  // candidates per trip: their (dependent, uncoalesced) loads are issued together
-    for (int c0 = threadIdx.x; c0 < B; c0 += G * blockDim.x) {
+    // (every thread runs every trip: the live list is compacted in a fixed order by a block scan, so that the candidate
+    //  blocks below, hence the published items, are the same from run to run)
+    for (int t0 = 0; t0 < B; t0 += G * blockDim.x) {
+      const int c0 = t0 + threadIdx.x;
       int row[G];
       double xi[G], b[G];
 #pragma unroll
-      for (int j = 0; j < G; ++j) { const int c = c0 + j * blockDim.x; row[j] = cand[(c < B) ? c : c0]; }  // written above by this thread
+      for (int j = 0; j < G; ++j) { const int c = c0 + j * blockDim.x; row[j] = (c < B) ? cand[c] : 0; }  // written above by this thread
 #pragma unroll
       for (int j = 0; j < G; ++j) xi[j] = xr[row[j]];
 #pragma unroll
@@ -399,18 +433,29 @@ __device__ inline void a2_generate(const A2Args& a, A2State& st, A2NodeSmem& S, 
 #pragma unroll
         for (int j = 0; j < G; ++j) b[j] += fabs(u[j]);
       }
+      unsigned keep = 0u;
 #pragma unroll
       for (int j = 0; j < G; ++j) {
         const int c = c0 + j * blockDim.x;
         if (c < B) {
           // (a NaN box, one NaN column, makes far NaN; a non-finite x_i makes it NaN or inf: the bound keeps the row)
           const double bb = b[j] + program_bound(a.prog, fmax(0.0, fmax(clo - xi[j], xi[j] - chi)), fmax(xi[j] - clo, chi - xi[j]));
-          if (!(bb * 1.000001 < 1e-14)) {  // NaN keeps the candidate
-            live[atomicAdd(&S.n_live, 1)] = c;
-            a.cand_xu[nd.cand_off + c] = make_double2(xi[j], b[j]);
-          }
+          if (!(bb * 1.000001 < 1e-14)) keep |= 1u << j;  // NaN keeps the candidate
         }
       }
+      const int base = S.n_live;
+      int total;
+      int pos = base + a2_block_scan(__popc(keep), S.redi, total);
+#pragma unroll
+      for (int j = 0; j < G; ++j) {
+        if (keep & (1u << j)) {
+          const int c = c0 + j * blockDim.x;
+          live[pos++] = c;
+          a.cand_xu[nd.cand_off + c] = make_double2(xi[j], b[j]);
+        }
+      }
+      if (threadIdx.x == 0) S.n_live = base + total;
+      __syncthreads();
     }
   }
   __syncthreads();
@@ -429,18 +474,90 @@ __device__ inline void a2_generate(const A2Args& a, A2State& st, A2NodeSmem& S, 
     if (split) my_chunks = (nd.n_cchunks - a.shard_rank + a.shard_count - 1) / a.shard_count;
     const int n_items = my_chunks * per_chunk;
     int4* work_next = a.work + (int64_t)nb * a.work_cap;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      S.flag = n_items ? atomicAdd(a.work_count + nb, n_items) : 0;
-      if (S.flag + n_items > a.work_cap) st.status = 2;  // cannot happen (the host sizes the list for the worst case): fail loudly
-    }
-    __syncthreads();
-    const int base = S.flag;
-    for (int t = threadIdx.x; t < n_items; t += blockDim.x) {
+    auto item = [&](int t) {
       const int ci = t / per_chunk, pi = t % per_chunk;
       const int lc = split ? (a.shard_rank + ci * a.shard_count) : ci;
       const int c0 = pi * ipc;
-      if (base + t < a.work_cap) work_next[base + t] = make_int4(nd.cchunk0 + lc, c0, min(ipc, n_live - c0), nid);
+      return make_int4(nd.cchunk0 + lc, c0, min(ipc, n_live - c0), nid);
+    };
+    __syncthreads();
+    if (!cull) {
+      if (threadIdx.x == 0) {
+        S.flag = n_items ? atomicAdd(a.work_count + nb, n_items) : 0;
+        if (S.flag + n_items > a.work_cap) st.status = 2;  // cannot happen (the host sizes the list for the worst case): fail loudly
+      }
+      __syncthreads();
+      const int base = S.flag;
+      for (int t = threadIdx.x; t < n_items; t += blockDim.x)
+        if (base + t < a.work_cap) work_next[base + t] = item(t);
+    } else {
+      // Chunk-level culling: an item whose whole chunk is bounded below the threshold for all of its candidates holds no
+      // unit that a2_eval would evaluate, so it is not published.  Per candidate block: the range of its coordinates and
+      // the largest sum_q |U(i, q)|; per chunk: its static range (a2_init_kernel) and the largest vmax of its groups.
+      // Every (candidate, group) pair of the item has a gap >= the (block, chunk) gap, a far end <= the block's, a U sum
+      // <= the block's and a vmax <= the chunk's, so this bound is >= the one a2_eval tests each pair with (vmax is
+      // final here: vnorm wrote it earlier in the iteration and nothing writes it before the next eval).  The margin is
+      // ten times a2_eval's, for the rounding the compiler may choose differently in the two kernels: an item survives
+      // whenever a unit of it could.  NaN anywhere keeps the item.
+      // The per-block ranges go to the multimap's slots (dead once the candidates are resolved).
+      double* s_blo = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(S.hkey) + 7) & ~uintptr_t(7));
+      double* s_bhi = s_blo + A2_PUB_BLOCKS;
+      double* s_bu = s_bhi + A2_PUB_BLOCKS;
+      for (int p0 = 0; p0 < per_chunk * ipc; p0 += blockDim.x) {  // ipc consecutive lanes hold one block (ipc divides 32)
+        const int p = p0 + threadIdx.x;
+        double lo = __longlong_as_double(0x7ff0000000000000ll), hi = -lo, u = 0.0;
+        bool bnan = false;
+        if (p < n_live) {
+          const double2 xu = a.cand_xu[nd.cand_off + live[p]];  // written above by this CTA
+          lo = hi = xu.x; u = xu.y;
+          bnan = (xu.x != xu.x) || (xu.y != xu.y);
+        }
+        for (int o = 1; o < ipc; o <<= 1) {
+          lo = fmin(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+          hi = fmax(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+          u = fmax(u, __shfl_xor_sync(0xffffffffu, u, o));
+          bnan |= __shfl_xor_sync(0xffffffffu, (int)bnan, o) != 0;
+        }
+        if (bnan) lo = hi = u = __longlong_as_double(0x7ff8000000000000ll);
+        if (p % ipc == 0 && p < n_live) { s_blo[p / ipc] = lo; s_bhi[p / ipc] = hi; s_bu[p / ipc] = u; }
+      }
+      __syncthreads();
+      constexpr int R = 32;  // items tested per thread and round (one bit each)
+      for (int r0 = 0; r0 < n_items; r0 += R * blockDim.x) {
+        unsigned keep = 0u;
+        for (int k = 0; k < R; ++k) {
+          const int t = r0 + k * blockDim.x + threadIdx.x;
+          if (t >= n_items) break;
+          const int4 w = item(t);
+          const int lc = w.x - nd.cchunk0, pi = w.y / ipc;
+          const double2 cb = __ldcg(a.cbox + w.x);
+          double vm = 0.0;
+          bool vnan = false;
+          for (int g = 0; g < A2_NGROUP && lc * A2_CHUNK + g * A2_GROUP < nd.n_cols; ++g) {
+            const double v = __ldcg(a.vmax + ((int64_t)w.x * A2_NGROUP + g));
+            vm = fmax(vm, v); vnan |= (v != v);
+          }
+          if (vnan) vm = __longlong_as_double(0x7ff8000000000000ll);
+          const double lo = s_blo[pi], hi = s_bhi[pi];
+          const double bb = program_bound(a.prog, fmax(0.0, fmax(cb.x - hi, lo - cb.y)), fmax(hi - cb.x, cb.y - lo)) + s_bu[pi] * vm;
+          if (!(bb * 1.00001 < 1e-14)) keep |= 1u << k;  // NaN keeps the item
+        }
+        int total;
+        const int off = a2_block_scan(__popc(keep), S.redi, total);
+        if (threadIdx.x == 0) {
+          S.flag = total ? atomicAdd(a.work_count + nb, total) : 0;
+          if (S.flag + total > a.work_cap) st.status = 2;  // cannot happen (the host sizes the list for the worst case): fail loudly
+        }
+        __syncthreads();
+        int q = S.flag + off;
+        for (int k = 0; k < R; ++k) {
+          if (keep & (1u << k)) {
+            if (q < a.work_cap) work_next[q] = item(r0 + k * blockDim.x + threadIdx.x);
+            ++q;
+          }
+        }
+        __syncthreads();  // (S.flag is rewritten by the next round)
+      }
     }
   }
   __syncthreads();
@@ -476,6 +593,35 @@ __global__ void __launch_bounds__(A2_NODE_THREADS) a2_init_kernel(A2Args a) {
     hi = block_max_signed(hi, S.red);
     if (__syncthreads_or(has_nan)) lo = hi = __longlong_as_double(0x7ff8000000000000ll);
     if (threadIdx.x == 0) { a.node_box[2 * nid] = lo; a.node_box[2 * nid + 1] = hi; }
+    // the same ranges per 128-column group (what a2_eval bounds a warp's columns by) and per column chunk (a2_generate's
+    // test before it publishes an item): the columns never change during a compute, so they are reduced once here
+    const int lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+    for (int g = threadIdx.x >> 5; g < nd.n_cchunks * A2_NGROUP; g += nw) {
+      const int w_lo = g * A2_GROUP;
+      const int w_n = min(A2_GROUP, nd.n_cols - w_lo);
+      if (w_n <= 0) break;  // (warp-uniform) the groups past the node's last column are never evaluated
+      double glo = __longlong_as_double(0x7ff0000000000000ll), ghi = -glo;
+      bool gnan = false;
+      for (int n = lane; n < w_n; n += 32) { const double xv = a.x[nd.col0 + w_lo + n]; glo = fmin(glo, xv); ghi = fmax(ghi, xv); gnan |= (xv != xv); }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        glo = fmin(glo, __shfl_xor_sync(0xffffffffu, glo, o));
+        ghi = fmax(ghi, __shfl_xor_sync(0xffffffffu, ghi, o));
+      }
+      if (__any_sync(0xffffffffu, gnan)) glo = ghi = __longlong_as_double(0x7ff8000000000000ll);
+      if (lane == 0) a.gbox[(int64_t)nd.cchunk0 * A2_NGROUP + g] = make_double2(glo, ghi);
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < nd.n_cchunks; c += blockDim.x) {
+      double clo = __longlong_as_double(0x7ff0000000000000ll), chi = -clo;
+      bool cnan = false;
+      for (int g = 0; g < A2_NGROUP && c * A2_CHUNK + g * A2_GROUP < nd.n_cols; ++g) {
+        const double2 b = a.gbox[(int64_t)(nd.cchunk0 + c) * A2_NGROUP + g];
+        clo = fmin(clo, b.x); chi = fmax(chi, b.y); cnan |= (b.x != b.x);
+      }
+      if (cnan) clo = chi = __longlong_as_double(0x7ff8000000000000ll);
+      a.cbox[nd.cchunk0 + c] = make_double2(clo, chi);
+    }
     __syncthreads();
   }
   a2_generate(a, st, S, nd, nid, 0);
@@ -497,7 +643,7 @@ __global__ void __launch_bounds__(A2_NODE_THREADS) a2_init_kernel(A2Args a) {
 template <class KFn, bool CULL>
 __device__ __forceinline__ void a2_eval_body(const A2Args& a, const A2Node& nd, int rank, int chunk, int c_first,
                                              int c_count, int ndim, KFn fn, int warp, unsigned long long& n_eval,
-                                             unsigned long long& n_fma) {
+                                             unsigned long long& n_fma, unsigned& n_live_units) {
   const int lc = chunk - nd.cchunk0;
   const int lane = threadIdx.x & 31;
   const int w_lo = lc * A2_CHUNK + warp * A2_GROUP;  // first column of this warp
@@ -518,22 +664,15 @@ __device__ __forceinline__ void a2_eval_body(const A2Args& a, const A2Node& nd, 
   const bool cull = CULL && a.vmax != nullptr;  // runtime switch: BGP_NO_CULL runs the exhaustive scan
   double vg = 0.0;
   if constexpr (CULL) if (cull) {
-    glo = __longlong_as_double(0x7ff0000000000000ll); ghi = -glo;
-    bool gnan = false;
-#pragma unroll
-    for (int e = 0; e < A2_EPT; ++e) { const double xv = xc[ncol[e]]; glo = fmin(glo, xv); ghi = fmax(ghi, xv); gnan |= (xv != xv); }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      glo = fmin(glo, __shfl_xor_sync(0xffffffffu, glo, o));
-      ghi = fmax(ghi, __shfl_xor_sync(0xffffffffu, ghi, o));
-    }
-    // fmin / fmax drop NaN: a group with a NaN column gets a NaN range, whose bound is NaN and keeps every candidate
-    if (__any_sync(0xffffffffu, gnan)) glo = ghi = __longlong_as_double(0x7ff8000000000000ll);
+    // the range of this warp's columns (a group with a NaN column has a NaN range, whose bound keeps every candidate)
+    const double2 gb = __ldcg(a.gbox + ((int64_t)chunk * A2_NGROUP + warp));
+    glo = gb.x; ghi = gb.y;
     vmaxg = a.vmax + ((int64_t)chunk * A2_NGROUP + warp);
     vg = __ldcg(vmaxg);
   }
 
   const int ncand = c_first + c_count;
+  bool unit_live = false;
   for (int cb0 = c_first; cb0 < ncand; cb0 += 32) {
     const bool valid = cb0 + lane < ncand;
     const int myc = valid ? live_list[cb0 + lane] : 0;  // index of the candidate in the node's batch
@@ -549,6 +688,7 @@ __device__ __forceinline__ void a2_eval_body(const A2Args& a, const A2Node& nd, 
       }
       live = __ballot_sync(0xffffffffu, keep);
     }
+    unit_live |= (live != 0u);
     n_eval += (unsigned long long)__popc(live) * (unsigned long long)w_n;
     n_fma += (unsigned long long)__popc(live) * (unsigned long long)w_n * (unsigned long long)rank;
     while (live) {
@@ -614,6 +754,7 @@ __device__ __forceinline__ void a2_eval_body(const A2Args& a, const A2Node& nd, 
       }
     }
   }
+  n_live_units += unit_live ? 1u : 0u;
 }
 
 // one instantiation per program shape: the specialised ones carry no interpreter and need far fewer registers
@@ -635,6 +776,7 @@ __global__ void __launch_bounds__(A2_THREADS, MINB) a2_eval_kernel(A2Args a) {
   const auto fn = ShapeEval<SHAPE>::make(&P, a.prog);
   constexpr bool CULL = shape_has_bound(SHAPE);
   unsigned long long n_eval = 0ull, n_fma = 0ull;
+  unsigned n_pulled = 0u, n_live_units = 0u;
   // work unit = (item, 128-column group); every WARP pulls its next unit from a global cursor: items differ wildly in cost
   // (fully culled ... 32 candidate rows to evaluate), a static deal leaves most of the chip idle behind the few heavy ones
   int* cursor = a.work_cursor + buf;
@@ -645,14 +787,19 @@ __global__ void __launch_bounds__(A2_THREADS, MINB) a2_eval_kernel(A2Args a) {
     if ((threadIdx.x & 31) == 0) u = atomicAdd(cursor, 1);
     u = __shfl_sync(0xffffffffu, u, 0);
     if (u >= n_units) break;
+    ++n_pulled;
     const int4 w = items[u / A2_NGROUP];
     const int grp = u % A2_NGROUP;
     const A2Node& nd = a.nodes[w.w];
     const int rank = a.states[w.w].rank;
-    if constexpr (SHAPE == BGP_SHAPE_GENERIC) a2_eval_body<decltype(fn), false>(a, nd, rank, w.x, w.y, w.z, P.ndim, fn, grp, n_eval, n_fma);
-    else a2_eval_body<decltype(fn), CULL>(a, nd, rank, w.x, w.y, w.z, 1, fn, grp, n_eval, n_fma);
+    if constexpr (SHAPE == BGP_SHAPE_GENERIC) a2_eval_body<decltype(fn), false>(a, nd, rank, w.x, w.y, w.z, P.ndim, fn, grp, n_eval, n_fma, n_live_units);
+    else a2_eval_body<decltype(fn), CULL>(a, nd, rank, w.x, w.y, w.z, 1, fn, grp, n_eval, n_fma, n_live_units);
   }
   if ((threadIdx.x & 31) == 0 && n_eval) { atomicAdd(a.stats + 3, n_eval); atomicAdd(a.stats + 1, n_fma); }
+  if ((threadIdx.x & 31) == 0 && n_pulled) {
+    atomicAdd(a.stats + A2_UNITS_PULLED, (unsigned long long)n_pulled);
+    atomicAdd(a.stats + A2_UNITS_LIVE, (unsigned long long)n_live_units);
+  }
 }
 inline void a2_eval_launch(int shape, dim3 grid, cudaStream_t s, const A2Args& a, int minb) {
   if (minb == 3 && shape != BGP_SHAPE_GENERIC) {

@@ -182,6 +182,14 @@ class HODLRSolver(object):
         _lib.check(self._lib.bgp_hodlr_last_draw_paths(self._ptr, c))
         return dict(zip(("lemire_redos", "truncated_batches", "sequential_draws", "partial_commits"), (int(v) for v in c)))
 
+    def eval_units(self):
+        """The last compute's candidate-evaluation work units: ``pulled`` by the evaluation kernel and ``live`` (at
+        least one candidate evaluated) (``include/bgp.h: bgp_hodlr_last_eval_units``)."""
+        self._require_computed()
+        c = (C.c_uint64 * 2)()
+        _lib.check(self._lib.bgp_hodlr_last_eval_units(self._ptr, c))
+        return dict(zip(("pulled", "live"), (int(v) for v in c)))
+
     def timing(self):
         t = (C.c_double * 5)()
         _lib.check(self._lib.bgp_hodlr_last_timing(self._ptr, t))

@@ -436,6 +436,12 @@ int bgp_hodlr_node_factors(const bgp_hodlr_t* h, int64_t node, double* out);
  * stream to the winning draw instead of taking the saved end-of-batch state.  All zero for rng_mode = REFERENCE, which
  * draws one row at a time.  BGP_ERR_NOT_COMPUTED before compute. */
 int bgp_hodlr_last_draw_paths(const bgp_hodlr_t* h, uint64_t* out4);
+/* Diagnostics: the work units of the per-node-stream ACA's candidate evaluation in the last compute
+ * (csrc/hodlr_aca2.cuh, a2_eval_kernel; one unit = one candidate block against 128 columns of the block).
+ * out2 = [0] units pulled by the evaluation kernel, [1] units in which at least one candidate survived the
+ * 128-column bound and was evaluated (all of [0] that have columns when bound culling is off).  Decisions never
+ * depend on these counts.  All zero for rng_mode = REFERENCE.  BGP_ERR_NOT_COMPUTED before compute. */
+int bgp_hodlr_last_eval_units(const bgp_hodlr_t* h, uint64_t* out2);
 /* Device-event timings of the last compute, ms: [0] leaves (build+factor; stream A, CONCURRENT with [1]),
  * [1] ACA (stream B, from the start of compute), [2] up-sweep (panel finalisation + leaf solves + level sweeps, from the
  * moment both streams have drained), [3] total compute, [4] last solve.  [3] ~ max([0], [1]) + host gap + [2]. */
