@@ -67,6 +67,7 @@ SIGNATURES = {
     "bgp_hodlr_grad_terms_local_dev": (C.c_int, [_p, _p, _p, _p, _p]),
     "bgp_dense_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
     "bgp_hodlr_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
+    "bgp_hodlr_predict_local_dev": (C.c_int, [_p, _specp, _p, _i64, _i32, _p, _i64, _i32, _p]),
     "bgp_dense_batch_create": (C.c_int, [C.POINTER(_p)]),
     "bgp_dense_batch_destroy": (None, [_p]),
     "bgp_dense_batch_log_likelihood": (C.c_int, [_p, _specp, _p, _i64, _i64, _p, _i64, _i32, _p, _p, _p, _p, _p]),

@@ -44,15 +44,15 @@ int kmat_matvec_batch_launch(const DevProgram* dprogs, int nd, int members, cons
 int64_t matvec_partial_size(int64_t n1, int64_t n2);
 int64_t predict_chunk_cols(int64_t n, int64_t multiple);
 int64_t predict_var_partial_size(int64_t n, int64_t c);
-int predict_var_batch_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
-                             double* var, int members, int64_t mstride, int64_t vstride, DevBuf<double>& scratch,
-                             cudaStream_t s);
+int predict_var_batch_launch(const double* B, int64_t ldb, const double* W, int64_t ldw, int64_t n, int64_t c,
+                             const double* kdiag, double* var, int members, int64_t mstride, int64_t vstride,
+                             DevBuf<double>& scratch, cudaStream_t s);
 void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, int64_t* klen_out);
 int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn,
                              int64_t K, bool lower, double* C, int64_t ldc, int members, int64_t abstride,
                              int64_t cstride, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
-int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
-                       double* var, DevBuf<double>& scratch, cudaStream_t s);
+int predict_var_launch(const double* B, int64_t ldb, const double* W, int64_t ldw, int64_t n, int64_t c,
+                       const double* kdiag, double* var, DevBuf<double>& scratch, cudaStream_t s);
 int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
                      bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
 
@@ -867,7 +867,7 @@ int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const doubl
       BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p, nc, h->d_x.p, n, dW.p, n, s));  // K(x, x*_chunk), N x nc
       BGP_TRY(dense_trsm_fwd_dev(h, dW.p, nc, n));
       BGP_TRY(kmat_diagonal_launch(dprog.p, dxs.p, dxs.p, nc, dkd.p, s));
-      BGP_TRY(predict_var_launch(dW.p, dW.p, n, n, nc, dkd.p, dvar.p, scratch, s));
+      BGP_TRY(predict_var_launch(dW.p, n, dW.p, n, n, nc, dkd.p, dvar.p, scratch, s));
       BGP_CUDA(cudaMemcpyAsync(out + j0, dvar.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));
     }
   } else {
@@ -1252,7 +1252,7 @@ int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec,
         BGP_TRY(kmat_general_batch_launch_auto(progs, dprogs, mc, xc, nc, h->d_x.p, n, h->d_W.p, ldw, n, h->d_fn, s));
         BGP_TRY(trsm_fwd_members(h->d_A.p, n, nn, h->d_W.p, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
         BGP_TRY(kmat_diagonal_launch(dprogs, xc, xc, nc, h->d_kd.p, s, mc, c));
-        BGP_TRY(predict_var_batch_launch(h->d_W.p, h->d_W.p, ldw, n, nc, h->d_kd.p, h->d_var.p, mc, n, c, h->d_vp, s));
+        BGP_TRY(predict_var_batch_launch(h->d_W.p, ldw, h->d_W.p, ldw, n, nc, h->d_kd.p, h->d_var.p, mc, n, c, h->d_vp, s));
         BGP_CUDA(cudaMemcpy2DAsync(out + c0 * ns + j0, sizeof(double) * ns, h->d_var.p, sizeof(double) * c,
                                    sizeof(double) * nc, mc, cudaMemcpyDeviceToHost, s));
       }

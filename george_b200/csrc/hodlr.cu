@@ -40,8 +40,10 @@ int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const
 int kmat_diagonal_launch(const DevProgram* dprog, const double* x1, const double* x2, int64_t n, double* out,
                          cudaStream_t s, int members = 1, int64_t ostride = 0);
 int64_t predict_chunk_cols(int64_t n, int64_t multiple);
-int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
-                       double* var, DevBuf<double>& scratch, cudaStream_t s);
+int64_t predict_var_partial_size(int64_t n, int64_t c);
+int predict_var_launch(const double* B, int64_t ldb, const double* W, int64_t ldw, int64_t n, int64_t c,
+                       const double* kdiag, double* var, DevBuf<double>& scratch, cudaStream_t s);
+void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, int64_t* klen_out);
 int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
                      bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
 bool comm_ready();
@@ -1467,12 +1469,157 @@ int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const 
   return BGP_OK;
 }
 
+// One handle's part of GP.predict's variance / covariance, over its own rows J = [row0, row0 + nloc) ([0, n) unsharded):
+//   VAR: out_j = (prior ? k(x*_j, x*_j) : 0) - sum_{i in J} B_ij W_ij                (ns)
+//   COV: out   = (prior ? K** : 0) - B[J]^T W[J]          (ns x ns, column-major ld ns: bgp_hodlr_predict's layout)
+// with B = K(x, x*) built for the rows J only and W = K^-1 B read in the rows J only, one test-point chunk of c columns
+// at a time.  The chunks, builds and contractions are bgp_hodlr_predict's, so on an unsharded handle with the prior the
+// result is its bits.  predict_own_prepare validates and reserves without touching the device, so that a collective
+// caller can agree on the outcome before anything runs; predict_own_begin then uploads xs and, for COV, builds the
+// prior and the resident B[J] (nloc x ns); predict_own_chunk contracts one chunk.
+struct PredictOwnRows {
+  DevProgram P;
+  DevBuf<DevProgram> dprog;
+  DevBuf<double> dxs, dB, dkd, dout, scratch;
+  DevBuf<GemmDesc> ddesc;
+  int64_t ns = 0, c = 0;
+  int32_t what = 0;
+  bool prior = false;
+};
+
+static int predict_own_prepare(bgp_hodlr* h, const bgp_kernel_spec_t* spec, int64_t ns, int32_t what, bool prior,
+                               PredictOwnRows* w) {
+  if (what != BGP_PREDICT_VAR && what != BGP_PREDICT_COV) { set_error("invalid prediction kind %d", what); return BGP_ERR_INVALID; }
+  if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
+  BGP_TRY(build_dev_program(spec, &w->P));
+  if (w->P.ndim != h->ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", w->P.ndim, h->ndim); return BGP_ERR_DIM; }
+  w->ns = ns; w->what = what; w->prior = prior;
+  if (ns == 0) return BGP_OK;
+  cudaStream_t s = h->sA;
+  const int64_t nloc = h->nloc;
+  const int64_t c = std::min(ns, predict_chunk_cols(h->n, 64)), tail = ns - (ns - 1) / c * c;
+  w->c = c;
+  BGP_TRY(w->dprog.reserve(1, s));
+  BGP_TRY(w->dxs.reserve((size_t)ns * h->ndim, s));
+  if (what == BGP_PREDICT_VAR) {
+    BGP_TRY(w->dB.reserve((size_t)nloc * c, s));
+    BGP_TRY(w->dkd.reserve((size_t)c, s));
+    BGP_TRY(w->dout.reserve((size_t)ns, s));
+    BGP_TRY(w->scratch.reserve((size_t)std::max(predict_var_partial_size(nloc, c), predict_var_partial_size(nloc, tail)), s));
+  } else {
+    BGP_TRY(w->dB.reserve((size_t)nloc * ns, s));
+    BGP_TRY(w->dout.reserve((size_t)ns * ns, s));
+    int64_t nsplit_c, nsplit_t, klen;  // predict_gemm_sub's split-K slices of a full chunk and of the tail
+    predict_gemm_plan(c, ns, nloc, &nsplit_c, &klen);
+    predict_gemm_plan(tail, ns, nloc, &nsplit_t, &klen);
+    BGP_TRY(w->scratch.reserve((size_t)std::max(nsplit_c * c, nsplit_t * tail) * ns, s));
+    BGP_TRY(w->ddesc.reserve((size_t)std::max(nsplit_c, nsplit_t), s));
+  }
+  return BGP_OK;
+}
+
+static int predict_own_begin(bgp_hodlr* h, PredictOwnRows& w, const double* xs) {
+  cudaStream_t s = h->sA;
+  BGP_TRY(upload_program(w.P, w.dprog, s));
+  BGP_CUDA(cudaMemcpyAsync(w.dxs.p, xs, sizeof(double) * w.ns * h->ndim, cudaMemcpyHostToDevice, s));
+  if (w.what == BGP_PREDICT_VAR) {
+    if (!w.prior) BGP_CUDA(cudaMemsetAsync(w.dkd.p, 0, sizeof(double) * w.c, s));
+    return BGP_OK;
+  }
+  if (w.prior) BGP_TRY(kmat_symmetric_launch_auto(w.P, w.dprog.p, w.dxs.p, w.ns, nullptr, w.dout.p, w.ns, s));
+  else BGP_CUDA(cudaMemsetAsync(w.dout.p, 0, sizeof(double) * w.ns * w.ns, s));
+  return kmat_general_launch_auto(w.P, w.dprog.p, w.dxs.p, w.ns, h->d_x.p + h->row0 * h->ndim, h->nloc, w.dB.p,
+                                  h->nloc, s);
+}
+
+// test points [j0, j0 + nc); Wc: the chunk's first column of W (global row 0), leading dimension ldw
+static int predict_own_chunk(bgp_hodlr* h, PredictOwnRows& w, int64_t j0, int64_t nc, const double* Wc, int64_t ldw) {
+  cudaStream_t s = h->sA;
+  const int64_t nloc = h->nloc;
+  if (w.what == BGP_PREDICT_VAR) {
+    const double* xc = w.dxs.p + j0 * h->ndim;
+    BGP_TRY(kmat_general_launch_auto(w.P, w.dprog.p, xc, nc, h->d_x.p + h->row0 * h->ndim, nloc, w.dB.p, nloc, s));
+    if (w.prior) BGP_TRY(kmat_diagonal_launch(w.dprog.p, xc, xc, nc, w.dkd.p, s));
+    return predict_var_launch(w.dB.p, nloc, Wc + h->row0, ldw, nloc, nc, w.dkd.p, w.dout.p + j0, w.scratch, s);
+  }
+  // rows j0.. of the column-major result are output COLUMNS j of the row-major one, as in bgp_hodlr_predict
+  return predict_gemm_sub(Wc + h->row0, ldw, w.dB.p, nloc, nc, w.ns, nloc, false, w.dout.p + j0, w.ns, w.scratch,
+                          w.ddesc, s);
+}
+
+// bgp_hodlr_predict on a shard with a matching communicator (include/bgp.h): per test-point chunk, this shard's rows of
+// B = K(x, x*) are built into the rows J of an N x c chunk, the collective solve fills the other rows from the other
+// shards and runs the top levels, and predict_own_chunk contracts over J; one all-reduce of the ns (VAR) or ns^2 (COV)
+// partial results ends it.  Every check and reservation comes before the first collective, and an all-reduce of a
+// status value turns a failure on any rank into an error on every rank, so no rank is left waiting in a later one.
+static int hodlr_predict_collective(bgp_hodlr* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
+                                    int32_t what, double* out) {
+  cudaStream_t s = h->sA;
+  const int64_t n = h->n;
+  PredictOwnRows w;
+  DevBuf<double> dW;
+  int st = predict_own_prepare(h, spec, ns, what, h->opts.shard_rank == 0, &w);
+  if (st == BGP_OK && ns == 0) return BGP_OK;  // ns is replicated: every rank returns here
+  if (st == BGP_OK) st = dW.alloc((size_t)n * w.c, s);
+  if (st == BGP_OK) {  // exchange_rows' staging for the solve's 64-column groups
+    int64_t rows_pad = 0;
+    for (int64_t r : h->shard_rows) rows_pad = std::max(rows_pad, r);
+    st = h->d_xsend.reserve((size_t)64 * rows_pad, s);
+    if (st == BGP_OK) st = h->d_xrecv.reserve((size_t)64 * rows_pad * h->opts.shard_count, s);
+  }
+  double failed = st == BGP_OK ? 0.0 : 1.0;
+  BGP_CUDA(cudaMemcpyAsync(h->d_scalar.p, &failed, sizeof(double), cudaMemcpyHostToDevice, s));
+  BGP_TRY(comm_allreduce_sum_f64(h->d_scalar.p, 1, s));
+  BGP_CUDA(cudaMemcpyAsync(&failed, h->d_scalar.p, sizeof(double), cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  if (st != BGP_OK) return st;
+  if (failed != 0.0) {
+    set_error("predict: %d other shard(s) could not validate or reserve their part", (int)failed);
+    return BGP_ERR_NOMEM;
+  }
+  BGP_TRY(predict_own_begin(h, w, xs));
+  const int nd = h->ndim;
+  for (int64_t j0 = 0; j0 < ns; j0 += w.c) {
+    const int64_t nc = std::min(w.c, ns - j0);
+    BGP_TRY(kmat_general_launch_auto(w.P, w.dprog.p, w.dxs.p + j0 * nd, nc, h->d_x.p + h->row0 * nd, h->nloc,
+                                     dW.p + h->row0, n, s));
+    BGP_TRY(hodlr_solve_dev(h, dW.p, nc, n, s, 0));
+    BGP_TRY(predict_own_chunk(h, w, j0, nc, dW.p, n));
+  }
+  const size_t count = (size_t)(what == BGP_PREDICT_VAR ? ns : ns * ns);
+  BGP_TRY(comm_allreduce_sum_f64(w.dout.p, count, s));
+  BGP_CUDA(cudaMemcpyAsync(out, w.dout.p, sizeof(double) * count, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  return BGP_OK;
+}
+
+// One handle's part of the prediction from the caller's solved W (include/bgp.h).  Issues no collective.
+int bgp_hodlr_predict_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
+                                int32_t what, const double* w_dev, int64_t ldw, int32_t add_prior, double* out) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (ns > 0 && !w_dev) { set_error("predict_local: w_dev is null"); return BGP_ERR_INVALID; }
+  if (ldw < h->n) { set_error("predict_local: ldw %lld < n %lld", (long long)ldw, (long long)h->n); return BGP_ERR_INVALID; }
+  PredictOwnRows w;
+  BGP_TRY(predict_own_prepare(h, spec, ns, what, add_prior != 0, &w));
+  if (ns == 0) return BGP_OK;
+  cudaStream_t s = h->sA;
+  BGP_TRY(predict_own_begin(h, w, xs));
+  for (int64_t j0 = 0; j0 < ns; j0 += w.c)
+    BGP_TRY(predict_own_chunk(h, w, j0, std::min(w.c, ns - j0), w_dev + j0 * ldw, ldw));
+  const size_t count = (size_t)(what == BGP_PREDICT_VAR ? ns : ns * ns);
+  BGP_CUDA(cudaMemcpyAsync(out, w.dout.p, sizeof(double) * count, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  return BGP_OK;
+}
+
 // GP.predict's variance / covariance on the stored factorisation.  The test points are streamed in chunks of a multiple
 // of 64 columns, so W = K^-1 B is solved in the same 64-column groups as apply_inverse and matches it bit for bit.
+// On a shard with a matching communicator the call is collective (hodlr_predict_collective).
 int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
                       double* out) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
-  if (h->opts.shard_count > 1) { set_error("predict is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  if (host_exchange(h)) { set_error("predict is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  if (h->opts.shard_count > 1) return hodlr_predict_collective(h, spec, xs, ns, what, out);
   if (what != BGP_PREDICT_VAR && what != BGP_PREDICT_COV) { set_error("invalid prediction kind %d", what); return BGP_ERR_INVALID; }
   if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
   DevProgram P;
@@ -1501,7 +1648,7 @@ int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
       BGP_CUDA(cudaMemcpyAsync(dW.p, dB.p, sizeof(double) * n * nc, cudaMemcpyDeviceToDevice, s));
       BGP_TRY(hodlr_solve_dev(h, dW.p, nc, n, s, 0));
       BGP_TRY(kmat_diagonal_launch(dprog.p, dxs.p, dxs.p, nc, dkd.p, s));
-      BGP_TRY(predict_var_launch(dB.p, dW.p, n, n, nc, dkd.p, dvar.p, scratch, s));
+      BGP_TRY(predict_var_launch(dB.p, n, dW.p, n, n, nc, dkd.p, dvar.p, scratch, s));
       BGP_CUDA(cudaMemcpyAsync(out + j0, dvar.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));
     }
   } else {

@@ -565,10 +565,10 @@ int64_t predict_chunk_cols(int64_t n, int64_t multiple) {
   return (c + multiple - 1) / multiple * multiple;
 }
 
-// partial[j * nsplit + b] = sum over the rows of split b of B[j*ld + i] * W[j*ld + i]; grid (c, nsplit, members):
+// partial[j * nsplit + b] = sum over the rows of split b of B[j*ldb + i] * W[j*ldw + i]; grid (c, nsplit, members):
 // member z reads B and W + z * mstride and writes partial + z * c * nsplit
-__global__ void __launch_bounds__(PV_THREADS) predict_var_partial_kernel(const double* __restrict__ B,
-                                                                         const double* __restrict__ W, int64_t ld,
+__global__ void __launch_bounds__(PV_THREADS) predict_var_partial_kernel(const double* __restrict__ B, int64_t ldb,
+                                                                         const double* __restrict__ W, int64_t ldw,
                                                                          int64_t n, int64_t rows_per_split,
                                                                          double* __restrict__ partial, int64_t mstride) {
   __shared__ double red[32];
@@ -577,8 +577,8 @@ __global__ void __launch_bounds__(PV_THREADS) predict_var_partial_kernel(const d
   partial += (int64_t)blockIdx.z * gridDim.x * gridDim.y;
   const int64_t j = blockIdx.x;
   const int64_t r0 = (int64_t)blockIdx.y * rows_per_split, r1 = min(n, r0 + rows_per_split);
-  const double* b = B + j * ld;
-  const double* w = W + j * ld;
+  const double* b = B + j * ldb;
+  const double* w = W + j * ldw;
   double s = 0.0;
   for (int64_t i = r0 + threadIdx.x; i < r1; i += PV_THREADS) s = fma(b[i], w[i], s);
   s = block_sum(s, red);
@@ -614,28 +614,29 @@ int64_t predict_var_partial_size(int64_t n, int64_t c) {
   return c * nsplit;
 }
 
-// var (c) = kdiag - colsum(B .* W); B, W: n x c column-major, leading dimension ld (B == W for the dense solver).
+// var (c) = kdiag - colsum(B .* W); B, W: n x c column-major, leading dimensions ldb and ldw (B == W for the dense
+// solver; a HODLR shard's B holds its own rows only, W all N).
 // `members` > 1: member b reads B and W + b * mstride and writes var + b * vstride from kdiag + b * vstride, in the
 // same two launches; scratch holds members * predict_var_partial_size(n, c).
-int predict_var_batch_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
-                             double* var, int members, int64_t mstride, int64_t vstride, DevBuf<double>& scratch,
-                             cudaStream_t s) {
+int predict_var_batch_launch(const double* B, int64_t ldb, const double* W, int64_t ldw, int64_t n, int64_t c,
+                             const double* kdiag, double* var, int members, int64_t mstride, int64_t vstride,
+                             DevBuf<double>& scratch, cudaStream_t s) {
   if (c <= 0 || members <= 0) return BGP_OK;
   int64_t nsplit, rows;
   predict_var_plan(n, c, &nsplit, &rows);
   if (c > 0x7fffffffLL || nsplit > 65535 || members > 65535) { set_error("predict: chunk too large for one launch"); return BGP_ERR_INVALID; }
   BGP_TRY(scratch.reserve((size_t)(c * nsplit * members), s));
   predict_var_partial_kernel<<<dim3((unsigned)c, (unsigned)nsplit, (unsigned)members), PV_THREADS, 0, s>>>(
-      B, W, ld, n, rows, scratch.p, mstride);
+      B, ldb, W, ldw, n, rows, scratch.p, mstride);
   BGP_LAUNCH_CHECK();
   predict_var_finish_kernel<<<dim3((unsigned)std::min<int64_t>((c + 255) / 256, 4 * (int64_t)num_sms()), (unsigned)members),
                               256, 0, s>>>(scratch.p, (int)nsplit, kdiag, c, var, vstride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
-int predict_var_launch(const double* B, const double* W, int64_t ld, int64_t n, int64_t c, const double* kdiag,
-                       double* var, DevBuf<double>& scratch, cudaStream_t s) {
-  return predict_var_batch_launch(B, W, ld, n, c, kdiag, var, 1, 0, 0, scratch, s);
+int predict_var_launch(const double* B, int64_t ldb, const double* W, int64_t ldw, int64_t n, int64_t c,
+                       const double* kdiag, double* var, DevBuf<double>& scratch, cudaStream_t s) {
+  return predict_var_batch_launch(B, ldb, W, ldw, n, c, kdiag, var, 1, 0, 0, scratch, s);
 }
 
 // C[j*ldc + i] += sum_s slices[s*m*nn + j*m + i], s ascending; `lower`: only i >= j, mirrored to C[i*ldc + j]

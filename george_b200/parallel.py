@@ -15,7 +15,9 @@ The reference has no distributed code; what shards is the algorithmic independen
 
 ``log|K|`` is an all-reduce of one double; a solve is: local sub-tree solve on the owned slice, one all-gather of the
 vector, top nodes redundantly.  The log-likelihood gradient (``grad_terms``) is that solve for alpha, each rank
-streaming K^-1 over the columns of its own rows, an all-reduce of ``g`` and an all-gather of the diagonal.
+streaming K^-1 over the columns of its own rows, an all-reduce of ``g`` and an all-gather of the diagonal.  The
+predictive variance / covariance (``predictive``) solves K(x, x*) chunk by chunk, each rank building its own rows and
+contracting over them, and ends with one all-reduce of the result.
 ``torch.distributed`` is plumbing only: it broadcasts the 128-byte NCCL unique id with
 which every rank initialises the library's communicator (``ensure_device_comm``).  All arithmetic and all data-path
 collectives are in ``csrc/hodlr.cu`` / ``csrc/comm.cu``.
@@ -29,6 +31,7 @@ import numpy as np
 
 from . import _lib
 from ._spec import flatten
+from .solvers.basic import BasicSolver
 
 __all__ = ["ShardedHODLRSolver", "shard_ranges", "allgather_padded"]
 
@@ -174,6 +177,15 @@ class ShardedHODLRSolver(object):
         _lib.check(lib.bgp_hodlr_grad_terms(self.solver._ptr, _lib.ptr(which), _lib.ptr(r), _lib.ptr(alpha),
                                             _lib.ptr(g), _lib.ptr(diag)))
         return alpha, g[:which.size], diag
+
+    def predictive(self, kernel, xs, what):
+        """``BasicSolver.predictive`` on the sharded factorisation: the variance (``what="var"``, ``(ns,)``) or
+        covariance (``"cov"``, ``(ns, ns)``) of ``GP.predict``.  Collective; ``xs`` replicated on every rank, and every
+        rank returns the same result.  Each rank builds and contracts K(x, x*) over its own rows only; the collectives
+        are the chunks' solves and one all-reduce of the result (``include/bgp.h: bgp_hodlr_predict``)."""
+        if self.solver is None or not self._computed:
+            raise RuntimeError("you must call 'compute' first")
+        return BasicSolver._predictive_call(self.solver._lib.bgp_hodlr_predict, self.solver._ptr, kernel, xs, what)
 
     def apply_sqrt(self, r):
         raise NotImplementedError("apply_sqrt is not implemented for the HODLRSolver")

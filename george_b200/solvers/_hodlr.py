@@ -16,6 +16,7 @@ import numpy as np
 
 from .. import _lib
 from .._spec import HodlrNodeInfo, HodlrOpts, flatten
+from .basic import BasicSolver
 
 RNG_MODES = {"pernode": 0, "reference": 1}
 
@@ -216,6 +217,19 @@ class HODLRSolver(object):
         _lib.check(self._lib.bgp_hodlr_grad_terms_local_dev(self._ptr, _lib.ptr(which), alpha_dev, _lib.ptr(g),
                                                             diag_dev))
         return g[:which.size]
+
+    def predict_local(self, kernel, xs, what, w_dev, ldw, add_prior):
+        """This handle's part of the predictive variance (``what="var"``, ``(ns,)``) or covariance (``"cov"``,
+        ``(ns, ns)``) over its own rows (``include/bgp.h: bgp_hodlr_predict_local_dev``), from ``w_dev``, a device
+        pointer to the full solved ``K^-1 K(x, x*)`` (``n x ns`` column-major, leading dimension ``ldw``).
+        ``add_prior`` adds ``k(x*, x*)``; summing every shard's part, with the prior on one of them, gives the
+        prediction.  Issues no collective."""
+        self._require_computed()
+
+        def call(ptr, spec, xs_p, ns, kind, out):
+            return self._lib.bgp_hodlr_predict_local_dev(ptr, spec, xs_p, ns, kind, w_dev, int(ldw),
+                                                         1 if add_prior else 0, out)
+        return BasicSolver._predictive_call(call, self._ptr, kernel, xs, what)
 
     def set_profiling(self, on=True):
         _lib.check(self._lib.bgp_hodlr_set_profiling(self._ptr, 1 if on else 0))

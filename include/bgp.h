@@ -224,9 +224,8 @@ int bgp_dense_last_timing(const bgp_dense_t* h, double* ms2);
  *   dense VAR  N*c + O(c)                 dense COV  N*ns + split-K slices (ns^2 each, at most max(ns^2, 2^27) in all)
  *   HODLR VAR  2*N*c + O(c)               HODLR COV  N*ns + N*c + split-K slices (c*ns each, at most max(c*ns, 2^27))
  * Errors: BGP_ERR_NOT_COMPUTED before compute and on a dense handle restored by bgp_dense_import_factor (no
- * coordinates); BGP_ERR_DIM when the spec's ndim differs from the handle's; BGP_ERR_INVALID on a sharded HODLR
- * factorisation, an unknown `what` or ns < 0; BGP_ERR_NOMEM when the workspace cannot be allocated.  ns == 0 writes
- * nothing.
+ * coordinates); BGP_ERR_DIM when the spec's ndim differs from the handle's; BGP_ERR_INVALID on a host-exchange HODLR
+ * shard, an unknown `what` or ns < 0; BGP_ERR_NOMEM when the workspace cannot be allocated.  ns == 0 writes nothing.
  * ------------------------------------------------------------------------------------------ */
 enum { BGP_PREDICT_VAR = 0, BGP_PREDICT_COV = 1 };
 int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
@@ -402,9 +401,34 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
  * than 64 kernel parameters and for a NULL alpha_dev (both before anything is launched). */
 int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const double* alpha_dev, double* g_part_out,
                                    double* diag_dev);
-/* The HODLR counterpart of bgp_dense_predict (see there for the outputs, workspace and errors). */
+/* The HODLR counterpart of bgp_dense_predict (see there for the outputs, workspace and errors).
+ * On a sharded factorisation with a matching communicator (see the multi-GPU block below) the call is COLLECTIVE, with
+ * spec, xs and ns replicated: per test-point chunk each shard builds its own rows J of K(x, x*) into an N x c chunk, the
+ * collective solve fills the other rows and runs the top levels, and the shard contracts over J
+ * (bgp_hodlr_predict_local_dev's arithmetic, the prior on shard 0 only); one all-reduce of ns (VAR) or ns^2 (COV)
+ * doubles adds the shards' parts, and every rank returns the same bits.  Everything is validated and reserved before
+ * the first collective, and one all-reduce of a status value makes a failure on any rank an error on every rank.  The
+ * number of chunks depends only on N, ns and BGP_PREDICT_CHUNK, which must therefore be the same on every rank.
+ * Device workspace per shard (doubles), besides the result and xs, with nloc = the shard's rows:
+ *   VAR  N*c + nloc*c + O(c)             COV  N*c + nloc*ns + split-K slices (c*ns each, at most max(c*ns, 2^27))
+ * A host-exchange shard returns BGP_ERR_INVALID, as before; it computes its part with bgp_hodlr_predict_local_dev. */
 int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
                       double* out);
+/* One shard's part of the prediction: with J = this handle's own rows [row0, row0 + rows) ([0, N) unsharded),
+ * B = K(x, x*) (N x ns) and P = B[J]^T W[J],
+ *   VAR: out[ns]        = (add_prior ? k(x*_j, x*_j) : 0) - P_jj
+ *   COV: out[i*ns + j]  = (add_prior ? K**(i,j) : 0) - P(i,j)     (row-major, bgp_hodlr_predict's orientation)
+ * from w_dev, the full solved K^-1 B on the device (N x ns column-major, leading dimension ldw >= N; on a
+ * host-exchange shard: solve_local_dev, the host's all-gather, solve_top_dev).  spec, xs and out as bgp_hodlr_predict.
+ * Only rows J of w_dev are read, and only rows J of B are built (x is replicated on every shard).  The test points run
+ * in bgp_hodlr_predict's chunks, so on an unsharded handle with add_prior = 1 the result is bit for bit what
+ * bgp_hodlr_predict returns.  Summing the P shards' outputs, add_prior = 1 on exactly one of them, gives the prediction.
+ * Issues no collective and works on any computed handle.  Workspace (doubles): VAR nloc*c + ns + O(c), COV nloc*ns +
+ * ns^2 + split-K slices.  Errors, before anything is launched: BGP_ERR_NOT_COMPUTED before compute and on a shard whose
+ * top levels are not finished; BGP_ERR_INVALID for an unknown `what`, ns < 0, a NULL w_dev with ns > 0 and ldw < N;
+ * BGP_ERR_DIM when the spec's ndim differs from the handle's.  ns == 0 writes nothing. */
+int bgp_hodlr_predict_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
+                                int32_t what, const double* w_dev, int64_t ldw, int32_t add_prior, double* out);
 
 /* Tree / index structure introspection (bit-exact parity target; hodlr.h:48-61).
  * Nodes are listed in the reference's PRE-ORDER construction order. */
@@ -481,7 +505,7 @@ int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n
  * opts.shard_rank, bgp_hodlr_compute[_dev] is COLLECTIVE and complete: local sub-tree, all-gather of the rows this shard
  * owns of the top-level factor panel (pack kernel -> ncclAllGather -> unpack kernels on the solver's stream), the nodes
  * above the cut, log-det all-reduce; apply_inverse / dot_solve are collective too (replicated right-hand side, one
- * all-gather of the locally solved slices).  WITHOUT a communicator (a "host-exchange shard": no communicator, or one
+ * all-gather of the locally solved slices), and so are grad_terms and predict.  WITHOUT a communicator (a "host-exchange shard": no communicator, or one
  * whose size or rank does not match) the same steps are exposed one by one so that a host can run the exchange itself.
  * The P shards may be P processes or P handles in one process, on any devices.  The call order is:
  *   1. bgp_hodlr_compute[_dev] on every shard (opts.shard_rank = s, opts.shard_count = P, rng_mode = per-node).  It
@@ -497,7 +521,9 @@ int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n
  * The full solves (bgp_hodlr_apply_inverse, bgp_hodlr_dot_solve[_dev], bgp_hodlr_get_inverse), like grad_terms,
  * predict and node_factors, return BGP_ERR_INVALID on a host-exchange shard: they need the other shards' rows.  The
  * gradient runs there as bgp_hodlr_grad_terms_local_dev on every shard with the solved alpha, the host summing g and
- * assembling the diag slices; with a matching communicator bgp_hodlr_grad_terms does all of it collectively.
+ * assembling the diag slices; with a matching communicator bgp_hodlr_grad_terms does all of it collectively.  The
+ * prediction runs there as bgp_hodlr_predict_local_dev on every shard with the solved K^-1 K(x, x*), the host summing
+ * the outputs (the prior on one shard); with a matching communicator bgp_hodlr_predict does it collectively.
  * bgp_hodlr_log_determinant on a host-exchange shard returns that shard's PARTIAL log-determinant: its own leaves and
  * sub-tree nodes, plus the nodes above the cut on shard 0 only, so the sum over the P shards is log det K.
  *   bgp_hodlr_top_panel(h, &ptr_dev, &row0, &rows, &cols, &ld): device pointer to the (N x cols) column-major panel of

@@ -2,7 +2,9 @@
 """Multi-GPU parity probe (run under torchrun): sharded HODLR (sub-tree per rank + one all-gather) must reproduce the
 single-GPU factorisation — same per-node RNG streams, so log-det / solve / gradient terms agree to rounding.  The
 gradient leg runs the collective grad_terms (each rank streams K^-1 over its own columns; all-reduce of g, all-gather of
-the diagonal) against the single-GPU grad_terms on rank 0."""
+the diagonal) against the single-GPU grad_terms on rank 0.  The predict leg runs the collective predictive (each rank
+builds and contracts K(x, x*) over its own rows; the chunks' solves and one all-reduce) for the variance and the
+covariance against the single-GPU bgp_hodlr_predict on rank 0, on the prior's scale."""
 import os, sys, json
 import numpy as np
 import torch
@@ -11,6 +13,7 @@ sys.path.insert(0, ".")
 from george_b200 import kernels, _lib
 from george_b200.parallel import ShardedHODLRSolver
 from george_b200.solvers._hodlr import HODLRSolver
+from george_b200.solvers.basic import BasicSolver
 
 rank = int(os.environ["RANK"]); local = int(os.environ["LOCAL_RANK"]); world = int(os.environ["WORLD_SIZE"])
 torch.cuda.set_device(local)
@@ -33,20 +36,27 @@ for name, kernel, n, ms, exhaust in [
     a = sh.apply_inverse(y)[:, 0]
     which = np.ones(len(kernel.get_parameter_vector(include_frozen=True)), dtype=np.uint32)
     ga, gg, gd = sh.grad_terms(y, which)  # collective
+    xs = np.random.default_rng(7).uniform(x.min() - 0.5, x.max() + 0.5, (300, 1))
+    pv, pc = sh.predictive(kernel, xs, "var"), sh.predictive(kernel, xs, "cov")  # collective
     if rank == 0:
         s = HODLRSolver(); s.compute(kernel, x[:, None], yerr, min_size=ms, tol=1e-10, seed=42, exhaust=exhaust)
         ld1, ds1 = s.log_determinant, s.dot_solve(y)
         a1 = s.apply_inverse(y)[:, 0]
         ga1, gg1, gd1 = np.empty(n), np.zeros(which.size), np.empty(n)
         _lib.check(s._lib.bgp_hodlr_grad_terms(s._ptr, _lib.ptr(which), _lib.ptr(y), _lib.ptr(ga1), _lib.ptr(gg1), _lib.ptr(gd1)))
+        pv1 = BasicSolver._predictive_call(s._lib.bgp_hodlr_predict, s._ptr, kernel, xs, "var")
+        pc1 = BasicSolver._predictive_call(s._lib.bgp_hodlr_predict, s._ptr, kernel, xs, "cov")
+        kss = np.max(np.abs(kernel.get_value(xs)))
+        p_rel = float(max(np.max(np.abs(pv - pv1)), np.max(np.abs(pc - pc1))) / kss)
         g_rel = float(np.max(np.abs(gg - gg1) / np.maximum(1.0, np.abs(gg1))))
         d_rel = float(np.linalg.norm(gd - gd1) / np.linalg.norm(gd1))
         good = abs(ld - ld1) <= 1e-10 * abs(ld1) and abs(ds - ds1) <= 1e-9 * abs(ds1) and np.linalg.norm(a - a1) <= 1e-9 * np.linalg.norm(a1)
         good = good and g_rel <= 1e-9 and d_rel <= 1e-9 and np.linalg.norm(ga - ga1) <= 1e-9 * np.linalg.norm(ga1)
+        good = good and p_rel <= 1e-9
         ok = ok and good
         print(json.dumps({"case": name, "world": world, "logdet_sharded": ld, "logdet_single": ld1, "dot_sharded": ds, "dot_single": ds1,
                           "solve_relerr": float(np.linalg.norm(a - a1) / np.linalg.norm(a1)), "grad_relerr": g_rel,
-                          "grad_diag_relerr": d_rel, "ok": bool(good)}))
+                          "grad_diag_relerr": d_rel, "predict_relerr": p_rel, "ok": bool(good)}))
 dist.barrier()
 if rank == 0:
     print("MGPU_CHECK", "PASS" if ok else "FAIL")
