@@ -23,6 +23,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libbgp_b200.so")
 BGP_OK, BGP_ERR_INVALID, BGP_ERR_DIM, BGP_ERR_NOT_COMPUTED, BGP_ERR_LINALG = 0, 1, 2, 3, 4
 BGP_ERR_CUDA, BGP_ERR_NO_DEVICE, BGP_ERR_RANK_CAPACITY, BGP_ERR_INDEX, BGP_ERR_NOMEM = 5, 6, 7, 8, 9
 BGP_PREDICT_VAR, BGP_PREDICT_COV = 0, 1
+BGP_SAMPLE_DMMA_ROWS = 8  # include/bgp.h: draws from which bgp_*_sample multiplies on the DMMA pipe
 
 
 class BGPError(RuntimeError):
@@ -68,6 +69,10 @@ SIGNATURES = {
     "bgp_dense_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
     "bgp_hodlr_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
     "bgp_hodlr_predict_local_dev": (C.c_int, [_p, _specp, _p, _i64, _i32, _p, _i64, _i32, _p]),
+    "bgp_mvn_sample": (C.c_int, [_p, _i64, _p, _p, _i64, C.c_double, _p]),
+    "bgp_dense_sample": (C.c_int, [_p, _specp, _p, _i64, _p, _p, _i64, C.c_double, _p]),
+    "bgp_hodlr_sample": (C.c_int, [_p, _specp, _p, _i64, _p, _p, _i64, C.c_double, _p]),
+    "bgp_sample_last_timing": (C.c_int, [_dp]),
     "bgp_dense_batch_create": (C.c_int, [C.POINTER(_p)]),
     "bgp_dense_batch_destroy": (None, [_p]),
     "bgp_dense_batch_log_likelihood": (C.c_int, [_p, _specp, _p, _i64, _i64, _p, _i64, _i32, _p, _p, _p, _p, _p]),

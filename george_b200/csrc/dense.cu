@@ -12,6 +12,7 @@
 #include "common.cuh"
 #include "gemm_dmma.cuh"
 #include "kernel_eval.cuh"
+#include "linalg.cuh"
 
 namespace bgp {
 int upload_program(const DevProgram& P, DevBuf<DevProgram>& buf, cudaStream_t s);
@@ -498,8 +499,8 @@ static int64_t dense_mid_block(int64_t OB) {
 // and go through grid.z).  gemm_info: the word the trailing updates test before running (a single factorisation
 // passes its info word so that nothing runs after a failed pivot; a batch passes nullptr, so a failed member's updates
 // run on its own slab's garbage, which no other member reads).
-static int dense_potrf_members(double* A, int64_t n, int64_t mstride, int members, int* info, const int* gemm_info,
-                               DevBuf<GemmDesc>& gdesc, cudaStream_t s) {
+int bgp::dense_potrf_members(double* A, int64_t n, int64_t mstride, int members, int* info, const int* gemm_info,
+                             DevBuf<GemmDesc>& gdesc, cudaStream_t s) {
   // all trailing-update descriptors of the factorisation, uploaded once
   std::vector<GemmDesc> descs;
   struct Step { int64_t k0; int nb; int64_t rem; int desc[3]; };
@@ -657,6 +658,31 @@ static int dense_potrs_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
 static int dense_trsm_fwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
   if (nrhs <= DS_MAX_RHS) BGP_TRY(h->d_tmp.reserve((size_t)h->n * DS_MAX_RHS, h->s));
   return trsm_fwd_members(h->d_A.p, h->n, 0, X, nrhs, ldx, 0, 1, h->d_tmp.p, h->n, h->s);
+}
+
+// GP.predict's covariance at the ns test points xs (host) into dC (ns x ns on the device, allocated here): every W chunk
+// stays resident (n*ns), then C = K** - W^T W (lower, mirrored: exactly symmetric).  P is the validated program of the
+// prediction's kernel.  bgp_dense_predict copies dC out; bgp_dense_sample draws from it on the device.
+static int dense_predict_cov_dev(bgp_dense* h, const DevProgram& P, const double* xs, int64_t ns, DevBuf<double>& dC) {
+  const int64_t n = h->n;
+  const int nd = h->ndim;
+  cudaStream_t s = h->s;
+  DevBuf<DevProgram> dprog;
+  DevBuf<double> dxs, dW, scratch;
+  DevBuf<GemmDesc> ddesc;
+  BGP_TRY(upload_program(P, dprog, s));
+  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
+  BGP_TRY(dxs.alloc((size_t)ns * nd, s));
+  BGP_TRY(dW.alloc((size_t)n * ns, s));
+  BGP_TRY(dC.alloc((size_t)ns * ns, s));
+  BGP_CUDA(cudaMemcpyAsync(dxs.p, xs, sizeof(double) * ns * nd, cudaMemcpyHostToDevice, s));
+  BGP_TRY(kmat_symmetric_launch_auto(P, dprog.p, dxs.p, ns, nullptr, dC.p, ns, s));
+  for (int64_t j0 = 0; j0 < ns; j0 += c) {
+    const int64_t nc = std::min(c, ns - j0);
+    BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p + j0 * nd, nc, h->d_x.p, n, dW.p + j0 * n, n, s));
+    BGP_TRY(dense_trsm_fwd_dev(h, dW.p + j0 * n, nc, n));
+  }
+  return predict_gemm_sub(dW.p, n, dW.p, n, ns, ns, n, true, dC.p, ns, scratch, ddesc, s);
 }
 
 extern "C" {
@@ -852,10 +878,9 @@ int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const doubl
   cudaStream_t s = h->s;
   DevBuf<DevProgram> dprog;
   DevBuf<double> dxs, dW, dkd, dvar, dC, scratch;
-  DevBuf<GemmDesc> ddesc;
-  BGP_TRY(upload_program(P, dprog, s));
-  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
   if (what == BGP_PREDICT_VAR) {
+    BGP_TRY(upload_program(P, dprog, s));
+    const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
     // workspace n*c + O(c): var_j = k(x*_j, x*_j) - ||L^-1 K(x, x*_j)||^2, chunk by chunk
     BGP_TRY(dxs.alloc((size_t)c * nd, s));
     BGP_TRY(dW.alloc((size_t)n * c, s));
@@ -871,22 +896,26 @@ int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const doubl
       BGP_CUDA(cudaMemcpyAsync(out + j0, dvar.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));
     }
   } else {
-    // every W chunk stays resident (n*ns), then C = K** - W^T W (lower, mirrored: exactly symmetric)
-    BGP_TRY(dxs.alloc((size_t)ns * nd, s));
-    BGP_TRY(dW.alloc((size_t)n * ns, s));
-    BGP_TRY(dC.alloc((size_t)ns * ns, s));
-    BGP_CUDA(cudaMemcpyAsync(dxs.p, xs, sizeof(double) * ns * nd, cudaMemcpyHostToDevice, s));
-    BGP_TRY(kmat_symmetric_launch_auto(P, dprog.p, dxs.p, ns, nullptr, dC.p, ns, s));
-    for (int64_t j0 = 0; j0 < ns; j0 += c) {
-      const int64_t nc = std::min(c, ns - j0);
-      BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p + j0 * nd, nc, h->d_x.p, n, dW.p + j0 * n, n, s));
-      BGP_TRY(dense_trsm_fwd_dev(h, dW.p + j0 * n, nc, n));
-    }
-    BGP_TRY(predict_gemm_sub(dW.p, n, dW.p, n, ns, ns, n, true, dC.p, ns, scratch, ddesc, s));
+    BGP_TRY(dense_predict_cov_dev(h, P, xs, ns, dC));
     BGP_CUDA(cudaMemcpyAsync(out, dC.p, sizeof(double) * ns * ns, cudaMemcpyDeviceToHost, s));
   }
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;
+}
+
+int bgp_dense_sample(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, const double* mean,
+                     const double* z, int64_t size, double jitter, double* out) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (!h->has_inputs) { set_error("the factor was imported: the handle holds no kernel/coordinates"); return BGP_ERR_NOT_COMPUTED; }
+  BGP_TRY(mvn_sample_check(ns, size, jitter));
+  DevProgram P;
+  BGP_TRY(build_dev_program(spec, &P));
+  if (P.ndim != h->ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", P.ndim, h->ndim); return BGP_ERR_DIM; }
+  if (ns == 0 || size == 0) return BGP_OK;
+  DevBuf<double> dC;
+  BGP_TRY(sample_mark(0, h->s));
+  BGP_TRY(dense_predict_cov_dev(h, P, xs, ns, dC));
+  return mvn_draw_host_io(dC.p, ns, mean, z, size, jitter, out, h->s);
 }
 
 int bgp_dense_export_factor(bgp_dense_t* h, double* out) {

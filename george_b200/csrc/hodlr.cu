@@ -19,6 +19,7 @@
 #include "hodlr_lu.cuh"
 #include "hodlr_aca2.cuh"
 #include "hodlr_leaf.cuh"
+#include "linalg.cuh"
 #include "kernel_eval.cuh"
 
 namespace bgp {
@@ -1612,6 +1613,36 @@ int bgp_hodlr_predict_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, c
   return BGP_OK;
 }
 
+// GP.predict's covariance on an unsharded handle into dC (ns x ns on the device, allocated here; row-major as
+// bgp_hodlr_predict returns it): B = K(x, x*) stays resident (n*ns), W one chunk (n*c): C[:, chunk] = K**[:, chunk] -
+// B^T W_chunk, in the reference's orientation (K_h^-1 is symmetric only to tol).  P is the validated program of the
+// prediction's kernel.  bgp_hodlr_predict copies dC out; bgp_hodlr_sample draws from it on the device.
+static int hodlr_predict_cov_dev(bgp_hodlr* h, const DevProgram& P, const double* xs, int64_t ns, DevBuf<double>& dC) {
+  const int64_t n = h->n;
+  const int nd = h->ndim;
+  cudaStream_t s = h->sA;
+  DevBuf<DevProgram> dprog;
+  DevBuf<double> dxs, dB, dW, scratch;
+  DevBuf<GemmDesc> ddesc;
+  BGP_TRY(upload_program(P, dprog, s));
+  const int64_t c = std::min(ns, predict_chunk_cols(n, 64));
+  BGP_TRY(dW.alloc((size_t)n * c, s));
+  BGP_TRY(dxs.alloc((size_t)ns * nd, s));
+  BGP_TRY(dB.alloc((size_t)n * ns, s));
+  BGP_TRY(dC.alloc((size_t)ns * ns, s));
+  BGP_CUDA(cudaMemcpyAsync(dxs.p, xs, sizeof(double) * ns * nd, cudaMemcpyHostToDevice, s));
+  BGP_TRY(kmat_symmetric_launch_auto(P, dprog.p, dxs.p, ns, nullptr, dC.p, ns, s));
+  BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p, ns, h->d_x.p, n, dB.p, n, s));
+  for (int64_t j0 = 0; j0 < ns; j0 += c) {
+    const int64_t nc = std::min(c, ns - j0);
+    BGP_CUDA(cudaMemcpyAsync(dW.p, dB.p + j0 * n, sizeof(double) * n * nc, cudaMemcpyDeviceToDevice, s));
+    BGP_TRY(hodlr_solve_dev(h, dW.p, nc, n, s, 0));
+    // column-major C (ld ns): rows j0.. of the chunk are output COLUMNS j of the row-major result
+    BGP_TRY(predict_gemm_sub(dW.p, n, dB.p, n, nc, ns, n, false, dC.p + j0, ns, scratch, ddesc, s));
+  }
+  return BGP_OK;
+}
+
 // GP.predict's variance / covariance on the stored factorisation.  The test points are streamed in chunks of a multiple
 // of 64 columns, so W = K^-1 B is solved in the same 64-column groups as apply_inverse and matches it bit for bit.
 // On a shard with a matching communicator the call is collective (hodlr_predict_collective).
@@ -1631,11 +1662,10 @@ int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
   cudaStream_t s = h->sA;
   DevBuf<DevProgram> dprog;
   DevBuf<double> dxs, dB, dW, dkd, dvar, dC, scratch;
-  DevBuf<GemmDesc> ddesc;
-  BGP_TRY(upload_program(P, dprog, s));
-  const int64_t c = std::min(ns, predict_chunk_cols(n, 64));
-  BGP_TRY(dW.alloc((size_t)n * c, s));
   if (what == BGP_PREDICT_VAR) {
+    BGP_TRY(upload_program(P, dprog, s));
+    const int64_t c = std::min(ns, predict_chunk_cols(n, 64));
+    BGP_TRY(dW.alloc((size_t)n * c, s));
     // workspace 2*n*c + O(c): var_j = k(x*_j, x*_j) - B_j . (K^-1 B)_j, chunk by chunk
     BGP_TRY(dxs.alloc((size_t)c * nd, s));
     BGP_TRY(dB.alloc((size_t)n * c, s));
@@ -1652,25 +1682,27 @@ int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
       BGP_CUDA(cudaMemcpyAsync(out + j0, dvar.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));
     }
   } else {
-    // B = K(x, x*) stays resident (n*ns), W one chunk (n*c): C[:, chunk] = K**[:, chunk] - B^T W_chunk, in the
-    // reference's orientation (K_h^-1 is symmetric only to tol)
-    BGP_TRY(dxs.alloc((size_t)ns * nd, s));
-    BGP_TRY(dB.alloc((size_t)n * ns, s));
-    BGP_TRY(dC.alloc((size_t)ns * ns, s));
-    BGP_CUDA(cudaMemcpyAsync(dxs.p, xs, sizeof(double) * ns * nd, cudaMemcpyHostToDevice, s));
-    BGP_TRY(kmat_symmetric_launch_auto(P, dprog.p, dxs.p, ns, nullptr, dC.p, ns, s));
-    BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p, ns, h->d_x.p, n, dB.p, n, s));
-    for (int64_t j0 = 0; j0 < ns; j0 += c) {
-      const int64_t nc = std::min(c, ns - j0);
-      BGP_CUDA(cudaMemcpyAsync(dW.p, dB.p + j0 * n, sizeof(double) * n * nc, cudaMemcpyDeviceToDevice, s));
-      BGP_TRY(hodlr_solve_dev(h, dW.p, nc, n, s, 0));
-      // column-major C (ld ns): rows j0.. of the chunk are output COLUMNS j of the row-major result
-      BGP_TRY(predict_gemm_sub(dW.p, n, dB.p, n, nc, ns, n, false, dC.p + j0, ns, scratch, ddesc, s));
-    }
+    BGP_TRY(hodlr_predict_cov_dev(h, P, xs, ns, dC));
     BGP_CUDA(cudaMemcpyAsync(out, dC.p, sizeof(double) * ns * ns, cudaMemcpyDeviceToHost, s));
   }
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;
+}
+
+// bgp_hodlr_predict's covariance drawn from on the device (include/bgp.h); unsharded handles only
+int bgp_hodlr_sample(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, const double* mean,
+                     const double* z, int64_t size, double jitter, double* out) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (h->opts.shard_count > 1) { set_error("sample is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  BGP_TRY(mvn_sample_check(ns, size, jitter));
+  DevProgram P;
+  BGP_TRY(build_dev_program(spec, &P));
+  if (P.ndim != h->ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", P.ndim, h->ndim); return BGP_ERR_DIM; }
+  if (ns == 0 || size == 0) return BGP_OK;
+  DevBuf<double> dC;
+  BGP_TRY(sample_mark(0, h->sA));
+  BGP_TRY(hodlr_predict_cov_dev(h, P, xs, ns, dC));
+  return mvn_draw_host_io(dC.p, ns, mean, z, size, jitter, out, h->sA);
 }
 
 int bgp_hodlr_num_nodes(const bgp_hodlr_t* h, int64_t* out) {

@@ -20,7 +20,7 @@ from ._spec import flatten, num_params, patch_specs
 from .modeling import ConstantModel, ModelSet
 from .solvers import BasicSolver, TrivialSolver
 from .solvers.basic import NONFINITE_RHS
-from .utils import multivariate_gaussian_samples
+from .utils import device_gaussian_samples, multivariate_gaussian_samples
 
 __all__ = ["GP"]
 
@@ -37,6 +37,19 @@ def _as_model(obj):
     except TypeError:
         return obj
     return ConstantModel(float(value))
+
+
+def _check_rng(rng):
+    if not isinstance(rng, (np.random.Generator, np.random.RandomState)):
+        raise TypeError("rng must be a numpy.random.Generator or numpy.random.RandomState, got {0}".format(
+            type(rng).__name__))
+
+
+def _check_size(size):
+    size = int(size)
+    if size < 0:
+        raise ValueError("size must be >= 0, got {0}".format(size))
+    return size
 
 
 def _is_number(obj):
@@ -680,17 +693,24 @@ class GP(ModelSet):
             kernel = self.kernel
 
         if not (return_var or return_cov):
-            # mean only: K(x*, x) alpha evaluated matrix-free on the device (csrc/kmat_ops.cu); the reference forms the
-            # (n*, N) matrix on the host (gp.py:524-528), which stops being possible long before N = 2^18
-            return kernel.matvec(xs, self._x, alpha) + self._call_mean(xs)
+            return self._predict_mean(alpha, xs, kernel)
+        return self._predict_spread(alpha, xs, return_var, kernel)
 
+    def _predict_mean(self, alpha, xs, kernel):
+        """K(x*, x) alpha + mean(x*), K(x*, x) alpha evaluated matrix-free on the device (csrc/kmat_ops.cu); the
+        reference forms the (n*, N) matrix on the host (gp.py:524-528), which stops being possible long before
+        N = 2^18."""
+        return kernel.matvec(xs, self._x, alpha) + self._call_mean(xs)
+
+    def _predict_spread(self, alpha, xs, return_var, kernel):
+        """``(mu, var)`` or ``(mu, cov)`` of :func:`predict`."""
         # variance / covariance from the stored factorisation on the device (BasicSolver, HODLRSolver): K(x*, x) and
         # K^-1 K(x, x*) stay there, streamed in column chunks.  Solvers without `predictive`, or that return None (a
         # pickled dense factor, a sharded tree), take the reference's host route below.
         predictive = getattr(self.solver, "predictive", None)
         out = predictive(kernel, xs, "var" if return_var else "cov") if predictive is not None else None
         if out is not None:
-            return kernel.matvec(xs, self._x, alpha) + self._call_mean(xs), out
+            return self._predict_mean(alpha, xs, kernel), out
         return self._predict_host(alpha, xs, return_var, kernel)
 
     def _predict_host(self, alpha, xs, return_var, kernel):
@@ -707,22 +727,89 @@ class GP(ModelSet):
         cov -= np.dot(Kxs, KinvKxs)
         return mu, cov
 
-    def sample_conditional(self, y, t, size=1):
-        mu, cov = self.predict(y, t)
-        return multivariate_gaussian_samples(cov, size, mean=mu)
+    def sample_conditional(self, y, t, size=1, *, rng=None, jitter=None):
+        """Draws from the conditional predictive distribution at ``t``: shape ``(ns,)`` when ``size == 1``, else
+        ``(size, ns)``.
 
-    def sample(self, t=None, size=1):
-        """Draw from the prior, at ``t`` or (``t is None``) at the computed coordinates via the Cholesky factor."""
+        With ``rng=None`` this is the reference's route: ``predict(y, t)`` and ``numpy.random.multivariate_normal``
+        (an SVD of the covariance on the host, drawing from numpy's global generator).
+
+        With ``rng`` (a ``numpy.random.Generator`` or ``RandomState``) the draws are ``mu + z @ L.T``, where ``z =
+        rng.standard_normal((size, ns))`` is drawn exactly once, after the argument checks and before any device call,
+        ``(mu, C)`` is what ``predict(y, t, return_cov=True)`` returns and ``L`` is the lower Cholesky factor of
+        ``sym(C) + jitter * I`` computed on the device, ``sym(C)`` mirroring the lower triangle of ``C`` (the HODLR
+        covariance is symmetric only to ``tol``).  ``jitter`` defaults to ``TINY``.  ``BasicSolver`` and
+        ``HODLRSolver`` build ``C`` on the device and never copy it to the host (``sample_predictive``); other
+        solvers sample from ``predict``'s covariance.  On ``ShardedHODLRSolver`` every rank returns the same draws
+        provided ``rng`` is seeded identically on every rank, as ``y`` and ``t`` are replicated.
+
+        If that matrix is not positive definite (a negative predictive variance, a NaN) the call raises
+        ``numpy.linalg.LinAlgError`` naming the failed leading minor, where the host route warns and draws anyway; the
+        GP stays as it was.
+        """
+        if rng is None:
+            if jitter is not None:
+                raise ValueError("jitter applies only to draws with an rng; the host route adds nothing")
+            mu, cov = self.predict(y, t)
+            return multivariate_gaussian_samples(cov, size, mean=mu)
+        _check_rng(rng)
+        jitter = TINY if jitter is None else float(jitter)
+        if not (np.isfinite(jitter) and jitter >= 0.0):
+            raise ValueError("jitter must be finite and >= 0, got {0}".format(jitter))
+        size = _check_size(size)
+        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
+            raise RuntimeError("You need to compute the model first")
+        self._check_dimensions(y)
+        xs = self.parse_samples(t)
+        z = rng.standard_normal((size, len(xs)))
+        if size == 0:
+            return np.empty((0, len(xs)), dtype=np.float64)
+        self.recompute()
+        alpha = self._compute_alpha(y, True)
+        draws = None
+        fused = getattr(self.solver, "sample_predictive", None)
+        if fused is not None:
+            draws = fused(self.kernel, xs, self._predict_mean(alpha, xs, self.kernel), z, jitter)
+        if draws is None:
+            mu, cov = self._predict_spread(alpha, xs, False, self.kernel)
+            draws = device_gaussian_samples(cov, z, mu, jitter)
+        return draws[0] if size == 1 else draws
+
+    def sample(self, t=None, size=1, *, rng=None):
+        """Draw from the prior, at ``t`` or (``t is None``) at the computed coordinates via the Cholesky factor.
+
+        With ``rng=None`` this is the reference's route (numpy's global generator; at ``t``, an SVD of
+        ``K(t, t) + TINY`` on the host).  With ``rng`` (a ``numpy.random.Generator`` or ``RandomState``) the normals are
+        ``rng.standard_normal((size, n))``, drawn once after the argument checks: at ``t`` the draws are those of
+        :func:`sample_conditional` with ``mu = mean(t)``, ``C = K(t, t)`` and ``jitter = TINY``; with ``t=None`` they
+        are ``solver.apply_sqrt(z) + mean(x)``."""
+        if rng is None:
+            if t is None:
+                self.recompute()
+                n = self._x.shape[0]
+                draws = self.solver.apply_sqrt(np.random.randn(size, n))
+                draws += self._call_mean(self._x)
+                return draws[0] if size == 1 else draws
+            x = self.parse_samples(t)
+            cov = self.get_matrix(x)
+            cov[np.diag_indices_from(cov)] += TINY
+            return multivariate_gaussian_samples(cov, size, mean=self._call_mean(x))
+        _check_rng(rng)
+        size = _check_size(size)
         if t is None:
+            if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
+                raise RuntimeError("You need to compute the model first")
+            z = rng.standard_normal((size, self._x.shape[0]))
             self.recompute()
-            n = self._x.shape[0]
-            draws = self.solver.apply_sqrt(np.random.randn(size, n))
+            draws = self.solver.apply_sqrt(z)
             draws += self._call_mean(self._x)
-            return draws[0] if size == 1 else draws
-        x = self.parse_samples(t)
-        cov = self.get_matrix(x)
-        cov[np.diag_indices_from(cov)] += TINY
-        return multivariate_gaussian_samples(cov, size, mean=self._call_mean(x))
+        else:
+            x = self.parse_samples(t)
+            z = rng.standard_normal((size, len(x)))
+            if size == 0:
+                return np.empty((0, len(x)), dtype=np.float64)
+            draws = device_gaussian_samples(self.get_matrix(x), z, self._call_mean(x), TINY)
+        return draws[0] if size == 1 else draws
 
     def get_matrix(self, x1, x2=None):
         x1 = self.parse_samples(x1)

@@ -217,6 +217,36 @@ class BasicSolver(object):
         _lib.check(fn(ptr, C.byref(spec), _lib.ptr(xs), ns, kinds[what], _lib.ptr(out)))
         return out
 
+    def sample_predictive(self, kernel, xs, mean, z, jitter):
+        """``mean + z @ L.T`` (``(size, ns)``) with ``L`` the lower Cholesky factor of ``sym(C) + jitter * I``, ``C``
+        the covariance :func:`predictive` returns for ``kernel`` at ``xs``: ``GP.sample_conditional``'s draws, with
+        ``C`` built, factorised and multiplied on the device without visiting the host
+        (``include/bgp.h: bgp_dense_sample``).  ``z``: ``(size, ns)`` standard normals.  Raises
+        ``numpy.linalg.LinAlgError`` when that matrix is not positive definite.  Returns ``None`` for a solver restored
+        from a pickle (it holds no coordinates): the caller then samples from the host's covariance."""
+        self._require()
+        if not getattr(self, "_has_inputs", True):
+            return None
+        return self._sample_call(self._handle.lib.bgp_dense_sample, self._handle.ptr, kernel, xs, mean, z, jitter)
+
+    @staticmethod
+    def _sample_call(fn, ptr, kernel, xs, mean, z, jitter):
+        xs = np.ascontiguousarray(xs, dtype=np.float64)
+        if xs.ndim == 1:
+            xs = xs[:, None]
+        spec = flatten(kernel)
+        if xs.ndim != 2 or xs.shape[1] != spec.ndim:
+            raise DimensionMismatch("dimension mismatch")
+        ns = xs.shape[0]
+        mean = np.ascontiguousarray(mean, dtype=np.float64)
+        z = np.ascontiguousarray(z, dtype=np.float64)
+        if mean.shape != (ns,) or z.ndim != 2 or z.shape[1] != ns:
+            raise ValueError("mean must have shape ({0},) and z (size, {0})".format(ns))
+        out = np.empty(z.shape, dtype=np.float64)
+        _lib.check(fn(ptr, C.byref(spec), _lib.ptr(xs), ns, _lib.ptr(mean), _lib.ptr(z), z.shape[0], float(jitter),
+                      _lib.ptr(out)))
+        return out
+
     @staticmethod
     def batch_log_likelihood(spec, params, x, yerr, r):
         """``(log_det, quad, info)``, each ``(B,)``, for ``B`` parameter vectors of one kernel program on the same

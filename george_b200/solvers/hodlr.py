@@ -69,6 +69,14 @@ class HODLRSolver(BasicSolver):
             return None
         return self._predictive_call(self.solver._lib.bgp_hodlr_predict, self.solver._ptr, kernel, xs, what)
 
+    def sample_predictive(self, kernel, xs, mean, z, jitter):
+        """``BasicSolver.sample_predictive`` on the HODLR factorisation (``include/bgp.h: bgp_hodlr_sample``); ``None``
+        on a sharded factorisation."""
+        self._require()
+        if self.solver.shard_count > 1:
+            return None
+        return self._sample_call(self.solver._lib.bgp_hodlr_sample, self.solver._ptr, kernel, xs, mean, z, jitter)
+
     def __getstate__(self):
         state = self.__dict__.copy()
         state["_computed"] = False

@@ -7,7 +7,9 @@ path; same public functions as the reference's ``src/george/utils.py:11-92``.
 import numpy as np
 from scipy.spatial import cKDTree
 
-__all__ = ["multivariate_gaussian_samples", "nd_sort_samples", "check_gradient"]
+from . import _lib
+
+__all__ = ["multivariate_gaussian_samples", "device_gaussian_samples", "nd_sort_samples", "check_gradient"]
 
 
 def multivariate_gaussian_samples(matrix, N, mean=None):
@@ -17,6 +19,24 @@ def multivariate_gaussian_samples(matrix, N, mean=None):
         mean = np.zeros(len(matrix))
     draws = np.random.multivariate_normal(mean, matrix, N)
     return draws[0] if N == 1 else draws
+
+
+def device_gaussian_samples(matrix, z, mean, jitter):
+    """``mean + z @ L.T`` (shape ``(size, ns)``) with ``L`` the lower Cholesky factor of ``sym(matrix) + jitter * I``,
+    computed on the device (``include/bgp.h: bgp_mvn_sample``).  ``sym`` mirrors the lower triangle of ``matrix``
+    (``(ns, ns)``); ``z`` (``(size, ns)``) holds the caller's standard normals, so the draws are reproducible from
+    them.  Raises ``numpy.linalg.LinAlgError`` when that matrix is not positive definite, where
+    :func:`multivariate_gaussian_samples` warns and draws anyway."""
+    matrix = np.ascontiguousarray(matrix, dtype=np.float64)
+    z = np.ascontiguousarray(z, dtype=np.float64)
+    mean = np.ascontiguousarray(mean, dtype=np.float64)
+    ns = len(mean)
+    if matrix.shape != (ns, ns) or z.ndim != 2 or z.shape[1] != ns:
+        raise ValueError("matrix must be (ns, ns) and z (size, ns) for a mean of length ns")
+    out = np.empty(z.shape, dtype=np.float64)
+    _lib.check(_lib.load().bgp_mvn_sample(_lib.ptr(matrix), ns, _lib.ptr(mean), _lib.ptr(z), z.shape[0],
+                                          float(jitter), _lib.ptr(out)))
+    return out
 
 
 def nd_sort_samples(samples):

@@ -430,6 +430,43 @@ int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
 int bgp_hodlr_predict_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
                                 int32_t what, const double* w_dev, int64_t ldw, int32_t add_prior, double* out);
 
+/* ------------------------------------------------------------------------------------------
+ * Draws from N(mean, C) on the device: GP.sample_conditional / GP.sample with a caller's random generator (the
+ * reference draws with numpy's multivariate_normal, an SVD of C on the host: utils.py:19-33, gp.py:547-599).
+ *   A   = sym(C) + jitter * I, sym(C) the LOWER triangle C[i*ns + j], i >= j, of the row-major C, mirrored
+ *   L   = the lower Cholesky factor of A (bgp_dense_compute's blocked Cholesky)
+ *   out[a*ns + j] = mean[j] + sum_{i <= j} z[a*ns + i] L(j, i)     (size x ns row-major: draws = mean + z L^T)
+ * mean (ns) and z (size x ns row-major, the caller's standard normals) are host arrays.  Fewer than
+ * BGP_SAMPLE_DMMA_ROWS draws run as one row of threads per draw (bgp_dense_apply_sqrt's arithmetic plus the mean: each
+ * draw reads L once); more run as a triangular GEMM on the DMMA pipe, one descriptor per 128 columns of out, its K
+ * stopping at the tile's last column.  Both add in a fixed order (no atomics): identical inputs give identical bits.
+ * bgp_mvn_sample takes C from the host.  bgp_dense_sample and bgp_hodlr_sample build C on the device exactly as the
+ * COV branch of bgp_dense_predict / bgp_hodlr_predict does (spec, xs, ns as there) and C never leaves the device, so
+ * bgp_dense_sample equals bgp_mvn_sample on bgp_dense_predict's output bit for bit; for HODLR the same holds wherever its
+ * predict is reproducible (N <= 1024, see bgp_dense_predict).
+ * Workspace (doubles): ns^2 (C, factorised in place) + (2 size + 1) ns, on top of the predict's for the fused entries.
+ * Errors: BGP_ERR_NOT_COMPUTED before compute and on a dense handle restored by bgp_dense_import_factor; BGP_ERR_DIM
+ * when the spec's ndim differs from the handle's; BGP_ERR_INVALID for ns < 0, size < 0, a negative or non-finite
+ * jitter and on any sharded HODLR handle (the sharded solver samples through bgp_mvn_sample on its collective
+ * prediction); BGP_ERR_NOMEM when the workspace cannot be allocated; BGP_ERR_LINALG, "k-th leading minor of the array
+ * is not positive definite", when A is not (a negative predictive variance, a NaN, a singular C with jitter 0).  The
+ * solver's handle is unchanged by any outcome.  ns == 0 or size == 0 writes nothing.
+ * ------------------------------------------------------------------------------------------ */
+/* Draws from which the product runs on the DMMA pipe.  On one H100 (700 W) the row path takes 0.05 / 0.13 ms for 1-7
+ * draws at ns = 256 / 1024 against 0.08 / 0.20 ms for the DMMA path, and loses at ns >= 4096 (0.82-0.90 vs 0.70 ms);
+ * tools/sample_bench.py, DESIGN.md §6. */
+#define BGP_SAMPLE_DMMA_ROWS 8
+int bgp_mvn_sample(const double* cov, int64_t ns, const double* mean, const double* z, int64_t size, double jitter,
+                   double* out);
+int bgp_dense_sample(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, const double* mean,
+                     const double* z, int64_t size, double jitter, double* out);
+int bgp_hodlr_sample(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, const double* mean,
+                     const double* z, int64_t size, double jitter, double* out);
+/* device-event timing (ms) of the calling thread's last successful sampling call: [0] the covariance (its build on
+ * the device for the fused entries, its upload for bgp_mvn_sample) and the upload of mean and z, [1] symmetrisation +
+ * Cholesky, [2] the product. */
+int bgp_sample_last_timing(double* ms3);
+
 /* Tree / index structure introspection (bit-exact parity target; hodlr.h:48-61).
  * Nodes are listed in the reference's PRE-ORDER construction order. */
 typedef struct bgp_hodlr_node_info {
