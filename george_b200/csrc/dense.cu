@@ -436,6 +436,12 @@ __global__ void square2_kernel(const double* __restrict__ yerr, double* __restri
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     diag[i] = yerr[i] * yerr[i];
 }
+// b[i] = a[i] + b[i]: the batched draws' mean, K(x*, x) alpha plus the mean model at x*, one IEEE add per entry as
+// GP.sample_conditional's host sum
+__global__ void add_into_kernel(const double* __restrict__ a, double* __restrict__ b, int64_t n) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    b[i] = a[i] + b[i];
+}
 // out (nr x n, row-major) = r (nr x n, row-major) @ U with U = L^T:  out[a][j] = sum_{i<=j} r[a][i] L[j][i]
 __global__ void apply_sqrt_kernel(const double* __restrict__ L, int64_t n, const double* __restrict__ r, int64_t nr,
                                   double* __restrict__ out) {
@@ -966,6 +972,11 @@ struct bgp_dense_batch {
   // variances and their partials, covariances and their split-K slices
   DevBuf<double> d_xs, d_mean, d_mvp, d_W, d_kd, d_var, d_vp, d_C, d_slices;
   DevBuf<GemmDesc> d_pdesc;
+  // bgp_dense_batch_sample: the means, normals and draws, the covariance factorisations' info words and the product's
+  // descriptors (apart from d_gdesc, which the factorisations use)
+  DevBuf<double> d_madd, d_z, d_draws;
+  DevBuf<int> d_dinfo;
+  DevBuf<GemmDesc> d_sdesc;
   // bgp_dense_batch_grad_terms: K_b^-1, the contraction partials and g
   DevBuf<double> d_inv, d_gp, d_g;
   DevBuf<unsigned> d_which;
@@ -1082,6 +1093,26 @@ static int batch_factor_chunk(bgp_dense_batch* h, const BatchPrograms& bp, int64
   return potrs_small_members(h->d_A.p, n, h->d_sol.p, 1, n, h->d_tmp.p, mc, mstride, n, s);
 }
 
+// members [c0, c0 + mc) after batch_factor_chunk: the steps of bgp_dense_predict's covariance path, member-indexed:
+// K**, every W chunk resident (W = L_b^-1 K_b(x, x*), test-point chunks of c columns), C_b = K** - W^T W into d_C
+// (member stride ns^2).  The W columns of all members are interleaved: column j of member m at W + (j * mc + m) * n, so
+// that the columns of a test-point chunk are one contiguous block (the few-column solve copies its result back in one
+// piece).  bgp_dense_batch_predict copies C out; bgp_dense_batch_sample draws from it on the device.
+static int batch_cov_chunk(bgp_dense_batch* h, const DevProgram* progs, const DevProgram* dprogs, int mc, int64_t n,
+                           int32_t ndim, int64_t ns, int64_t c) {
+  cudaStream_t s = h->s;
+  const int64_t nn = n * n, ldw = (int64_t)mc * n;
+  BGP_TRY(kmat_symmetric_batch_launch_auto(progs, dprogs, mc, h->d_xs.p, ns, nullptr, h->d_C.p, ns * ns, h->d_fn, s));
+  for (int64_t j0 = 0; j0 < ns; j0 += c) {
+    const int64_t nc = std::min(c, ns - j0);
+    BGP_TRY(kmat_general_batch_launch_auto(progs, dprogs, mc, h->d_xs.p + j0 * ndim, nc, h->d_x.p, n,
+                                           h->d_W.p + j0 * ldw, ldw, n, h->d_fn, s));
+    BGP_TRY(trsm_fwd_members(h->d_A.p, n, nn, h->d_W.p + j0 * ldw, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
+  }
+  return predict_gemm_sub_members(h->d_W.p, ldw, h->d_W.p, ldw, ns, ns, n, true, h->d_C.p, ns, mc, n, ns * ns,
+                                  h->d_slices, h->d_pdesc, s);
+}
+
 extern "C" {
 
 int bgp_dense_batch_create(bgp_dense_batch_t** out) {
@@ -1099,6 +1130,7 @@ void bgp_dense_batch_destroy(bgp_dense_batch_t* h) {
   h->d_xs.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_kd.release();
   h->d_var.release(); h->d_vp.release(); h->d_C.release(); h->d_slices.release(); h->d_pdesc.release();
   h->d_inv.release(); h->d_gp.release(); h->d_g.release(); h->d_which.release();
+  h->d_madd.release(); h->d_z.release(); h->d_draws.release(); h->d_dinfo.release(); h->d_sdesc.release();
   if (h->s) {
     cudaStreamSynchronize(h->s);
     cudaStreamDestroy(h->s);
@@ -1270,8 +1302,7 @@ int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec,
                                      h->d_mvp.p, s));
     if (ns > 0)
       BGP_CUDA(cudaMemcpyAsync(mean + c0 * ns, h->d_mean.p, sizeof(double) * mc * ns, cudaMemcpyDeviceToHost, s));
-    // W columns of all members interleaved: column j of member m at W + (j * mc + m) * n, so that the columns of a
-    // test-point chunk are one contiguous block (the few-column solve copies its result back in one piece)
+    // W columns of all members interleaved, as in batch_cov_chunk
     const int64_t ldw = (int64_t)mc * n;
     if (var) {
       // the steps of bgp_dense_predict's variance loop, member-indexed
@@ -1286,16 +1317,7 @@ int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec,
                                    sizeof(double) * nc, mc, cudaMemcpyDeviceToHost, s));
       }
     } else if (cov && ns > 0) {
-      // the steps of bgp_dense_predict's covariance path, member-indexed: K**, every W chunk resident, C = K** - W^T W
-      BGP_TRY(kmat_symmetric_batch_launch_auto(progs, dprogs, mc, h->d_xs.p, ns, nullptr, h->d_C.p, ns * ns, h->d_fn, s));
-      for (int64_t j0 = 0; j0 < ns; j0 += c) {
-        const int64_t nc = std::min(c, ns - j0);
-        BGP_TRY(kmat_general_batch_launch_auto(progs, dprogs, mc, h->d_xs.p + j0 * ndim, nc, h->d_x.p, n,
-                                               h->d_W.p + j0 * ldw, ldw, n, h->d_fn, s));
-        BGP_TRY(trsm_fwd_members(h->d_A.p, n, nn, h->d_W.p + j0 * ldw, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
-      }
-      BGP_TRY(predict_gemm_sub_members(h->d_W.p, ldw, h->d_W.p, ldw, ns, ns, n, true, h->d_C.p, ns, mc, n, ns * ns,
-                                       h->d_slices, h->d_pdesc, s));
+      BGP_TRY(batch_cov_chunk(h, progs, dprogs, mc, n, ndim, ns, c));
       BGP_CUDA(cudaMemcpyAsync(out + c0 * ns * ns, h->d_C.p, sizeof(double) * mc * ns * ns, cudaMemcpyDeviceToHost, s));
     }
     BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
@@ -1307,6 +1329,92 @@ int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec,
     if (info[b] == 0) continue;
     for (int64_t j = 0; j < ns; ++j) mean[b * ns + j] = std::nan("");
     for (int64_t j = 0; j < osize; ++j) out[b * osize + j] = std::nan("");
+  }
+  return BGP_OK;
+}
+
+int bgp_dense_batch_sample(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
+                           int64_t P, const double* x, int64_t n, int32_t ndim, const double* yerr, const double* r,
+                           const double* xs, int64_t ns, const double* mean_add, const double* z, int64_t size,
+                           double jitter, double* draws, int32_t* info, int32_t* draw_info) {
+  BGP_TRY(mvn_sample_check(ns, size, jitter));
+  BatchPrograms bp;
+  BGP_TRY(batch_begin(h, spec, params, B, P, x, n, ndim, &bp));
+  if (B == 0) return BGP_OK;
+  cudaStream_t s = h->s;
+  const bool draw = ns > 0 && size > 0;
+  const int64_t nn = n * n;
+  // bgp_dense_batch_predict's COV workspace (the single path's test-point chunk and split-K plan) plus z, the draws
+  // and the mean
+  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
+  const int64_t mvp = matvec_partial_size(ns, n);
+  int64_t gsplit = 1, gklen = 0;
+  if (draw) predict_gemm_plan(ns, ns, n, &gsplit, &gklen);
+  const int64_t tmp_cols = DS_MAX_RHS;
+  const int64_t per_member = nn + (4 + tmp_cols) * n + ns + mvp + n * ns + ns * ns * (1 + gsplit) + 2 * size * ns + ns;
+  int64_t chunk = batch_chunk_members(per_member, B);
+  // one launch per step for the chunk: the split-K product and the draws' DMMA product each take one descriptor per
+  // member and slice, at most 65535 per launch
+  chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, 65535 / gsplit));
+  if (draw && mvn_product_descs(ns, size) > 0)
+    chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, 65535 / mvn_product_descs(ns, size)));
+  auto release = [&] {
+    h->d_A.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_C.release();
+    h->d_slices.release(); h->d_tmp.release(); h->d_madd.release(); h->d_z.release(); h->d_draws.release();
+  };
+  auto reserve = [&](int64_t m) -> int {
+    BGP_TRY(h->d_A.reserve((size_t)(nn * m), s));
+    BGP_TRY(h->d_tmp.reserve((size_t)(n * m * tmp_cols), s));
+    BGP_TRY(h->d_mean.reserve((size_t)std::max<int64_t>(1, ns * m), s));
+    BGP_TRY(h->d_mvp.reserve((size_t)std::max<int64_t>(1, mvp * m), s));
+    if (draw) {
+      BGP_TRY(h->d_W.reserve((size_t)(n * ns * m), s));
+      BGP_TRY(h->d_C.reserve((size_t)(ns * ns * m), s));
+      BGP_TRY(h->d_slices.reserve((size_t)(ns * ns * gsplit * m), s));
+      BGP_TRY(h->d_madd.reserve((size_t)(ns * m), s));
+      BGP_TRY(h->d_z.reserve((size_t)(size * ns * m), s));
+      BGP_TRY(h->d_draws.reserve((size_t)(size * ns * m), s));
+    }
+    return BGP_OK;
+  };
+  BGP_TRY(batch_reserve_chunk(&chunk, reserve, release));
+  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, tmp_cols));
+  BGP_TRY(h->d_dinfo.reserve((size_t)chunk, s));
+  BGP_TRY(h->d_xs.reserve((size_t)std::max<int64_t>(1, ns * ndim), s));
+  if (ns > 0) BGP_CUDA(cudaMemcpyAsync(h->d_xs.p, xs, sizeof(double) * ns * ndim, cudaMemcpyHostToDevice, s));
+  const int64_t dsize = size * ns;  // a member's draws
+  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
+    const int mc = (int)std::min(chunk, B - c0);
+    const DevProgram* progs = bp.progs.data() + c0;
+    const DevProgram* dprogs = h->d_prog.p + c0;
+    // the steps of bgp_dense_batch_predict (factor, alpha, mean, COV), then those of bgp_dense_sample's draw with a
+    // member index.  A member whose K is not positive definite runs every later step on its own slabs, which no other
+    // member reads; nothing synchronises inside the chunk.
+    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
+    if (draw) {
+      BGP_TRY(kmat_matvec_batch_launch(dprogs, ndim, mc, h->d_xs.p, ns, h->d_x.p, n, h->d_sol.p, n, h->d_mean.p, ns,
+                                       h->d_mvp.p, s));
+      BGP_CUDA(cudaMemcpyAsync(h->d_madd.p, mean_add + c0 * ns, sizeof(double) * mc * ns, cudaMemcpyHostToDevice, s));
+      BGP_CUDA(cudaMemcpyAsync(h->d_z.p, z + c0 * dsize, sizeof(double) * mc * dsize, cudaMemcpyHostToDevice, s));
+      add_into_kernel<<<(unsigned)std::min<int64_t>((mc * ns + 255) / 256, 1184), 256, 0, s>>>(h->d_mean.p, h->d_madd.p,
+                                                                                              mc * ns);
+      BGP_LAUNCH_CHECK();
+      BGP_TRY(batch_cov_chunk(h, progs, dprogs, mc, n, ndim, ns, c));
+      BGP_TRY(mvn_factor_members(h->d_C.p, ns, jitter, mc, h->d_dinfo.p, nullptr, h->d_gdesc, s));
+      BGP_TRY(mvn_product_members(h->d_C.p, ns, h->d_madd.p, ns, h->d_z.p, size, h->d_draws.p, mc, h->d_sdesc, s));
+      BGP_CUDA(cudaMemcpyAsync(draws + c0 * dsize, h->d_draws.p, sizeof(double) * mc * dsize, cudaMemcpyDeviceToHost, s));
+      BGP_CUDA(cudaMemcpyAsync(draw_info + c0, h->d_dinfo.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
+    } else {
+      for (int m = 0; m < mc; ++m) draw_info[c0 + m] = 0;
+    }
+    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaStreamSynchronize(s));
+  }
+  for (int64_t b = 0; b < B; ++b) {
+    if (!bp.valid[b]) info[b] = -1;
+    if (info[b] != 0) draw_info[b] = 0;
+    if (info[b] == 0 && draw_info[b] == 0) continue;
+    for (int64_t j = 0; j < dsize; ++j) draws[b * dsize + j] = std::nan("");
   }
   return BGP_OK;
 }

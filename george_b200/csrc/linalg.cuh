@@ -18,6 +18,17 @@ int dense_potrf_members(double* A, int64_t n, int64_t mstride, int members, int*
 // BGP_ERR_LINALG ("%d-th leading minor ...") when A is not positive definite; nothing is written to out then.
 int mvn_draw_dev(double* C, int64_t ns, const double* mean, double* z, int64_t size, double jitter, double* out,
                  DevBuf<int>& info, DevBuf<GemmDesc>& gdesc, cudaStream_t s);
+// The two halves of mvn_draw_dev for `members` draws at once, one launch per step for all of them (member m: C + m ns^2,
+// mean + m * mstride, z and out + m * size * ns); mvn_draw_dev runs them with one member and checks info in between.
+//   mvn_factor_members: A_m = sym(C_m) + jitter * I factorised in place, info[m] its dpotrf index (gemm_info as in
+//     dense_potrf_members: a batch passes nullptr, so a failed member's steps run on its own slab only).
+//   mvn_product_members: zero the upper triangles, then out = mean + z L^T (rows below BGP_SAMPLE_DMMA_ROWS draws, the
+//     DMMA GEMM from it with mvn_product_descs(ns, size) descriptors per member, uploaded to gdesc).
+int mvn_factor_members(double* C, int64_t ns, double jitter, int members, int* info, const int* gemm_info,
+                       DevBuf<GemmDesc>& gdesc, cudaStream_t s);
+int mvn_product_members(double* C, int64_t ns, const double* mean, int64_t mstride, double* z, int64_t size,
+                        double* out, int members, DevBuf<GemmDesc>& gdesc, cudaStream_t s);
+int64_t mvn_product_descs(int64_t ns, int64_t size);
 // mvn_draw_dev with mean, z and out on the host (synchronises s)
 int mvn_draw_host_io(double* C, int64_t ns, const double* mean, const double* z, int64_t size, double jitter,
                      double* out, cudaStream_t s);

@@ -20,9 +20,12 @@ constexpr int SP_T = 32;  // tile of the symmetrisation
 // (rows bi, columns bj; C[i*n + j], i >= j) onto the mirrored positions C[j*n + i] through shared memory, so both the
 // read and the write are coalesced.  The positions written (i > j) are never read and the diagonal is read and written
 // by the same thread, so the CTAs need no ordering.  A is its own transpose: column-major, as the Cholesky reads it.
-__global__ void __launch_bounds__(256) sample_sym_kernel(double* __restrict__ C, int64_t n, double jitter) {
+// Member blockIdx.z works on C + blockIdx.z * cstride.
+__global__ void __launch_bounds__(256) sample_sym_kernel(double* __restrict__ C, int64_t n, double jitter,
+                                                         int64_t cstride) {
   const int64_t bi = blockIdx.y, bj = blockIdx.x;
   if (bj > bi) return;
+  C += blockIdx.z * cstride;
   __shared__ double t[SP_T][SP_T + 1];
   const int tx = threadIdx.x & (SP_T - 1), ty = threadIdx.x / SP_T;
   for (int r = ty; r < SP_T; r += 256 / SP_T) {
@@ -38,28 +41,34 @@ __global__ void __launch_bounds__(256) sample_sym_kernel(double* __restrict__ C,
 }
 
 // zero the strict upper triangle of the column-major factor (entries (i, j), i < j, at L[j*n + i]), which the
-// factorisation leaves holding A, so that the product may read whole tiles of L
-__global__ void sample_zero_upper_kernel(double* __restrict__ L, int64_t n) {
+// factorisation leaves holding A, so that the product may read whole tiles of L; member blockIdx.z at L + z * lstride
+__global__ void sample_zero_upper_kernel(double* __restrict__ L, int64_t n, int64_t lstride) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  L += blockIdx.z * lstride;
   for (int64_t j = blockIdx.y; j < n; j += gridDim.y)
     if (i < j) L[j * n + i] = 0.0;
 }
 
 // few draws: out[a][j] = mean[j] + sum_{i<=j} z[a][i] L[j][i], the arithmetic of apply_sqrt_kernel (dense.cu) plus the
-// mean; one thread per output entry, the row of L it needs read coalesced across the CTA
+// mean; one thread per output entry, the row of L it needs read coalesced across the CTA.  Member blockIdx.z reads
+// L + z * lstride, mean + z * mstride and z, out + z * zstride.
 __global__ void sample_rows_kernel(const double* __restrict__ L, int64_t n, const double* __restrict__ z,
-                                   const double* __restrict__ mean, double* __restrict__ out) {
+                                   const double* __restrict__ mean, double* __restrict__ out, int64_t lstride,
+                                   int64_t mstride, int64_t zstride) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t a = blockIdx.y;
+  const int64_t a = blockIdx.y, m = blockIdx.z;
   if (j >= n) return;
+  L += m * lstride; mean += m * mstride; z += m * zstride; out += m * zstride;
   double s = 0.0;
   for (int64_t i = 0; i <= j; ++i) s += z[a * n + i] * L[i * n + j];  // L[j][i] column-major = L[i*n + j]
   out[a * n + j] = mean[j] + s;
 }
 
-// many draws, the operands of gemm_dmma's C -= A'B': out starts as the mean in every row and z is negated (exactly)
+// many draws, the operands of gemm_dmma's C -= A'B': out starts as the mean in every row and z is negated (exactly);
+// member blockIdx.z on z, out + z * total (its size x n draws) and mean + z * mstride
 __global__ void sample_dmma_operands_kernel(double* __restrict__ z, const double* __restrict__ mean,
-                                            double* __restrict__ out, int64_t n, int64_t total) {
+                                            double* __restrict__ out, int64_t n, int64_t total, int64_t mstride) {
+  z += blockIdx.z * total; out += blockIdx.z * total; mean += blockIdx.z * mstride;
   for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < total; p += (int64_t)gridDim.x * blockDim.x) {
     z[p] = -z[p];
     out[p] = mean[p % n];
@@ -90,16 +99,72 @@ int mvn_sample_check(int64_t ns, int64_t size, double jitter) {
   return BGP_OK;
 }
 
+int mvn_factor_members(double* C, int64_t ns, double jitter, int members, int* info, const int* gemm_info,
+                       DevBuf<GemmDesc>& gdesc, cudaStream_t s) {
+  const unsigned T = (unsigned)((ns + SP_T - 1) / SP_T);
+  sample_sym_kernel<<<dim3(T, T, (unsigned)members), 256, 0, s>>>(C, ns, jitter, ns * ns);
+  BGP_LAUNCH_CHECK();
+  BGP_CUDA(cudaMemsetAsync(info, 0, sizeof(int) * members, s));
+  return dense_potrf_members(C, ns, ns * ns, members, info, gemm_info, gdesc, s);
+}
+
+int64_t mvn_product_descs(int64_t ns, int64_t size) {
+  if (size < BGP_SAMPLE_DMMA_ROWS) return 0;
+  const int64_t slab = std::min<int64_t>(size, (int64_t)65535 * GD_BN);
+  return (size + slab - 1) / slab * ((ns + GD_BM - 1) / GD_BM);
+}
+
+int mvn_product_members(double* C, int64_t ns, const double* mean, int64_t mstride, double* z, int64_t size,
+                        double* out, int members, DevBuf<GemmDesc>& gdesc, cudaStream_t s) {
+  const unsigned mb = (unsigned)members;
+  const int64_t total = size * ns;  // a member's draws
+  sample_zero_upper_kernel<<<dim3((unsigned)((ns + 255) / 256), (unsigned)std::min<int64_t>(ns, 65535), mb), 256, 0,
+                             s>>>(C, ns, ns * ns);
+  BGP_LAUNCH_CHECK();
+  if (size < BGP_SAMPLE_DMMA_ROWS) {
+    sample_rows_kernel<<<dim3((unsigned)((ns + 127) / 128), (unsigned)size, mb), 128, 0, s>>>(C, ns, z, mean, out,
+                                                                                              ns * ns, mstride, total);
+    BGP_LAUNCH_CHECK();
+    return BGP_OK;
+  }
+  sample_dmma_operands_kernel<<<dim3((unsigned)std::min<int64_t>((total + 255) / 256, 4096), 1, mb), 256, 0, s>>>(
+      z, mean, out, ns, total, mstride);
+  BGP_LAUNCH_CHECK();
+  // column-major view: out^T (ns x size, ld ns) -= L (-z)^T.  One descriptor per member, per 128 rows of out^T (= 128
+  // columns of out) and per slab of at most 65535 * 128 draws (the grid's y limit); the tile of rows j0.. stops K at
+  // its last row, so the blocks of L above the diagonal are neither read nor multiplied.  Every member's descriptors
+  // have the geometry of a single draw's, so its bits do not depend on the number of members.
+  const int64_t slab = std::min<int64_t>(size, (int64_t)65535 * GD_BN);
+  std::vector<GemmDesc> descs;
+  for (int m = 0; m < members; ++m) {
+    const double* Lm = C + m * ns * ns;
+    double* zm = z + m * total;
+    double* om = out + m * total;
+    for (int64_t a0 = 0; a0 < size; a0 += slab)
+      for (int64_t j0 = 0; j0 < ns; j0 += GD_BM) {
+        GemmDesc d;
+        d.A = Lm + j0; d.lda = ns;                // A'(m, k) = L[j0 + m][k] = C[k*ns + j0 + m]
+        d.B = zm + a0 * ns; d.ldb = ns;           // B'(k, a) = -z[a0 + a][k]
+        d.C = om + a0 * ns + j0; d.ldc = ns;      // C(m, a) = out[a0 + a][j0 + m]
+        d.M = (int)std::min<int64_t>(GD_BM, ns - j0);
+        d.N = (int)std::min(slab, size - a0);
+        d.K = (int)std::min<int64_t>(j0 + GD_BM, ns);
+        d.mode = GD_SUB;
+        descs.push_back(d);
+      }
+  }
+  BGP_TRY(gdesc.reserve(descs.size(), s));
+  BGP_CUDA(cudaMemcpyAsync(gdesc.p, descs.data(), sizeof(GemmDesc) * descs.size(), cudaMemcpyHostToDevice, s));
+  // descs is pageable host memory: the copy above has been staged before cudaMemcpyAsync returned
+  return gemm_dmma_launch<false, true>(gdesc.p, (int)descs.size(), GD_BM, (int)slab, nullptr, s);
+}
+
 int mvn_draw_dev(double* C, int64_t ns, const double* mean, double* z, int64_t size, double jitter, double* out,
                  DevBuf<int>& info, DevBuf<GemmDesc>& gdesc, cudaStream_t s) {
   if (ns == 0 || size == 0) return BGP_OK;
   BGP_TRY(sample_mark(1, s));
-  const unsigned T = (unsigned)((ns + SP_T - 1) / SP_T);
-  sample_sym_kernel<<<dim3(T, T), 256, 0, s>>>(C, ns, jitter);
-  BGP_LAUNCH_CHECK();
   BGP_TRY(info.reserve(1, s));
-  BGP_CUDA(cudaMemsetAsync(info.p, 0, sizeof(int), s));
-  BGP_TRY(dense_potrf_members(C, ns, 0, 1, info.p, info.p, gdesc, s));
+  BGP_TRY(mvn_factor_members(C, ns, jitter, 1, info.p, info.p, gdesc, s));
   BGP_TRY(sample_mark(2, s));
   int h_info = 0;
   BGP_CUDA(cudaMemcpyAsync(&h_info, info.p, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -109,39 +174,7 @@ int mvn_draw_dev(double* C, int64_t ns, const double* mean, double* z, int64_t s
               h_info);
     return BGP_ERR_LINALG;
   }
-  sample_zero_upper_kernel<<<dim3((unsigned)((ns + 255) / 256), (unsigned)std::min<int64_t>(ns, 65535)), 256, 0, s>>>(
-      C, ns);
-  BGP_LAUNCH_CHECK();
-  if (size < BGP_SAMPLE_DMMA_ROWS) {
-    sample_rows_kernel<<<dim3((unsigned)((ns + 127) / 128), (unsigned)size), 128, 0, s>>>(C, ns, z, mean, out);
-    BGP_LAUNCH_CHECK();
-    return sample_mark(3, s);
-  }
-  const int64_t total = size * ns;
-  sample_dmma_operands_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 4096), 256, 0, s>>>(z, mean, out, ns,
-                                                                                                     total);
-  BGP_LAUNCH_CHECK();
-  // column-major view: out^T (ns x size, ld ns) -= L (-z)^T.  One descriptor per 128 rows of out^T (= 128 columns of
-  // out) and per slab of at most 65535 * 128 draws (the grid's y limit); the tile of rows j0.. stops K at its last
-  // row, so the blocks of L above the diagonal are neither read nor multiplied.
-  const int64_t slab = std::min<int64_t>(size, (int64_t)65535 * GD_BN);
-  std::vector<GemmDesc> descs;
-  for (int64_t a0 = 0; a0 < size; a0 += slab)
-    for (int64_t j0 = 0; j0 < ns; j0 += GD_BM) {
-      GemmDesc d;
-      d.A = C + j0; d.lda = ns;                 // A'(m, k) = L[j0 + m][k] = C[k*ns + j0 + m]
-      d.B = z + a0 * ns; d.ldb = ns;            // B'(k, a) = -z[a0 + a][k]
-      d.C = out + a0 * ns + j0; d.ldc = ns;     // C(m, a) = out[a0 + a][j0 + m]
-      d.M = (int)std::min<int64_t>(GD_BM, ns - j0);
-      d.N = (int)std::min(slab, size - a0);
-      d.K = (int)std::min<int64_t>(j0 + GD_BM, ns);
-      d.mode = GD_SUB;
-      descs.push_back(d);
-    }
-  BGP_TRY(gdesc.reserve(descs.size(), s));
-  BGP_CUDA(cudaMemcpyAsync(gdesc.p, descs.data(), sizeof(GemmDesc) * descs.size(), cudaMemcpyHostToDevice, s));
-  BGP_TRY((gemm_dmma_launch<false, true>(gdesc.p, (int)descs.size(), GD_BM, (int)slab, nullptr, s)));
-  // descs is pageable host memory: the copy above has been staged before cudaMemcpyAsync returned
+  BGP_TRY(mvn_product_members(C, ns, mean, 0, z, size, out, 1, gdesc, s));
   return sample_mark(3, s);
 }
 

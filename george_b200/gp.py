@@ -480,13 +480,30 @@ class GP(ModelSet):
 
     def _batch_predict_device(self, batch, vectors, y, xs, what):
         """The batched dense path of :func:`batch_predict`; ``None`` when the kernel has no valid device program."""
-        members = self._batch_members(vectors, y, self._residual,
-                                      lambda y, c: y - (c + np.zeros(len(y))))  # GP._residual of a ConstantModel
+        members = self._batch_predict_members(vectors, y)
         if members is None:
             return None
         spec, full, kpar, sigma, resid, fact_err, mean_err = members
-        nb, ns, n_mean = len(vectors), len(xs), self.mean.full_size
-        # the mean model at x*, what GP.predict adds last (a non-finite constant already failed in the residual)
+        mean_xs, xs_err = self._batch_mean_at(full, xs)
+        mu, out, info = batch(spec, kpar, self._x, sigma, resid, xs, what)
+        for b in range(len(vectors)):  # the loop's order: white noise, factorisation, residual, mean at x*
+            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
+            exc = exc if exc is not None else (mean_err[b] if mean_err[b] is not None else xs_err[b])
+            if exc is not None:
+                raise exc
+        mu += mean_xs
+        return mu if what is None else (mu, out)
+
+    def _batch_predict_members(self, vectors, y):
+        """:func:`_batch_members` with the residual of :func:`predict` (``GP._residual``)."""
+        return self._batch_members(vectors, y, self._residual,
+                                   lambda y, c: y - (c + np.zeros(len(y))))  # GP._residual of a ConstantModel
+
+    def _batch_mean_at(self, full, xs):
+        """``(mean_xs, xs_err)``: the mean model at ``xs`` for each member's full parameter vector (``(B, ns)``), what
+        ``GP.predict`` adds last to the kernel part of its mean, and the exception member ``b``'s evaluation raised,
+        or ``None`` (a non-finite constant already failed in the residual)."""
+        nb, ns, n_mean = len(full), len(xs), self.mean.full_size
         mean_xs, xs_err = np.zeros((nb, ns), dtype=np.float64), [None] * nb
         for b in range(nb):
             if type(self.mean) is ConstantModel:
@@ -496,14 +513,7 @@ class GP(ModelSet):
                 mean_xs[b] = self._swap_eval(self.mean, full[b, :n_mean], lambda: self._call_mean(xs))
             except Exception as exc:
                 xs_err[b] = exc
-        mu, out, info = batch(spec, kpar, self._x, sigma, resid, xs, what)
-        for b in range(nb):  # the loop's order: white noise, factorisation, residual, mean at x*
-            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
-            exc = exc if exc is not None else (mean_err[b] if mean_err[b] is not None else xs_err[b])
-            if exc is not None:
-                raise exc
-        mu += mean_xs
-        return mu if what is None else (mu, out)
+        return mean_xs, xs_err
 
     def lnlikelihood(self, y, quiet=False):
         warnings.warn("'lnlikelihood' is deprecated. Use 'log_likelihood'", DeprecationWarning)
@@ -774,6 +784,95 @@ class GP(ModelSet):
             mu, cov = self._predict_spread(alpha, xs, False, self.kernel)
             draws = device_gaussian_samples(cov, z, mu, jitter)
         return draws[0] if size == 1 else draws
+
+    def batch_sample_conditional(self, vectors, y, t, size=1, *, rng=None, jitter=None):
+        """:func:`sample_conditional` at many parameter vectors: ``(B, ns)`` when ``size == 1``, else ``(B, size,
+        ns)``, entry ``b`` being bit for bit what ``gp.set_parameter_vector(vectors[b]); gp.sample_conditional(y, t,
+        size, rng=rng, jitter=jitter)`` returns, run over ``b`` in order on the computed ``x`` and ``yerr``: posterior
+        predictive draws for each sample of a chain in one call.  The GP is left as it was: parameter vector,
+        factorisation, cached solve and dirty flags.
+
+        With ``rng`` (a ``numpy.random.Generator`` or ``RandomState``) the normals are drawn on the host, one
+        ``rng.standard_normal((size, ns))`` per member in member order, all of them after the argument checks and
+        before any device call.  When no member fails the generator ends where that loop leaves it; when one fails it
+        has still advanced by all ``B`` members' normals.  ``rng=None`` runs that loop itself (the reference's host
+        route, numpy's global generator).
+
+        The argument checks (``rng``, ``jitter``, ``size``, a computed model, the shape of ``vectors``, ``y``'s length,
+        ``t``'s dimension) come first and raise what :func:`sample_conditional` (or, for ``vectors``,
+        :func:`batch_predict`) raises.  Then a failing member raises the exception the loop would raise first, with its
+        type and message: white noise, factorisation, residual, mean at ``t``, and a predictive covariance that is not
+        positive definite.  With no members, ``size == 0`` or no test points nothing is computed and the empty result
+        is returned, the generator advanced as the loop would advance it; with no test points the loop would still
+        factorise every member, which is skipped here as in :func:`batch_predict`.
+
+        Solvers with a ``batch_sample`` hook (``BasicSolver``) factorise, predict and draw for all members in one
+        batched pass on the device; any other solver (``HODLRSolver``, ``ShardedHODLRSolver``, ``TrivialSolver``,
+        plug-ins) and a kernel without a valid device program take that loop.
+
+        :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
+        """
+        if rng is None:
+            if jitter is not None:
+                raise ValueError("jitter applies only to draws with an rng; the host route adds nothing")
+        else:
+            _check_rng(rng)
+            jitter = TINY if jitter is None else float(jitter)
+            if not (np.isfinite(jitter) and jitter >= 0.0):
+                raise ValueError("jitter must be finite and >= 0, got {0}".format(jitter))
+        size = _check_size(size)
+        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
+            raise RuntimeError("You need to compute the model first")
+        vectors = np.asarray(vectors, dtype=np.float64)
+        if vectors.ndim != 2 or vectors.shape[1] != len(self):
+            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        self._check_dimensions(y)
+        xs = self.parse_samples(t)
+        nb, ns = len(vectors), len(xs)
+        shape = (nb, ns) if size == 1 else (nb, size, ns)
+        if nb == 0:
+            return np.empty(shape, dtype=np.float64)
+        if rng is not None and (size == 0 or ns == 0):
+            for _ in range(nb):
+                rng.standard_normal((size, ns))
+            return np.empty(shape, dtype=np.float64)
+        batch = getattr(self.solver_type, "batch_sample", None)
+        if batch is not None and rng is not None:
+            out = self._batch_sample_device(batch, vectors, y, xs, size, rng, jitter)
+            if out is not None:
+                return out
+        state = self._batch_state()
+        try:
+            res = []
+            for v in vectors:
+                self.set_parameter_vector(v)
+                res.append(self.sample_conditional(y, t, size, rng=rng, jitter=jitter))
+        finally:
+            self._batch_restore(state)
+        return np.stack(res)
+
+    def _batch_sample_device(self, batch, vectors, y, xs, size, rng, jitter):
+        """The batched dense path of :func:`batch_sample_conditional`; ``None`` when the kernel has no valid device
+        program (nothing has been drawn from ``rng`` then)."""
+        members = self._batch_predict_members(vectors, y)
+        if members is None:
+            return None
+        spec, full, kpar, sigma, resid, fact_err, mean_err = members
+        nb, ns = len(vectors), len(xs)
+        z = np.empty((nb, size, ns), dtype=np.float64)
+        for b in range(nb):
+            z[b] = rng.standard_normal((size, ns))
+        mean_xs, xs_err = self._batch_mean_at(full, xs)
+        draws, info, draw_info = batch(spec, kpar, self._x, sigma, resid, xs, mean_xs, z, jitter)
+        for b in range(nb):  # the loop's order: white noise, factorisation, residual, mean at x*, covariance
+            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
+            exc = exc if exc is not None else (mean_err[b] if mean_err[b] is not None else xs_err[b])
+            if exc is None and draw_info[b] != 0:
+                exc = LinAlgError("%d-th leading minor of the array is not positive definite (a larger jitter adds "
+                                  "more to the diagonal)" % draw_info[b])
+            if exc is not None:
+                raise exc
+        return draws[:, 0] if size == 1 else draws
 
     def sample(self, t=None, size=1, *, rng=None):
         """Draw from the prior, at ``t`` or (``t is None``) at the computed coordinates via the Cholesky factor.

@@ -376,6 +376,53 @@ class BasicSolver(object):
             _lib.ptr(info)))
         return mean, out, info
 
+    @staticmethod
+    def batch_sample(spec, params, x, yerr, r, xs, mean_add, z, jitter):
+        """``(draws, info, draw_info)`` for ``B`` parameter vectors of one kernel program on the same ``x``: member
+        ``b`` factorises as in :func:`batch_log_likelihood` and draws ``mu_b + z[b] @ L_b.T`` (``(B, size, ns)``) as
+        :func:`sample_predictive` does, ``mu_b`` being the kernel part of ``GP.predict``'s mean plus ``mean_add[b]``
+        and ``L_b`` the lower Cholesky factor of ``sym(C_b) + jitter * I`` with ``C_b`` the member's predictive
+        covariance (``include/bgp.h: bgp_dense_batch_sample``).  ``info`` is that of :func:`batch_log_likelihood`;
+        ``draw_info[b]`` is 0 or the leading minor of that matrix which is not positive definite (0 where ``info[b]``
+        is not); a failed member's draws are NaN.  Every draw is bit-identical to :func:`compute` with member ``b``'s
+        spec and yerr followed by :func:`sample_predictive`.  ``xs``: ``(ns,)`` or ``(ns, ndim)``; ``mean_add``:
+        ``(B, ns)``; ``z``: ``(B, size, ns)`` standard normals."""
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.ndim == 1:
+            x = x[:, None]
+        xs = np.ascontiguousarray(xs, dtype=np.float64)
+        if xs.ndim == 1:
+            xs = xs[:, None]
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
+        r = np.ascontiguousarray(r, dtype=np.float64)
+        mean_add = np.ascontiguousarray(mean_add, dtype=np.float64)
+        z = np.ascontiguousarray(z, dtype=np.float64)
+        if x.ndim != 2 or x.shape[0] == 0:
+            raise ValueError("x must have shape (n, ndim) with n > 0")
+        n, ndim = x.shape
+        if params.ndim != 2 or params.shape[1] != num_params(spec):
+            raise ValueError("params must have shape (B, {0})".format(num_params(spec)))
+        nb = params.shape[0]
+        if yerr.shape != (nb, n) or r.shape != (nb, n):
+            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
+        if ndim != spec.ndim or xs.ndim != 2 or xs.shape[1] != ndim:
+            raise DimensionMismatch("dimension mismatch")
+        ns = xs.shape[0]
+        if mean_add.shape != (nb, ns) or z.ndim != 3 or z.shape[0] != nb or z.shape[2] != ns:
+            raise ValueError("mean_add must have shape ({0}, {1}) and z ({0}, size, {1})".format(nb, ns))
+        draws = np.empty(z.shape, dtype=np.float64)
+        info = np.zeros(nb, dtype=np.int32)
+        draw_info = np.zeros(nb, dtype=np.int32)
+        if nb == 0:
+            return draws, info, draw_info
+        h = _get_batch_handle()
+        _lib.check(h.lib.bgp_dense_batch_sample(
+            h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim, _lib.ptr(yerr),
+            _lib.ptr(r), _lib.ptr(xs), ns, _lib.ptr(mean_add), _lib.ptr(z), z.shape[1], float(jitter),
+            _lib.ptr(draws), _lib.ptr(info), _lib.ptr(draw_info)))
+        return draws, info, draw_info
+
     # Device handles cannot be pickled.  Like the reference (which pickles its numpy factor, tests/test_pickle.py:21-36:
     # "Unpickled GP shouldn't need to be computed") the Cholesky factor travels with the pickle and is re-uploaded.
     def __getstate__(self):

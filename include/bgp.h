@@ -311,6 +311,38 @@ int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec,
                             double* mean,                                    /* B x ns                       */
                             double* out,                                     /* B x ns, B x ns x ns, or NULL */
                             int32_t* info);
+/* Batched draws (GP.batch_sample_conditional): for the same B members as bgp_dense_batch_predict (spec, params, x,
+ * yerr, r, xs), what bgp_dense_sample draws for each member from its predictive covariance:
+ *   draws[(b*size + a)*ns + j] = mu_b[j] + sum_{i <= j} z[(b*size + a)*ns + i] L_b(j, i)
+ * with mu_b = (K_b(x*, x) K_b^-1 r_b) + mean_add[b*ns + j] (the kernel part of GP.predict's mean plus the mean model at
+ * x*, one IEEE add as the host sums them) and L_b the lower Cholesky factor of sym(C_b) + jitter * I, C_b the member's
+ * BGP_PREDICT_COV output.  mean_add (B x ns), z (B x size x ns, the caller's standard normals) and draws are host
+ * arrays.  Each member's draws are bit-identical to bgp_dense_sample(mean = bgp_kmat_matvec(xs, x, alpha) + mean_add[b])
+ * on a handle computed with member b's spec and yerr: the covariance steps are bgp_dense_batch_predict's, and the
+ * symmetrisation, the factorisation and the product (rows below BGP_SAMPLE_DMMA_ROWS draws, the DMMA GEMM from it with
+ * one descriptor per member, 128 columns and draw slab) are bgp_dense_sample's with a member index.  A member's draws
+ * therefore do not depend on B, its position or the chunking.
+ *   info[b]       as bgp_dense_batch_predict reports it (0, the leading-minor index of K_b, -1 for an invalid program)
+ *   draw_info[b]  0, or the leading-minor index of sym(C_b) + jitter * I (bgp_dense_sample's BGP_ERR_LINALG); 0 where
+ *                 info[b] != 0
+ * A failed member's draws are NaN and do not disturb the other members: its later steps run on its own slabs, and
+ * nothing synchronises inside a chunk.  Members run in chunks that fit in 4 GiB of device memory (BGP_BATCH_CHUNK
+ * overrides it), capped so that the split-K covariance product and the draws' DMMA product are one launch each; every
+ * step of a chunk is one launch for all its members, so the launch count depends on n, ns, size and the number of
+ * chunks, never on B within a chunk.
+ * Device workspace per member (doubles): bgp_dense_batch_predict's with COV, plus 2 size ns + ns (z, the draws, the
+ * mean).  Shared: B programs, x, xs.  The handle keeps it for the next call.
+ * Errors: those of bgp_dense_batch_predict and of bgp_dense_sample's argument checks (BGP_ERR_INVALID for ns < 0,
+ * size < 0, a negative or non-finite jitter).  A member that is not positive definite, in K or in the covariance, is
+ * not an error.  B == 0 writes nothing; ns == 0 or size == 0 factorises (info) and draws nothing (draw_info 0). */
+int bgp_dense_batch_sample(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params,
+                           int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
+                           const double* yerr, const double* r,          /* B x n                      */
+                           const double* xs, int64_t ns,
+                           const double* mean_add,                       /* B x ns: mean model at xs    */
+                           const double* z, int64_t size, double jitter, /* B x size x ns              */
+                           double* draws,                                /* B x size x ns              */
+                           int32_t* info, int32_t* draw_info);
 
 /* ------------------------------------------------------------------------------------------
  * HODLR solver.  Replaces _hodlr.HODLRSolver (src/george/solvers/_hodlr.cpp:115-204) and the
