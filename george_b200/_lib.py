@@ -63,11 +63,15 @@ SIGNATURES = {
     "bgp_kmat_matvec": (C.c_int, [_specp, _p, _i64, _p, _i64, _p, _p, _i64, _p]),
     "bgp_kmat_matvec_dev": (C.c_int, [_specp, _p, _i64, _p, _i64, _p, _p, _i64, _p]),
     "bgp_kmat_gradient_contract": (C.c_int, [_specp, _p, _p, _i64, _p, _p]),
+    "bgp_kmat_x1_gradient_matvec": (C.c_int, [_specp, _p, _i64, _p, _i64, _p, _i64, C.c_double, _i32, _p]),
+    "bgp_kmat_x1_gradient_matvec_dev": (C.c_int, [_specp, _p, _i64, _p, _i64, _p, _i64, C.c_double, _i32, _p]),
     "bgp_dense_grad_terms": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_grad_terms": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_grad_terms_local_dev": (C.c_int, [_p, _p, _p, _p, _p]),
     "bgp_dense_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
     "bgp_hodlr_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),
+    "bgp_dense_predict_grad": (C.c_int, [_p, _specp, _p, _i64, _p, _p]),
+    "bgp_hodlr_predict_grad": (C.c_int, [_p, _specp, _p, _i64, _p, _p]),
     "bgp_hodlr_predict_local_dev": (C.c_int, [_p, _specp, _p, _i64, _i32, _p, _i64, _i32, _p]),
     "bgp_mvn_sample": (C.c_int, [_p, _i64, _p, _p, _i64, C.c_double, _p]),
     "bgp_dense_sample": (C.c_int, [_p, _specp, _p, _i64, _p, _p, _i64, C.c_double, _p]),

@@ -52,6 +52,9 @@ void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, in
 int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn,
                              int64_t K, bool lower, double* C, int64_t ldc, int members, int64_t abstride,
                              int64_t cstride, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
+int kmat_x1_grad_matvec_launch(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1,
+                               const double* x2, int64_t n2, const double* V, int64_t ldv, double scale, int add_prior,
+                               double* out, DevBuf<double>& scratch, cudaStream_t s);
 int predict_var_launch(const double* B, int64_t ldb, const double* W, int64_t ldw, int64_t n, int64_t c,
                        const double* kdiag, double* var, DevBuf<double>& scratch, cudaStream_t s);
 int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
@@ -635,10 +638,10 @@ static int trsm_fwd_members(const double* L, int64_t n, int64_t lstride, double*
 // member and zero strides.  Up to DS_MAX_RHS right-hand sides go through the one-launch step kernels with the scratch Y
 // (members blocks of xstride >= n * nrhs doubles); more through the forward sweep of trsm_fwd_members and the
 // backward sweep below.
-static int potrs_members(const double* L, int64_t n, int64_t lstride, double* X, int64_t nrhs, int64_t ldx,
-                         int64_t xstride, int members, double* Y, cudaStream_t s) {
-  if (nrhs <= DS_MAX_RHS) return potrs_small_members(L, n, X, (int)nrhs, ldx, Y, members, lstride, xstride, s);
-  BGP_TRY(trsm_fwd_members(L, n, lstride, X, nrhs, ldx, xstride, members, nullptr, 0, s));  // forward: L y = b
+// X (n x nrhs, column-major ldx) <- L^-T X in place, block by block from the bottom: the backward half of
+// potrs_members for more than DS_MAX_RHS right-hand sides (any nrhs works).  Member m: L + m * lstride, X + m * xstride.
+static int trsm_bwd_block_members(const double* L, int64_t n, int64_t lstride, double* X, int64_t nrhs, int64_t ldx,
+                                  int64_t xstride, int members, cudaStream_t s) {
   const unsigned mb = (unsigned)members;
   const unsigned cb = (unsigned)((nrhs + 127) / 128);
   const int64_t last = ((n - 1) / DN_NB) * DN_NB;
@@ -656,6 +659,13 @@ static int potrs_members(const double* L, int64_t n, int64_t lstride, double* X,
   return BGP_OK;
 }
 
+static int potrs_members(const double* L, int64_t n, int64_t lstride, double* X, int64_t nrhs, int64_t ldx,
+                         int64_t xstride, int members, double* Y, cudaStream_t s) {
+  if (nrhs <= DS_MAX_RHS) return potrs_small_members(L, n, X, (int)nrhs, ldx, Y, members, lstride, xstride, s);
+  BGP_TRY(trsm_fwd_members(L, n, lstride, X, nrhs, ldx, xstride, members, nullptr, 0, s));  // forward: L y = b
+  return trsm_bwd_block_members(L, n, lstride, X, nrhs, ldx, xstride, members, s);
+}
+
 static int dense_potrs_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
   if (nrhs <= DS_MAX_RHS) BGP_TRY(h->d_tmp.reserve((size_t)h->n * DS_MAX_RHS, h->s));
   return potrs_members(h->d_A.p, h->n, 0, X, nrhs, ldx, 0, 1, h->d_tmp.p, h->s);
@@ -664,6 +674,32 @@ static int dense_potrs_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
 static int dense_trsm_fwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
   if (nrhs <= DS_MAX_RHS) BGP_TRY(h->d_tmp.reserve((size_t)h->n * DS_MAX_RHS, h->s));
   return trsm_fwd_members(h->d_A.p, h->n, 0, X, nrhs, ldx, 0, 1, h->d_tmp.p, h->n, h->s);
+}
+
+// X (n x nrhs, column-major ldx) <- L^-T X: the backward half of dense_potrs_dev, so that dense_trsm_fwd_dev followed by
+// this is K^-1.  Few right-hand sides go through the one-launch step kernels of potrs_small_members, which read the
+// forward result from a copy in d_tmp; more through trsm_bwd_block_members.
+static int dense_trsm_bwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
+  const int64_t n = h->n;
+  cudaStream_t s = h->s;
+  if (nrhs > DS_MAX_RHS) return trsm_bwd_block_members(h->d_A.p, n, 0, X, nrhs, ldx, 0, 1, s);
+  BGP_TRY(h->d_tmp.reserve((size_t)n * DS_MAX_RHS, s));
+  double* Y = h->d_tmp.p;
+  BGP_CUDA(cudaMemcpy2DAsync(Y, sizeof(double) * n, X, sizeof(double) * ldx, sizeof(double) * n, nrhs,
+                             cudaMemcpyDeviceToDevice, s));
+  cudaFuncSetAttribute(trsv_bwd_step_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_BWD_SMEM);
+  cudaFuncSetAttribute(trsv_bwd_step_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_BWD_SMEM);
+  cudaFuncSetAttribute(trsv_bwd_step_kernel<DS_MAX_RHS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_BWD_SMEM);
+  const int nr = (int)nrhs;
+  for (int64_t k0 = ((n - 1) / DN_NB) * DN_NB; k0 >= 0; k0 -= DN_NB) {
+    const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
+    const dim3 g((unsigned)std::max<int64_t>(1, (k0 + DS_COLS - 1) / DS_COLS), 1);
+    if (nr == 1) trsv_bwd_step_kernel<1><<<g, 256, DS_BWD_SMEM, s>>>(h->d_A.p, n, k0, nb, Y, n, X, ldx, nr, 0, 0);
+    else if (nr <= 4) trsv_bwd_step_kernel<4><<<g, 256, DS_BWD_SMEM, s>>>(h->d_A.p, n, k0, nb, Y, n, X, ldx, nr, 0, 0);
+    else trsv_bwd_step_kernel<DS_MAX_RHS><<<g, 256, DS_BWD_SMEM, s>>>(h->d_A.p, n, k0, nb, Y, n, X, ldx, nr, 0, 0);
+    BGP_LAUNCH_CHECK();
+  }
+  return BGP_OK;
 }
 
 // GP.predict's covariance at the ns test points xs (host) into dC (ns x ns on the device, allocated here): every W chunk
@@ -904,6 +940,48 @@ int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const doubl
   } else {
     BGP_TRY(dense_predict_cov_dev(h, P, xs, ns, dC));
     BGP_CUDA(cudaMemcpyAsync(out, dC.p, sizeof(double) * ns * ns, cudaMemcpyDeviceToHost, s));
+  }
+  BGP_CUDA(cudaStreamSynchronize(s));
+  return BGP_OK;
+}
+
+// GP.grad_predict's var and dvar: bgp_dense_predict's VAR chunks, then per chunk W <- L^-T W (= K^-1 K(x, x*_chunk))
+// in place and dvar = dprior - 2 sum_j d1 k(x*, x_j) W_j (kmat_x1_grad_matvec_launch)
+int bgp_dense_predict_grad(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, double* var,
+                           double* dvar) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (!h->has_inputs) { set_error("the factor was imported: the handle holds no kernel/coordinates"); return BGP_ERR_NOT_COMPUTED; }
+  if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
+  DevProgram P;
+  BGP_TRY(build_dev_program(spec, &P));
+  if (P.ndim != h->ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", P.ndim, h->ndim); return BGP_ERR_DIM; }
+  if (P.ndim > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, P.ndim); return BGP_ERR_INVALID; }
+  if (ns == 0) return BGP_OK;
+  const int64_t n = h->n;
+  const int nd = h->ndim;
+  cudaStream_t s = h->s;
+  DevBuf<DevProgram> dprog;
+  DevBuf<double> dxs, dW, dkd, dvar_c, ddvar, scratch;
+  BGP_TRY(upload_program(P, dprog, s));
+  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
+  // workspace n*c + O(c * ndim): bgp_dense_predict's VAR workspace plus the chunk's dvar
+  BGP_TRY(dxs.alloc((size_t)c * nd, s));
+  BGP_TRY(dW.alloc((size_t)n * c, s));
+  BGP_TRY(dkd.alloc((size_t)c, s));
+  BGP_TRY(dvar_c.alloc((size_t)c, s));
+  BGP_TRY(ddvar.alloc((size_t)c * nd, s));
+  for (int64_t j0 = 0; j0 < ns; j0 += c) {
+    const int64_t nc = std::min(c, ns - j0);
+    // the steps of bgp_dense_predict's VAR loop
+    BGP_CUDA(cudaMemcpyAsync(dxs.p, xs + j0 * nd, sizeof(double) * nc * nd, cudaMemcpyHostToDevice, s));
+    BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p, nc, h->d_x.p, n, dW.p, n, s));
+    BGP_TRY(dense_trsm_fwd_dev(h, dW.p, nc, n));
+    BGP_TRY(kmat_diagonal_launch(dprog.p, dxs.p, dxs.p, nc, dkd.p, s));
+    BGP_TRY(predict_var_launch(dW.p, n, dW.p, n, n, nc, dkd.p, dvar_c.p, scratch, s));
+    BGP_CUDA(cudaMemcpyAsync(var + j0, dvar_c.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));
+    BGP_TRY(dense_trsm_bwd_dev(h, dW.p, nc, n));
+    BGP_TRY(kmat_x1_grad_matvec_launch(P, dprog.p, dxs.p, nc, h->d_x.p, n, dW.p, n, -2.0, 1, ddvar.p, scratch, s));
+    BGP_CUDA(cudaMemcpyAsync(dvar + j0 * nd, ddvar.p, sizeof(double) * nc * nd, cudaMemcpyDeviceToHost, s));
   }
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;

@@ -44,6 +44,9 @@ int64_t predict_chunk_cols(int64_t n, int64_t multiple);
 int64_t predict_var_partial_size(int64_t n, int64_t c);
 int predict_var_launch(const double* B, int64_t ldb, const double* W, int64_t ldw, int64_t n, int64_t c,
                        const double* kdiag, double* var, DevBuf<double>& scratch, cudaStream_t s);
+int kmat_x1_grad_matvec_launch(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1,
+                               const double* x2, int64_t n2, const double* V, int64_t ldv, double scale, int add_prior,
+                               double* out, DevBuf<double>& scratch, cudaStream_t s);
 void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, int64_t* klen_out);
 int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
                      bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
@@ -1684,6 +1687,49 @@ int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
   } else {
     BGP_TRY(hodlr_predict_cov_dev(h, P, xs, ns, dC));
     BGP_CUDA(cudaMemcpyAsync(out, dC.p, sizeof(double) * ns * ns, cudaMemcpyDeviceToHost, s));
+  }
+  BGP_CUDA(cudaStreamSynchronize(s));
+  return BGP_OK;
+}
+
+// GP.grad_predict's var and dvar: bgp_hodlr_predict's VAR chunks, whose W is already K_h^-1 K(x, x*_chunk), then
+// dvar = dprior - 2 sum_j d1 k(x*, x_j) W_j (kmat_x1_grad_matvec_launch).  Unsharded handles only.
+int bgp_hodlr_predict_grad(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, double* var,
+                           double* dvar) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (host_exchange(h) || h->opts.shard_count > 1) { set_error("predict_grad is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
+  DevProgram P;
+  BGP_TRY(build_dev_program(spec, &P));
+  if (P.ndim != h->ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", P.ndim, h->ndim); return BGP_ERR_DIM; }
+  if (P.ndim > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, P.ndim); return BGP_ERR_INVALID; }
+  if (ns == 0) return BGP_OK;
+  const int64_t n = h->n;
+  const int nd = h->ndim;
+  cudaStream_t s = h->sA;
+  DevBuf<DevProgram> dprog;
+  DevBuf<double> dxs, dB, dW, dkd, dvar_c, ddvar, scratch;
+  BGP_TRY(upload_program(P, dprog, s));
+  const int64_t c = std::min(ns, predict_chunk_cols(n, 64));
+  // workspace 2*n*c + O(c * ndim): bgp_hodlr_predict's VAR workspace plus the chunk's dvar
+  BGP_TRY(dW.alloc((size_t)n * c, s));
+  BGP_TRY(dxs.alloc((size_t)c * nd, s));
+  BGP_TRY(dB.alloc((size_t)n * c, s));
+  BGP_TRY(dkd.alloc((size_t)c, s));
+  BGP_TRY(dvar_c.alloc((size_t)c, s));
+  BGP_TRY(ddvar.alloc((size_t)c * nd, s));
+  for (int64_t j0 = 0; j0 < ns; j0 += c) {
+    const int64_t nc = std::min(c, ns - j0);
+    // the steps of bgp_hodlr_predict's VAR loop
+    BGP_CUDA(cudaMemcpyAsync(dxs.p, xs + j0 * nd, sizeof(double) * nc * nd, cudaMemcpyHostToDevice, s));
+    BGP_TRY(kmat_general_launch_auto(P, dprog.p, dxs.p, nc, h->d_x.p, n, dB.p, n, s));
+    BGP_CUDA(cudaMemcpyAsync(dW.p, dB.p, sizeof(double) * n * nc, cudaMemcpyDeviceToDevice, s));
+    BGP_TRY(hodlr_solve_dev(h, dW.p, nc, n, s, 0));
+    BGP_TRY(kmat_diagonal_launch(dprog.p, dxs.p, dxs.p, nc, dkd.p, s));
+    BGP_TRY(predict_var_launch(dB.p, n, dW.p, n, n, nc, dkd.p, dvar_c.p, scratch, s));
+    BGP_CUDA(cudaMemcpyAsync(var + j0, dvar_c.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));
+    BGP_TRY(kmat_x1_grad_matvec_launch(P, dprog.p, dxs.p, nc, h->d_x.p, n, dW.p, n, -2.0, 1, ddvar.p, scratch, s));
+    BGP_CUDA(cudaMemcpyAsync(dvar + j0 * nd, ddvar.p, sizeof(double) * nc * nd, cudaMemcpyDeviceToHost, s));
   }
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;

@@ -10,6 +10,9 @@
 //                             formed.
 //   predict_var_* / predict_gemm_sub  GP.predict's variance and covariance from K(x, x*) and K^-1 K(x, x*) chunks
 //                            that the solvers stream (dense.cu, hodlr.cu; reference gp.py:534-545).
+//   kmat_x1_grad_matvec_kernel  out_i = sum_j dk(x1_i, x2_j)/dx1_i V_ji  -> GP.grad_predict's dmu (V = alpha, shared)
+//                            and dvar (V = K^-1 K(x, x*), one column per test point); the (n1, n2, ndim) gradient
+//                            tensor is never formed.
 //
 // Roofline: matvec is FP64-ALU bound (one covariance evaluation per (i, j), no HBM traffic beyond x and V);
 // the contraction reads A once -> HBM bound at 8 B per pair for cheap kernels, FP64 bound for the gradient of
@@ -225,6 +228,158 @@ int kmat_matvec_batch_launch(const DevProgram* dprogs, int nd, int members, cons
   const int blocks = (int)std::min<int64_t>((n1 + 255) / 256, 8 * (int64_t)num_sms());
   kmat_matvec_reduce_kernel<<<dim3(blocks, members), 256, 0, s>>>(partial, n1, (int)nsplit, 1, nullptr, V, n2, out, n1,
                                                                   pstride, vstride, ostride);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Input-gradient contraction (GP.grad_predict):
+//     out[i*nd + q] = (add_prior ? d k(x1_i, x1_i) / d x1_iq : 0) + scale * sum_j d k(x1_i, x2_j) / d x1_iq * V_ji
+// V_ji = V[j] (ldv == 0: one vector shared by every i, the mean's alpha) or V[i*ldv + j] (column i of an n2 x n1
+// column-major matrix, the variance's W = K^-1 K(x, x*)).  The prior term d k(x, x)/dx = (d1 + d2) k(x, x) is taken as
+// 2 d1 k(x, x), every kernel being symmetric; it is 0 for stationary leaves.
+// Tiles of XG_TI test points against staged XG_TJ-point chunks of x2, as the matvec; the chunks are split over
+// blockIdx.y when there are few test points.  One warp takes one test point at a time with its lanes along j, so W is
+// read coalesced (8 * n2 * n1 bytes in all, the kernel's only large HBM traffic).  Each warp's sum over a chunk goes to
+// a per-point accumulator in shared memory owned by that warp; per-CTA partials are summed over the splits in a fixed
+// order by x1_grad_reduce_kernel.  No atomics: identical calls give identical bits.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int XG_TI = 32;
+constexpr int XG_TJ = 512;
+constexpr int XG_THREADS = 256;
+constexpr int XG_WARPS = XG_THREADS / 32;
+
+static size_t x1_grad_smem(int nd) {
+  return ((sizeof(DevProgram) + 15) & ~size_t(15)) +
+         sizeof(double) * ((size_t)XG_TI * nd + (size_t)XG_TJ * nd + XG_TJ + (size_t)XG_TI * nd);
+}
+
+// partial[(split * n1 + i) * nd + q] = sum_{j in split's chunks} d k(x1_i, x2_j) / d x1_iq V_ji
+template <int SHAPE>
+__global__ void __launch_bounds__(XG_THREADS) kmat_x1_grad_matvec_kernel(const DevProgram* __restrict__ gprog,
+                                                                         const double* __restrict__ x1, int64_t n1,
+                                                                         const double* __restrict__ x2, int64_t n2,
+                                                                         const double* __restrict__ V, int64_t ldv,
+                                                                         double* __restrict__ partial,
+                                                                         int chunks_per_split) {
+  using Eval = X1GradEval<SHAPE>;
+  constexpr int NDMAX = Eval::type::NDMAX;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  DevProgram* prog = reinterpret_cast<DevProgram*>(smem_raw);
+  const int nd = gprog->ndim;
+  double* sx1 = reinterpret_cast<double*>(smem_raw + ((sizeof(DevProgram) + 15) & ~size_t(15)));
+  double* sx2 = sx1 + XG_TI * nd;
+  double* sv = sx2 + XG_TJ * nd;  // the chunk of V (ldv == 0)
+  double* sacc = sv + XG_TJ;      // XG_TI x nd: per-point sums, point p owned by warp p % XG_WARPS
+  stage_program(prog, gprog);
+  const int64_t i0 = (int64_t)blockIdx.x * XG_TI;
+  const int ni = (int)min((int64_t)XG_TI, n1 - i0);
+  for (int t = threadIdx.x; t < ni * nd; t += XG_THREADS) sx1[t] = x1[i0 * nd + t];
+  for (int t = threadIdx.x; t < XG_TI * nd; t += XG_THREADS) sacc[t] = 0.0;
+  __syncthreads();
+  const typename Eval::type fn = Eval::make(prog);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+
+  const int64_t nchunks = (n2 + XG_TJ - 1) / XG_TJ;
+  const int64_t c_begin = (int64_t)blockIdx.y * chunks_per_split;
+  const int64_t c_end = min(nchunks, c_begin + chunks_per_split);
+  for (int64_t ch = c_begin; ch < c_end; ++ch) {
+    const int64_t j0 = ch * XG_TJ;
+    const int nj = (int)min((int64_t)XG_TJ, n2 - j0);
+    __syncthreads();  // previous iteration's readers are done with sx2 / sv
+    for (int t = threadIdx.x; t < nj * nd; t += XG_THREADS) sx2[t] = x2[j0 * nd + t];
+    if (ldv == 0)
+      for (int t = threadIdx.x; t < nj; t += XG_THREADS) sv[t] = V[j0 + t];
+    __syncthreads();
+    for (int p = warp; p < ni; p += XG_WARPS) {
+      const double* xi = sx1 + p * nd;
+      const double* w = V + (i0 + p) * ldv + j0;
+      double acc[NDMAX];
+#pragma unroll
+      for (int q = 0; q < NDMAX; ++q) acc[q] = 0.0;
+      for (int j = lane; j < nj; j += 32) {
+        const double v = ldv ? w[j] : sv[j];
+        double g[NDMAX];
+        fn(xi, sx2 + j * nd, g);
+#pragma unroll
+        for (int q = 0; q < NDMAX; ++q)
+          if (q < nd) acc[q] = fma(g[q], v, acc[q]);
+      }
+#pragma unroll
+      for (int q = 0; q < NDMAX; ++q) {
+        if (q < nd) {  // uniform across the warp
+          const double s = warp_sum(acc[q]);
+          if (lane == 0) sacc[p * nd + q] += s;
+        }
+      }
+    }
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < ni * nd; t += XG_THREADS) partial[((int64_t)blockIdx.y * n1 + i0) * nd + t] = sacc[t];
+}
+
+// out[i*nd + q] = (add_prior ? 2 d1 k(x1_i, x1_i)_q : 0) + scale * sum_s partial[(s*n1 + i)*nd + q], s ascending
+__global__ void x1_grad_reduce_kernel(const DevProgram* __restrict__ gprog, const double* __restrict__ x1, int64_t n1,
+                                      const double* __restrict__ partial, int64_t nsplit, double scale, int add_prior,
+                                      double* __restrict__ out) {
+  const int nd = gprog->ndim;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n1; i += (int64_t)gridDim.x * blockDim.x) {
+    double g[BGP_MAX_DIM];
+    if (add_prior) kernel_x_gradient<true>(*gprog, 1, x1 + i * nd, x1 + i * nd, g);
+    for (int q = 0; q < nd; ++q) {
+      double s = 0.0;
+      for (int64_t sp = 0; sp < nsplit; ++sp) s += partial[(sp * n1 + i) * nd + q];
+      s = scale * s;
+      out[i * nd + q] = add_prior ? 2.0 * g[q] + s : s;
+    }
+  }
+}
+
+// the column split of one contraction: nsplit groups of cps XG_TJ-point chunks (~8 CTAs per SM, as matvec_plan)
+static int x1_grad_plan(int64_t n1, int64_t n2, int64_t* nsplit_out, int* cps_out) {
+  const int64_t row_tiles = (n1 + XG_TI - 1) / XG_TI;
+  const int64_t nchunks = (n2 + XG_TJ - 1) / XG_TJ;
+  int64_t nsplit = std::max<int64_t>(1, std::min<int64_t>(nchunks, (8 * (int64_t)num_sms() + row_tiles - 1) / row_tiles));
+  const int cps = (int)std::max<int64_t>(1, (nchunks + nsplit - 1) / nsplit);
+  nsplit = nchunks > 0 ? (nchunks + cps - 1) / cps : 0;
+  if (row_tiles > 0x7fffffffLL || nsplit > 65535) { set_error("kmat_x1_gradient_matvec: problem too large for one launch"); return BGP_ERR_INVALID; }
+  *nsplit_out = nsplit;
+  *cps_out = cps;
+  return BGP_OK;
+}
+
+// out (n1 x nd, row-major) as described above; P is the validated program behind dprog (its shape selects the
+// evaluator), x1 / x2 / V / out device pointers.  scratch: the partials (nsplit * n1 * nd doubles).
+int kmat_x1_grad_matvec_launch(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1,
+                               const double* x2, int64_t n2, const double* V, int64_t ldv, double scale, int add_prior,
+                               double* out, DevBuf<double>& scratch, cudaStream_t s) {
+  const int nd = P.ndim;
+  if (nd > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, nd); return BGP_ERR_INVALID; }
+  if (n1 <= 0) return BGP_OK;
+  int64_t nsplit;
+  int cps;
+  BGP_TRY(x1_grad_plan(n1, n2, &nsplit, &cps));
+  if (nsplit > 0) {
+    BGP_TRY(scratch.reserve((size_t)(nsplit * n1 * nd), s));
+    const size_t smem = x1_grad_smem(nd);
+    const dim3 grid((unsigned)((n1 + XG_TI - 1) / XG_TI), (unsigned)nsplit);
+#define BGP_X1G_LAUNCH(SH)                                                                                   \
+  {                                                                                                         \
+    cudaFuncSetAttribute(kmat_x1_grad_matvec_kernel<SH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+    kmat_x1_grad_matvec_kernel<SH><<<grid, XG_THREADS, smem, s>>>(dprog, x1, n1, x2, n2, V, ldv, scratch.p, cps);  \
+  }
+    switch (P.shape) {
+      case BGP_SHAPE_EXPSQ: BGP_X1G_LAUNCH(BGP_SHAPE_EXPSQ); break;
+      case BGP_SHAPE_M32: BGP_X1G_LAUNCH(BGP_SHAPE_M32); break;
+      case BGP_SHAPE_M52: BGP_X1G_LAUNCH(BGP_SHAPE_M52); break;
+      case BGP_SHAPE_EXP: BGP_X1G_LAUNCH(BGP_SHAPE_EXP); break;
+      default: BGP_X1G_LAUNCH(BGP_SHAPE_GENERIC); break;
+    }
+#undef BGP_X1G_LAUNCH
+    BGP_LAUNCH_CHECK();
+  }
+  const int blocks = (int)std::min<int64_t>((n1 + 127) / 128, 8 * (int64_t)num_sms());
+  x1_grad_reduce_kernel<<<blocks, 128, 0, s>>>(dprog, x1, n1, scratch.p, nsplit, scale, add_prior, out);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
@@ -763,6 +918,54 @@ int bgp_kmat_matvec_dev(const bgp_kernel_spec_t* spec, const double* x1_dev, int
   DevBuf<double> scratch;
   BGP_TRY(upload_program(P, dprog, 0));
   BGP_TRY(kmat_matvec_launch(dprog.p, P.ndim, x1_dev, n1, x2_dev, n2, diag_dev, v_dev, n2, nrhs, out_dev, n1, scratch, 0));
+  BGP_CUDA(cudaStreamSynchronize(0));
+  return BGP_OK;
+}
+
+static int x1_gradient_matvec_args(const DevProgram& P, int64_t n1, int64_t n2, int64_t ldv) {
+  if (n1 < 0 || n2 < 0) { set_error("negative size"); return BGP_ERR_INVALID; }
+  if (ldv != 0 && ldv < n2) { set_error("dimension mismatch: ldv %lld is neither 0 nor >= n2 %lld", (long long)ldv, (long long)n2); return BGP_ERR_DIM; }
+  if (P.ndim > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, P.ndim); return BGP_ERR_INVALID; }
+  return BGP_OK;
+}
+
+int bgp_kmat_x1_gradient_matvec(const bgp_kernel_spec_t* spec, const double* x1, int64_t n1, const double* x2,
+                                int64_t n2, const double* v, int64_t ldv, double scale, int32_t add_prior, double* out) {
+  BGP_TRY(require_device());
+  DevProgram P;
+  BGP_TRY(build_dev_program(spec, &P));
+  BGP_TRY(x1_gradient_matvec_args(P, n1, n2, ldv));
+  if (n1 == 0) return BGP_OK;
+  cudaStream_t s = 0;
+  const int nd = P.ndim;
+  const int64_t nv = ldv == 0 ? n2 : ldv * (n1 - 1) + n2;
+  DevBuf<DevProgram> dprog;
+  DevBuf<double> dx1, dx2, dv, dout, scratch;
+  BGP_TRY(upload_program(P, dprog, s));
+  BGP_TRY(dx1.alloc((size_t)n1 * nd, s));
+  BGP_CUDA(cudaMemcpyAsync(dx1.p, x1, sizeof(double) * n1 * nd, cudaMemcpyHostToDevice, s));
+  BGP_TRY(dx2.alloc((size_t)std::max<int64_t>(n2, 1) * nd, s));
+  if (n2) BGP_CUDA(cudaMemcpyAsync(dx2.p, x2, sizeof(double) * n2 * nd, cudaMemcpyHostToDevice, s));
+  BGP_TRY(dv.alloc((size_t)std::max<int64_t>(nv, 1), s));
+  if (nv) BGP_CUDA(cudaMemcpyAsync(dv.p, v, sizeof(double) * nv, cudaMemcpyHostToDevice, s));
+  BGP_TRY(dout.alloc((size_t)n1 * nd, s));
+  BGP_TRY(kmat_x1_grad_matvec_launch(P, dprog.p, dx1.p, n1, dx2.p, n2, dv.p, ldv, scale, add_prior, dout.p, scratch, s));
+  BGP_CUDA(cudaMemcpyAsync(out, dout.p, sizeof(double) * n1 * nd, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  return BGP_OK;
+}
+
+int bgp_kmat_x1_gradient_matvec_dev(const bgp_kernel_spec_t* spec, const double* x1_dev, int64_t n1,
+                                    const double* x2_dev, int64_t n2, const double* v_dev, int64_t ldv, double scale,
+                                    int32_t add_prior, double* out_dev) {
+  BGP_TRY(require_device());
+  DevProgram P;
+  BGP_TRY(build_dev_program(spec, &P));
+  BGP_TRY(x1_gradient_matvec_args(P, n1, n2, ldv));
+  DevBuf<DevProgram> dprog;
+  DevBuf<double> scratch;
+  BGP_TRY(upload_program(P, dprog, 0));
+  BGP_TRY(kmat_x1_grad_matvec_launch(P, dprog.p, x1_dev, n1, x2_dev, n2, v_dev, ldv, scale, add_prior, out_dev, scratch, 0));
   BGP_CUDA(cudaStreamSynchronize(0));
   return BGP_OK;
 }

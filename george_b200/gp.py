@@ -16,7 +16,7 @@ import numpy as np
 from numpy.linalg import LinAlgError
 
 from . import _lib, kernels
-from ._spec import flatten, num_params, patch_specs
+from ._spec import BGP_MAX_DIM, flatten, num_params, patch_specs
 from .modeling import ConstantModel, ModelSet
 from .solvers import BasicSolver, TrivialSolver
 from .solvers.basic import NONFINITE_RHS
@@ -730,12 +730,61 @@ class GP(ModelSet):
 
         KinvKxs = self.solver.apply_inverse(Kxs.T)
         if return_var:
-            var = kernel.get_value(xs, diag=True)
-            var -= np.sum(Kxs.T * KinvKxs, axis=0)
-            return mu, var
+            return mu, self._host_var(Kxs, KinvKxs, xs, kernel)
         cov = kernel.get_value(xs)
         cov -= np.dot(Kxs, KinvKxs)
         return mu, cov
+
+    @staticmethod
+    def _host_var(Kxs, KinvKxs, xs, kernel):
+        var = kernel.get_value(xs, diag=True)
+        var -= np.sum(Kxs.T * KinvKxs, axis=0)
+        return var
+
+    def grad_predict(self, y, t, return_var=False, cache=True, kernel=None):
+        """The predictive mean (and variance) at ``t`` with their gradients with respect to the test points:
+        ``(mu, dmu)``, or ``(mu, var, dmu, dvar)`` with ``return_var``.  ``mu`` and ``var`` (``(ns,)``) are bit for bit
+        what :func:`predict` returns with ``return_cov=False`` / ``return_var=True`` and the same ``cache`` and
+        ``kernel``; ``dmu[i, q] = d mu_i / d t_iq`` and ``dvar[i, q] = d var_i / d t_iq`` (``(ns, ndim)``, also for a
+        1-D ``t``).  Each output depends on its own test point only, so this is the whole Jacobian: what an optimiser
+        of an acquisition function (``mu + kappa * sqrt(var)``, expected improvement) needs per step.
+
+        With ``B = K(x, t)`` and ``W = K^-1 B``: ``dmu_i = sum_j d1 k(t_i, x_j) alpha_j`` and ``dvar_i = d k(t_i, t_i)
+        / d t_i - 2 sum_j d1 k(t_i, x_j) W_ji``, the true derivatives for every metric (:func:`Kernel.get_x1_gradient`
+        keeps the reference's values, which differ for a general metric).  The contractions run on the device without
+        the ``(ns, N, ndim)`` gradient tensor; ``BasicSolver`` and ``HODLRSolver`` stream ``var`` and ``dvar`` through
+        the stored factorisation (``predictive_grad``), every other solver (``TrivialSolver``, ``ShardedHODLRSolver``,
+        a pickled dense solver, plug-ins) contracts the ``solver.apply_inverse(B)`` of :func:`predict`'s host route.
+
+        A ``ConstantModel`` mean adds nothing to ``dmu``; any other mean model raises ``NotImplementedError`` (the
+        modeling protocol has no input gradient).  Inputs of more than 8 dimensions raise ``ValueError``.
+        """
+        if type(self.mean) is not ConstantModel:
+            raise NotImplementedError("grad_predict needs the mean model's gradient with respect to the inputs, which "
+                                      "the modeling protocol does not provide; only a constant mean is supported")
+        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
+            raise RuntimeError("You need to compute the model first")
+        xs = self.parse_samples(t)
+        if xs.shape[1] > BGP_MAX_DIM:
+            raise ValueError("input-coordinate gradients support at most {0} dimensions (got {1})".format(
+                BGP_MAX_DIM, xs.shape[1]))
+        self.recompute()
+        alpha = self._compute_alpha(y, cache)
+        if kernel is None:
+            kernel = self.kernel
+        mu = self._predict_mean(alpha, xs, kernel)
+        dmu = kernel.kernel.x1_gradient_matvec(xs, self._x, alpha)
+        if not return_var:
+            return mu, dmu
+        hook = getattr(self.solver, "predictive_grad", None)
+        out = hook(kernel, xs) if hook is not None else None
+        if out is None:
+            Kxs = kernel.get_value(xs, self._x)
+            KinvKxs = self.solver.apply_inverse(Kxs.T)
+            out = (self._host_var(Kxs, KinvKxs, xs, kernel),
+                   kernel.kernel.x1_gradient_matvec(xs, self._x, KinvKxs, scale=-2.0, add_prior=True))
+        var, dvar = out
+        return mu, var, dmu, dvar
 
     def sample_conditional(self, y, t, size=1, *, rng=None, jitter=None):
         """Draws from the conditional predictive distribution at ``t``: shape ``(ns,)`` when ``size == 1``, else

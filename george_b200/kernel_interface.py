@@ -135,6 +135,27 @@ class KernelInterface(object):
                                                           _lib.ptr(A), _lib.ptr(out)))
         return out
 
+    def x1_gradient_matvec(self, x1, x2, v, scale=1.0, add_prior=False):
+        """``out[i, q] = (add_prior ? d k(x1_i, x1_i) / d x1_iq : 0) + scale * sum_j d k(x1_i, x2_j) / d x1_iq V_ji``
+        (``(n1, ndim)``) without the ``(n1, n2, ndim)`` gradient tensor, ``V_ji = v[j]`` for ``v`` of shape ``(n2,)`` and
+        ``v[j, i]`` for ``(n2, n1)``: ``GP.grad_predict``'s ``dmu`` (``v = alpha``) and, with ``scale=-2`` and
+        ``add_prior``, its ``dvar`` (``v = K^-1 K(x, x1)``).  True derivatives for every metric, where
+        :func:`x1_gradient_general` returns the reference's values (include/bgp.h: bgp_kmat_x1_gradient_matvec)."""
+        x1, x2 = _as2d(x1, self.ndim), _as2d(x2, self.ndim)
+        v = np.asarray(v, dtype=np.float64)
+        n1, n2 = x1.shape[0], x2.shape[0]
+        if v.shape == (n2,):
+            v, ldv = np.ascontiguousarray(v), 0
+        elif v.shape == (n2, n1):
+            v, ldv = np.asfortranarray(v), n2
+        else:
+            raise DimensionMismatch("dimension mismatch")
+        out = np.empty((n1, self.ndim), dtype=np.float64)
+        _lib.check(_lib.load().bgp_kmat_x1_gradient_matvec(C.byref(self._spec), _lib.ptr(x1), n1, _lib.ptr(x2), n2,
+                                                           _lib.ptr(v), ldv, float(scale), 1 if add_prior else 0,
+                                                           _lib.ptr(out)))
+        return out
+
     def _x_gradient(self, fn, x1, x2):
         x1, x2 = _as2d(x1, self.ndim), _as2d(x2, self.ndim)
         out = np.empty((x1.shape[0], x2.shape[0], self.ndim), dtype=np.float64)

@@ -217,6 +217,30 @@ class BasicSolver(object):
         _lib.check(fn(ptr, C.byref(spec), _lib.ptr(xs), ns, kinds[what], _lib.ptr(out)))
         return out
 
+    def predictive_grad(self, kernel, xs):
+        """``(var, dvar)`` for ``GP.grad_predict``: ``var`` (``(ns,)``) is bit for bit :func:`predictive`'s variance
+        and ``dvar[j, q] = d var_j / d xs_jq`` (``(ns, ndim)``), both computed on the device from the stored factor
+        (``include/bgp.h: bgp_dense_predict_grad``).  Returns ``None`` for a solver restored from a pickle (it holds no
+        coordinates): the caller then takes the host path."""
+        self._require()
+        if not getattr(self, "_has_inputs", True):
+            return None
+        return self._predictive_grad_call(self._handle.lib.bgp_dense_predict_grad, self._handle.ptr, kernel, xs)
+
+    @staticmethod
+    def _predictive_grad_call(fn, ptr, kernel, xs):
+        xs = np.ascontiguousarray(xs, dtype=np.float64)
+        if xs.ndim == 1:
+            xs = xs[:, None]
+        spec = flatten(kernel)
+        if xs.ndim != 2 or xs.shape[1] != spec.ndim:
+            raise DimensionMismatch("dimension mismatch")
+        ns = xs.shape[0]
+        var = np.empty(ns, dtype=np.float64)
+        dvar = np.empty((ns, spec.ndim), dtype=np.float64)
+        _lib.check(fn(ptr, C.byref(spec), _lib.ptr(xs), ns, _lib.ptr(var), _lib.ptr(dvar)))
+        return var, dvar
+
     def sample_predictive(self, kernel, xs, mean, z, jitter):
         """``mean + z @ L.T`` (``(size, ns)``) with ``L`` the lower Cholesky factor of ``sym(C) + jitter * I``, ``C``
         the covariance :func:`predictive` returns for ``kernel`` at ``xs``: ``GP.sample_conditional``'s draws, with

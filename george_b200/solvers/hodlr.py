@@ -70,6 +70,14 @@ class HODLRSolver(BasicSolver):
             return None
         return self._predictive_call(self.solver._lib.bgp_hodlr_predict, self.solver._ptr, kernel, xs, what)
 
+    def predictive_grad(self, kernel, xs):
+        """``BasicSolver.predictive_grad`` on the HODLR factorisation (``include/bgp.h: bgp_hodlr_predict_grad``);
+        ``None`` on a sharded factorisation."""
+        self._require()
+        if self.solver.shard_count > 1:
+            return None
+        return self._predictive_grad_call(self.solver._lib.bgp_hodlr_predict_grad, self.solver._ptr, kernel, xs)
+
     def sample_predictive(self, kernel, xs, mean, z, jitter):
         """``BasicSolver.sample_predictive`` on the HODLR factorisation (``include/bgp.h: bgp_hodlr_sample``); ``None``
         on a sharded factorisation."""

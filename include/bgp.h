@@ -169,6 +169,22 @@ int bgp_kmat_matvec_dev(const bgp_kernel_spec_t* spec, const double* x1_dev, int
                         int64_t n2, const double* diag_dev, const double* v_dev, int64_t nrhs, double* out_dev);
 int bgp_kmat_gradient_contract(const bgp_kernel_spec_t* spec, const uint32_t* which, const double* x, int64_t n,
                                const double* A, double* out /* n_params */);
+/* bgp_kmat_x1_gradient_matvec: input gradients contracted with a vector or with one column per point of x1,
+ *   out[i*ndim + q] = (add_prior ? d k(x1_i, x1_i) / d x1_iq : 0) + scale * sum_j d k(x1_i, x2_j) / d x1_iq * V_ji
+ * with V_ji = v[j] when ldv == 0 (one shared vector of n2 entries: GP.grad_predict's dmu with v = alpha, scale 1,
+ * add_prior 0) and V_ji = v[i*ldv + j] when ldv >= n2 (column i of an n2 x n1 column-major matrix: dvar with
+ * v = K^-1 K(x, x1), scale -2, add_prior 1).  The prior term is the derivative of the prior variance k(x, x), taken as
+ * 2 d k(x, x2)/dx at x2 = x (every kernel is symmetric); it is 0 for stationary kernels.  Unlike
+ * bgp_kmat_x1_gradient_general (the reference's values, L^-1 r for a general metric M = L L^T) the derivative is the
+ * true one for every metric.  The (n1, n2, ndim) gradient tensor is never formed; partial sums are added in a fixed
+ * order (no atomics), so identical calls return identical bits.  Errors: BGP_ERR_INVALID for ndim > BGP_MAX_DIM or a
+ * negative size, BGP_ERR_DIM for 0 < ldv < n2.  n1 == 0 writes nothing; n2 == 0 gives the prior term alone. */
+int bgp_kmat_x1_gradient_matvec(const bgp_kernel_spec_t* spec, const double* x1, int64_t n1, const double* x2,
+                                int64_t n2, const double* v, int64_t ldv, double scale, int32_t add_prior,
+                                double* out /* n1*ndim */);
+int bgp_kmat_x1_gradient_matvec_dev(const bgp_kernel_spec_t* spec, const double* x1_dev, int64_t n1,
+                                    const double* x2_dev, int64_t n2, const double* v_dev, int64_t ldv, double scale,
+                                    int32_t add_prior, double* out_dev);
 
 /* ------------------------------------------------------------------------------------------
  * Dense solver.  Replaces BasicSolver (src/george/solvers/basic.py:51-121): kernel matrix +
@@ -230,6 +246,16 @@ int bgp_dense_last_timing(const bgp_dense_t* h, double* ms2);
 enum { BGP_PREDICT_VAR = 0, BGP_PREDICT_COV = 1 };
 int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
                       double* out);
+/* Gradients of the predictive variance with respect to the test points (GP.grad_predict):
+ *   var[j]            = bgp_*_predict's VAR output, bit for bit (the same chunks and steps);
+ *   dvar[j*ndim + q]  = d var_j / d x*_jq = (d1 + d2) k(x*_j, x*_j)_q - 2 sum_i d k(x*_j, x_i) / d x*_jq W_ij
+ * with W = K^-1 K(x, x*) per chunk: dense, the backward sweep L^-T applied in place to the chunk's L^-1 K(x, x*) once
+ * var is reduced; HODLR, the chunk's K_h^-1 K(x, x*) of the VAR path.  The contraction is bgp_kmat_x1_gradient_matvec's
+ * (true derivatives for every metric), so identical calls return identical bits as far as the solve does.  Device
+ * workspace: the VAR path's plus O(c * ndim).  Errors: those of bgp_*_predict, and BGP_ERR_INVALID for ndim >
+ * BGP_MAX_DIM and on any sharded HODLR handle, all checked before anything is launched.  ns == 0 writes nothing. */
+int bgp_dense_predict_grad(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, double* var,
+                           double* dvar);
 
 /* ------------------------------------------------------------------------------------------
  * Batched log-likelihood terms (GP.batch_log_likelihood): B parameter vectors of one kernel program on the same x,
@@ -446,6 +472,9 @@ int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const 
  * A host-exchange shard returns BGP_ERR_INVALID, as before; it computes its part with bgp_hodlr_predict_local_dev. */
 int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
                       double* out);
+/* The HODLR counterpart of bgp_dense_predict_grad (see there); unsharded handles only. */
+int bgp_hodlr_predict_grad(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, double* var,
+                           double* dvar);
 /* One shard's part of the prediction: with J = this handle's own rows [row0, row0 + rows) ([0, N) unsharded),
  * B = K(x, x*) (N x ns) and P = B[J]^T W[J],
  *   VAR: out[ns]        = (add_prior ? k(x*_j, x*_j) : 0) - P_jj
