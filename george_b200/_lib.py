@@ -51,6 +51,7 @@ SIGNATURES = {
     "bgp_launch_count": (C.c_uint64, []),
     "bgp_spec_validate": (C.c_int, [_specp]),
     "bgp_spec_num_params": (C.c_int, [_specp, C.POINTER(C.c_int)]),
+    "bgp_spec_paths": (C.c_int, [_specp, C.POINTER(_i32)]),
     "bgp_kmat_symmetric": (C.c_int, [_specp, _p, _i64, _p]),
     "bgp_kmat_general": (C.c_int, [_specp, _p, _i64, _p, _i64, _p]),
     "bgp_kmat_diagonal": (C.c_int, [_specp, _p, _p, _i64, _p]),

@@ -761,6 +761,19 @@ static int kmat_xgrad_host(const bgp_kernel_spec_t* spec, int side, const double
 
 extern "C" {
 
+int bgp_spec_paths(const bgp_kernel_spec_t* spec, int32_t* out) {
+  DevProgram P;
+  BGP_TRY(build_dev_program(spec, &P));
+  FastShape F;
+  const bool fast = detect_fast_shape(P, &F);
+  out[0] = P.shape;
+  out[1] = (P.flags & BGP_FLAG_FAST1D) ? 1 : 0;
+  out[2] = fast ? F.shape : 0;
+  out[3] = fast ? F.nd : 0;
+  out[4] = fast && F.axis ? 1 : 0;
+  return BGP_OK;
+}
+
 int bgp_kmat_x1_gradient_general(const bgp_kernel_spec_t* spec, const double* x1, int64_t n1, const double* x2,
                                  int64_t n2, double* out) {
   return kmat_xgrad_host(spec, 1, x1, n1, x2, n2, out);

@@ -120,6 +120,14 @@ typedef struct bgp_kernel_spec {
 int bgp_spec_validate(const bgp_kernel_spec_t* spec);
 /* Total number of hyper-parameters = Kernel::size() (kernels.h:56, 2005). */
 int bgp_spec_num_params(const bgp_kernel_spec_t* spec, int* n_params);
+/* Diagnostics: which evaluator the library picks for a program (host only, no device needed; changes nothing).
+ *   out[0] the 1-D program shape of the specialised evaluators (csrc/kernel_eval.cuh BGP_SHAPE_*, 0 = interpreter),
+ *          used by the ACA, the HODLR leaves, the matvec and the x1-gradient contraction;
+ *   out[1] 1 when the interpreter takes its 1-D shortcut (every leaf a function of x1 - x2 on one input dimension);
+ *   out[2] the profile of the kernel-matrix builds' specialised evaluator (BGP_SHAPE_EXPSQ..EXP, 0 = interpreter),
+ *   out[3] its number of input dimensions, out[4] 1 for an axis-aligned metric, 0 for an isotropic one.
+ * BGP_KMAT_GENERIC, which turns the specialised kernel-matrix builds off, is not reflected in out[2..4]. */
+int bgp_spec_paths(const bgp_kernel_spec_t* spec, int32_t* out /* 5 */);
 
 /* ------------------------------------------------------------------------------------------
  * Kernel-matrix build.  Replaces KernelInterface::value_symmetric / value_general / value_diagonal
