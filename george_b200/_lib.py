@@ -83,6 +83,8 @@ SIGNATURES = {
     "bgp_dense_batch_log_likelihood": (C.c_int, [_p, _specp, _p, _i64, _i64, _p, _i64, _i32, _p, _p, _p, _p, _p]),
     "bgp_dense_batch_predict": (C.c_int, [_p, _specp, _p, _i64, _i64, _p, _i64, _i32, _p, _p, _p, _i64, _i32, _p, _p,
                                           _p]),
+    "bgp_dense_batch_predict_grad": (C.c_int, [_p, _specp, _p, _i64, _i64, _p, _i64, _i32, _p, _p, _p, _i64, _i32, _p,
+                                               _p, _p, _p, _p]),
     "bgp_dense_batch_sample": (C.c_int, [_p, _specp, _p, _i64, _i64, _p, _i64, _i32, _p, _p, _p, _i64, _p, _p, _i64,
                                          C.c_double, _p, _p, _p]),
     "bgp_dense_batch_grad_terms": (C.c_int, [_p, _specp, _p, _i64, _i64, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p,

@@ -55,6 +55,11 @@ int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int6
 int kmat_x1_grad_matvec_launch(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1,
                                const double* x2, int64_t n2, const double* V, int64_t ldv, double scale, int add_prior,
                                double* out, DevBuf<double>& scratch, cudaStream_t s);
+int kmat_x1_grad_matvec_members(const DevProgram* P, const DevProgram* dprogs, int members, const double* x1,
+                                int64_t n1, const double* x2, int64_t n2, const double* V, int64_t ldv,
+                                int64_t vstride, double scale, int add_prior, double* out, int64_t ostride,
+                                DevBuf<double>& scratch, cudaStream_t s);
+int64_t x1_grad_partial_size(int64_t n1, int64_t n2, int nd);
 int predict_var_launch(const double* B, int64_t ldb, const double* W, int64_t ldw, int64_t n, int64_t c,
                        const double* kdiag, double* var, DevBuf<double>& scratch, cudaStream_t s);
 int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
@@ -676,30 +681,36 @@ static int dense_trsm_fwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx
   return trsm_fwd_members(h->d_A.p, h->n, 0, X, nrhs, ldx, 0, 1, h->d_tmp.p, h->n, h->s);
 }
 
-// X (n x nrhs, column-major ldx) <- L^-T X: the backward half of dense_potrs_dev, so that dense_trsm_fwd_dev followed by
-// this is K^-1.  Few right-hand sides go through the one-launch step kernels of potrs_small_members, which read the
-// forward result from a copy in d_tmp; more through trsm_bwd_block_members.
-static int dense_trsm_bwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
-  const int64_t n = h->n;
-  cudaStream_t s = h->s;
-  if (nrhs > DS_MAX_RHS) return trsm_bwd_block_members(h->d_A.p, n, 0, X, nrhs, ldx, 0, 1, s);
-  BGP_TRY(h->d_tmp.reserve((size_t)n * DS_MAX_RHS, s));
-  double* Y = h->d_tmp.p;
-  BGP_CUDA(cudaMemcpy2DAsync(Y, sizeof(double) * n, X, sizeof(double) * ldx, sizeof(double) * n, nrhs,
-                             cudaMemcpyDeviceToDevice, s));
+// X (n x nrhs, column-major ldx) <- L^-T X: the backward half of potrs_members, so that trsm_fwd_members followed by
+// this is K^-1.  `members` factors at once (member m: L + m * lstride, X + m * xstride); a single solve passes one member
+// and zero strides.  Few right-hand sides go through the one-launch step kernels of potrs_small_members, which read the
+// forward result from a copy in Y (X's layout: leading dimension ldy, member stride xstride, so ldy >= (members - 1) *
+// xstride + n); more through trsm_bwd_block_members.
+static int trsm_bwd_members(const double* L, int64_t n, int64_t lstride, double* X, int64_t nrhs, int64_t ldx,
+                            int64_t xstride, int members, double* Y, int64_t ldy, cudaStream_t s) {
+  if (nrhs > DS_MAX_RHS) return trsm_bwd_block_members(L, n, lstride, X, nrhs, ldx, xstride, members, s);
+  const unsigned mb = (unsigned)members;
+  BGP_CUDA(cudaMemcpy2DAsync(Y, sizeof(double) * ldy, X, sizeof(double) * ldx,
+                             sizeof(double) * ((int64_t)(members - 1) * xstride + n), nrhs, cudaMemcpyDeviceToDevice, s));
   cudaFuncSetAttribute(trsv_bwd_step_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_BWD_SMEM);
   cudaFuncSetAttribute(trsv_bwd_step_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_BWD_SMEM);
   cudaFuncSetAttribute(trsv_bwd_step_kernel<DS_MAX_RHS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DS_BWD_SMEM);
   const int nr = (int)nrhs;
   for (int64_t k0 = ((n - 1) / DN_NB) * DN_NB; k0 >= 0; k0 -= DN_NB) {
     const int nb = (int)std::min<int64_t>(DN_NB, n - k0);
-    const dim3 g((unsigned)std::max<int64_t>(1, (k0 + DS_COLS - 1) / DS_COLS), 1);
-    if (nr == 1) trsv_bwd_step_kernel<1><<<g, 256, DS_BWD_SMEM, s>>>(h->d_A.p, n, k0, nb, Y, n, X, ldx, nr, 0, 0);
-    else if (nr <= 4) trsv_bwd_step_kernel<4><<<g, 256, DS_BWD_SMEM, s>>>(h->d_A.p, n, k0, nb, Y, n, X, ldx, nr, 0, 0);
-    else trsv_bwd_step_kernel<DS_MAX_RHS><<<g, 256, DS_BWD_SMEM, s>>>(h->d_A.p, n, k0, nb, Y, n, X, ldx, nr, 0, 0);
+    const dim3 g((unsigned)std::max<int64_t>(1, (k0 + DS_COLS - 1) / DS_COLS), mb);
+    if (nr == 1) trsv_bwd_step_kernel<1><<<g, 256, DS_BWD_SMEM, s>>>(L, n, k0, nb, Y, ldy, X, ldx, nr, lstride, xstride);
+    else if (nr <= 4) trsv_bwd_step_kernel<4><<<g, 256, DS_BWD_SMEM, s>>>(L, n, k0, nb, Y, ldy, X, ldx, nr, lstride, xstride);
+    else trsv_bwd_step_kernel<DS_MAX_RHS><<<g, 256, DS_BWD_SMEM, s>>>(L, n, k0, nb, Y, ldy, X, ldx, nr, lstride, xstride);
     BGP_LAUNCH_CHECK();
   }
   return BGP_OK;
+}
+
+// X (n x nrhs, column-major ldx) <- L^-T X on the handle's factor, the scratch Y in d_tmp
+static int dense_trsm_bwd_dev(bgp_dense* h, double* X, int64_t nrhs, int64_t ldx) {
+  if (nrhs <= DS_MAX_RHS) BGP_TRY(h->d_tmp.reserve((size_t)h->n * DS_MAX_RHS, h->s));
+  return trsm_bwd_members(h->d_A.p, h->n, 0, X, nrhs, ldx, 0, 1, h->d_tmp.p, h->n, h->s);
 }
 
 // GP.predict's covariance at the ns test points xs (host) into dC (ns x ns on the device, allocated here): every W chunk
@@ -1058,6 +1069,8 @@ struct bgp_dense_batch {
   // bgp_dense_batch_grad_terms: K_b^-1, the contraction partials and g
   DevBuf<double> d_inv, d_gp, d_g;
   DevBuf<unsigned> d_which;
+  // bgp_dense_batch_predict_grad: dmu, a test-point chunk of dvar and the input-gradient contraction's partials
+  DevBuf<double> d_dmu, d_dvar, d_xgp;
 };
 
 // members per chunk: as many members of per_member doubles as fit in 4 GiB, at least one; BGP_BATCH_CHUNK=<members>
@@ -1209,6 +1222,7 @@ void bgp_dense_batch_destroy(bgp_dense_batch_t* h) {
   h->d_var.release(); h->d_vp.release(); h->d_C.release(); h->d_slices.release(); h->d_pdesc.release();
   h->d_inv.release(); h->d_gp.release(); h->d_g.release(); h->d_which.release();
   h->d_madd.release(); h->d_z.release(); h->d_draws.release(); h->d_dinfo.release(); h->d_sdesc.release();
+  h->d_dmu.release(); h->d_dvar.release(); h->d_xgp.release();
   if (h->s) {
     cudaStreamSynchronize(h->s);
     cudaStreamDestroy(h->s);
@@ -1407,6 +1421,113 @@ int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec,
     if (info[b] == 0) continue;
     for (int64_t j = 0; j < ns; ++j) mean[b * ns + j] = std::nan("");
     for (int64_t j = 0; j < osize; ++j) out[b * osize + j] = std::nan("");
+  }
+  return BGP_OK;
+}
+
+int bgp_dense_batch_predict_grad(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
+                                 int64_t P, const double* x, int64_t n, int32_t ndim, const double* yerr,
+                                 const double* r, const double* xs, int64_t ns, int32_t with_var, double* mean,
+                                 double* dmu, double* var, double* dvar, int32_t* info) {
+  if (ndim > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, ndim); return BGP_ERR_INVALID; }
+  if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
+  if (with_var && (!var || !dvar)) { set_error("with_var needs the var and dvar outputs"); return BGP_ERR_INVALID; }
+  BatchPrograms bp;
+  BGP_TRY(batch_begin(h, spec, params, B, P, x, n, ndim, &bp));
+  if (B == 0) return BGP_OK;
+  cudaStream_t s = h->s;
+  const int64_t nn = n * n;
+  const int64_t nd = ndim;
+  // bgp_dense_batch_predict's mean and VAR workspace (the single path's test-point chunk), plus dmu, a chunk of dvar
+  // and the contraction partials (the larger of dmu's and a dvar chunk's: they run one after the other)
+  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
+  const int64_t tail = c > 0 ? ns - (ns - 1) / c * c : 0;
+  const int64_t mvp = matvec_partial_size(ns, n);
+  const int64_t vp = with_var ? std::max(predict_var_partial_size(n, c), predict_var_partial_size(n, tail)) : 0;
+  int64_t xgp = x1_grad_partial_size(ns, n, ndim);
+  if (with_var) xgp = std::max(xgp, std::max(x1_grad_partial_size(c, n, ndim), x1_grad_partial_size(tail, n, ndim)));
+  const int64_t tmp_cols = with_var ? DS_MAX_RHS : 1;
+  // doubles per member (see include/bgp.h)
+  int64_t per_member = nn + (4 + tmp_cols) * n + ns + mvp + ns * nd + xgp;
+  if (with_var) per_member += n * c + 2 * c + vp + c * nd;
+  int64_t chunk = batch_chunk_members(per_member, B);
+  auto release = [&] {
+    h->d_A.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_kd.release();
+    h->d_var.release(); h->d_vp.release(); h->d_tmp.release(); h->d_dmu.release(); h->d_dvar.release();
+    h->d_xgp.release();
+  };
+  auto reserve = [&](int64_t m) -> int {
+    BGP_TRY(h->d_A.reserve((size_t)(nn * m), s));
+    BGP_TRY(h->d_tmp.reserve((size_t)(n * m * tmp_cols), s));
+    BGP_TRY(h->d_mean.reserve((size_t)std::max<int64_t>(1, ns * m), s));
+    BGP_TRY(h->d_mvp.reserve((size_t)std::max<int64_t>(1, mvp * m), s));
+    BGP_TRY(h->d_dmu.reserve((size_t)std::max<int64_t>(1, ns * nd * m), s));
+    BGP_TRY(h->d_xgp.reserve((size_t)std::max<int64_t>(1, xgp * m), s));
+    if (with_var) {
+      BGP_TRY(h->d_W.reserve((size_t)std::max<int64_t>(1, n * c * m), s));
+      BGP_TRY(h->d_kd.reserve((size_t)std::max<int64_t>(1, c * m), s));
+      BGP_TRY(h->d_var.reserve((size_t)std::max<int64_t>(1, c * m), s));
+      BGP_TRY(h->d_vp.reserve((size_t)std::max<int64_t>(1, vp * m), s));
+      BGP_TRY(h->d_dvar.reserve((size_t)std::max<int64_t>(1, c * nd * m), s));
+    }
+    return BGP_OK;
+  };
+  BGP_TRY(batch_reserve_chunk(&chunk, reserve, release));
+  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, tmp_cols));
+  BGP_TRY(h->d_xs.reserve((size_t)std::max<int64_t>(1, ns * nd), s));
+  if (ns > 0) BGP_CUDA(cudaMemcpyAsync(h->d_xs.p, xs, sizeof(double) * ns * nd, cudaMemcpyHostToDevice, s));
+  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
+    const int mc = (int)std::min(chunk, B - c0);
+    const DevProgram* progs = bp.progs.data() + c0;
+    const DevProgram* dprogs = h->d_prog.p + c0;
+    // the steps of bgp_dense_batch_predict (factor, alpha, mean, VAR), then those of bgp_dense_predict_grad, with a
+    // member index.  A member whose K is not positive definite runs the later steps on its own slabs.
+    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
+    if (ns > 0) {
+      BGP_TRY(kmat_matvec_batch_launch(dprogs, ndim, mc, h->d_xs.p, ns, h->d_x.p, n, h->d_sol.p, n, h->d_mean.p, ns,
+                                       h->d_mvp.p, s));
+      BGP_CUDA(cudaMemcpyAsync(mean + c0 * ns, h->d_mean.p, sizeof(double) * mc * ns, cudaMemcpyDeviceToHost, s));
+      // dmu_b = sum_j d1 k_b(x*, x_j) alpha_bj: GP.grad_predict's kernel.x1_gradient_matvec(xs, x, alpha)
+      BGP_TRY(kmat_x1_grad_matvec_members(progs, dprogs, mc, h->d_xs.p, ns, h->d_x.p, n, h->d_sol.p, 0, n, 1.0, 0,
+                                          h->d_dmu.p, ns * nd, h->d_xgp, s));
+      BGP_CUDA(cudaMemcpyAsync(dmu + c0 * ns * nd, h->d_dmu.p, sizeof(double) * mc * ns * nd, cudaMemcpyDeviceToHost, s));
+    }
+    // W columns of all members interleaved, as in batch_cov_chunk
+    const int64_t ldw = (int64_t)mc * n;
+    if (with_var) {
+      for (int64_t j0 = 0; j0 < ns; j0 += c) {
+        const int64_t nc = std::min(c, ns - j0);
+        const double* xc = h->d_xs.p + j0 * nd;
+        // bgp_dense_batch_predict's variance steps
+        BGP_TRY(kmat_general_batch_launch_auto(progs, dprogs, mc, xc, nc, h->d_x.p, n, h->d_W.p, ldw, n, h->d_fn, s));
+        BGP_TRY(trsm_fwd_members(h->d_A.p, n, nn, h->d_W.p, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
+        BGP_TRY(kmat_diagonal_launch(dprogs, xc, xc, nc, h->d_kd.p, s, mc, c));
+        BGP_TRY(predict_var_batch_launch(h->d_W.p, ldw, h->d_W.p, ldw, n, nc, h->d_kd.p, h->d_var.p, mc, n, c, h->d_vp, s));
+        BGP_CUDA(cudaMemcpy2DAsync(var + c0 * ns + j0, sizeof(double) * ns, h->d_var.p, sizeof(double) * c,
+                                   sizeof(double) * nc, mc, cudaMemcpyDeviceToHost, s));
+        // bgp_dense_predict_grad's: W <- L_b^-T W = K_b^-1 K_b(x, x*), dvar = dprior - 2 sum_j d1 k_b(x*, x_j) W_j
+        BGP_TRY(trsm_bwd_members(h->d_A.p, n, nn, h->d_W.p, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
+        BGP_TRY(kmat_x1_grad_matvec_members(progs, dprogs, mc, xc, nc, h->d_x.p, n, h->d_W.p, ldw, n, -2.0, 1,
+                                            h->d_dvar.p, c * nd, h->d_xgp, s));
+        BGP_CUDA(cudaMemcpy2DAsync(dvar + (c0 * ns + j0) * nd, sizeof(double) * ns * nd, h->d_dvar.p,
+                                   sizeof(double) * c * nd, sizeof(double) * nc * nd, mc, cudaMemcpyDeviceToHost, s));
+      }
+    }
+    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaStreamSynchronize(s));
+  }
+  const double nan = std::nan("");
+  for (int64_t b = 0; b < B; ++b) {
+    if (!bp.valid[b]) info[b] = -1;
+    if (info[b] == 0) continue;
+    for (int64_t j = 0; j < ns; ++j) {
+      mean[b * ns + j] = nan;
+      if (with_var) var[b * ns + j] = nan;
+    }
+    for (int64_t j = 0; j < ns * nd; ++j) {
+      dmu[b * ns * nd + j] = nan;
+      if (with_var) dvar[b * ns * nd + j] = nan;
+    }
   }
   return BGP_OK;
 }

@@ -436,6 +436,9 @@ static int run_aca2(bgp_hodlr* h, const std::vector<AcaDesc>& descs, std::vector
   const bool cull = shape_has_bound(h->prog.shape) && !getenv("BGP_NO_CULL");  // BGP_NO_CULL: exhaustive scan (tests compare both)
   if (cull) {
     BGP_TRY(h->d_vmax.reserve((size_t)ncc * A2_NGROUP, s));
+    // a2_generate and a2_eval read vmax before a node's first factor writes it, scaled by sum_q |U(i, q)| = 0: a stale
+    // NaN or Inf left in reused device memory would turn that 0 into NaN and keep candidates the bound rules out
+    BGP_CUDA(cudaMemsetAsync(h->d_vmax.p, 0, sizeof(double) * ncc * A2_NGROUP, s));
     BGP_TRY(h->d_cand_xu.reserve((size_t)cand_total, s));
     BGP_TRY(h->d_gbox.reserve((size_t)ncc * A2_NGROUP, s));
     BGP_TRY(h->d_cbox.reserve((size_t)ncc, s));

@@ -243,6 +243,8 @@ int kmat_matvec_batch_launch(const DevProgram* dprogs, int nd, int members, cons
 // read coalesced (8 * n2 * n1 bytes in all, the kernel's only large HBM traffic).  Each warp's sum over a chunk goes to
 // a per-point accumulator in shared memory owned by that warp; per-CTA partials are summed over the splits in a fixed
 // order by x1_grad_reduce_kernel.  No atomics: identical calls give identical bits.
+// Member blockIdx.z of a batch (bgp_dense_batch_predict_grad) contracts with its own program gprog[z] and V + z * vstride
+// and writes partial + z * pstride; x1 and x2 are shared.  A single contraction launches one member with zero strides.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int XG_TI = 32;
 constexpr int XG_TJ = 512;
@@ -261,7 +263,11 @@ __global__ void __launch_bounds__(XG_THREADS) kmat_x1_grad_matvec_kernel(const D
                                                                          const double* __restrict__ x2, int64_t n2,
                                                                          const double* __restrict__ V, int64_t ldv,
                                                                          double* __restrict__ partial,
-                                                                         int chunks_per_split) {
+                                                                         int chunks_per_split, int64_t vstride,
+                                                                         int64_t pstride) {
+  gprog += blockIdx.z;
+  V += blockIdx.z * vstride;
+  partial += blockIdx.z * pstride;
   using Eval = X1GradEval<SHAPE>;
   constexpr int NDMAX = Eval::type::NDMAX;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -319,9 +325,13 @@ __global__ void __launch_bounds__(XG_THREADS) kmat_x1_grad_matvec_kernel(const D
 }
 
 // out[i*nd + q] = (add_prior ? 2 d1 k(x1_i, x1_i)_q : 0) + scale * sum_s partial[(s*n1 + i)*nd + q], s ascending
+// (member blockIdx.y: the prior term of gprog[y], partial + y * pstride, out + y * ostride)
 __global__ void x1_grad_reduce_kernel(const DevProgram* __restrict__ gprog, const double* __restrict__ x1, int64_t n1,
                                       const double* __restrict__ partial, int64_t nsplit, double scale, int add_prior,
-                                      double* __restrict__ out) {
+                                      double* __restrict__ out, int64_t pstride, int64_t ostride) {
+  gprog += blockIdx.y;
+  partial += blockIdx.y * pstride;
+  out += blockIdx.y * ostride;
   const int nd = gprog->ndim;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n1; i += (int64_t)gridDim.x * blockDim.x) {
     double g[BGP_MAX_DIM];
@@ -348,27 +358,50 @@ static int x1_grad_plan(int64_t n1, int64_t n2, int64_t* nsplit_out, int* cps_ou
   return BGP_OK;
 }
 
-// out (n1 x nd, row-major) as described above; P is the validated program behind dprog (its shape selects the
-// evaluator), x1 / x2 / V / out device pointers.  scratch: the partials (nsplit * n1 * nd doubles).
-int kmat_x1_grad_matvec_launch(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1,
-                               const double* x2, int64_t n2, const double* V, int64_t ldv, double scale, int add_prior,
-                               double* out, DevBuf<double>& scratch, cudaStream_t s) {
-  const int nd = P.ndim;
+// partials of one member's contraction (doubles): nsplit * n1 * nd, nsplit from x1_grad_plan
+int64_t x1_grad_partial_size(int64_t n1, int64_t n2, int nd) {
+  int64_t nsplit;
+  int cps;
+  if (n1 <= 0 || x1_grad_plan(n1, n2, &nsplit, &cps) != BGP_OK) return 0;
+  return nsplit * n1 * nd;
+}
+
+// `members` contractions on the same x1 (n1 points) and x2 (n2 points), in one launch of each kernel: member m uses the
+// host program P[m] (device copy dprogs + m), reads V + m * vstride (ldv as above) and writes out + m * ostride (n1 x nd,
+// row-major).  The split plan depends on (n1, n2) alone and the evaluator on P[0].shape, so every member's partials
+// and their reduction order are those of a one-member call; members whose shapes differ are refused, since the
+// specialised and the interpreted evaluators round differently.  x1 / x2 / V / out are device pointers; scratch holds
+// members * x1_grad_partial_size(n1, n2, nd) partials.
+int kmat_x1_grad_matvec_members(const DevProgram* P, const DevProgram* dprogs, int members, const double* x1,
+                                int64_t n1, const double* x2, int64_t n2, const double* V, int64_t ldv,
+                                int64_t vstride, double scale, int add_prior, double* out, int64_t ostride,
+                                DevBuf<double>& scratch, cudaStream_t s) {
+  if (members <= 0) return BGP_OK;
+  const int nd = P[0].ndim;
   if (nd > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, nd); return BGP_ERR_INVALID; }
+  if (members > 65535) { set_error("kmat_x1_gradient_matvec: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
+  for (int m = 1; m < members; ++m)
+    if (P[m].shape != P[0].shape || P[m].ndim != nd) {
+      set_error("kmat_x1_gradient_matvec: members differ in program structure");
+      return BGP_ERR_INVALID;
+    }
   if (n1 <= 0) return BGP_OK;
+  const unsigned mb = (unsigned)members;
   int64_t nsplit;
   int cps;
   BGP_TRY(x1_grad_plan(n1, n2, &nsplit, &cps));
+  const int64_t pstride = nsplit * n1 * nd;
   if (nsplit > 0) {
-    BGP_TRY(scratch.reserve((size_t)(nsplit * n1 * nd), s));
+    BGP_TRY(scratch.reserve((size_t)(pstride * members), s));
     const size_t smem = x1_grad_smem(nd);
-    const dim3 grid((unsigned)((n1 + XG_TI - 1) / XG_TI), (unsigned)nsplit);
+    const dim3 grid((unsigned)((n1 + XG_TI - 1) / XG_TI), (unsigned)nsplit, mb);
 #define BGP_X1G_LAUNCH(SH)                                                                                   \
   {                                                                                                         \
     cudaFuncSetAttribute(kmat_x1_grad_matvec_kernel<SH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-    kmat_x1_grad_matvec_kernel<SH><<<grid, XG_THREADS, smem, s>>>(dprog, x1, n1, x2, n2, V, ldv, scratch.p, cps);  \
+    kmat_x1_grad_matvec_kernel<SH><<<grid, XG_THREADS, smem, s>>>(dprogs, x1, n1, x2, n2, V, ldv, scratch.p, cps,  \
+                                                                  vstride, pstride);                        \
   }
-    switch (P.shape) {
+    switch (P[0].shape) {
       case BGP_SHAPE_EXPSQ: BGP_X1G_LAUNCH(BGP_SHAPE_EXPSQ); break;
       case BGP_SHAPE_M32: BGP_X1G_LAUNCH(BGP_SHAPE_M32); break;
       case BGP_SHAPE_M52: BGP_X1G_LAUNCH(BGP_SHAPE_M52); break;
@@ -379,9 +412,18 @@ int kmat_x1_grad_matvec_launch(const DevProgram& P, const DevProgram* dprog, con
     BGP_LAUNCH_CHECK();
   }
   const int blocks = (int)std::min<int64_t>((n1 + 127) / 128, 8 * (int64_t)num_sms());
-  x1_grad_reduce_kernel<<<blocks, 128, 0, s>>>(dprog, x1, n1, scratch.p, nsplit, scale, add_prior, out);
+  x1_grad_reduce_kernel<<<dim3((unsigned)blocks, mb), 128, 0, s>>>(dprogs, x1, n1, scratch.p, nsplit, scale, add_prior,
+                                                                   out, pstride, ostride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
+}
+
+// out (n1 x nd, row-major) as described above; P is the validated program behind dprog (its shape selects the
+// evaluator), x1 / x2 / V / out device pointers.  scratch: the partials (nsplit * n1 * nd doubles).
+int kmat_x1_grad_matvec_launch(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1,
+                               const double* x2, int64_t n2, const double* V, int64_t ldv, double scale, int add_prior,
+                               double* out, DevBuf<double>& scratch, cudaStream_t s) {
+  return kmat_x1_grad_matvec_members(&P, dprog, 1, x1, n1, x2, n2, V, ldv, 0, scale, add_prior, out, 0, scratch, s);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -786,6 +786,79 @@ class GP(ModelSet):
         var, dvar = out
         return mu, var, dmu, dvar
 
+    def batch_grad_predict(self, vectors, y, t, return_var=False, kernel=None):
+        """:func:`grad_predict` at many parameter vectors: ``(mu, dmu)``, or ``(mu, var, dmu, dvar)`` with
+        ``return_var``; ``mu`` and ``var`` are ``(B, ns)``, ``dmu`` and ``dvar`` ``(B, ns, ndim)`` (also for a 1-D
+        ``t``).  Entry ``b`` is bit for bit what ``gp.set_parameter_vector(vectors[b]); gp.grad_predict(y, t,
+        return_var=...)`` returns on the computed ``x`` and ``yerr``: an acquisition function averaged over a sampler's
+        chain (the integrated acquisition of Snoek, Larochelle and Adams, 2012) and its gradient in one call.  The GP
+        is left as it was: parameter vector, factorisation, cached solve and dirty flags.
+
+        The checks that do not depend on the member come first, with :func:`grad_predict`'s and :func:`batch_predict`'s
+        exceptions: a mean model other than a ``ConstantModel`` (``NotImplementedError``), a model that has not been
+        computed, the shape of ``vectors``, ``y``'s length, ``t``'s dimension and more than 8 input dimensions.  Then
+        a failing member raises the exception the loop would raise first, with its type and message (white noise,
+        factorisation, residual).  With no members or no test points nothing is computed and the empty results are
+        returned.
+
+        Solvers with a ``batch_predict_grad`` hook (``BasicSolver``) factorise all members and compute their means,
+        variances and gradients in one batched pass on the device; any other solver (``HODLRSolver``,
+        ``ShardedHODLRSolver``, ``TrivialSolver``, plug-ins), an explicit ``kernel`` and a kernel without a valid
+        device program take that loop.
+
+        :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
+        """
+        if type(self.mean) is not ConstantModel:
+            raise NotImplementedError("grad_predict needs the mean model's gradient with respect to the inputs, which "
+                                      "the modeling protocol does not provide; only a constant mean is supported")
+        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
+            raise RuntimeError("You need to compute the model first")
+        vectors = np.asarray(vectors, dtype=np.float64)
+        if vectors.ndim != 2 or vectors.shape[1] != len(self):
+            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        self._check_dimensions(y)
+        xs = self.parse_samples(t)
+        if xs.shape[1] > BGP_MAX_DIM:
+            raise ValueError("input-coordinate gradients support at most {0} dimensions (got {1})".format(
+                BGP_MAX_DIM, xs.shape[1]))
+        nb, ns, nd = len(vectors), len(xs), xs.shape[1]
+        if nb == 0 or ns == 0:
+            mu, dmu = np.empty((nb, ns), dtype=np.float64), np.empty((nb, ns, nd), dtype=np.float64)
+            if not return_var:
+                return mu, dmu
+            return mu, np.empty((nb, ns), dtype=np.float64), dmu, np.empty((nb, ns, nd), dtype=np.float64)
+        batch = getattr(self.solver_type, "batch_predict_grad", None)
+        if batch is not None and kernel is None:
+            out = self._batch_grad_predict_device(batch, vectors, y, xs, return_var)
+            if out is not None:
+                return out
+        state = self._batch_state()
+        try:
+            res = []
+            for v in vectors:
+                self.set_parameter_vector(v)
+                res.append(self.grad_predict(y, t, return_var=return_var, kernel=kernel))
+        finally:
+            self._batch_restore(state)
+        return tuple(np.stack([r[k] for r in res]) for k in range(len(res[0])))
+
+    def _batch_grad_predict_device(self, batch, vectors, y, xs, return_var):
+        """The batched dense path of :func:`batch_grad_predict`; ``None`` when the kernel has no valid device
+        program."""
+        members = self._batch_predict_members(vectors, y)
+        if members is None:
+            return None
+        spec, full, kpar, sigma, resid, fact_err, mean_err = members
+        mean_xs, xs_err = self._batch_mean_at(full, xs)
+        mu, var, dmu, dvar, info = batch(spec, kpar, self._x, sigma, resid, xs, return_var)
+        for b in range(len(vectors)):  # the loop's order: white noise, factorisation, residual
+            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
+            exc = exc if exc is not None else (mean_err[b] if mean_err[b] is not None else xs_err[b])
+            if exc is not None:
+                raise exc
+        mu += mean_xs  # a constant mean adds nothing to dmu
+        return (mu, var, dmu, dvar) if return_var else (mu, dmu)
+
     def sample_conditional(self, y, t, size=1, *, rng=None, jitter=None):
         """Draws from the conditional predictive distribution at ``t``: shape ``(ns,)`` when ``size == 1``, else
         ``(size, ns)``.

@@ -401,6 +401,50 @@ class BasicSolver(object):
         return mean, out, info
 
     @staticmethod
+    def batch_predict_grad(spec, params, x, yerr, r, xs, return_var):
+        """``(mean, var, dmu, dvar, info)`` for ``B`` parameter vectors of one kernel program on the same ``x``: member
+        ``b`` factorises as in :func:`batch_log_likelihood`; ``mean`` (``(B, ns)``) is :func:`batch_predict`'s,
+        ``dmu[b]`` (``(B, ns, ndim)``) the contraction ``kernel.x1_gradient_matvec(xs, x, K_b^-1 r[b])`` and, with
+        ``return_var``, ``var`` (``(B, ns)``) and ``dvar`` (``(B, ns, ndim)``) are what :func:`predictive_grad` returns
+        for the member; otherwise both are ``None`` (``include/bgp.h: bgp_dense_batch_predict_grad``).  ``info`` is that
+        of :func:`batch_log_likelihood`; a failed member's rows are NaN.  Every entry is bit-identical to
+        :func:`compute` with member ``b``'s spec and yerr followed by ``apply_inverse(r[b])``, ``kernel.matvec``,
+        ``kernel.x1_gradient_matvec`` and :func:`predictive_grad`.  ``xs``: ``(ns,)`` or ``(ns, ndim)``."""
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.ndim == 1:
+            x = x[:, None]
+        xs = np.ascontiguousarray(xs, dtype=np.float64)
+        if xs.ndim == 1:
+            xs = xs[:, None]
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
+        r = np.ascontiguousarray(r, dtype=np.float64)
+        if x.ndim != 2 or x.shape[0] == 0:
+            raise ValueError("x must have shape (n, ndim) with n > 0")
+        n, ndim = x.shape
+        if params.ndim != 2 or params.shape[1] != num_params(spec):
+            raise ValueError("params must have shape (B, {0})".format(num_params(spec)))
+        nb = params.shape[0]
+        if yerr.shape != (nb, n) or r.shape != (nb, n):
+            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
+        if ndim != spec.ndim or xs.ndim != 2 or xs.shape[1] != ndim:
+            raise DimensionMismatch("dimension mismatch")
+        ns = xs.shape[0]
+        mean = np.empty((nb, ns), dtype=np.float64)
+        dmu = np.empty((nb, ns, ndim), dtype=np.float64)
+        var = np.empty((nb, ns), dtype=np.float64) if return_var else None
+        dvar = np.empty((nb, ns, ndim), dtype=np.float64) if return_var else None
+        info = np.zeros(nb, dtype=np.int32)
+        if nb == 0:
+            return mean, var, dmu, dvar, info
+        h = _get_batch_handle()
+        _lib.check(h.lib.bgp_dense_batch_predict_grad(
+            h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim, _lib.ptr(yerr),
+            _lib.ptr(r), _lib.ptr(xs), ns, 1 if return_var else 0, _lib.ptr(mean), _lib.ptr(dmu),
+            _lib.ptr(var) if return_var else None, _lib.ptr(dvar) if return_var else None, _lib.ptr(info)))
+        return mean, var, dmu, dvar, info
+
+    @staticmethod
     def batch_sample(spec, params, x, yerr, r, xs, mean_add, z, jitter):
         """``(draws, info, draw_info)`` for ``B`` parameter vectors of one kernel program on the same ``x``: member
         ``b`` factorises as in :func:`batch_log_likelihood` and draws ``mu_b + z[b] @ L_b.T`` (``(B, size, ns)``) as

@@ -345,6 +345,40 @@ int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec,
                             double* mean,                                    /* B x ns                       */
                             double* out,                                     /* B x ns, B x ns x ns, or NULL */
                             int32_t* info);
+/* Batched predictive gradients (GP.batch_grad_predict): for the same B members as bgp_dense_batch_predict (spec,
+ * params, x, yerr, r, xs), what bgp_dense_predict_grad and the input-gradient contraction give each member:
+ *   mean[b*ns + j]            as bgp_dense_batch_predict
+ *   dmu[(b*ns + j)*ndim + q]  = sum_i d k_b(x*_j, x_i) / d x*_jq alpha_bi      (alpha_b = K_b^-1 r_b)
+ *   with_var != 0:
+ *   var[b*ns + j]             as bgp_dense_batch_predict with BGP_PREDICT_VAR
+ *   dvar[(b*ns + j)*ndim + q] = 2 d1 k_b(x*_j, x*_j)_q - 2 sum_i d k_b(x*_j, x_i) / d x*_jq (K_b^-1 K_b(x, x*_j))_i
+ * Every entry is bit-identical to the single path on member b's spec and yerr: bgp_dense_apply_inverse of r_b (one
+ * right-hand side), bgp_kmat_matvec and bgp_kmat_x1_gradient_matvec(xs, x, alpha) for mean and dmu, bgp_dense_predict_grad
+ * after bgp_dense_compute for var and dvar.  The steps of a member chunk are bgp_dense_batch_predict's (factor, alpha,
+ * mean, the VAR chunks) followed by bgp_dense_predict_grad's backward sweep L_b^-T and contraction per test-point
+ * chunk, each with a member index and with the single path's split and chunk decisions (test-point chunks of
+ * predict_chunk_cols(n) columns, BGP_PREDICT_CHUNK applies alike; the contraction's evaluator is the one the single
+ * path picks from the program's shape).  A member's results therefore do not depend on B, its position or the
+ * chunking.  info[b] as in bgp_dense_batch_log_likelihood; a failed member's rows of every output are NaN and do not
+ * disturb the other members.
+ * Members run in chunks that fit in 4 GiB of device memory (BGP_BATCH_CHUNK=<members> overrides it); every step of a
+ * chunk is one launch for all its members, so the launch count depends on n, ns, with_var and the number of chunks,
+ * never on B within a chunk.
+ * Device workspace per member (doubles): bgp_dense_batch_predict's (mean only without with_var, VAR with it) plus
+ * ns ndim (dmu) + P_xg, and with with_var c ndim (a chunk of dvar); P_xg = nsplit * m * ndim contraction partials for
+ * the larger of the m = ns (dmu) and m = c (dvar) contractions, nsplit <= ceil(n / 512).  Shared: B programs, x, xs.
+ * The handle keeps it for the next call.
+ * Errors: those of bgp_dense_batch_log_likelihood; BGP_ERR_INVALID for ndim > BGP_MAX_DIM (before anything else),
+ * ns < 0, or with_var without var or dvar.  B == 0 writes nothing; ns == 0 factorises (info) and writes no rows. */
+int bgp_dense_batch_predict_grad(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params,
+                                 int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
+                                 const double* yerr, const double* r,       /* B x n, row-major            */
+                                 const double* xs, int64_t ns, int32_t with_var,
+                                 double* mean,                               /* B x ns                      */
+                                 double* dmu,                                /* B x ns x ndim               */
+                                 double* var,                                /* B x ns, or NULL             */
+                                 double* dvar,                               /* B x ns x ndim, or NULL      */
+                                 int32_t* info);                             /* B                           */
 /* Batched draws (GP.batch_sample_conditional): for the same B members as bgp_dense_batch_predict (spec, params, x,
  * yerr, r, xs), what bgp_dense_sample draws for each member from its predictive covariance:
  *   draws[(b*size + a)*ns + j] = mu_b[j] + sum_{i <= j} z[(b*size + a)*ns + i] L_b(j, i)
