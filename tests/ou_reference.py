@@ -1,0 +1,197 @@
+# -*- coding: utf-8 -*-
+"""Closed-form references for ``c * ExpKernel(m)`` on sorted 1-D inputs (test infrastructure; numpy only).
+
+On sorted points this covariance is that of an Ornstein-Uhlenbeck process, and its Cholesky factor is known entry by
+entry.  Let ``l = sqrt(m)`` (``ExpKernel`` evaluates ``exp(-sqrt(r^2))`` with ``r^2 = (x_i - x_j)^2 / m``),
+
+    K_ij = c exp(-|x_i - x_j| / l),   rho_j = exp(-(x_j - x_{j-1}) / l),   s_0 = 1,   s_j = sqrt(1 - rho_j^2).
+
+Then ``K = L L^T`` with
+
+    L_ij = sqrt(c) exp(-(x_i - x_j) / l) s_j    (i >= j),   0 above the diagonal.
+
+Proof: for i >= k, ``(L L^T)_ik = c exp(-(x_i - x_k) / l) sum_{j <= k} E_j s_j^2`` with
+``E_j = exp(-2 (x_k - x_j) / l)``.  Since ``E_j rho_j^2 = E_{j-1}``, each term ``E_j s_j^2 = E_j - E_{j-1}`` for
+j >= 1 and ``E_0 s_0^2 = E_0``, so the sum telescopes to ``E_k = 1`` and ``(L L^T)_ik = K_ik``.
+
+Everything else follows in O(n):
+
+* ``log det K = n log c + 2 sum_j log s_j``;
+* ``L = sqrt(c) A diag(s)`` with ``A_ij = exp(-(x_i - x_j) / l)`` (i >= j), and ``A^-1`` is unit lower bidiagonal with
+  ``-rho_j`` below the diagonal, so ``(L^-1 z)_j = (z_j - rho_j z_{j-1}) / (sqrt(c) s_j)`` and
+  ``(L^-T w)_j = (w_j / s_j - rho_{j+1} w_{j+1} / s_{j+1}) / sqrt(c)``;
+* ``K^-1 = L^-T L^-1`` is tridiagonal: ``c K^-1_jj = 1 / s_j^2 + rho_{j+1}^2 / s_{j+1}^2`` and
+  ``c K^-1_{j,j+1} = -rho_{j+1} / s_{j+1}^2``;
+* ``o = z L^T`` is the AR(1) recursion ``o_j = rho_j o_{j-1} + sqrt(c) s_j z_j``;
+* for theta = (log c, log m), ``dK/dlog c = K`` and ``dK/dlog m = D / 2`` with ``D_ij = K_ij |x_i - x_j| / l``
+  (``d sqrt(r^2) / dlog m = -sqrt(r^2) / 2``).  The gradient terms of ``grad_terms``,
+  ``g_p = sum_ij (alpha alpha^T - K^-1)_ij dK_ij/dtheta_p`` with ``alpha = K^-1 r``, are therefore
+  ``g_c = r . alpha - n`` and ``g_m = alpha^T D alpha / 2 - tr(K^-1 D) / 2``.  D is semi-separable: ``D a`` takes one
+  forward and one backward sweep, and ``tr(K^-1 D)`` needs only the first off-diagonal of K^-1 (D's diagonal is 0).
+
+Every recursion runs on the ratios ``rho_j`` and the scaled gaps ``(x_j - x_{j-1}) / l``, never on ``exp(+-x / l)``,
+so nothing overflows however long the interval.  All arithmetic is ``np.longdouble`` (x87 80-bit on x86-64, eps
+1.1e-19), so for well-conditioned K (gaps of at least 0.2 l give rho <= 0.82 and cond(K) <= 10) the distance of a
+float64 result from these values is the float64 result's own error.
+"""
+import numpy as np
+
+LD = np.longdouble
+assert np.finfo(LD).nmant >= 63, (
+    "np.longdouble has a {0}-bit mantissa here: the extended-precision reference needs the 80-bit x87 format"
+    .format(np.finfo(LD).nmant))
+
+# Test points see the data within this many length scales: a dropped term of the predictive mean or variance is below
+# exp(-100) = 3.7e-44 of c, far below longdouble rounding.
+PREDICT_WINDOW = 100
+
+
+class OU(object):
+    """The closed forms for ``K = c * ExpKernel(m)`` evaluated at the sorted points ``x`` (``(n,)`` or ``(n, 1)``)."""
+
+    def __init__(self, x, c, m):
+        x = np.asarray(x, dtype=np.float64).reshape(-1)
+        if x.size > 1 and not np.all(np.diff(x) > 0):
+            raise ValueError("x must be strictly increasing")
+        self.n = x.size
+        self.x = x.astype(LD)
+        self.c = LD(c)
+        self.ell = np.sqrt(LD(m))
+        self.sqrtc = np.sqrt(self.c)
+        # delta_j = (x_j - x_{j-1}) / l and rho_j = exp(-delta_j) for j >= 1; delta_0 = rho_0 = 0, s_0 = 1
+        self.delta = np.zeros(self.n, dtype=LD)
+        self.delta[1:] = np.diff(self.x) / self.ell
+        self.rho = np.exp(-self.delta)
+        self.rho[0] = 0
+        s2 = -np.expm1(-2 * self.delta)  # 1 - rho^2 without cancellation
+        s2[0] = 1
+        self.s2 = s2
+        self.s = np.sqrt(s2)
+
+    # ---- the factor ---------------------------------------------------------------------------------------------
+    def logdet(self):
+        """``log det K``."""
+        return self.n * np.log(self.c) + 2 * np.sum(np.log(self.s))
+
+    def chol_columns(self, cols):
+        """``L[:, cols]`` (``(n, len(cols))``), entry by entry."""
+        cols = np.asarray(cols, dtype=np.int64)
+        out = np.zeros((self.n, cols.size), dtype=LD)
+        for k, j in enumerate(cols):
+            out[j:, k] = self.sqrtc * self.s[j] * np.exp(-(self.x[j:] - self.x[j]) / self.ell)
+        return out
+
+    def inv_chol(self, z):
+        """``L^-1 z`` for ``z`` of shape ``(n,)`` or ``(n, k)``."""
+        z = np.asarray(z, dtype=LD)
+        rho, s = (self.rho, self.s) if z.ndim == 1 else (self.rho[:, None], self.s[:, None])
+        prev = np.zeros_like(z)
+        prev[1:] = z[:-1]
+        return (z - rho * prev) / (self.sqrtc * s)
+
+    def inv_chol_t(self, w):
+        """``L^-T w`` for ``w`` of shape ``(n,)`` or ``(n, k)``."""
+        w = np.asarray(w, dtype=LD)
+        rho, s = (self.rho, self.s) if w.ndim == 1 else (self.rho[:, None], self.s[:, None])
+        q = w / s
+        nxt = np.zeros_like(q)
+        nxt[:-1] = rho[1:] * q[1:]
+        return (q - nxt) / self.sqrtc
+
+    def solve(self, b):
+        """``K^-1 b`` for ``b`` of shape ``(n,)`` or ``(n, k)``."""
+        return self.inv_chol_t(self.inv_chol(b))
+
+    def inv_tridiag(self):
+        """``(d, e)``: the diagonal (``(n,)``) and the first off-diagonal (``(n - 1,)``, ``e_j = K^-1_{j,j+1}``) of the
+        tridiagonal K^-1."""
+        d = 1 / self.s2
+        d[:-1] += self.rho[1:] ** 2 / self.s2[1:]
+        e = -self.rho[1:] / self.s2[1:]
+        return d / self.c, e / self.c
+
+    def sqrt_rows(self, z):
+        """``z @ L^T`` for ``z`` of shape ``(n,)`` or ``(k, n)``: the AR(1) recursion, one sweep over the points."""
+        z = np.asarray(z, dtype=LD)
+        zz = z.reshape(-1, self.n)
+        out = np.empty_like(zz)
+        o = np.zeros(zz.shape[0], dtype=LD)
+        w = self.sqrtc * self.s
+        for j in range(self.n):
+            o = self.rho[j] * o + w[j] * zz[:, j]
+            out[:, j] = o
+        return out.reshape(z.shape)
+
+    # ---- the log-likelihood gradient ------------------------------------------------------------------------------
+    def apply_d(self, a):
+        """``D a`` for a vector ``a``, ``D_ij = K_ij |x_i - x_j| / l``, in one forward and one backward sweep.
+
+        Forward: ``P_i = sum_{j<i} exp(-(x_i - x_j)/l) a_j`` and ``Q_i = sum_{j<i} exp(-(x_i - x_j)/l) (x_i - x_j)/l a_j``
+        obey ``P_i = rho_i (P_{i-1} + a_{i-1})`` and ``Q_i = rho_i (Q_{i-1} + delta_i (P_{i-1} + a_{i-1}))``; the
+        backward sweep is the mirror image.  ``(D a)_i = c (Q_i + Q'_i)``."""
+        a = np.asarray(a, dtype=LD).tolist()
+        rho, dl = self.rho.tolist(), self.delta.tolist()
+        n = self.n
+        out = [LD(0)] * n
+        P = Q = LD(0)
+        for i in range(1, n):
+            t = P + a[i - 1]
+            Q = rho[i] * (Q + dl[i] * t)
+            P = rho[i] * t
+            out[i] = Q
+        P = Q = LD(0)
+        for i in range(n - 2, -1, -1):
+            t = P + a[i + 1]
+            Q = rho[i + 1] * (Q + dl[i + 1] * t)
+            P = rho[i + 1] * t
+            out[i] += Q
+        return self.c * np.array(out, dtype=LD)
+
+    def trace_kinv_d(self):
+        """``tr(K^-1 D) = 2 sum_j K^-1_{j,j+1} D_{j,j+1}``, with ``D_{j,j+1} = c rho_{j+1} delta_{j+1}``."""
+        _, e = self.inv_tridiag()
+        return 2 * np.sum(e * self.c * self.rho[1:] * self.delta[1:])
+
+    def grad_terms(self, r):
+        """``(alpha, g, diag)`` of ``grad_terms`` for theta = (log c, log m): ``alpha = K^-1 r``, ``g`` (``(2,)``) and
+        ``diag = alpha^2 - diag(K^-1)``."""
+        r = np.asarray(r, dtype=LD)
+        alpha = self.solve(r)
+        g_c = r @ alpha - self.n
+        g_m = (alpha @ self.apply_d(alpha) - self.trace_kinv_d()) / 2
+        d, _ = self.inv_tridiag()
+        return alpha, np.array([g_c, g_m], dtype=LD), alpha ** 2 - d
+
+    # ---- prediction -------------------------------------------------------------------------------------------------
+    def predict(self, t, alpha):
+        """``(mean, var)`` at the test points ``t``: ``mean = K(t, x) alpha`` and ``var = c - |w|^2`` with
+        ``w = L^-1 K(x, t)``, over the points within ``PREDICT_WINDOW`` length scales of each test point (``w`` is
+        exactly 0 past the first point at or above t, and below ``exp(-PREDICT_WINDOW)`` further down)."""
+        t = np.asarray(t, dtype=np.float64).reshape(-1)
+        alpha = np.asarray(alpha, dtype=LD)
+        x64 = self.x.astype(np.float64)
+        span = float(PREDICT_WINDOW * self.ell)
+        mean = np.empty(t.size, dtype=LD)
+        var = np.empty(t.size, dtype=LD)
+        for k, tk in enumerate(t):
+            lo = int(np.searchsorted(x64, tk - span, side="left"))
+            hi = int(np.searchsorted(x64, tk + span, side="right"))
+            lo1 = max(lo - 1, 0)
+            kt = self.c * np.exp(-np.abs(self.x[lo1:hi] - LD(tk)) / self.ell)  # K(x_j, t) for j in [lo1, hi)
+            cur = kt[lo - lo1:]
+            prev = np.empty_like(cur)  # K(x_{j-1}, t); rho_0 = 0 makes the first row's value irrelevant
+            prev[1:] = cur[:-1]
+            prev[0] = kt[0] if lo1 < lo else 0
+            w = (cur - self.rho[lo:hi] * prev) / (self.sqrtc * self.s[lo:hi])
+            mean[k] = cur @ alpha[lo:hi]
+            var[k] = self.c - w @ w
+        return mean, var
+
+
+def exp_problem(n, ell, seed, x0=0.0, gap=(0.2, 1.0)):
+    """Sorted points with gaps drawn from ``uniform(*gap) * ell``, starting at ``x0``."""
+    rng = np.random.default_rng(seed)
+    x = np.empty(n)
+    x[0] = x0
+    x[1:] = x0 + np.cumsum(rng.uniform(gap[0], gap[1], n - 1) * ell)
+    return x

@@ -1,0 +1,118 @@
+# -*- coding: utf-8 -*-
+"""``tests/ou_reference.py`` against the O(n^3) longdouble references of ``tests/hiprec.py`` on the oracle's K.
+
+The closed forms are what the large-index GPU tests (``test_gpu_zz_large_index.py``) compare the solvers with at sizes
+where no O(n^3) reference runs, so each quantity they use is pinned here at n <= 500: the factor's columns, log det,
+solves, the tridiagonal K^-1, ``z L^T``, ``D a``, the gradient terms (against ``einsum`` over the oracle's gradient
+tensor, which also fixes the factor 1/2 and the sign of the ``log m`` derivative) and the predictive mean and variance.
+The differences are the float64 rounding of K's entries carried through cond(K) <= 10 (largest measured: 7.7e-16, in
+K^-1 and the gradient's diagonal; bar 1e-14).
+"""
+import numpy as np
+import pytest
+
+import hiprec
+import ou_reference
+
+LD = np.longdouble
+TOL = 1e-14
+
+# (n, c, m, gap): gaps are uniform(gap) * sqrt(m); the last case spans ~1100 length scales, so the far entries of the
+# float64 K underflow to 0 while the closed form keeps them (exp(-1100) ~ 1e-478 in longdouble)
+CASES = [(1, 1.0, 1.0, (0.2, 1.0)), (2, 0.7, 2.0, (0.2, 1.0)), (65, 1.0, 1.0, (0.2, 1.0)),
+         (300, 2.5, 0.04, (0.2, 1.0)), (500, 0.3, 9.0, (0.2, 1.0)), (500, 1.7, 0.5, (1.5, 3.0))]
+
+
+def _case(n, c, m, gap):
+    from george_b200 import kernels
+    from george_b200._spec import flatten
+    import oracle
+    x = ou_reference.exp_problem(n, np.sqrt(m), seed=n, x0=-0.3 * n * np.sqrt(m), gap=gap)
+    kernel = c * kernels.ExpKernel(m)
+    spec = flatten(kernel)
+    K = oracle.value_symmetric(spec, x[:, None])
+    return x, kernel, spec, K, ou_reference.OU(x, c, m)
+
+
+def _rel(A, Ref):
+    Ref = np.asarray(Ref, dtype=LD)
+    den = np.max(np.abs(Ref))
+    return float(np.max(np.abs(np.asarray(A, dtype=LD) - Ref)) / (den if den > 0 else 1))
+
+
+@pytest.mark.parametrize("n,c,m,gap", CASES)
+def test_closed_forms_match_the_longdouble_factorisation(oracle, n, c, m, gap):
+    x, kernel, spec, K, ou = _case(n, c, m, gap)
+    if gap[0] > 1:
+        assert np.sum(K == 0) > n * n // 10  # the case it is meant to be (12 % of the entries)
+    L = hiprec.chol_ld(K)
+    assert abs(float(ou.logdet() - hiprec.logdet_ld(L))) <= TOL * max(1.0, abs(float(hiprec.logdet_ld(L))))
+    assert _rel(ou.chol_columns(np.arange(n)), L) <= TOL
+    cols = sorted({0, n // 2, n - 1})
+    assert np.array_equal(ou.chol_columns(cols), ou.chol_columns(np.arange(n))[:, cols])
+
+    rng = np.random.default_rng(n + 1)
+    B = rng.standard_normal((n, 3))
+    X = hiprec.solve_ld(L, B)
+    assert _rel(ou.solve(B), X) <= TOL
+    assert _rel(ou.solve(B[:, 0]), X[:, 0]) <= TOL
+    assert _rel(ou.inv_chol(B), _lower_solve(L, B)) <= TOL
+
+    Kinv = hiprec.solve_ld(L, np.eye(n))
+    d, e = ou.inv_tridiag()
+    T = np.diag(d)
+    if n > 1:
+        T += np.diag(e, 1) + np.diag(e, -1)
+    assert _rel(T, Kinv) <= TOL
+
+    Z = rng.standard_normal((4, n))
+    assert _rel(ou.sqrt_rows(Z), Z.astype(LD) @ L.T) <= TOL
+    assert _rel(ou.sqrt_rows(Z[0]), Z[0].astype(LD) @ L.T) <= TOL
+
+
+def _lower_solve(L, B):
+    X = np.array(B, dtype=LD)
+    for i in range(L.shape[0]):
+        X[i] = (X[i] - L[i, :i] @ X[:i]) / L[i, i]
+    return X
+
+
+@pytest.mark.parametrize("n,c,m,gap", CASES)
+def test_gradient_terms_match_the_oracle_gradient_tensor(oracle, n, c, m, gap):
+    x, kernel, spec, K, ou = _case(n, c, m, gap)
+    assert list(kernel.get_parameter_names(include_frozen=True)) == ["k1:log_constant", "k2:metric:log_M_0_0"]
+    L = hiprec.chol_ld(K)
+    Kinv = hiprec.solve_ld(L, np.eye(n))
+    dK = oracle.gradient_general(spec, [1, 1], x[:, None], x[:, None]).astype(LD)
+    # D = 2 dK/dlog m
+    a = np.random.default_rng(n + 2).standard_normal(n)
+    assert _rel(ou.apply_d(a), 2 * dK[:, :, 1] @ a.astype(LD)) <= TOL
+    assert abs(float(ou.trace_kinv_d() - 2 * np.sum(Kinv * dK[:, :, 1]))) <= TOL * max(1.0, float(np.sum(np.abs(Kinv * dK[:, :, 1]))))
+
+    r = np.sin(x / np.sqrt(m)) + 0.5
+    alpha_ref = Kinv @ r.astype(LD)
+    A = np.outer(alpha_ref, alpha_ref) - Kinv
+    g_ref = np.einsum("ijk,ij->k", dK, A)
+    scale = np.einsum("ijk,ij->k", np.abs(dK), np.abs(A))
+    alpha, g, diag = ou.grad_terms(r)
+    assert _rel(alpha, alpha_ref) <= TOL
+    assert np.all(np.abs(g - g_ref) <= TOL * scale), (g, g_ref, scale)
+    assert _rel(diag, np.diag(A)) <= TOL
+
+
+@pytest.mark.parametrize("n,c,m,gap", CASES)
+def test_prediction_matches_the_dense_formulas(oracle, n, c, m, gap):
+    x, kernel, spec, K, ou = _case(n, c, m, gap)
+    L = hiprec.chol_ld(K)
+    ell = np.sqrt(m)
+    rng = np.random.default_rng(n + 3)
+    # inside the data, on a data point, and beyond either end
+    t = np.concatenate((rng.uniform(x[0], x[-1], 16), [x[n // 2], x[0] - 0.7 * ell, x[-1] + 2.0 * ell]))
+    y = rng.standard_normal(n)
+    alpha = hiprec.solve_ld(L, y)
+    Kts = oracle.value_general(spec, t[:, None], x[:, None]).astype(LD)
+    W = _lower_solve(L, Kts.T)
+    mean, var = ou.predict(t, ou.solve(y))
+    assert _rel(mean, Kts @ alpha) <= TOL
+    assert np.max(np.abs(var - (LD(c) - np.sum(W * W, axis=0)))) <= TOL * c
+    assert abs(float(var[16])) <= TOL * c  # no variance left at a data point
