@@ -1051,8 +1051,18 @@ int bgp_dense_last_timing(const bgp_dense_t* h, double* ms2) {
 }  // extern "C"
 
 // ---- batched log-likelihood terms and predictions: many parameter vectors of one kernel program on the same x -------
-struct bgp_dense_batch {
+// The stream is a base so that it is destroyed after the buffers: each DevBuf destructor issues its cudaFreeAsync on
+// it, then the stream is synchronised and destroyed.
+struct BatchStream {
   cudaStream_t s = nullptr;
+  ~BatchStream() {
+    if (s) {
+      cudaStreamSynchronize(s);
+      cudaStreamDestroy(s);
+    }
+  }
+};
+struct bgp_dense_batch : BatchStream {
   DevBuf<DevProgram> d_prog;
   DevBuf<double> d_x, d_yerr, d_diag, d_r, d_sol, d_tmp, d_A, d_out, d_fn;
   DevBuf<int> d_info;
@@ -1132,19 +1142,6 @@ static int batch_begin(bgp_dense_batch* h, const bgp_kernel_spec_t* spec, const 
   return BGP_OK;
 }
 
-// the chunk size for the device buffers reserve(chunk) allocates: halved while they do not fit, BGP_ERR_NOMEM when one
-// member does not; release() frees what a failed attempt left allocated
-template <class Reserve, class Release>
-static int batch_reserve_chunk(int64_t* chunk, Reserve reserve, Release release) {
-  for (;;) {
-    const int st = reserve(*chunk);
-    if (st == BGP_OK) return BGP_OK;
-    if (st != BGP_ERR_NOMEM || *chunk == 1) return st;
-    release();
-    *chunk = (*chunk + 1) / 2;
-  }
-}
-
 // the shared buffers of a chunk of `chunk` members (d_A is reserved by the caller) and the programs and x of all B
 static int batch_reserve_common(bgp_dense_batch* h, const BatchPrograms& bp, const double* x, int64_t n, int32_t ndim,
                                 int64_t chunk, int64_t tmp_cols) {
@@ -1160,6 +1157,13 @@ static int batch_reserve_common(bgp_dense_batch* h, const BatchPrograms& bp, con
   BGP_TRY(h->d_info.reserve((size_t)chunk, s));
   BGP_CUDA(cudaMemcpyAsync(h->d_prog.p, bp.progs.data(), sizeof(DevProgram) * B, cudaMemcpyHostToDevice, s));
   BGP_CUDA(cudaMemcpyAsync(h->d_x.p, x, sizeof(double) * n * ndim, cudaMemcpyHostToDevice, s));
+  return BGP_OK;
+}
+
+// the test points of the predictive entry points in d_xs (at least one double)
+static int batch_upload_xs(bgp_dense_batch* h, const double* xs, int64_t ns, int32_t ndim) {
+  BGP_TRY(h->d_xs.reserve((size_t)std::max<int64_t>(1, ns * ndim), h->s));
+  if (ns > 0) BGP_CUDA(cudaMemcpyAsync(h->d_xs.p, xs, sizeof(double) * ns * ndim, cudaMemcpyHostToDevice, h->s));
   return BGP_OK;
 }
 
@@ -1184,7 +1188,108 @@ static int batch_factor_chunk(bgp_dense_batch* h, const BatchPrograms& bp, int64
   return potrs_small_members(h->d_A.p, n, h->d_sol.p, 1, n, h->d_tmp.p, mc, mstride, n, s);
 }
 
-// members [c0, c0 + mc) after batch_factor_chunk: the steps of bgp_dense_predict's covariance path, member-indexed:
+// a device buffer of a member chunk: `per` doubles per member, at least one double in all
+struct ChunkBuf {
+  DevBuf<double>* buf;
+  int64_t per;
+};
+// a host output of a batched entry point: member b's row of `len` doubles at p + b * len (p may be null)
+struct BatchOut {
+  double* p;
+  int64_t len;
+};
+
+// The member chunking of every batched entry point, after batch_begin with B > 0.  A chunk has as many members as
+// the per-member workspace allows (batch_chunk_members), at most `cap` (one launch's descriptors), halved while the
+// chunk buffers `bufs` do not fit (BGP_ERR_NOMEM when one member's do not); then come the shared buffers and
+// setup(chunk), the entry point's own.  Each chunk of mc members from c0 runs batch_factor_chunk, then step(c0, mc,
+// progs, dprogs) with the members' host and device programs, copies the info words and synchronises.  Last, a member
+// whose program failed validation gets info = -1, and every output row of a member with info != 0 is NaN.
+template <class Setup, class Step>
+static int batch_run(bgp_dense_batch* h, const BatchPrograms& bp, const double* x, int64_t n, int32_t ndim,
+                     const double* yerr, const double* r, int64_t per_member, int64_t cap, int64_t tmp_cols,
+                     const std::vector<ChunkBuf>& bufs, Setup setup, Step step, int32_t* info,
+                     std::initializer_list<BatchOut> outs) {
+  cudaStream_t s = h->s;
+  const int64_t B = (int64_t)bp.progs.size();
+  int64_t chunk = std::max<int64_t>(1, std::min(batch_chunk_members(per_member, B), cap));
+  for (;;) {
+    int st = BGP_OK;
+    for (const ChunkBuf& b : bufs)
+      if ((st = b.buf->reserve((size_t)std::max<int64_t>(1, b.per * chunk), s)) != BGP_OK) break;
+    if (st == BGP_OK) break;
+    if (st != BGP_ERR_NOMEM || chunk == 1) return st;
+    for (const ChunkBuf& b : bufs) b.buf->release();
+    chunk = (chunk + 1) / 2;
+  }
+  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, tmp_cols));
+  BGP_TRY(setup(chunk));
+  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
+    const int mc = (int)std::min(chunk, B - c0);
+    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
+    BGP_TRY(step(c0, mc, bp.progs.data() + c0, h->d_prog.p + c0));
+    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaStreamSynchronize(s));
+  }
+  for (int64_t b = 0; b < B; ++b) {
+    if (!bp.valid[b]) info[b] = -1;
+    if (info[b] == 0) continue;
+    for (const BatchOut& o : outs)
+      if (o.p) std::fill(o.p + b * o.len, o.p + (b + 1) * o.len, std::nan(""));
+  }
+  return BGP_OK;
+}
+
+// The test-point chunking of the predictive entry points: chunks of c test points (the single path's
+// predict_chunk_cols(n, 1), whatever the number of members) ending in a ragged tail, the mean matvec's partials per
+// member, a VAR chunk's partials (var) and the split-K plan of the COV product (cov)
+struct BatchTestPlan {
+  int64_t c, tail, mvp, vp = 0, gsplit = 1;
+  BatchTestPlan(int64_t n, int64_t ns, bool var, bool cov)
+      : c(std::min(ns, predict_chunk_cols(n, 1))), tail(c > 0 ? ns - (ns - 1) / c * c : 0),
+        mvp(matvec_partial_size(ns, n)) {
+    if (var) vp = std::max(predict_var_partial_size(n, c), predict_var_partial_size(n, tail));
+    int64_t gklen = 0;
+    if (cov && ns > 0) predict_gemm_plan(ns, ns, n, &gsplit, &gklen);
+  }
+};
+
+// members [0, mc) after batch_factor_chunk: log_det_b into d_out and quad_b = r_b^T K_b^-1 r_b, a fixed-order dot of
+// r_b and alpha_b, into d_out + chunk
+static int batch_loglik_chunk(bgp_dense_batch* h, int mc, int64_t n, int64_t chunk) {
+  logdet_diag_kernel<<<(unsigned)mc, 1024, 0, h->s>>>(h->d_A.p, n, n, h->d_out.p, n * n);
+  BGP_LAUNCH_CHECK();
+  dot_rows_kernel<<<(unsigned)mc, 256, 0, h->s>>>(h->d_r.p, h->d_sol.p, n, h->d_out.p + chunk);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
+// members [0, mc) after batch_factor_chunk: mean_b = K_b(x*, x) alpha_b into d_mean (member stride ns), the matvec
+// GP.predict computes for its mean
+static int batch_mean_chunk(bgp_dense_batch* h, const DevProgram* dprogs, int32_t ndim, int mc, int64_t n, int64_t ns) {
+  return kmat_matvec_batch_launch(dprogs, ndim, mc, h->d_xs.p, ns, h->d_x.p, n, h->d_sol.p, n, h->d_mean.p, ns,
+                                  h->d_mvp.p, h->s);
+}
+
+// members [0, mc) after batch_factor_chunk, test points [j0, j0 + nc) of a VAR chunk of c: the steps of
+// bgp_dense_predict's variance loop, member-indexed.  W = L_b^-1 K_b(x, x*) (d_W, the columns of all members
+// interleaved as in batch_cov_chunk), k(x*, x*) and the variances (d_var, member stride c), copied to var + j0 on the
+// host (member stride ns).
+static int batch_var_chunk(bgp_dense_batch* h, const DevProgram* progs, const DevProgram* dprogs, int mc, int64_t n,
+                           int32_t ndim, int64_t c, int64_t j0, int64_t nc, double* var, int64_t ns) {
+  cudaStream_t s = h->s;
+  const int64_t ldw = (int64_t)mc * n;
+  const double* xc = h->d_xs.p + j0 * ndim;
+  BGP_TRY(kmat_general_batch_launch_auto(progs, dprogs, mc, xc, nc, h->d_x.p, n, h->d_W.p, ldw, n, h->d_fn, s));
+  BGP_TRY(trsm_fwd_members(h->d_A.p, n, n * n, h->d_W.p, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
+  BGP_TRY(kmat_diagonal_launch(dprogs, xc, xc, nc, h->d_kd.p, s, mc, c));
+  BGP_TRY(predict_var_batch_launch(h->d_W.p, ldw, h->d_W.p, ldw, n, nc, h->d_kd.p, h->d_var.p, mc, n, c, h->d_vp, s));
+  BGP_CUDA(cudaMemcpy2DAsync(var + j0, sizeof(double) * ns, h->d_var.p, sizeof(double) * c, sizeof(double) * nc, mc,
+                             cudaMemcpyDeviceToHost, s));
+  return BGP_OK;
+}
+
+// members [0, mc) after batch_factor_chunk: the steps of bgp_dense_predict's covariance path, member-indexed:
 // K**, every W chunk resident (W = L_b^-1 K_b(x, x*), test-point chunks of c columns), C_b = K** - W^T W into d_C
 // (member stride ns^2).  The W columns of all members are interleaved: column j of member m at W + (j * mc + m) * n, so
 // that the columns of a test-point chunk are one contiguous block (the few-column solve copies its result back in one
@@ -1212,23 +1317,7 @@ int bgp_dense_batch_create(bgp_dense_batch_t** out) {
   return BGP_OK;
 }
 
-void bgp_dense_batch_destroy(bgp_dense_batch_t* h) {
-  if (!h) return;
-  if (h->s) cudaStreamSynchronize(h->s);
-  h->d_prog.release(); h->d_x.release(); h->d_yerr.release(); h->d_diag.release(); h->d_r.release();
-  h->d_sol.release(); h->d_tmp.release(); h->d_A.release(); h->d_out.release(); h->d_fn.release();
-  h->d_info.release(); h->d_gdesc.release();
-  h->d_xs.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_kd.release();
-  h->d_var.release(); h->d_vp.release(); h->d_C.release(); h->d_slices.release(); h->d_pdesc.release();
-  h->d_inv.release(); h->d_gp.release(); h->d_g.release(); h->d_which.release();
-  h->d_madd.release(); h->d_z.release(); h->d_draws.release(); h->d_dinfo.release(); h->d_sdesc.release();
-  h->d_dmu.release(); h->d_dvar.release(); h->d_xgp.release();
-  if (h->s) {
-    cudaStreamSynchronize(h->s);
-    cudaStreamDestroy(h->s);
-  }
-  delete h;
-}
+void bgp_dense_batch_destroy(bgp_dense_batch_t* h) { delete h; }
 
 int bgp_dense_batch_log_likelihood(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params,
                                    int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
@@ -1238,31 +1327,20 @@ int bgp_dense_batch_log_likelihood(bgp_dense_batch_t* h, const bgp_kernel_spec_t
   BGP_TRY(batch_begin(h, spec, params, B, P, x, n, ndim, &bp));
   if (B == 0) return BGP_OK;
   cudaStream_t s = h->s;
-  int64_t chunk = batch_chunk_members(n * n, B);
-  const size_t nn = (size_t)n * (size_t)n;
-  // the matrices of a chunk; a smaller chunk when they do not fit, BGP_ERR_NOMEM when one member does not
-  BGP_TRY(batch_reserve_chunk(&chunk, [&](int64_t c) { return h->d_A.reserve(nn * (size_t)c, s); }, [] {}));
-  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, 1));
-  BGP_TRY(h->d_out.reserve((size_t)2 * chunk, s));
-  const int64_t mstride = (int64_t)nn;
-  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
-    const int mc = (int)std::min(chunk, B - c0);
-    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
-    logdet_diag_kernel<<<(unsigned)mc, 1024, 0, s>>>(h->d_A.p, n, n, h->d_out.p, mstride);
-    BGP_LAUNCH_CHECK();
-    // quad = r^T K^-1 r: a fixed-order dot per member of r and the solve above
-    dot_rows_kernel<<<(unsigned)mc, 256, 0, s>>>(h->d_r.p, h->d_sol.p, n, h->d_out.p + chunk);
-    BGP_LAUNCH_CHECK();
+  const int64_t nn = n * n;
+  int64_t chunk = 0;
+  auto setup = [&](int64_t c) {
+    chunk = c;
+    return h->d_out.reserve((size_t)2 * c, s);
+  };
+  auto step = [&](int64_t c0, int mc, const DevProgram*, const DevProgram*) -> int {
+    BGP_TRY(batch_loglik_chunk(h, mc, n, chunk));
     BGP_CUDA(cudaMemcpyAsync(log_det + c0, h->d_out.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, s));
     BGP_CUDA(cudaMemcpyAsync(quad + c0, h->d_out.p + chunk, sizeof(double) * mc, cudaMemcpyDeviceToHost, s));
-    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
-    BGP_CUDA(cudaStreamSynchronize(s));
-  }
-  for (int64_t b = 0; b < B; ++b) {
-    if (!bp.valid[b]) info[b] = -1;
-    if (info[b] != 0) log_det[b] = quad[b] = std::nan("");
-  }
-  return BGP_OK;
+    return BGP_OK;
+  };
+  return batch_run(h, bp, x, n, ndim, yerr, r, nn, 65535, 1, {{&h->d_A, nn}}, setup, step, info,
+                   {{log_det, 1}, {quad, 1}});
 }
 
 int bgp_dense_batch_grad_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
@@ -1280,57 +1358,34 @@ int bgp_dense_batch_grad_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* sp
   const int64_t nt = (n + 31) / 32;  // the contraction's 32 x 32 tiles
   // doubles per member (see include/bgp.h): factor, K^-1, the vectors of batch_reserve_common, partials, g
   const int64_t per_member = 2 * nn + (4 + tmp_cols) * n + nt * nt * P + P;
-  int64_t chunk = batch_chunk_members(per_member, B);
-  auto release = [&] { h->d_A.release(); h->d_inv.release(); h->d_gp.release(); h->d_g.release(); };
-  auto reserve = [&](int64_t m) -> int {
-    BGP_TRY(h->d_A.reserve((size_t)(nn * m), s));
-    BGP_TRY(h->d_inv.reserve((size_t)(nn * m), s));
-    BGP_TRY(h->d_gp.reserve((size_t)std::max<int64_t>(1, nt * nt * P * m), s));
-    BGP_TRY(h->d_g.reserve((size_t)std::max<int64_t>(1, P * m), s));
+  int64_t chunk = 0;
+  auto setup = [&](int64_t c) -> int {
+    chunk = c;
+    BGP_TRY(h->d_out.reserve((size_t)2 * c, s));
+    BGP_TRY(h->d_which.reserve((size_t)std::max<int64_t>(1, P), s));
+    if (P > 0) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * P, cudaMemcpyHostToDevice, s));
     return BGP_OK;
   };
-  BGP_TRY(batch_reserve_chunk(&chunk, reserve, release));
-  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, tmp_cols));
-  BGP_TRY(h->d_out.reserve((size_t)2 * chunk, s));
-  BGP_TRY(h->d_which.reserve((size_t)std::max<int64_t>(1, P), s));
-  if (P > 0) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * P, cudaMemcpyHostToDevice, s));
-  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
-    const int mc = (int)std::min(chunk, B - c0);
-    // the steps of bgp_dense_compute and bgp_dense_grad_terms, member-indexed: factor and alpha (d_sol), log_det and
-    // quad as bgp_dense_batch_log_likelihood computes them
-    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
-    logdet_diag_kernel<<<(unsigned)mc, 1024, 0, s>>>(h->d_A.p, n, n, h->d_out.p, nn);
-    BGP_LAUNCH_CHECK();
-    dot_rows_kernel<<<(unsigned)mc, 256, 0, s>>>(h->d_r.p, h->d_sol.p, n, h->d_out.p + chunk);
-    BGP_LAUNCH_CHECK();
+  // the steps of bgp_dense_compute and bgp_dense_grad_terms, member-indexed: log_det and quad as
+  // bgp_dense_batch_log_likelihood computes them
+  auto step = [&](int64_t c0, int mc, const DevProgram*, const DevProgram* dprogs) -> int {
+    BGP_TRY(batch_loglik_chunk(h, mc, n, chunk));
     // K_b^-1 by solving against the identity
     BGP_TRY(fill_identity_members(h->d_inv.p, n, mc, s));
     BGP_TRY(potrs_members(h->d_A.p, n, nn, h->d_inv.p, n, n, nn, mc, h->d_tmp.p, s));
     // g_b and diag(alpha_b alpha_b^T - K_b^-1); the diagonal goes to d_diag, whose yerr^2 the build above consumed
-    BGP_TRY(kmat_grad_contract_members(h->d_prog.p + c0, (int)P, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, nn,
-                                       h->d_sol.p, n, 1.0, -1.0, h->d_g.p, P, diag ? h->d_diag.p : nullptr, n, mc,
-                                       h->d_gp, s));
+    BGP_TRY(kmat_grad_contract_members(dprogs, (int)P, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, nn, h->d_sol.p, n,
+                                       1.0, -1.0, h->d_g.p, P, diag ? h->d_diag.p : nullptr, n, mc, h->d_gp, s));
     if (log_det) BGP_CUDA(cudaMemcpyAsync(log_det + c0, h->d_out.p, sizeof(double) * mc, cudaMemcpyDeviceToHost, s));
     if (quad) BGP_CUDA(cudaMemcpyAsync(quad + c0, h->d_out.p + chunk, sizeof(double) * mc, cudaMemcpyDeviceToHost, s));
     if (alpha) BGP_CUDA(cudaMemcpyAsync(alpha + c0 * n, h->d_sol.p, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
     if (diag) BGP_CUDA(cudaMemcpyAsync(diag + c0 * n, h->d_diag.p, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
     if (g && P > 0) BGP_CUDA(cudaMemcpyAsync(g + c0 * P, h->d_g.p, sizeof(double) * mc * P, cudaMemcpyDeviceToHost, s));
-    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
-    BGP_CUDA(cudaStreamSynchronize(s));
-  }
-  const double nan = std::nan("");
-  for (int64_t b = 0; b < B; ++b) {
-    if (!bp.valid[b]) info[b] = -1;
-    if (info[b] == 0) continue;
-    if (log_det) log_det[b] = nan;
-    if (quad) quad[b] = nan;
-    for (int64_t i = 0; i < n; ++i) {
-      if (alpha) alpha[b * n + i] = nan;
-      if (diag) diag[b * n + i] = nan;
-    }
-    if (g) for (int64_t q = 0; q < P; ++q) g[b * P + q] = nan;
-  }
-  return BGP_OK;
+    return BGP_OK;
+  };
+  return batch_run(h, bp, x, n, ndim, yerr, r, per_member, 65535, tmp_cols,
+                   {{&h->d_A, nn}, {&h->d_inv, nn}, {&h->d_gp, nt * nt * P}, {&h->d_g, P}}, setup, step, info,
+                   {{log_det, 1}, {quad, 1}, {alpha, n}, {diag, n}, {g, P}});
 }
 
 int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
@@ -1344,85 +1399,32 @@ int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec,
   cudaStream_t s = h->s;
   const bool var = out && what == BGP_PREDICT_VAR, cov = out && what == BGP_PREDICT_COV;
   const int64_t nn = n * n;
-  // test-point chunk of the W columns: the single path's (predict_chunk_cols(n, 1)), whatever the number of members
-  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
-  const int64_t tail = c > 0 ? ns - (ns - 1) / c * c : 0;
-  const int64_t mvp = matvec_partial_size(ns, n);
-  const int64_t vp = var ? std::max(predict_var_partial_size(n, c), predict_var_partial_size(n, tail)) : 0;
-  int64_t gsplit = 1, gklen = 0;
-  if (cov && ns > 0) predict_gemm_plan(ns, ns, n, &gsplit, &gklen);
+  const BatchTestPlan tp(n, ns, var, cov);
   const int64_t tmp_cols = (var || cov) ? DS_MAX_RHS : 1;
   // doubles per member (see include/bgp.h)
-  int64_t per_member = nn + (4 + tmp_cols) * n + ns + mvp;
-  if (var) per_member += n * c + 2 * c + vp;
-  if (cov) per_member += n * ns + ns * ns * (1 + gsplit);
-  int64_t chunk = batch_chunk_members(per_member, B);
-  if (cov) chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, 65535 / gsplit));  // one DMMA launch per chunk
-  auto release = [&] {
-    h->d_A.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_kd.release();
-    h->d_var.release(); h->d_vp.release(); h->d_C.release(); h->d_slices.release(); h->d_tmp.release();
-  };
-  auto reserve = [&](int64_t m) -> int {
-    BGP_TRY(h->d_A.reserve((size_t)(nn * m), s));
-    BGP_TRY(h->d_tmp.reserve((size_t)(n * m * tmp_cols), s));
-    BGP_TRY(h->d_mean.reserve((size_t)std::max<int64_t>(1, ns * m), s));
-    BGP_TRY(h->d_mvp.reserve((size_t)std::max<int64_t>(1, mvp * m), s));
+  int64_t per_member = nn + (4 + tmp_cols) * n + ns + tp.mvp;
+  if (var) per_member += n * tp.c + 2 * tp.c + tp.vp;
+  if (cov) per_member += n * ns + ns * ns * (1 + tp.gsplit);
+  std::vector<ChunkBuf> bufs = {{&h->d_A, nn}, {&h->d_tmp, n * tmp_cols}, {&h->d_mean, ns}, {&h->d_mvp, tp.mvp}};
+  if (var) bufs.insert(bufs.end(), {{&h->d_W, n * tp.c}, {&h->d_kd, tp.c}, {&h->d_var, tp.c}, {&h->d_vp, tp.vp}});
+  if (cov) bufs.insert(bufs.end(), {{&h->d_W, n * ns}, {&h->d_C, ns * ns}, {&h->d_slices, ns * ns * tp.gsplit}});
+  auto step = [&](int64_t c0, int mc, const DevProgram* progs, const DevProgram* dprogs) -> int {
+    BGP_TRY(batch_mean_chunk(h, dprogs, ndim, mc, n, ns));
+    if (ns > 0)
+      BGP_CUDA(cudaMemcpyAsync(mean + c0 * ns, h->d_mean.p, sizeof(double) * mc * ns, cudaMemcpyDeviceToHost, s));
     if (var) {
-      BGP_TRY(h->d_W.reserve((size_t)std::max<int64_t>(1, n * c * m), s));
-      BGP_TRY(h->d_kd.reserve((size_t)std::max<int64_t>(1, c * m), s));
-      BGP_TRY(h->d_var.reserve((size_t)std::max<int64_t>(1, c * m), s));
-      BGP_TRY(h->d_vp.reserve((size_t)std::max<int64_t>(1, vp * m), s));
-    }
-    if (cov) {
-      BGP_TRY(h->d_W.reserve((size_t)std::max<int64_t>(1, n * ns * m), s));
-      BGP_TRY(h->d_C.reserve((size_t)std::max<int64_t>(1, ns * ns * m), s));
-      BGP_TRY(h->d_slices.reserve((size_t)std::max<int64_t>(1, ns * ns * gsplit * m), s));
+      for (int64_t j0 = 0; j0 < ns; j0 += tp.c)
+        BGP_TRY(batch_var_chunk(h, progs, dprogs, mc, n, ndim, tp.c, j0, std::min(tp.c, ns - j0), out + c0 * ns, ns));
+    } else if (cov && ns > 0) {
+      BGP_TRY(batch_cov_chunk(h, progs, dprogs, mc, n, ndim, ns, tp.c));
+      BGP_CUDA(cudaMemcpyAsync(out + c0 * ns * ns, h->d_C.p, sizeof(double) * mc * ns * ns, cudaMemcpyDeviceToHost, s));
     }
     return BGP_OK;
   };
-  BGP_TRY(batch_reserve_chunk(&chunk, reserve, release));
-  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, tmp_cols));
-  BGP_TRY(h->d_xs.reserve((size_t)std::max<int64_t>(1, ns * ndim), s));
-  if (ns > 0) BGP_CUDA(cudaMemcpyAsync(h->d_xs.p, xs, sizeof(double) * ns * ndim, cudaMemcpyHostToDevice, s));
-  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
-    const int mc = (int)std::min(chunk, B - c0);
-    const DevProgram* progs = bp.progs.data() + c0;
-    const DevProgram* dprogs = h->d_prog.p + c0;
-    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
-    // mean_b = K_b(x*, x) alpha_b, the matvec GP.predict computes for its mean
-    BGP_TRY(kmat_matvec_batch_launch(dprogs, ndim, mc, h->d_xs.p, ns, h->d_x.p, n, h->d_sol.p, n, h->d_mean.p, ns,
-                                     h->d_mvp.p, s));
-    if (ns > 0)
-      BGP_CUDA(cudaMemcpyAsync(mean + c0 * ns, h->d_mean.p, sizeof(double) * mc * ns, cudaMemcpyDeviceToHost, s));
-    // W columns of all members interleaved, as in batch_cov_chunk
-    const int64_t ldw = (int64_t)mc * n;
-    if (var) {
-      // the steps of bgp_dense_predict's variance loop, member-indexed
-      for (int64_t j0 = 0; j0 < ns; j0 += c) {
-        const int64_t nc = std::min(c, ns - j0);
-        const double* xc = h->d_xs.p + j0 * ndim;
-        BGP_TRY(kmat_general_batch_launch_auto(progs, dprogs, mc, xc, nc, h->d_x.p, n, h->d_W.p, ldw, n, h->d_fn, s));
-        BGP_TRY(trsm_fwd_members(h->d_A.p, n, nn, h->d_W.p, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
-        BGP_TRY(kmat_diagonal_launch(dprogs, xc, xc, nc, h->d_kd.p, s, mc, c));
-        BGP_TRY(predict_var_batch_launch(h->d_W.p, ldw, h->d_W.p, ldw, n, nc, h->d_kd.p, h->d_var.p, mc, n, c, h->d_vp, s));
-        BGP_CUDA(cudaMemcpy2DAsync(out + c0 * ns + j0, sizeof(double) * ns, h->d_var.p, sizeof(double) * c,
-                                   sizeof(double) * nc, mc, cudaMemcpyDeviceToHost, s));
-      }
-    } else if (cov && ns > 0) {
-      BGP_TRY(batch_cov_chunk(h, progs, dprogs, mc, n, ndim, ns, c));
-      BGP_CUDA(cudaMemcpyAsync(out + c0 * ns * ns, h->d_C.p, sizeof(double) * mc * ns * ns, cudaMemcpyDeviceToHost, s));
-    }
-    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
-    BGP_CUDA(cudaStreamSynchronize(s));
-  }
-  const int64_t osize = var ? ns : cov ? ns * ns : 0;
-  for (int64_t b = 0; b < B; ++b) {
-    if (!bp.valid[b]) info[b] = -1;
-    if (info[b] == 0) continue;
-    for (int64_t j = 0; j < ns; ++j) mean[b * ns + j] = std::nan("");
-    for (int64_t j = 0; j < osize; ++j) out[b * osize + j] = std::nan("");
-  }
-  return BGP_OK;
+  // COV: one DMMA launch per chunk, one descriptor per member and split-K slice
+  return batch_run(h, bp, x, n, ndim, yerr, r, per_member, 65535 / tp.gsplit, tmp_cols, bufs,
+                   [&](int64_t) { return batch_upload_xs(h, xs, ns, ndim); }, step, info,
+                   {{mean, ns}, {out, var ? ns : cov ? ns * ns : 0}});
 }
 
 int bgp_dense_batch_predict_grad(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
@@ -1438,98 +1440,48 @@ int bgp_dense_batch_predict_grad(bgp_dense_batch_t* h, const bgp_kernel_spec_t* 
   cudaStream_t s = h->s;
   const int64_t nn = n * n;
   const int64_t nd = ndim;
-  // bgp_dense_batch_predict's mean and VAR workspace (the single path's test-point chunk), plus dmu, a chunk of dvar
-  // and the contraction partials (the larger of dmu's and a dvar chunk's: they run one after the other)
-  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
-  const int64_t tail = c > 0 ? ns - (ns - 1) / c * c : 0;
-  const int64_t mvp = matvec_partial_size(ns, n);
-  const int64_t vp = with_var ? std::max(predict_var_partial_size(n, c), predict_var_partial_size(n, tail)) : 0;
+  // bgp_dense_batch_predict's mean and VAR workspace, plus dmu, a chunk of dvar and the contraction partials (the
+  // larger of dmu's and a dvar chunk's: they run one after the other)
+  const BatchTestPlan tp(n, ns, with_var, false);
+  const int64_t c = tp.c;
   int64_t xgp = x1_grad_partial_size(ns, n, ndim);
-  if (with_var) xgp = std::max(xgp, std::max(x1_grad_partial_size(c, n, ndim), x1_grad_partial_size(tail, n, ndim)));
+  if (with_var) xgp = std::max(xgp, std::max(x1_grad_partial_size(c, n, ndim), x1_grad_partial_size(tp.tail, n, ndim)));
   const int64_t tmp_cols = with_var ? DS_MAX_RHS : 1;
   // doubles per member (see include/bgp.h)
-  int64_t per_member = nn + (4 + tmp_cols) * n + ns + mvp + ns * nd + xgp;
-  if (with_var) per_member += n * c + 2 * c + vp + c * nd;
-  int64_t chunk = batch_chunk_members(per_member, B);
-  auto release = [&] {
-    h->d_A.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_kd.release();
-    h->d_var.release(); h->d_vp.release(); h->d_tmp.release(); h->d_dmu.release(); h->d_dvar.release();
-    h->d_xgp.release();
-  };
-  auto reserve = [&](int64_t m) -> int {
-    BGP_TRY(h->d_A.reserve((size_t)(nn * m), s));
-    BGP_TRY(h->d_tmp.reserve((size_t)(n * m * tmp_cols), s));
-    BGP_TRY(h->d_mean.reserve((size_t)std::max<int64_t>(1, ns * m), s));
-    BGP_TRY(h->d_mvp.reserve((size_t)std::max<int64_t>(1, mvp * m), s));
-    BGP_TRY(h->d_dmu.reserve((size_t)std::max<int64_t>(1, ns * nd * m), s));
-    BGP_TRY(h->d_xgp.reserve((size_t)std::max<int64_t>(1, xgp * m), s));
-    if (with_var) {
-      BGP_TRY(h->d_W.reserve((size_t)std::max<int64_t>(1, n * c * m), s));
-      BGP_TRY(h->d_kd.reserve((size_t)std::max<int64_t>(1, c * m), s));
-      BGP_TRY(h->d_var.reserve((size_t)std::max<int64_t>(1, c * m), s));
-      BGP_TRY(h->d_vp.reserve((size_t)std::max<int64_t>(1, vp * m), s));
-      BGP_TRY(h->d_dvar.reserve((size_t)std::max<int64_t>(1, c * nd * m), s));
-    }
-    return BGP_OK;
-  };
-  BGP_TRY(batch_reserve_chunk(&chunk, reserve, release));
-  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, tmp_cols));
-  BGP_TRY(h->d_xs.reserve((size_t)std::max<int64_t>(1, ns * nd), s));
-  if (ns > 0) BGP_CUDA(cudaMemcpyAsync(h->d_xs.p, xs, sizeof(double) * ns * nd, cudaMemcpyHostToDevice, s));
-  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
-    const int mc = (int)std::min(chunk, B - c0);
-    const DevProgram* progs = bp.progs.data() + c0;
-    const DevProgram* dprogs = h->d_prog.p + c0;
-    // the steps of bgp_dense_batch_predict (factor, alpha, mean, VAR), then those of bgp_dense_predict_grad, with a
-    // member index.  A member whose K is not positive definite runs the later steps on its own slabs.
-    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
+  int64_t per_member = nn + (4 + tmp_cols) * n + ns + tp.mvp + ns * nd + xgp;
+  if (with_var) per_member += n * c + 2 * c + tp.vp + c * nd;
+  std::vector<ChunkBuf> bufs = {{&h->d_A, nn},       {&h->d_tmp, n * tmp_cols}, {&h->d_mean, ns},
+                                {&h->d_mvp, tp.mvp}, {&h->d_dmu, ns * nd},      {&h->d_xgp, xgp}};
+  if (with_var)
+    bufs.insert(bufs.end(), {{&h->d_W, n * c}, {&h->d_kd, c}, {&h->d_var, c}, {&h->d_vp, tp.vp}, {&h->d_dvar, c * nd}});
+  // the steps of bgp_dense_batch_predict (factor, alpha, mean, VAR), then those of bgp_dense_predict_grad, with a
+  // member index.  A member whose K is not positive definite runs the later steps on its own slabs.
+  auto step = [&](int64_t c0, int mc, const DevProgram* progs, const DevProgram* dprogs) -> int {
     if (ns > 0) {
-      BGP_TRY(kmat_matvec_batch_launch(dprogs, ndim, mc, h->d_xs.p, ns, h->d_x.p, n, h->d_sol.p, n, h->d_mean.p, ns,
-                                       h->d_mvp.p, s));
+      BGP_TRY(batch_mean_chunk(h, dprogs, ndim, mc, n, ns));
       BGP_CUDA(cudaMemcpyAsync(mean + c0 * ns, h->d_mean.p, sizeof(double) * mc * ns, cudaMemcpyDeviceToHost, s));
       // dmu_b = sum_j d1 k_b(x*, x_j) alpha_bj: GP.grad_predict's kernel.x1_gradient_matvec(xs, x, alpha)
       BGP_TRY(kmat_x1_grad_matvec_members(progs, dprogs, mc, h->d_xs.p, ns, h->d_x.p, n, h->d_sol.p, 0, n, 1.0, 0,
                                           h->d_dmu.p, ns * nd, h->d_xgp, s));
       BGP_CUDA(cudaMemcpyAsync(dmu + c0 * ns * nd, h->d_dmu.p, sizeof(double) * mc * ns * nd, cudaMemcpyDeviceToHost, s));
     }
-    // W columns of all members interleaved, as in batch_cov_chunk
+    if (!with_var) return BGP_OK;
     const int64_t ldw = (int64_t)mc * n;
-    if (with_var) {
-      for (int64_t j0 = 0; j0 < ns; j0 += c) {
-        const int64_t nc = std::min(c, ns - j0);
-        const double* xc = h->d_xs.p + j0 * nd;
-        // bgp_dense_batch_predict's variance steps
-        BGP_TRY(kmat_general_batch_launch_auto(progs, dprogs, mc, xc, nc, h->d_x.p, n, h->d_W.p, ldw, n, h->d_fn, s));
-        BGP_TRY(trsm_fwd_members(h->d_A.p, n, nn, h->d_W.p, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
-        BGP_TRY(kmat_diagonal_launch(dprogs, xc, xc, nc, h->d_kd.p, s, mc, c));
-        BGP_TRY(predict_var_batch_launch(h->d_W.p, ldw, h->d_W.p, ldw, n, nc, h->d_kd.p, h->d_var.p, mc, n, c, h->d_vp, s));
-        BGP_CUDA(cudaMemcpy2DAsync(var + c0 * ns + j0, sizeof(double) * ns, h->d_var.p, sizeof(double) * c,
-                                   sizeof(double) * nc, mc, cudaMemcpyDeviceToHost, s));
-        // bgp_dense_predict_grad's: W <- L_b^-T W = K_b^-1 K_b(x, x*), dvar = dprior - 2 sum_j d1 k_b(x*, x_j) W_j
-        BGP_TRY(trsm_bwd_members(h->d_A.p, n, nn, h->d_W.p, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
-        BGP_TRY(kmat_x1_grad_matvec_members(progs, dprogs, mc, xc, nc, h->d_x.p, n, h->d_W.p, ldw, n, -2.0, 1,
-                                            h->d_dvar.p, c * nd, h->d_xgp, s));
-        BGP_CUDA(cudaMemcpy2DAsync(dvar + (c0 * ns + j0) * nd, sizeof(double) * ns * nd, h->d_dvar.p,
-                                   sizeof(double) * c * nd, sizeof(double) * nc * nd, mc, cudaMemcpyDeviceToHost, s));
-      }
+    for (int64_t j0 = 0; j0 < ns; j0 += c) {
+      const int64_t nc = std::min(c, ns - j0);
+      BGP_TRY(batch_var_chunk(h, progs, dprogs, mc, n, ndim, c, j0, nc, var + c0 * ns, ns));
+      // bgp_dense_predict_grad's: W <- L_b^-T W = K_b^-1 K_b(x, x*), dvar = dprior - 2 sum_j d1 k_b(x*, x_j) W_j
+      BGP_TRY(trsm_bwd_members(h->d_A.p, n, nn, h->d_W.p, nc, ldw, n, mc, h->d_tmp.p, ldw, s));
+      BGP_TRY(kmat_x1_grad_matvec_members(progs, dprogs, mc, h->d_xs.p + j0 * nd, nc, h->d_x.p, n, h->d_W.p, ldw, n,
+                                          -2.0, 1, h->d_dvar.p, c * nd, h->d_xgp, s));
+      BGP_CUDA(cudaMemcpy2DAsync(dvar + (c0 * ns + j0) * nd, sizeof(double) * ns * nd, h->d_dvar.p,
+                                 sizeof(double) * c * nd, sizeof(double) * nc * nd, mc, cudaMemcpyDeviceToHost, s));
     }
-    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
-    BGP_CUDA(cudaStreamSynchronize(s));
-  }
-  const double nan = std::nan("");
-  for (int64_t b = 0; b < B; ++b) {
-    if (!bp.valid[b]) info[b] = -1;
-    if (info[b] == 0) continue;
-    for (int64_t j = 0; j < ns; ++j) {
-      mean[b * ns + j] = nan;
-      if (with_var) var[b * ns + j] = nan;
-    }
-    for (int64_t j = 0; j < ns * nd; ++j) {
-      dmu[b * ns * nd + j] = nan;
-      if (with_var) dvar[b * ns * nd + j] = nan;
-    }
-  }
-  return BGP_OK;
+    return BGP_OK;
+  };
+  return batch_run(h, bp, x, n, ndim, yerr, r, per_member, 65535, tmp_cols, bufs,
+                   [&](int64_t) { return batch_upload_xs(h, xs, ns, ndim); }, step, info,
+                   {{mean, ns}, {var, with_var ? ns : 0}, {dmu, ns * nd}, {dvar, with_var ? ns * nd : 0}});
 }
 
 int bgp_dense_batch_sample(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
@@ -1543,77 +1495,52 @@ int bgp_dense_batch_sample(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, 
   cudaStream_t s = h->s;
   const bool draw = ns > 0 && size > 0;
   const int64_t nn = n * n;
-  // bgp_dense_batch_predict's COV workspace (the single path's test-point chunk and split-K plan) plus z, the draws
-  // and the mean
-  const int64_t c = std::min(ns, predict_chunk_cols(n, 1));
-  const int64_t mvp = matvec_partial_size(ns, n);
-  int64_t gsplit = 1, gklen = 0;
-  if (draw) predict_gemm_plan(ns, ns, n, &gsplit, &gklen);
+  const int64_t dsize = size * ns;  // a member's draws
+  // bgp_dense_batch_predict's COV workspace plus z, the draws and the mean
+  const BatchTestPlan tp(n, ns, false, draw);
   const int64_t tmp_cols = DS_MAX_RHS;
-  const int64_t per_member = nn + (4 + tmp_cols) * n + ns + mvp + n * ns + ns * ns * (1 + gsplit) + 2 * size * ns + ns;
-  int64_t chunk = batch_chunk_members(per_member, B);
+  const int64_t per_member =
+      nn + (4 + tmp_cols) * n + ns + tp.mvp + n * ns + ns * ns * (1 + tp.gsplit) + 2 * dsize + ns;
   // one launch per step for the chunk: the split-K product and the draws' DMMA product each take one descriptor per
   // member and slice, at most 65535 per launch
-  chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, 65535 / gsplit));
-  if (draw && mvn_product_descs(ns, size) > 0)
-    chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, 65535 / mvn_product_descs(ns, size)));
-  auto release = [&] {
-    h->d_A.release(); h->d_mean.release(); h->d_mvp.release(); h->d_W.release(); h->d_C.release();
-    h->d_slices.release(); h->d_tmp.release(); h->d_madd.release(); h->d_z.release(); h->d_draws.release();
+  int64_t cap = 65535 / tp.gsplit;
+  if (draw && mvn_product_descs(ns, size) > 0) cap = std::min<int64_t>(cap, 65535 / mvn_product_descs(ns, size));
+  std::vector<ChunkBuf> bufs = {{&h->d_A, nn}, {&h->d_tmp, n * tmp_cols}, {&h->d_mean, ns}, {&h->d_mvp, tp.mvp}};
+  if (draw)
+    bufs.insert(bufs.end(), {{&h->d_W, n * ns}, {&h->d_C, ns * ns}, {&h->d_slices, ns * ns * tp.gsplit},
+                             {&h->d_madd, ns}, {&h->d_z, dsize}, {&h->d_draws, dsize}});
+  auto setup = [&](int64_t c) -> int {
+    BGP_TRY(h->d_dinfo.reserve((size_t)c, s));
+    return batch_upload_xs(h, xs, ns, ndim);
   };
-  auto reserve = [&](int64_t m) -> int {
-    BGP_TRY(h->d_A.reserve((size_t)(nn * m), s));
-    BGP_TRY(h->d_tmp.reserve((size_t)(n * m * tmp_cols), s));
-    BGP_TRY(h->d_mean.reserve((size_t)std::max<int64_t>(1, ns * m), s));
-    BGP_TRY(h->d_mvp.reserve((size_t)std::max<int64_t>(1, mvp * m), s));
-    if (draw) {
-      BGP_TRY(h->d_W.reserve((size_t)(n * ns * m), s));
-      BGP_TRY(h->d_C.reserve((size_t)(ns * ns * m), s));
-      BGP_TRY(h->d_slices.reserve((size_t)(ns * ns * gsplit * m), s));
-      BGP_TRY(h->d_madd.reserve((size_t)(ns * m), s));
-      BGP_TRY(h->d_z.reserve((size_t)(size * ns * m), s));
-      BGP_TRY(h->d_draws.reserve((size_t)(size * ns * m), s));
+  // the steps of bgp_dense_batch_predict (factor, alpha, mean, COV), then those of bgp_dense_sample's draw with a
+  // member index.  A member whose K is not positive definite runs every later step on its own slabs, which no other
+  // member reads; nothing synchronises inside the chunk.
+  auto step = [&](int64_t c0, int mc, const DevProgram* progs, const DevProgram* dprogs) -> int {
+    if (!draw) {
+      for (int m = 0; m < mc; ++m) draw_info[c0 + m] = 0;
+      return BGP_OK;
     }
+    BGP_TRY(batch_mean_chunk(h, dprogs, ndim, mc, n, ns));
+    BGP_CUDA(cudaMemcpyAsync(h->d_madd.p, mean_add + c0 * ns, sizeof(double) * mc * ns, cudaMemcpyHostToDevice, s));
+    BGP_CUDA(cudaMemcpyAsync(h->d_z.p, z + c0 * dsize, sizeof(double) * mc * dsize, cudaMemcpyHostToDevice, s));
+    add_into_kernel<<<(unsigned)std::min<int64_t>((mc * ns + 255) / 256, 1184), 256, 0, s>>>(h->d_mean.p, h->d_madd.p,
+                                                                                            mc * ns);
+    BGP_LAUNCH_CHECK();
+    BGP_TRY(batch_cov_chunk(h, progs, dprogs, mc, n, ndim, ns, tp.c));
+    BGP_TRY(mvn_factor_members(h->d_C.p, ns, jitter, mc, h->d_dinfo.p, nullptr, h->d_gdesc, s));
+    BGP_TRY(mvn_product_members(h->d_C.p, ns, h->d_madd.p, ns, h->d_z.p, size, h->d_draws.p, mc, h->d_sdesc, s));
+    BGP_CUDA(cudaMemcpyAsync(draws + c0 * dsize, h->d_draws.p, sizeof(double) * mc * dsize, cudaMemcpyDeviceToHost, s));
+    BGP_CUDA(cudaMemcpyAsync(draw_info + c0, h->d_dinfo.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
     return BGP_OK;
   };
-  BGP_TRY(batch_reserve_chunk(&chunk, reserve, release));
-  BGP_TRY(batch_reserve_common(h, bp, x, n, ndim, chunk, tmp_cols));
-  BGP_TRY(h->d_dinfo.reserve((size_t)chunk, s));
-  BGP_TRY(h->d_xs.reserve((size_t)std::max<int64_t>(1, ns * ndim), s));
-  if (ns > 0) BGP_CUDA(cudaMemcpyAsync(h->d_xs.p, xs, sizeof(double) * ns * ndim, cudaMemcpyHostToDevice, s));
-  const int64_t dsize = size * ns;  // a member's draws
-  for (int64_t c0 = 0; c0 < B; c0 += chunk) {
-    const int mc = (int)std::min(chunk, B - c0);
-    const DevProgram* progs = bp.progs.data() + c0;
-    const DevProgram* dprogs = h->d_prog.p + c0;
-    // the steps of bgp_dense_batch_predict (factor, alpha, mean, COV), then those of bgp_dense_sample's draw with a
-    // member index.  A member whose K is not positive definite runs every later step on its own slabs, which no other
-    // member reads; nothing synchronises inside the chunk.
-    BGP_TRY(batch_factor_chunk(h, bp, c0, mc, n, yerr, r));
-    if (draw) {
-      BGP_TRY(kmat_matvec_batch_launch(dprogs, ndim, mc, h->d_xs.p, ns, h->d_x.p, n, h->d_sol.p, n, h->d_mean.p, ns,
-                                       h->d_mvp.p, s));
-      BGP_CUDA(cudaMemcpyAsync(h->d_madd.p, mean_add + c0 * ns, sizeof(double) * mc * ns, cudaMemcpyHostToDevice, s));
-      BGP_CUDA(cudaMemcpyAsync(h->d_z.p, z + c0 * dsize, sizeof(double) * mc * dsize, cudaMemcpyHostToDevice, s));
-      add_into_kernel<<<(unsigned)std::min<int64_t>((mc * ns + 255) / 256, 1184), 256, 0, s>>>(h->d_mean.p, h->d_madd.p,
-                                                                                              mc * ns);
-      BGP_LAUNCH_CHECK();
-      BGP_TRY(batch_cov_chunk(h, progs, dprogs, mc, n, ndim, ns, c));
-      BGP_TRY(mvn_factor_members(h->d_C.p, ns, jitter, mc, h->d_dinfo.p, nullptr, h->d_gdesc, s));
-      BGP_TRY(mvn_product_members(h->d_C.p, ns, h->d_madd.p, ns, h->d_z.p, size, h->d_draws.p, mc, h->d_sdesc, s));
-      BGP_CUDA(cudaMemcpyAsync(draws + c0 * dsize, h->d_draws.p, sizeof(double) * mc * dsize, cudaMemcpyDeviceToHost, s));
-      BGP_CUDA(cudaMemcpyAsync(draw_info + c0, h->d_dinfo.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
-    } else {
-      for (int m = 0; m < mc; ++m) draw_info[c0 + m] = 0;
-    }
-    BGP_CUDA(cudaMemcpyAsync(info + c0, h->d_info.p, sizeof(int) * mc, cudaMemcpyDeviceToHost, s));
-    BGP_CUDA(cudaStreamSynchronize(s));
-  }
+  BGP_TRY(batch_run(h, bp, x, n, ndim, yerr, r, per_member, cap, tmp_cols, bufs, setup, step, info, {{draws, dsize}}));
+  // a failed member has no draw_info; a failed draw's rows are NaN as well
   for (int64_t b = 0; b < B; ++b) {
-    if (!bp.valid[b]) info[b] = -1;
-    if (info[b] != 0) draw_info[b] = 0;
-    if (info[b] == 0 && draw_info[b] == 0) continue;
-    for (int64_t j = 0; j < dsize; ++j) draws[b * dsize + j] = std::nan("");
+    if (info[b] != 0)
+      draw_info[b] = 0;
+    else if (draw_info[b] != 0)
+      std::fill(draws + b * dsize, draws + (b + 1) * dsize, std::nan(""));
   }
   return BGP_OK;
 }

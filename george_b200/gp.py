@@ -45,6 +45,32 @@ def _check_rng(rng):
             type(rng).__name__))
 
 
+def _sampling_jitter(rng, jitter):
+    """The ``rng`` / ``jitter`` checks of the conditional draws: the jitter the device draws add (``TINY`` by
+    default), ``None`` without ``rng``, where no jitter may be given."""
+    if rng is None:
+        if jitter is not None:
+            raise ValueError("jitter applies only to draws with an rng; the host route adds nothing")
+        return None
+    _check_rng(rng)
+    jitter = TINY if jitter is None else float(jitter)
+    if not (np.isfinite(jitter) and jitter >= 0.0):
+        raise ValueError("jitter must be finite and >= 0, got {0}".format(jitter))
+    return jitter
+
+
+def _check_grad_predict_mean(mean):
+    if type(mean) is not ConstantModel:
+        raise NotImplementedError("grad_predict needs the mean model's gradient with respect to the inputs, which "
+                                  "the modeling protocol does not provide; only a constant mean is supported")
+
+
+def _check_grad_predict_dim(xs):
+    if xs.shape[1] > BGP_MAX_DIM:
+        raise ValueError("input-coordinate gradients support at most {0} dimensions (got {1})".format(
+            BGP_MAX_DIM, xs.shape[1]))
+
+
 def _check_size(size):
     size = int(size)
     if size < 0:
@@ -234,13 +260,16 @@ class GP(ModelSet):
         self.computed = True
         self._alpha = None
 
+    def _require_computed(self):
+        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
+            raise RuntimeError("You need to compute the model first")
+
     def recompute(self, quiet=False, **kwargs):
         """Refactorise if the kernel changed since the last ``compute``.  With ``quiet`` a failed factorisation
         returns ``False`` instead of raising."""
         if self.computed:
             return True
-        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
-            raise RuntimeError("You need to compute the model first")
+        self._require_computed()
         try:
             self.compute(self._x, np.sqrt(self._yerr2), **kwargs)
         except (ValueError, LinAlgError):
@@ -274,11 +303,7 @@ class GP(ModelSet):
 
         :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
         """
-        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
-            raise RuntimeError("You need to compute the model first")
-        vectors = np.asarray(vectors, dtype=np.float64)
-        if vectors.ndim != 2 or vectors.shape[1] != len(self):
-            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        vectors = self._batch_vectors(vectors)
         if vectors.shape[0] == 0:
             return np.empty(0, dtype=np.float64)
         batch = getattr(self.solver_type, "batch_log_likelihood", None)
@@ -286,30 +311,35 @@ class GP(ModelSet):
             out = self._batch_device(batch, vectors, y, quiet)
             if out is not None:
                 return out
-        return self._batch_loop(vectors, y, quiet)
+        return np.array(self._batch_loop(vectors, lambda: self.log_likelihood(y, quiet=quiet)), dtype=np.float64)
 
-    def _batch_state(self):
-        return (self.get_parameter_vector(include_frozen=True), [m.dirty for m in self.models.values()],
-                dict((k, self.__dict__[k]) for k in ("_computed", "solver", "_alpha", "_y", "_const", "_x", "_yerr2")
-                     if k in self.__dict__))
+    def _batch_vectors(self, vectors):
+        """The checks of every ``batch_*`` method that come before its own: a computed model and ``vectors`` of shape
+        ``(B, len(gp))``, returned as a float64 array."""
+        self._require_computed()
+        vectors = np.asarray(vectors, dtype=np.float64)
+        if vectors.ndim != 2 or vectors.shape[1] != len(self):
+            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        return vectors
 
-    def _batch_restore(self, state):
-        vector, dirty, attrs = state
-        self.set_parameter_vector(vector, include_frozen=True)
-        for m, d in zip(self.models.values(), dirty):
-            m.dirty = d
-        self.__dict__.update(attrs)
-
-    def _batch_loop(self, vectors, y, quiet):
-        state = self._batch_state()
+    def _batch_loop(self, vectors, fn):
+        """The per-vector path of the ``batch_*`` methods: ``[fn() for each member]`` with ``set_parameter_vector``
+        called for the member before ``fn``.  The GP is left as it was: parameter vector, factorisation, cached solve
+        and dirty flags."""
+        vector, dirty = self.get_parameter_vector(include_frozen=True), [m.dirty for m in self.models.values()]
+        attrs = dict((k, self.__dict__[k]) for k in ("_computed", "solver", "_alpha", "_y", "_const", "_x", "_yerr2")
+                     if k in self.__dict__)
         try:
-            out = np.empty(len(vectors), dtype=np.float64)
-            for b, v in enumerate(vectors):
+            res = []
+            for v in vectors:
                 self.set_parameter_vector(v)
-                out[b] = self.log_likelihood(y, quiet=quiet)
-            return out
+                res.append(fn())
+            return res
         finally:
-            self._batch_restore(state)
+            self.set_parameter_vector(vector, include_frozen=True)
+            for m, d in zip(self.models.values(), dirty):
+                m.dirty = d
+            self.__dict__.update(attrs)
 
     def _swap_eval(self, model, vector, fn):
         """``fn()`` with only ``model``'s full parameter vector set to ``vector``; the model is restored after."""
@@ -398,6 +428,25 @@ class GP(ModelSet):
             return e
         return ValueError("invalid kernel")
 
+    def _raise_member_error(self, spec, kpar, info, fact_err, *later):
+        """Raise the exception the per-vector loop meets first, member by member: the white noise or the
+        factorisation (``fact_err``, ``info``), then the first of ``later`` (per-member lists of an exception or
+        ``None``, in the loop's order)."""
+        for b in range(len(info)):
+            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
+            for errs in later:
+                if exc is None:
+                    exc = errs[b]
+            if exc is not None:
+                raise exc
+
+    def _batch_ll(self, log_det, quad):
+        """GP.compute / GP.log_likelihood over the members, in the same order of operations."""
+        const = -0.5 * (len(self._x) * np.log(2 * np.pi) + log_det)
+        ll = const - 0.5 * quad
+        ll[~np.isfinite(ll)] = -np.inf
+        return ll
+
     def _batch_device(self, batch, vectors, y, quiet):
         """The batched dense path of :func:`batch_log_likelihood`; ``None`` when the kernel has no valid device
         program."""
@@ -406,12 +455,8 @@ class GP(ModelSet):
         if members is None:
             return None
         spec, _, kpar, sigma, resid, fact_err, mean_err = members
-        n = len(self._x)
         log_det, quad, info = batch(spec, kpar, self._x, sigma, resid)
-        # GP.compute / GP.log_likelihood, in the same order of operations
-        const = -0.5 * (n * np.log(2 * np.pi) + log_det)
-        ll = const - 0.5 * quad
-        ll[~np.isfinite(ll)] = -np.inf
+        ll = self._batch_ll(log_det, quad)
         for b in range(len(vectors)):
             exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
             if exc is not None:
@@ -444,11 +489,7 @@ class GP(ModelSet):
 
         :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
         """
-        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
-            raise RuntimeError("You need to compute the model first")
-        vectors = np.asarray(vectors, dtype=np.float64)
-        if vectors.ndim != 2 or vectors.shape[1] != len(self):
-            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        vectors = self._batch_vectors(vectors)
         self._check_dimensions(y)
         xs = self.parse_samples(t)
         what = "var" if return_var else ("cov" if return_cov else None)
@@ -463,17 +504,8 @@ class GP(ModelSet):
             out = self._batch_predict_device(batch, vectors, y, xs, what)
             if out is not None:
                 return out
-        return self._batch_predict_loop(vectors, y, t, return_cov, return_var, kernel)
-
-    def _batch_predict_loop(self, vectors, y, t, return_cov, return_var, kernel):
-        state = self._batch_state()
-        try:
-            res = []
-            for v in vectors:
-                self.set_parameter_vector(v)
-                res.append(self.predict(y, t, return_cov=return_cov, return_var=return_var, kernel=kernel))
-        finally:
-            self._batch_restore(state)
+        res = self._batch_loop(vectors, lambda: self.predict(y, t, return_cov=return_cov, return_var=return_var,
+                                                             kernel=kernel))
         if not (return_var or return_cov):
             return np.stack(res)
         return np.stack([r[0] for r in res]), np.stack([r[1] for r in res])
@@ -486,11 +518,7 @@ class GP(ModelSet):
         spec, full, kpar, sigma, resid, fact_err, mean_err = members
         mean_xs, xs_err = self._batch_mean_at(full, xs)
         mu, out, info = batch(spec, kpar, self._x, sigma, resid, xs, what)
-        for b in range(len(vectors)):  # the loop's order: white noise, factorisation, residual, mean at x*
-            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
-            exc = exc if exc is not None else (mean_err[b] if mean_err[b] is not None else xs_err[b])
-            if exc is not None:
-                raise exc
+        self._raise_member_error(spec, kpar, info, fact_err, mean_err, xs_err)  # residual, mean at x*
         mu += mean_xs
         return mu if what is None else (mu, out)
 
@@ -594,11 +622,7 @@ class GP(ModelSet):
 
         :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
         """
-        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
-            raise RuntimeError("You need to compute the model first")
-        vectors = np.asarray(vectors, dtype=np.float64)
-        if vectors.ndim != 2 or vectors.shape[1] != len(self):
-            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        vectors = self._batch_vectors(vectors)
         self._check_dimensions(y)
         out = None
         if len(vectors) == 0:
@@ -607,39 +631,23 @@ class GP(ModelSet):
         if out is None and batch is not None and (len(self.white_noise) or len(self.kernel)):
             out = self._batch_grad_device(batch, vectors, y, quiet, return_log_likelihood)
         if out is None:
-            out = self._batch_grad_loop(vectors, y, quiet, return_log_likelihood)
+            res = self._batch_loop(vectors, lambda: (self.log_likelihood(y, quiet=quiet) if return_log_likelihood
+                                                     else np.nan, self.grad_log_likelihood(y, quiet=quiet)))
+            out = np.array([r[0] for r in res], dtype=np.float64), np.stack([r[1] for r in res])
         return out if return_log_likelihood else out[1]
-
-    def _batch_grad_loop(self, vectors, y, quiet, return_ll):
-        state = self._batch_state()
-        try:
-            ll = np.empty(len(vectors), dtype=np.float64)
-            grad = np.empty((len(vectors), len(self)), dtype=np.float64)
-            for b, v in enumerate(vectors):
-                self.set_parameter_vector(v)
-                if return_ll:
-                    ll[b] = self.log_likelihood(y, quiet=quiet)
-                grad[b] = self.grad_log_likelihood(y, quiet=quiet)
-            return ll, grad
-        finally:
-            self._batch_restore(state)
 
     def _batch_grad_device(self, batch, vectors, y, quiet, return_ll):
         """The batched dense path of :func:`batch_grad_log_likelihood`: ``(ll, grad)``, or ``None`` when the kernel
         has no valid device program or more than ``_MAX_GRAD_PARAMS`` parameters."""
         # one residual serves both terms: GP._residual (the gradient's) and GP._residual_of (the value's) round alike
-        members = self._batch_members(vectors, y, self._residual,
-                                      lambda y, c: y - (c + np.zeros(len(y))))  # GP._residual of a ConstantModel
+        members = self._batch_predict_members(vectors, y)
         if members is None or members[2].shape[1] > _MAX_GRAD_PARAMS:
             return None
         spec, full, kpar, sigma, resid, fact_err, mean_err = members
-        nb, n = len(vectors), len(self._x)
+        nb = len(vectors)
         mask = self.kernel.unfrozen_mask
         log_det, quad, alpha, g, diag, info = batch(spec, kpar, self._x, sigma, resid, mask.astype(np.uint32))
-        # GP.compute / GP.log_likelihood, in the same order of operations
-        const = -0.5 * (n * np.log(2 * np.pi) + log_det)
-        ll = const - 0.5 * quad
-        ll[~np.isfinite(ll)] = -np.inf
+        ll = self._batch_ll(log_det, quad)
         # GP.grad_log_likelihood member by member, with its operations
         n_mean, n_wn, n_k = len(self.mean), len(self.white_noise), len(self.kernel)
         full_mean, full_wn = self.mean.full_size, self.white_noise.full_size
@@ -759,15 +767,10 @@ class GP(ModelSet):
         A ``ConstantModel`` mean adds nothing to ``dmu``; any other mean model raises ``NotImplementedError`` (the
         modeling protocol has no input gradient).  Inputs of more than 8 dimensions raise ``ValueError``.
         """
-        if type(self.mean) is not ConstantModel:
-            raise NotImplementedError("grad_predict needs the mean model's gradient with respect to the inputs, which "
-                                      "the modeling protocol does not provide; only a constant mean is supported")
-        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
-            raise RuntimeError("You need to compute the model first")
+        _check_grad_predict_mean(self.mean)
+        self._require_computed()
         xs = self.parse_samples(t)
-        if xs.shape[1] > BGP_MAX_DIM:
-            raise ValueError("input-coordinate gradients support at most {0} dimensions (got {1})".format(
-                BGP_MAX_DIM, xs.shape[1]))
+        _check_grad_predict_dim(xs)
         self.recompute()
         alpha = self._compute_alpha(y, cache)
         if kernel is None:
@@ -808,19 +811,11 @@ class GP(ModelSet):
 
         :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
         """
-        if type(self.mean) is not ConstantModel:
-            raise NotImplementedError("grad_predict needs the mean model's gradient with respect to the inputs, which "
-                                      "the modeling protocol does not provide; only a constant mean is supported")
-        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
-            raise RuntimeError("You need to compute the model first")
-        vectors = np.asarray(vectors, dtype=np.float64)
-        if vectors.ndim != 2 or vectors.shape[1] != len(self):
-            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        _check_grad_predict_mean(self.mean)
+        vectors = self._batch_vectors(vectors)
         self._check_dimensions(y)
         xs = self.parse_samples(t)
-        if xs.shape[1] > BGP_MAX_DIM:
-            raise ValueError("input-coordinate gradients support at most {0} dimensions (got {1})".format(
-                BGP_MAX_DIM, xs.shape[1]))
+        _check_grad_predict_dim(xs)
         nb, ns, nd = len(vectors), len(xs), xs.shape[1]
         if nb == 0 or ns == 0:
             mu, dmu = np.empty((nb, ns), dtype=np.float64), np.empty((nb, ns, nd), dtype=np.float64)
@@ -832,14 +827,7 @@ class GP(ModelSet):
             out = self._batch_grad_predict_device(batch, vectors, y, xs, return_var)
             if out is not None:
                 return out
-        state = self._batch_state()
-        try:
-            res = []
-            for v in vectors:
-                self.set_parameter_vector(v)
-                res.append(self.grad_predict(y, t, return_var=return_var, kernel=kernel))
-        finally:
-            self._batch_restore(state)
+        res = self._batch_loop(vectors, lambda: self.grad_predict(y, t, return_var=return_var, kernel=kernel))
         return tuple(np.stack([r[k] for r in res]) for k in range(len(res[0])))
 
     def _batch_grad_predict_device(self, batch, vectors, y, xs, return_var):
@@ -851,11 +839,7 @@ class GP(ModelSet):
         spec, full, kpar, sigma, resid, fact_err, mean_err = members
         mean_xs, xs_err = self._batch_mean_at(full, xs)
         mu, var, dmu, dvar, info = batch(spec, kpar, self._x, sigma, resid, xs, return_var)
-        for b in range(len(vectors)):  # the loop's order: white noise, factorisation, residual
-            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
-            exc = exc if exc is not None else (mean_err[b] if mean_err[b] is not None else xs_err[b])
-            if exc is not None:
-                raise exc
+        self._raise_member_error(spec, kpar, info, fact_err, mean_err, xs_err)  # residual, mean at x*
         mu += mean_xs  # a constant mean adds nothing to dmu
         return (mu, var, dmu, dvar) if return_var else (mu, dmu)
 
@@ -879,18 +863,12 @@ class GP(ModelSet):
         ``numpy.linalg.LinAlgError`` naming the failed leading minor, where the host route warns and draws anyway; the
         GP stays as it was.
         """
+        jitter = _sampling_jitter(rng, jitter)
         if rng is None:
-            if jitter is not None:
-                raise ValueError("jitter applies only to draws with an rng; the host route adds nothing")
             mu, cov = self.predict(y, t)
             return multivariate_gaussian_samples(cov, size, mean=mu)
-        _check_rng(rng)
-        jitter = TINY if jitter is None else float(jitter)
-        if not (np.isfinite(jitter) and jitter >= 0.0):
-            raise ValueError("jitter must be finite and >= 0, got {0}".format(jitter))
         size = _check_size(size)
-        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
-            raise RuntimeError("You need to compute the model first")
+        self._require_computed()
         self._check_dimensions(y)
         xs = self.parse_samples(t)
         z = rng.standard_normal((size, len(xs)))
@@ -934,20 +912,9 @@ class GP(ModelSet):
 
         :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
         """
-        if rng is None:
-            if jitter is not None:
-                raise ValueError("jitter applies only to draws with an rng; the host route adds nothing")
-        else:
-            _check_rng(rng)
-            jitter = TINY if jitter is None else float(jitter)
-            if not (np.isfinite(jitter) and jitter >= 0.0):
-                raise ValueError("jitter must be finite and >= 0, got {0}".format(jitter))
+        jitter = _sampling_jitter(rng, jitter)
         size = _check_size(size)
-        if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
-            raise RuntimeError("You need to compute the model first")
-        vectors = np.asarray(vectors, dtype=np.float64)
-        if vectors.ndim != 2 or vectors.shape[1] != len(self):
-            raise ValueError("vectors must have shape (B, {0}), got {1}".format(len(self), vectors.shape))
+        vectors = self._batch_vectors(vectors)
         self._check_dimensions(y)
         xs = self.parse_samples(t)
         nb, ns = len(vectors), len(xs)
@@ -963,15 +930,7 @@ class GP(ModelSet):
             out = self._batch_sample_device(batch, vectors, y, xs, size, rng, jitter)
             if out is not None:
                 return out
-        state = self._batch_state()
-        try:
-            res = []
-            for v in vectors:
-                self.set_parameter_vector(v)
-                res.append(self.sample_conditional(y, t, size, rng=rng, jitter=jitter))
-        finally:
-            self._batch_restore(state)
-        return np.stack(res)
+        return np.stack(self._batch_loop(vectors, lambda: self.sample_conditional(y, t, size, rng=rng, jitter=jitter)))
 
     def _batch_sample_device(self, batch, vectors, y, xs, size, rng, jitter):
         """The batched dense path of :func:`batch_sample_conditional`; ``None`` when the kernel has no valid device
@@ -986,14 +945,9 @@ class GP(ModelSet):
             z[b] = rng.standard_normal((size, ns))
         mean_xs, xs_err = self._batch_mean_at(full, xs)
         draws, info, draw_info = batch(spec, kpar, self._x, sigma, resid, xs, mean_xs, z, jitter)
-        for b in range(nb):  # the loop's order: white noise, factorisation, residual, mean at x*, covariance
-            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
-            exc = exc if exc is not None else (mean_err[b] if mean_err[b] is not None else xs_err[b])
-            if exc is None and draw_info[b] != 0:
-                exc = LinAlgError("%d-th leading minor of the array is not positive definite (a larger jitter adds "
-                                  "more to the diagonal)" % draw_info[b])
-            if exc is not None:
-                raise exc
+        cov_err = [LinAlgError("%d-th leading minor of the array is not positive definite (a larger jitter adds more "
+                               "to the diagonal)" % d) if d != 0 else None for d in draw_info]
+        self._raise_member_error(spec, kpar, info, fact_err, mean_err, xs_err, cov_err)  # residual, mean at x*, cov
         return draws[:, 0] if size == 1 else draws
 
     def sample(self, t=None, size=1, *, rng=None):
@@ -1018,8 +972,7 @@ class GP(ModelSet):
         _check_rng(rng)
         size = _check_size(size)
         if t is None:
-            if not (hasattr(self, "_x") and hasattr(self, "_yerr2")):
-                raise RuntimeError("You need to compute the model first")
+            self._require_computed()
             z = rng.standard_normal((size, self._x.shape[0]))
             self.recompute()
             draws = self.solver.apply_sqrt(z)

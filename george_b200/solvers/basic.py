@@ -27,32 +27,20 @@ def _check_finite(b):
 __all__ = ["BasicSolver"]
 
 
-class _DenseHandle(object):
-    """Owns a ``bgp_dense_t*``; never pickled."""
+class _Handle(object):
+    """Owns a pointer that the library function ``create`` makes and ``destroy`` frees (a ``bgp_dense_t*`` or the
+    ``bgp_dense_batch_t*`` workspace of the ``batch_*`` statics); never pickled."""
 
-    def __init__(self):
+    def __init__(self, create, destroy):
         self.lib = _lib.load()
         self.ptr = C.c_void_p()
-        _lib.check(self.lib.bgp_dense_create(C.byref(self.ptr)))
-
-    def __del__(self):
-        if getattr(self, "ptr", None) is not None and self.ptr:
-            self.lib.bgp_dense_destroy(self.ptr)
-            self.ptr = None
-
-
-class _BatchHandle(object):
-    """Owns a ``bgp_dense_batch_t*`` (device workspace of ``BasicSolver.batch_log_likelihood`` / ``batch_predict``)."""
-
-    def __init__(self):
-        self.lib = _lib.load()
-        self.ptr = C.c_void_p()
-        _lib.check(self.lib.bgp_dense_batch_create(C.byref(self.ptr)))
+        self._destroy = getattr(self.lib, destroy)
+        _lib.check(getattr(self.lib, create)(C.byref(self.ptr)))
 
     def __del__(self):
         if getattr(self, "ptr", None) is not None and self.ptr:
             try:
-                self.lib.bgp_dense_batch_destroy(self.ptr)
+                self._destroy(self.ptr)
             except Exception:  # interpreter shutdown
                 pass
             self.ptr = None
@@ -66,8 +54,62 @@ _batch_handle = None
 def _get_batch_handle():
     global _batch_handle
     if _batch_handle is None:
-        _batch_handle = _BatchHandle()
+        _batch_handle = _Handle("bgp_dense_batch_create", "bgp_dense_batch_destroy")
     return _batch_handle
+
+
+def _points(a):
+    """``a`` as contiguous float64, a 1-D array as one column."""
+    a = np.ascontiguousarray(a, dtype=np.float64)
+    return a[:, None] if a.ndim == 1 else a
+
+
+def _test_points(kernel, xs):
+    """``(spec, xs)`` for the ``_*_call`` statics: ``kernel``'s program and the test points as ``(ns, ndim)``."""
+    xs = _points(xs)
+    spec = flatten(kernel)
+    if xs.ndim != 2 or xs.shape[1] != spec.ndim:
+        raise DimensionMismatch("dimension mismatch")  # what kernel.get_value(xs, x) raises
+    return spec, xs
+
+
+def _batch_inputs(spec, params, x, yerr, r, xs=None, which=None):
+    """``(x, xs, params, yerr, r, which)`` normalised and checked for the ``batch_*`` statics: ``x`` ``(n, ndim)``,
+    ``params`` ``(B, num_params(spec))``, ``yerr`` and ``r`` ``(B, n)``, ``which`` (when given) ``(P,)``, then the
+    dimension of the program, ``x`` and ``xs`` (when given, ``(ns, ndim)``)."""
+    x = _points(x)
+    if xs is not None:
+        xs = _points(xs)
+    params = np.ascontiguousarray(params, dtype=np.float64)
+    yerr = np.ascontiguousarray(yerr, dtype=np.float64)
+    r = np.ascontiguousarray(r, dtype=np.float64)
+    if which is not None:
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+    if x.ndim != 2 or x.shape[0] == 0:
+        raise ValueError("x must have shape (n, ndim) with n > 0")
+    n, ndim = x.shape
+    npar = num_params(spec)
+    if params.ndim != 2 or params.shape[1] != npar:
+        raise ValueError("params must have shape (B, {0})".format(npar))
+    nb = params.shape[0]
+    if yerr.shape != (nb, n) or r.shape != (nb, n):
+        raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
+    if which is not None and which.shape != (npar,):
+        raise ValueError("which must have shape ({0},)".format(npar))
+    if ndim != spec.ndim or (xs is not None and (xs.ndim != 2 or xs.shape[1] != ndim)):
+        raise DimensionMismatch("dimension mismatch")
+    return x, xs, params, yerr, r, which
+
+
+def _batch_call(name, spec, params, x, yerr, r, *rest):
+    """The library's batched entry point ``name`` on the shared workspace, with the members' common arguments followed
+    by ``rest``; nothing for no members."""
+    nb, (n, ndim) = params.shape[0], x.shape
+    if nb == 0:
+        return
+    h = _get_batch_handle()
+    _lib.check(getattr(h.lib, name)(h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim,
+                                    _lib.ptr(yerr), _lib.ptr(r), *rest))
 
 
 class BasicSolver(object):
@@ -99,14 +141,12 @@ class BasicSolver(object):
 
     def compute(self, x, yerr):
         """Build K(x, x) + diag(yerr^2) on the device and Cholesky-factorise it (basic.py:51-70)."""
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        if x.ndim == 1:
-            x = x[:, None]
+        x = _points(x)
         n, ndim = x.shape
         yerr = np.ascontiguousarray(np.broadcast_to(np.asarray(yerr, dtype=np.float64), (n,)))
         spec = flatten(self.kernel)
         if self._handle is None:
-            self._handle = _DenseHandle()
+            self._handle = _Handle("bgp_dense_create", "bgp_dense_destroy")
         lib = self._handle.lib
         self._computed = False
         _lib.check(lib.bgp_dense_compute(self._handle.ptr, C.byref(spec), _lib.ptr(x), n, ndim, _lib.ptr(yerr)))
@@ -206,12 +246,7 @@ class BasicSolver(object):
         kinds = {"var": _lib.BGP_PREDICT_VAR, "cov": _lib.BGP_PREDICT_COV}
         if what not in kinds:
             raise ValueError("what must be 'var' or 'cov'")
-        xs = np.ascontiguousarray(xs, dtype=np.float64)
-        if xs.ndim == 1:
-            xs = xs[:, None]
-        spec = flatten(kernel)
-        if xs.ndim != 2 or xs.shape[1] != spec.ndim:
-            raise DimensionMismatch("dimension mismatch")  # what kernel.get_value(xs, x) raises
+        spec, xs = _test_points(kernel, xs)
         ns = xs.shape[0]
         out = np.empty((ns,) if what == "var" else (ns, ns), dtype=np.float64)
         _lib.check(fn(ptr, C.byref(spec), _lib.ptr(xs), ns, kinds[what], _lib.ptr(out)))
@@ -229,12 +264,7 @@ class BasicSolver(object):
 
     @staticmethod
     def _predictive_grad_call(fn, ptr, kernel, xs):
-        xs = np.ascontiguousarray(xs, dtype=np.float64)
-        if xs.ndim == 1:
-            xs = xs[:, None]
-        spec = flatten(kernel)
-        if xs.ndim != 2 or xs.shape[1] != spec.ndim:
-            raise DimensionMismatch("dimension mismatch")
+        spec, xs = _test_points(kernel, xs)
         ns = xs.shape[0]
         var = np.empty(ns, dtype=np.float64)
         dvar = np.empty((ns, spec.ndim), dtype=np.float64)
@@ -255,12 +285,7 @@ class BasicSolver(object):
 
     @staticmethod
     def _sample_call(fn, ptr, kernel, xs, mean, z, jitter):
-        xs = np.ascontiguousarray(xs, dtype=np.float64)
-        if xs.ndim == 1:
-            xs = xs[:, None]
-        spec = flatten(kernel)
-        if xs.ndim != 2 or xs.shape[1] != spec.ndim:
-            raise DimensionMismatch("dimension mismatch")
+        spec, xs = _test_points(kernel, xs)
         ns = xs.shape[0]
         mean = np.ascontiguousarray(mean, dtype=np.float64)
         z = np.ascontiguousarray(z, dtype=np.float64)
@@ -281,31 +306,13 @@ class BasicSolver(object):
         ``(n,)`` or ``(n, ndim)``, ``yerr`` and ``r`` ``(B, n)``.  The members run in chunks on the device; a
         member's ``log_det`` is bit-identical to :attr:`log_determinant` after :func:`compute` with its spec and
         yerr."""
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        if x.ndim == 1:
-            x = x[:, None]
-        params = np.ascontiguousarray(params, dtype=np.float64)
-        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
-        r = np.ascontiguousarray(r, dtype=np.float64)
-        if x.ndim != 2 or x.shape[0] == 0:
-            raise ValueError("x must have shape (n, ndim) with n > 0")
-        n, ndim = x.shape
-        if params.ndim != 2 or params.shape[1] != num_params(spec):
-            raise ValueError("params must have shape (B, {0})".format(num_params(spec)))
+        x, _, params, yerr, r, _ = _batch_inputs(spec, params, x, yerr, r)
         nb = params.shape[0]
-        if yerr.shape != (nb, n) or r.shape != (nb, n):
-            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
-        if ndim != spec.ndim:
-            raise DimensionMismatch("dimension mismatch")
         log_det = np.empty(nb, dtype=np.float64)
         quad = np.empty(nb, dtype=np.float64)
         info = np.zeros(nb, dtype=np.int32)
-        if nb == 0:
-            return log_det, quad, info
-        h = _get_batch_handle()
-        _lib.check(h.lib.bgp_dense_batch_log_likelihood(
-            h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim, _lib.ptr(yerr),
-            _lib.ptr(r), _lib.ptr(log_det), _lib.ptr(quad), _lib.ptr(info)))
+        _batch_call("bgp_dense_batch_log_likelihood", spec, params, x, yerr, r, _lib.ptr(log_det), _lib.ptr(quad),
+                    _lib.ptr(info))
         return log_det, quad, info
 
     @staticmethod
@@ -317,39 +324,16 @@ class BasicSolver(object):
         :func:`batch_log_likelihood`; a failed member's rows are NaN.  A member's ``alpha``, ``g``, ``diag`` and
         ``log_det`` are bit-identical to :func:`compute` with its spec and yerr followed by :func:`grad_terms`.  More
         than 64 kernel parameters raise ``ValueError`` before anything is solved."""
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        if x.ndim == 1:
-            x = x[:, None]
-        params = np.ascontiguousarray(params, dtype=np.float64)
-        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
-        r = np.ascontiguousarray(r, dtype=np.float64)
-        which = np.ascontiguousarray(which, dtype=np.uint32)
-        if x.ndim != 2 or x.shape[0] == 0:
-            raise ValueError("x must have shape (n, ndim) with n > 0")
-        n, ndim = x.shape
-        npar = num_params(spec)
-        if params.ndim != 2 or params.shape[1] != npar:
-            raise ValueError("params must have shape (B, {0})".format(npar))
-        nb = params.shape[0]
-        if yerr.shape != (nb, n) or r.shape != (nb, n):
-            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
-        if which.shape != (npar,):
-            raise ValueError("which must have shape ({0},)".format(npar))
-        if ndim != spec.ndim:
-            raise DimensionMismatch("dimension mismatch")
+        x, _, params, yerr, r, which = _batch_inputs(spec, params, x, yerr, r, which=which)
+        nb, n, npar = params.shape[0], x.shape[0], params.shape[1]
         log_det = np.empty(nb, dtype=np.float64)
         quad = np.empty(nb, dtype=np.float64)
         alpha = np.empty((nb, n), dtype=np.float64)
         g = np.empty((nb, npar), dtype=np.float64)
         diag = np.empty((nb, n), dtype=np.float64)
         info = np.zeros(nb, dtype=np.int32)
-        if nb == 0:
-            return log_det, quad, alpha, g, diag, info
-        h = _get_batch_handle()
-        _lib.check(h.lib.bgp_dense_batch_grad_terms(
-            h.ptr, C.byref(spec), _lib.ptr(params), nb, npar, _lib.ptr(x), n, ndim, _lib.ptr(yerr), _lib.ptr(r),
-            _lib.ptr(which), _lib.ptr(log_det), _lib.ptr(quad), _lib.ptr(alpha), _lib.ptr(diag), _lib.ptr(g),
-            _lib.ptr(info)))
+        _batch_call("bgp_dense_batch_grad_terms", spec, params, x, yerr, r, _lib.ptr(which), _lib.ptr(log_det),
+                    _lib.ptr(quad), _lib.ptr(alpha), _lib.ptr(diag), _lib.ptr(g), _lib.ptr(info))
         return log_det, quad, alpha, g, diag, info
 
     @staticmethod
@@ -364,26 +348,8 @@ class BasicSolver(object):
         kinds = {None: 0, "var": _lib.BGP_PREDICT_VAR, "cov": _lib.BGP_PREDICT_COV}
         if what not in kinds:
             raise ValueError("what must be None, 'var' or 'cov'")
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        if x.ndim == 1:
-            x = x[:, None]
-        xs = np.ascontiguousarray(xs, dtype=np.float64)
-        if xs.ndim == 1:
-            xs = xs[:, None]
-        params = np.ascontiguousarray(params, dtype=np.float64)
-        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
-        r = np.ascontiguousarray(r, dtype=np.float64)
-        if x.ndim != 2 or x.shape[0] == 0:
-            raise ValueError("x must have shape (n, ndim) with n > 0")
-        n, ndim = x.shape
-        if params.ndim != 2 or params.shape[1] != num_params(spec):
-            raise ValueError("params must have shape (B, {0})".format(num_params(spec)))
-        nb = params.shape[0]
-        if yerr.shape != (nb, n) or r.shape != (nb, n):
-            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
-        if ndim != spec.ndim or xs.ndim != 2 or xs.shape[1] != ndim:
-            raise DimensionMismatch("dimension mismatch")
-        ns = xs.shape[0]
+        x, xs, params, yerr, r, _ = _batch_inputs(spec, params, x, yerr, r, xs=xs)
+        nb, ns = params.shape[0], xs.shape[0]
         mean = np.empty((nb, ns), dtype=np.float64)
         out = None
         if what == "var":
@@ -391,13 +357,8 @@ class BasicSolver(object):
         elif what == "cov":
             out = np.empty((nb, ns, ns), dtype=np.float64)
         info = np.zeros(nb, dtype=np.int32)
-        if nb == 0:
-            return mean, out, info
-        h = _get_batch_handle()
-        _lib.check(h.lib.bgp_dense_batch_predict(
-            h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim, _lib.ptr(yerr),
-            _lib.ptr(r), _lib.ptr(xs), ns, kinds[what], _lib.ptr(mean), _lib.ptr(out) if out is not None else None,
-            _lib.ptr(info)))
+        _batch_call("bgp_dense_batch_predict", spec, params, x, yerr, r, _lib.ptr(xs), ns, kinds[what], _lib.ptr(mean),
+                    _lib.ptr(out) if out is not None else None, _lib.ptr(info))
         return mean, out, info
 
     @staticmethod
@@ -410,38 +371,16 @@ class BasicSolver(object):
         of :func:`batch_log_likelihood`; a failed member's rows are NaN.  Every entry is bit-identical to
         :func:`compute` with member ``b``'s spec and yerr followed by ``apply_inverse(r[b])``, ``kernel.matvec``,
         ``kernel.x1_gradient_matvec`` and :func:`predictive_grad`.  ``xs``: ``(ns,)`` or ``(ns, ndim)``."""
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        if x.ndim == 1:
-            x = x[:, None]
-        xs = np.ascontiguousarray(xs, dtype=np.float64)
-        if xs.ndim == 1:
-            xs = xs[:, None]
-        params = np.ascontiguousarray(params, dtype=np.float64)
-        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
-        r = np.ascontiguousarray(r, dtype=np.float64)
-        if x.ndim != 2 or x.shape[0] == 0:
-            raise ValueError("x must have shape (n, ndim) with n > 0")
-        n, ndim = x.shape
-        if params.ndim != 2 or params.shape[1] != num_params(spec):
-            raise ValueError("params must have shape (B, {0})".format(num_params(spec)))
-        nb = params.shape[0]
-        if yerr.shape != (nb, n) or r.shape != (nb, n):
-            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
-        if ndim != spec.ndim or xs.ndim != 2 or xs.shape[1] != ndim:
-            raise DimensionMismatch("dimension mismatch")
-        ns = xs.shape[0]
+        x, xs, params, yerr, r, _ = _batch_inputs(spec, params, x, yerr, r, xs=xs)
+        nb, (ns, ndim) = params.shape[0], xs.shape
         mean = np.empty((nb, ns), dtype=np.float64)
         dmu = np.empty((nb, ns, ndim), dtype=np.float64)
         var = np.empty((nb, ns), dtype=np.float64) if return_var else None
         dvar = np.empty((nb, ns, ndim), dtype=np.float64) if return_var else None
         info = np.zeros(nb, dtype=np.int32)
-        if nb == 0:
-            return mean, var, dmu, dvar, info
-        h = _get_batch_handle()
-        _lib.check(h.lib.bgp_dense_batch_predict_grad(
-            h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim, _lib.ptr(yerr),
-            _lib.ptr(r), _lib.ptr(xs), ns, 1 if return_var else 0, _lib.ptr(mean), _lib.ptr(dmu),
-            _lib.ptr(var) if return_var else None, _lib.ptr(dvar) if return_var else None, _lib.ptr(info)))
+        _batch_call("bgp_dense_batch_predict_grad", spec, params, x, yerr, r, _lib.ptr(xs), ns, 1 if return_var else 0,
+                    _lib.ptr(mean), _lib.ptr(dmu), _lib.ptr(var) if return_var else None,
+                    _lib.ptr(dvar) if return_var else None, _lib.ptr(info))
         return mean, var, dmu, dvar, info
 
     @staticmethod
@@ -455,40 +394,17 @@ class BasicSolver(object):
         is not); a failed member's draws are NaN.  Every draw is bit-identical to :func:`compute` with member ``b``'s
         spec and yerr followed by :func:`sample_predictive`.  ``xs``: ``(ns,)`` or ``(ns, ndim)``; ``mean_add``:
         ``(B, ns)``; ``z``: ``(B, size, ns)`` standard normals."""
-        x = np.ascontiguousarray(x, dtype=np.float64)
-        if x.ndim == 1:
-            x = x[:, None]
-        xs = np.ascontiguousarray(xs, dtype=np.float64)
-        if xs.ndim == 1:
-            xs = xs[:, None]
-        params = np.ascontiguousarray(params, dtype=np.float64)
-        yerr = np.ascontiguousarray(yerr, dtype=np.float64)
-        r = np.ascontiguousarray(r, dtype=np.float64)
+        x, xs, params, yerr, r, _ = _batch_inputs(spec, params, x, yerr, r, xs=xs)
         mean_add = np.ascontiguousarray(mean_add, dtype=np.float64)
         z = np.ascontiguousarray(z, dtype=np.float64)
-        if x.ndim != 2 or x.shape[0] == 0:
-            raise ValueError("x must have shape (n, ndim) with n > 0")
-        n, ndim = x.shape
-        if params.ndim != 2 or params.shape[1] != num_params(spec):
-            raise ValueError("params must have shape (B, {0})".format(num_params(spec)))
-        nb = params.shape[0]
-        if yerr.shape != (nb, n) or r.shape != (nb, n):
-            raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
-        if ndim != spec.ndim or xs.ndim != 2 or xs.shape[1] != ndim:
-            raise DimensionMismatch("dimension mismatch")
-        ns = xs.shape[0]
+        nb, ns = params.shape[0], xs.shape[0]
         if mean_add.shape != (nb, ns) or z.ndim != 3 or z.shape[0] != nb or z.shape[2] != ns:
             raise ValueError("mean_add must have shape ({0}, {1}) and z ({0}, size, {1})".format(nb, ns))
         draws = np.empty(z.shape, dtype=np.float64)
         info = np.zeros(nb, dtype=np.int32)
         draw_info = np.zeros(nb, dtype=np.int32)
-        if nb == 0:
-            return draws, info, draw_info
-        h = _get_batch_handle()
-        _lib.check(h.lib.bgp_dense_batch_sample(
-            h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim, _lib.ptr(yerr),
-            _lib.ptr(r), _lib.ptr(xs), ns, _lib.ptr(mean_add), _lib.ptr(z), z.shape[1], float(jitter),
-            _lib.ptr(draws), _lib.ptr(info), _lib.ptr(draw_info)))
+        _batch_call("bgp_dense_batch_sample", spec, params, x, yerr, r, _lib.ptr(xs), ns, _lib.ptr(mean_add), _lib.ptr(z),
+                    z.shape[1], float(jitter), _lib.ptr(draws), _lib.ptr(info), _lib.ptr(draw_info))
         return draws, info, draw_info
 
     # Device handles cannot be pickled.  Like the reference (which pickles its numpy factor, tests/test_pickle.py:21-36:
@@ -511,7 +427,7 @@ class BasicSolver(object):
         if factor is not None:
             self._has_inputs = False
             try:
-                self._handle = _DenseHandle()
+                self._handle = _Handle("bgp_dense_create", "bgp_dense_destroy")
                 _lib.check(self._handle.lib.bgp_dense_import_factor(self._handle.ptr, _lib.ptr(factor), self._n,
                                                                    float(self._log_det)))
             except Exception:  # no device where it was unpickled: refactorise lazily on first use
