@@ -6,6 +6,9 @@
   north-star bar 1e-6; log-likelihood identical (1e-9) between the two RNG-independent ways of computing the quadratic
   form (dot_solve vs y . apply_inverse); two computes give the same log-det to 1e-12.
 * config 4 (Matern52 3-D, N = 32768, dense Cholesky): the same round trip through the dense solver.
+
+Configs 2 and 5 (bench.py's cfg2 and cfg5, N = 65536, 131072 and 2^20, unsharded and in eight shards) are held to
+golden vectors of the CPU oracle at full size in tests/test_gpu_zz_workloads.py.
 """
 import numpy as np
 import pytest
