@@ -4,14 +4,18 @@
 //
 // The leaf is factorised in 32-column panels, left to right.  A panel (rows k0.., columns k0..k0+31) is built in shared
 // memory, brought up to date there and written to global memory once, final:
-//   (1) build: the panel's kernel entries on and below the diagonal, evaluated by the whole CTA (the 1-D shapes through
-//       ShapeEval, the same arithmetic as the interpreter);
+//   (1) build: the panel's kernel entries on and below the diagonal, evaluated by the whole CTA, LF_BUILD_ILP
+//       independent entries per thread in flight (the 1-D shapes through ShapeEval, the same arithmetic as the
+//       interpreter);
 //   (2) update: panel -= L(k0:, 0:k0) D L(k0:k0+32, 0:k0)^T on the tensor pipe (mma.sync.m8n8k4.f64): 16 x 32 output
 //       tiles dealt to the 8 warps, both operands read straight from the finished columns in global memory (this CTA
 //       wrote them, so they come from L1 / L2), the D scaling applied to the B fragment on the fly, no barrier inside;
-//   (3) the 32 x 32 diagonal block: LDL^T by one warp, lane = row, the row in registers and each column of L broadcast
-//       by shuffles;
-//   (4) the rows below it: L21 = A21 L11^-T D^-1, one row per thread, written to global memory.
+//   (3) the 32 x 32 diagonal block: right-looking LDL^T by one warp in shared memory, lane = row, with a rolled loop
+//       (a fully unrolled register version is ~7k instructions run once per panel by one warp: it streamed through the
+//       instruction cache and cost more than the rest of the panel).  The same warp eliminates the identity alongside,
+//       which leaves W = L11^-T D^-1 in shared memory;
+//   (4) the rows below it: L21 = A21 W on the tensor pipe, 16 x 32 tiles dealt to the 8 warps, written to global memory
+//       from the accumulators.
 // No entry of the leaf is read back and rewritten in global memory.
 #pragma once
 
@@ -23,8 +27,24 @@ namespace bgp {
 constexpr int LF_THREADS = 256;
 constexpr int LF_NB = 32;
 constexpr int LF_MAX_LEAF = 768;
+constexpr int LF_LDW = 40;  // leading dimension of W: the B fragments of phase (4) read it without bank conflicts
 
-__host__ __device__ inline int lf_panel_ld(int max_m) { return ((max_m + 15) / 16) * 16 + 4; }
+// panel leading dimension: = 8 (mod 16) doubles, so that the A fragments (4 columns x 8 rows) fill two bank wavefronts
+__host__ __device__ inline int lf_panel_ld(int max_m) { return ((max_m + 15) / 16) * 16 + 8; }
+
+// dst[j * ds] -= f * src[j * ss] for j in [lo, hi]: 8 shared-memory loads issued before their stores (one at a time,
+// each load would wait for the store before it, which the compiler cannot tell apart from an alias)
+__device__ __forceinline__ void lf_axpy(double* dst, int ds, const double* src, int ss, int lo, int hi, double f) {
+  for (int j0 = lo; j0 <= hi; j0 += 8) {
+    double a[8], b[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u)
+      if (j0 + u <= hi) { a[u] = dst[(j0 + u) * ds]; b[u] = src[(j0 + u) * ss]; }
+#pragma unroll
+    for (int u = 0; u < 8; ++u)
+      if (j0 + u <= hi) dst[(j0 + u) * ds] = a[u] - f * b[u];
+  }
+}
 
 template <int SHAPE>
 __global__ void __launch_bounds__(LF_THREADS, 2) leaf_factor_kernel(const DevProgram* __restrict__ gprog,
@@ -34,13 +54,14 @@ __global__ void __launch_bounds__(LF_THREADS, 2) leaf_factor_kernel(const DevPro
                                                                     double* __restrict__ Lbuf,
                                                                     double* __restrict__ leaf_logdet, int ldp) {
   // dynamic shared memory: the panel [LF_NB][ldp] (column c, leaf row k0 + i at pn[c * ldp + i]), D of the finished
-  // columns [ldp], and for the interpreter the staged program
+  // columns [ldp], W = L11^-T D^-1 of the current panel [LF_NB][LF_LDW] (W(q, n) at w11[q * LF_LDW + n]), and for the
+  // interpreter the staged program
   extern __shared__ __align__(16) double lf_smem[];
   double* pn = lf_smem;
   double* dall = lf_smem + LF_NB * ldp;
-  DevProgram* P = reinterpret_cast<DevProgram*>(lf_smem + (LF_NB + 1) * ldp);
+  double* w11 = dall + ldp;
+  DevProgram* P = reinterpret_cast<DevProgram*>(w11 + LF_NB * LF_LDW);
   __shared__ double red[32];
-  __shared__ double dinv[LF_NB];
   if constexpr (SHAPE == BGP_SHAPE_GENERIC) stage_program(P, gprog);
   __syncthreads();
   const auto fn = ShapeEval<SHAPE>::make(P, gprog);
@@ -49,23 +70,30 @@ __global__ void __launch_bounds__(LF_THREADS, 2) leaf_factor_kernel(const DevPro
   double* A = Lbuf + lf.off;
   const double* xs = x + (int64_t)lf.start * nd;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int lr = lane >> 2, lc = lane & 3;  // mma.m8n8k4 fragment coordinates
 
+  // independent kernel evaluations per thread in flight in the build (the interpreter keeps one: its stack is large)
+  constexpr int LF_BUILD_ILP = SHAPE == BGP_SHAPE_GENERIC ? 1 : 4;
   double logdet = 0.0;
   for (int k0 = 0; k0 < m; k0 += LF_NB) {
     const int nb = min(LF_NB, m - k0), rem = m - k0;
     // (1) build
-    for (int t = threadIdx.x; t < nb * rem; t += LF_THREADS) {
-      const int c = t / rem, i = t - c * rem;
-      if (i >= c) {
-        double v = fn(xs + (int64_t)(k0 + i) * nd, xs + (int64_t)(k0 + c) * nd);
-        if (i == c) v += diag[lf.start + k0 + i];
-        pn[c * ldp + i] = v;
+    for (int t0 = threadIdx.x; t0 < nb * rem; t0 += LF_BUILD_ILP * LF_THREADS) {
+      double v[LF_BUILD_ILP];
+#pragma unroll
+      for (int u = 0; u < LF_BUILD_ILP; ++u) {
+        const int t = t0 + u * LF_THREADS, c = t / rem, i = t - c * rem;
+        v[u] = (t < nb * rem && i >= c) ? fn(xs + (int64_t)(k0 + i) * nd, xs + (int64_t)(k0 + c) * nd) : 0.0;
+      }
+#pragma unroll
+      for (int u = 0; u < LF_BUILD_ILP; ++u) {
+        const int t = t0 + u * LF_THREADS, c = t / rem, i = t - c * rem;
+        if (t < nb * rem && i >= c) pn[c * ldp + i] = (i == c) ? v[u] + diag[lf.start + k0 + i] : v[u];
       }
     }
     __syncthreads();
     // (2) update from the finished columns 0..k0-1
     if (k0 > 0) {
-      const int lr = lane >> 2, lc = lane & 3;
       const int n_tiles = (rem + 15) / 16;
       bool bok[4];
 #pragma unroll
@@ -109,56 +137,74 @@ __global__ void __launch_bounds__(LF_THREADS, 2) leaf_factor_kernel(const DevPro
       }
       __syncthreads();
     }
-    // (3) warp 0: LDL^T of the diagonal block, lane = row
+    // (3) warp 0: LDL^T of the diagonal block, lane = row i, and T = L11^-1 (starting from the identity, row i of T
+    // takes the same eliminations as row i of the block); then W = T^T D^-1
     if (warp == 0) {
-      double w[LF_NB];
-#pragma unroll
-      for (int j = 0; j < LF_NB; ++j) w[j] = (j <= lane && lane < nb) ? pn[j * ldp + lane] : 0.0;
-#pragma unroll
-      for (int k = 0; k < LF_NB; ++k) {
-        if (k < nb) {
-          const double d = __shfl_sync(0xffffffffu, w[k], k);
-          const double l = (lane > k && lane < nb) ? w[k] / d : 0.0;
-          if (lane > k) w[k] = l;
+      double* t11 = w11;  // T(i, j) at t11[j * LF_LDW + i]
+      for (int j = 0; j < LF_NB; ++j) t11[j * LF_LDW + lane] = (j == lane) ? 1.0 : 0.0;
+      __syncwarp();
+      for (int k = 0; k < nb; ++k) {
+        const double d = pn[k * ldp + k];
+        const bool below = lane > k && lane < nb;
+        const double l = below ? pn[k * ldp + lane] / d : 0.0;
+        if (below) pn[k * ldp + lane] = l;
+        __syncwarp();
+        if (below) {
           const double ld = l * d;
-#pragma unroll
-          for (int j = k + 1; j < LF_NB; ++j) {
-            const double lj = __shfl_sync(0xffffffffu, l, j);
-            if (j <= lane) w[j] -= ld * lj;
-          }
+          lf_axpy(pn + lane, ldp, pn + k * ldp, 1, k + 1, lane, ld);
+          lf_axpy(t11 + lane, LF_LDW, t11 + k, LF_LDW, 0, k, l);
         }
+        __syncwarp();
       }
       if (lane < nb) {
+        const double d = pn[lane * ldp + lane];
+        const double dinv = 1.0 / d;
         double* col = A + (int64_t)k0 * m + k0 + lane;  // row k0 + lane of the leaf
-        double d = 0.0;
-#pragma unroll
-        for (int j = 0; j < LF_NB; ++j) {
-          if (j < lane) { pn[j * ldp + lane] = w[j]; col[(int64_t)j * m] = w[j]; }
-          if (j == lane) d = w[j];
-        }
+        for (int j = 0; j < lane; ++j) col[(int64_t)j * m] = pn[j * ldp + lane];
         col[(int64_t)lane * m] = d;
         dall[k0 + lane] = d;
-        dinv[lane] = 1.0 / d;
         logdet += log(fabs(d));
+        for (int j = 0; j <= lane; ++j) t11[j * LF_LDW + lane] *= dinv;
       }
     }
     __syncthreads();
     // (4) the rows below the diagonal block (there are some only when the panel is full: nb == LF_NB)
-    const volatile double* l11 = pn;  // (volatile: read where used, not hoisted out of the row loop into 528 registers)
-    for (int i = LF_NB + threadIdx.x; i < rem; i += LF_THREADS) {
-      double w[LF_NB];
+    if (rem > LF_NB) {
+      const int n_tiles = (rem - LF_NB + 15) / 16;
+      for (int t = warp; t < n_tiles; t += LF_THREADS / 32) {
+        const int r0 = LF_NB + t * 16;
+        bool aok[2];
 #pragma unroll
-      for (int j = 0; j < LF_NB; ++j) w[j] = pn[j * ldp + i];
+        for (int a = 0; a < 2; ++a) aok[a] = r0 + a * 8 + lr < rem;
+        double acc[2][4][2];
 #pragma unroll
-      for (int j = 0; j < LF_NB; ++j) {
-        double s = w[j];
+        for (int a = 0; a < 2; ++a)
 #pragma unroll
-        for (int q = 0; q < j; ++q) s -= w[q] * l11[q * ldp + j];
-        w[j] = s;
+          for (int b = 0; b < 4; ++b) { acc[a][b][0] = 0.0; acc[a][b][1] = 0.0; }
+#pragma unroll
+        for (int q0 = 0; q0 < LF_NB; q0 += 4) {
+          const int q = q0 + lc;
+          double af[2], bf[4];
+#pragma unroll
+          for (int a = 0; a < 2; ++a) af[a] = aok[a] ? pn[q * ldp + r0 + a * 8 + lr] : 0.0;
+#pragma unroll
+          for (int b = 0; b < 4; ++b) bf[b] = w11[q * LF_LDW + b * 8 + lr];
+#pragma unroll
+          for (int a = 0; a < 2; ++a)
+#pragma unroll
+            for (int b = 0; b < 4; ++b) dmma884(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
+        }
+#pragma unroll
+        for (int a = 0; a < 2; ++a) {
+          const int i = r0 + a * 8 + lr;
+          if (i < rem) {
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) A[(int64_t)(k0 + b * 8 + 2 * lc + e) * m + k0 + i] = acc[a][b][e];
+          }
+        }
       }
-      double* row = A + (int64_t)k0 * m + k0 + i;
-#pragma unroll
-      for (int j = 0; j < LF_NB; ++j) row[(int64_t)j * m] = w[j] * dinv[j];
     }
     __syncthreads();
   }
@@ -168,7 +214,8 @@ __global__ void __launch_bounds__(LF_THREADS, 2) leaf_factor_kernel(const DevPro
 
 // dynamic shared memory of leaf_factor_kernel<SHAPE> for leaves of up to max_m rows
 __host__ inline size_t lf_smem_bytes(int shape, int max_m) {
-  return sizeof(double) * (size_t)(LF_NB + 1) * lf_panel_ld(max_m) + (shape == BGP_SHAPE_GENERIC ? sizeof(DevProgram) : 0);
+  return sizeof(double) * ((size_t)(LF_NB + 1) * lf_panel_ld(max_m) + LF_NB * LF_LDW) +
+         (shape == BGP_SHAPE_GENERIC ? sizeof(DevProgram) : 0);
 }
 
 template <int SHAPE>
