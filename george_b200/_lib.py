@@ -74,6 +74,7 @@ SIGNATURES = {
     "bgp_dense_predict_grad": (C.c_int, [_p, _specp, _p, _i64, _p, _p]),
     "bgp_hodlr_predict_grad": (C.c_int, [_p, _specp, _p, _i64, _p, _p]),
     "bgp_hodlr_predict_local_dev": (C.c_int, [_p, _specp, _p, _i64, _i32, _p, _i64, _i32, _p]),
+    "bgp_hodlr_predict_grad_local_dev": (C.c_int, [_p, _specp, _p, _i64, _p, _i64, _i32, _p, _p]),
     "bgp_mvn_sample": (C.c_int, [_p, _i64, _p, _p, _i64, C.c_double, _p]),
     "bgp_dense_sample": (C.c_int, [_p, _specp, _p, _i64, _p, _p, _i64, C.c_double, _p]),
     "bgp_hodlr_sample": (C.c_int, [_p, _specp, _p, _i64, _p, _p, _i64, C.c_double, _p]),

@@ -47,6 +47,7 @@ int predict_var_launch(const double* B, int64_t ldb, const double* W, int64_t ld
 int kmat_x1_grad_matvec_launch(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1,
                                const double* x2, int64_t n2, const double* V, int64_t ldv, double scale, int add_prior,
                                double* out, DevBuf<double>& scratch, cudaStream_t s);
+int64_t x1_grad_partial_size(int64_t n1, int64_t n2, int nd);
 void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, int64_t* klen_out);
 int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
                      bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
@@ -1480,27 +1481,30 @@ int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const 
 //   VAR: out_j = (prior ? k(x*_j, x*_j) : 0) - sum_{i in J} B_ij W_ij                (ns)
 //   COV: out   = (prior ? K** : 0) - B[J]^T W[J]          (ns x ns, column-major ld ns: bgp_hodlr_predict's layout)
 // with B = K(x, x*) built for the rows J only and W = K^-1 B read in the rows J only, one test-point chunk of c columns
-// at a time.  The chunks, builds and contractions are bgp_hodlr_predict's, so on an unsharded handle with the prior the
-// result is its bits.  predict_own_prepare validates and reserves without touching the device, so that a collective
-// caller can agree on the outcome before anything runs; predict_own_begin then uploads xs and, for COV, builds the
-// prior and the resident B[J] (nloc x ns); predict_own_chunk contracts one chunk.
+// at a time.  With `grad` (VAR only) each chunk also contracts GP.grad_predict's variance gradient over J:
+//   dvar_jq = (prior ? d k(x*_j, x*_j) / d x*_jq : 0) - 2 sum_{i in J} d k(x*_j, x_i) / d x*_jq W_ij   (ns x ndim)
+// The chunks, builds and contractions are bgp_hodlr_predict's (and bgp_hodlr_predict_grad's), so on an unsharded handle
+// with the prior the result is its bits.  predict_own_prepare validates and reserves without touching the device, so
+// that a collective caller can agree on the outcome before anything runs; predict_own_begin then uploads xs and, for
+// COV, builds the prior and the resident B[J] (nloc x ns); predict_own_chunk contracts one chunk.
 struct PredictOwnRows {
   DevProgram P;
   DevBuf<DevProgram> dprog;
-  DevBuf<double> dxs, dB, dkd, dout, scratch;
+  DevBuf<double> dxs, dB, dkd, dout, ddvar, scratch;
   DevBuf<GemmDesc> ddesc;
   int64_t ns = 0, c = 0;
   int32_t what = 0;
-  bool prior = false;
+  bool prior = false, grad = false;
 };
 
 static int predict_own_prepare(bgp_hodlr* h, const bgp_kernel_spec_t* spec, int64_t ns, int32_t what, bool prior,
-                               PredictOwnRows* w) {
+                               bool grad, PredictOwnRows* w) {
   if (what != BGP_PREDICT_VAR && what != BGP_PREDICT_COV) { set_error("invalid prediction kind %d", what); return BGP_ERR_INVALID; }
   if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
   BGP_TRY(build_dev_program(spec, &w->P));
   if (w->P.ndim != h->ndim) { set_error("dimension mismatch: kernel ndim %d, input ndim %d", w->P.ndim, h->ndim); return BGP_ERR_DIM; }
-  w->ns = ns; w->what = what; w->prior = prior;
+  if (grad && w->P.ndim > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, w->P.ndim); return BGP_ERR_INVALID; }
+  w->ns = ns; w->what = what; w->prior = prior; w->grad = grad;
   if (ns == 0) return BGP_OK;
   cudaStream_t s = h->sA;
   const int64_t nloc = h->nloc;
@@ -1512,7 +1516,12 @@ static int predict_own_prepare(bgp_hodlr* h, const bgp_kernel_spec_t* spec, int6
     BGP_TRY(w->dB.reserve((size_t)nloc * c, s));
     BGP_TRY(w->dkd.reserve((size_t)c, s));
     BGP_TRY(w->dout.reserve((size_t)ns, s));
-    BGP_TRY(w->scratch.reserve((size_t)std::max(predict_var_partial_size(nloc, c), predict_var_partial_size(nloc, tail)), s));
+    int64_t sc = std::max(predict_var_partial_size(nloc, c), predict_var_partial_size(nloc, tail));
+    if (grad) {  // the variance gradient's partials share the scratch with the variance's
+      BGP_TRY(w->ddvar.reserve((size_t)ns * h->ndim, s));
+      sc = std::max(sc, std::max(x1_grad_partial_size(c, nloc, h->ndim), x1_grad_partial_size(tail, nloc, h->ndim)));
+    }
+    BGP_TRY(w->scratch.reserve((size_t)sc, s));
   } else {
     BGP_TRY(w->dB.reserve((size_t)nloc * ns, s));
     BGP_TRY(w->dout.reserve((size_t)ns * ns, s));
@@ -1547,25 +1556,30 @@ static int predict_own_chunk(bgp_hodlr* h, PredictOwnRows& w, int64_t j0, int64_
     const double* xc = w.dxs.p + j0 * h->ndim;
     BGP_TRY(kmat_general_launch_auto(w.P, w.dprog.p, xc, nc, h->d_x.p + h->row0 * h->ndim, nloc, w.dB.p, nloc, s));
     if (w.prior) BGP_TRY(kmat_diagonal_launch(w.dprog.p, xc, xc, nc, w.dkd.p, s));
-    return predict_var_launch(w.dB.p, nloc, Wc + h->row0, ldw, nloc, nc, w.dkd.p, w.dout.p + j0, w.scratch, s);
+    BGP_TRY(predict_var_launch(w.dB.p, nloc, Wc + h->row0, ldw, nloc, nc, w.dkd.p, w.dout.p + j0, w.scratch, s));
+    if (!w.grad) return BGP_OK;
+    return kmat_x1_grad_matvec_launch(w.P, w.dprog.p, xc, nc, h->d_x.p + h->row0 * h->ndim, nloc, Wc + h->row0, ldw,
+                                      -2.0, w.prior ? 1 : 0, w.ddvar.p + j0 * h->ndim, w.scratch, s);
   }
   // rows j0.. of the column-major result are output COLUMNS j of the row-major one, as in bgp_hodlr_predict
   return predict_gemm_sub(Wc + h->row0, ldw, w.dB.p, nloc, nc, w.ns, nloc, false, w.dout.p + j0, w.ns, w.scratch,
                           w.ddesc, s);
 }
 
-// bgp_hodlr_predict on a shard with a matching communicator (include/bgp.h): per test-point chunk, this shard's rows of
-// B = K(x, x*) are built into the rows J of an N x c chunk, the collective solve fills the other rows from the other
-// shards and runs the top levels, and predict_own_chunk contracts over J; one all-reduce of the ns (VAR) or ns^2 (COV)
-// partial results ends it.  Every check and reservation comes before the first collective, and an all-reduce of a
-// status value turns a failure on any rank into an error on every rank, so no rank is left waiting in a later one.
+// bgp_hodlr_predict and bgp_hodlr_predict_grad on a shard with a matching communicator (include/bgp.h): per test-point
+// chunk, this shard's rows of B = K(x, x*) are built into the rows J of an N x c chunk, the collective solve fills the
+// other rows from the other shards and runs the top levels, and predict_own_chunk contracts over J; one all-reduce of
+// the ns (VAR) or ns^2 (COV) partial results ends it, followed with `grad` by one of the ns x ndim dvar.  The first is
+// the prediction's own, so a sharded grad_predict's var has predict's bits.  Every check and reservation comes before
+// the first collective, and an all-reduce of a status value turns a failure on any rank into an error on every rank,
+// so no rank is left waiting in a later one.
 static int hodlr_predict_collective(bgp_hodlr* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
-                                    int32_t what, double* out) {
+                                    int32_t what, bool grad, double* out, double* dvar) {
   cudaStream_t s = h->sA;
   const int64_t n = h->n;
   PredictOwnRows w;
   DevBuf<double> dW;
-  int st = predict_own_prepare(h, spec, ns, what, h->opts.shard_rank == 0, &w);
+  int st = predict_own_prepare(h, spec, ns, what, h->opts.shard_rank == 0, grad, &w);
   if (st == BGP_OK && ns == 0) return BGP_OK;  // ns is replicated: every rank returns here
   if (st == BGP_OK) st = dW.alloc((size_t)n * w.c, s);
   if (st == BGP_OK) {  // exchange_rows' staging for the solve's 64-column groups
@@ -1596,18 +1610,24 @@ static int hodlr_predict_collective(bgp_hodlr* h, const bgp_kernel_spec_t* spec,
   const size_t count = (size_t)(what == BGP_PREDICT_VAR ? ns : ns * ns);
   BGP_TRY(comm_allreduce_sum_f64(w.dout.p, count, s));
   BGP_CUDA(cudaMemcpyAsync(out, w.dout.p, sizeof(double) * count, cudaMemcpyDeviceToHost, s));
+  if (grad) {
+    BGP_TRY(comm_allreduce_sum_f64(w.ddvar.p, (size_t)(ns * nd), s));
+    BGP_CUDA(cudaMemcpyAsync(dvar, w.ddvar.p, sizeof(double) * ns * nd, cudaMemcpyDeviceToHost, s));
+  }
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;
 }
 
-// One handle's part of the prediction from the caller's solved W (include/bgp.h).  Issues no collective.
-int bgp_hodlr_predict_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
-                                int32_t what, const double* w_dev, int64_t ldw, int32_t add_prior, double* out) {
+// One handle's part of the prediction (and with `grad` its variance gradient into dvar) from the caller's solved W
+// (include/bgp.h).  Issues no collective.
+static int hodlr_predict_local(bgp_hodlr* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
+                               bool grad, const double* w_dev, int64_t ldw, int32_t add_prior, double* out,
+                               double* dvar) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
   if (ns > 0 && !w_dev) { set_error("predict_local: w_dev is null"); return BGP_ERR_INVALID; }
   if (ldw < h->n) { set_error("predict_local: ldw %lld < n %lld", (long long)ldw, (long long)h->n); return BGP_ERR_INVALID; }
   PredictOwnRows w;
-  BGP_TRY(predict_own_prepare(h, spec, ns, what, add_prior != 0, &w));
+  BGP_TRY(predict_own_prepare(h, spec, ns, what, add_prior != 0, grad, &w));
   if (ns == 0) return BGP_OK;
   cudaStream_t s = h->sA;
   BGP_TRY(predict_own_begin(h, w, xs));
@@ -1615,8 +1635,19 @@ int bgp_hodlr_predict_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, c
     BGP_TRY(predict_own_chunk(h, w, j0, std::min(w.c, ns - j0), w_dev + j0 * ldw, ldw));
   const size_t count = (size_t)(what == BGP_PREDICT_VAR ? ns : ns * ns);
   BGP_CUDA(cudaMemcpyAsync(out, w.dout.p, sizeof(double) * count, cudaMemcpyDeviceToHost, s));
+  if (grad) BGP_CUDA(cudaMemcpyAsync(dvar, w.ddvar.p, sizeof(double) * ns * h->ndim, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;
+}
+
+int bgp_hodlr_predict_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
+                                int32_t what, const double* w_dev, int64_t ldw, int32_t add_prior, double* out) {
+  return hodlr_predict_local(h, spec, xs, ns, what, false, w_dev, ldw, add_prior, out, nullptr);
+}
+
+int bgp_hodlr_predict_grad_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
+                                     const double* w_dev, int64_t ldw, int32_t add_prior, double* var, double* dvar) {
+  return hodlr_predict_local(h, spec, xs, ns, BGP_PREDICT_VAR, true, w_dev, ldw, add_prior, var, dvar);
 }
 
 // GP.predict's covariance on an unsharded handle into dC (ns x ns on the device, allocated here; row-major as
@@ -1656,7 +1687,7 @@ int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
                       double* out) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
   if (host_exchange(h)) { set_error("predict is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
-  if (h->opts.shard_count > 1) return hodlr_predict_collective(h, spec, xs, ns, what, out);
+  if (h->opts.shard_count > 1) return hodlr_predict_collective(h, spec, xs, ns, what, false, out, nullptr);
   if (what != BGP_PREDICT_VAR && what != BGP_PREDICT_COV) { set_error("invalid prediction kind %d", what); return BGP_ERR_INVALID; }
   if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
   DevProgram P;
@@ -1696,11 +1727,13 @@ int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
 }
 
 // GP.grad_predict's var and dvar: bgp_hodlr_predict's VAR chunks, whose W is already K_h^-1 K(x, x*_chunk), then
-// dvar = dprior - 2 sum_j d1 k(x*, x_j) W_j (kmat_x1_grad_matvec_launch).  Unsharded handles only.
+// dvar = dprior - 2 sum_j d1 k(x*, x_j) W_j (kmat_x1_grad_matvec_launch).  On a shard with a matching communicator the
+// call is collective (hodlr_predict_collective).
 int bgp_hodlr_predict_grad(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, double* var,
                            double* dvar) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
-  if (host_exchange(h) || h->opts.shard_count > 1) { set_error("predict_grad is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  if (host_exchange(h)) { set_error("predict_grad is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  if (h->opts.shard_count > 1) return hodlr_predict_collective(h, spec, xs, ns, BGP_PREDICT_VAR, true, var, dvar);
   if (ns < 0) { set_error("negative number of test points"); return BGP_ERR_INVALID; }
   DevProgram P;
   BGP_TRY(build_dev_program(spec, &P));

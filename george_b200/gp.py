@@ -761,8 +761,9 @@ class GP(ModelSet):
         / d t_i - 2 sum_j d1 k(t_i, x_j) W_ji``, the true derivatives for every metric (:func:`Kernel.get_x1_gradient`
         keeps the reference's values, which differ for a general metric).  The contractions run on the device without
         the ``(ns, N, ndim)`` gradient tensor; ``BasicSolver`` and ``HODLRSolver`` stream ``var`` and ``dvar`` through
-        the stored factorisation (``predictive_grad``), every other solver (``TrivialSolver``, ``ShardedHODLRSolver``,
-        a pickled dense solver, plug-ins) contracts the ``solver.apply_inverse(B)`` of :func:`predict`'s host route.
+        the stored factorisation (``predictive_grad``), ``ShardedHODLRSolver`` likewise with each rank contracting its
+        own rows (collective), and every other solver (``TrivialSolver``, a pickled dense solver, plug-ins without a
+        ``predictive_grad`` hook) contracts the ``solver.apply_inverse(B)`` of :func:`predict`'s host route.
 
         A ``ConstantModel`` mean adds nothing to ``dmu``; any other mean model raises ``NotImplementedError`` (the
         modeling protocol has no input gradient).  Inputs of more than 8 dimensions raise ``ValueError``.

@@ -187,6 +187,16 @@ class ShardedHODLRSolver(object):
             raise RuntimeError("you must call 'compute' first")
         return BasicSolver._predictive_call(self.solver._lib.bgp_hodlr_predict, self.solver._ptr, kernel, xs, what)
 
+    def predictive_grad(self, kernel, xs):
+        """``BasicSolver.predictive_grad`` on the sharded factorisation: ``(var, dvar)`` for ``GP.grad_predict``, ``var``
+        bit for bit what :func:`predictive` returns for ``"var"``.  Collective; ``xs`` replicated on every rank, and every
+        rank returns the same result.  Each rank builds and contracts K(x, x*) and its test-point gradient over its own
+        rows only; the collectives are the chunks' solves and two all-reduces, ``var``'s as in :func:`predictive` and then
+        ``dvar``'s (``include/bgp.h: bgp_hodlr_predict_grad``)."""
+        if self.solver is None or not self._computed:
+            raise RuntimeError("you must call 'compute' first")
+        return BasicSolver._predictive_grad_call(self.solver._lib.bgp_hodlr_predict_grad, self.solver._ptr, kernel, xs)
+
     def apply_sqrt(self, r):
         raise NotImplementedError("apply_sqrt is not implemented for the HODLRSolver")
 

@@ -231,6 +231,19 @@ class HODLRSolver(object):
                                                          1 if add_prior else 0, out)
         return BasicSolver._predictive_call(call, self._ptr, kernel, xs, what)
 
+    def predict_grad_local(self, kernel, xs, w_dev, ldw, add_prior):
+        """This handle's part ``(var, dvar)`` of ``GP.grad_predict``'s variance and its test-point gradient over its own
+        rows (``include/bgp.h: bgp_hodlr_predict_grad_local_dev``), from ``w_dev`` as in :func:`predict_local`.  ``var``
+        (``(ns,)``) is :func:`predict_local`'s ``"var"`` part bit for bit; ``dvar`` is ``(ns, ndim)``.  ``add_prior`` adds
+        the prior's terms; summing every shard's parts, with the prior on one of them, gives the gradient.  Issues no
+        collective."""
+        self._require_computed()
+
+        def call(ptr, spec, xs_p, ns, var, dvar):
+            return self._lib.bgp_hodlr_predict_grad_local_dev(ptr, spec, xs_p, ns, w_dev, int(ldw),
+                                                              1 if add_prior else 0, var, dvar)
+        return BasicSolver._predictive_grad_call(call, self._ptr, kernel, xs)
+
     def set_profiling(self, on=True):
         _lib.check(self._lib.bgp_hodlr_set_profiling(self._ptr, 1 if on else 0))
 

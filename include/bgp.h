@@ -261,7 +261,7 @@ int bgp_dense_predict(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const doubl
  * var is reduced; HODLR, the chunk's K_h^-1 K(x, x*) of the VAR path.  The contraction is bgp_kmat_x1_gradient_matvec's
  * (true derivatives for every metric), so identical calls return identical bits as far as the solve does.  Device
  * workspace: the VAR path's plus O(c * ndim).  Errors: those of bgp_*_predict, and BGP_ERR_INVALID for ndim >
- * BGP_MAX_DIM and on any sharded HODLR handle, all checked before anything is launched.  ns == 0 writes nothing. */
+ * BGP_MAX_DIM and on a host-exchange HODLR shard, all checked before anything is launched.  ns == 0 writes nothing. */
 int bgp_dense_predict_grad(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, double* var,
                            double* dvar);
 
@@ -514,7 +514,15 @@ int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const 
  * A host-exchange shard returns BGP_ERR_INVALID, as before; it computes its part with bgp_hodlr_predict_local_dev. */
 int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
                       double* out);
-/* The HODLR counterpart of bgp_dense_predict_grad (see there); unsharded handles only. */
+/* The HODLR counterpart of bgp_dense_predict_grad (see there).
+ * On a sharded factorisation with a matching communicator the call is COLLECTIVE, as bgp_hodlr_predict is, with spec,
+ * xs and ns replicated: per test-point chunk each shard builds its rows J of K(x, x*) into an N x c chunk, the
+ * collective solve fills the other rows and runs the top levels, and the shard contracts var and dvar over J
+ * (bgp_hodlr_predict_grad_local_dev's arithmetic, the prior on shard 0 only).  Two all-reduces end it: the ns doubles of
+ * var, exactly as bgp_hodlr_predict issues it (so var is bgp_hodlr_predict's VAR output bit for bit on every rank), then
+ * the ns * ndim of dvar.  Validation, reservation and the status all-reduce come before the first collective, as in
+ * bgp_hodlr_predict.  Device workspace per shard (doubles), besides the results and xs: N*c + nloc*c + O(c * ndim).
+ * A host-exchange shard returns BGP_ERR_INVALID; it computes its part with bgp_hodlr_predict_grad_local_dev. */
 int bgp_hodlr_predict_grad(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, double* var,
                            double* dvar);
 /* One shard's part of the prediction: with J = this handle's own rows [row0, row0 + rows) ([0, N) unsharded),
@@ -532,6 +540,17 @@ int bgp_hodlr_predict_grad(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const 
  * BGP_ERR_DIM when the spec's ndim differs from the handle's.  ns == 0 writes nothing. */
 int bgp_hodlr_predict_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
                                 int32_t what, const double* w_dev, int64_t ldw, int32_t add_prior, double* out);
+/* One shard's part of the variance gradient (GP.grad_predict): with J, B and w_dev as in bgp_hodlr_predict_local_dev,
+ *   var[j]            = bgp_hodlr_predict_local_dev's VAR output for the same arguments, bit for bit
+ *   dvar[j*ndim + q]  = (add_prior ? d k(x*_j, x*_j) / d x*_jq : 0) - 2 sum_{i in J} d k(x*_j, x_i) / d x*_jq W_ij
+ * (dvar (ns x ndim) row-major, as bgp_hodlr_predict_grad).  Only rows J of w_dev are read, and only rows J of B are
+ * built.  The chunks, contraction plan and evaluator are bgp_hodlr_predict_grad's, so on an unsharded handle with
+ * add_prior = 1 and w_dev = apply_inverse's K^-1 B both outputs are its bits.  Summing the P shards' outputs, add_prior
+ * = 1 on exactly one of them, gives var and dvar.  Issues no collective.  Workspace (doubles): the VAR part's plus
+ * ns * ndim + O(c * ndim).  Errors: those of bgp_hodlr_predict_local_dev, and BGP_ERR_INVALID for ndim > BGP_MAX_DIM,
+ * all before anything is launched.  ns == 0 writes nothing. */
+int bgp_hodlr_predict_grad_local_dev(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns,
+                                     const double* w_dev, int64_t ldw, int32_t add_prior, double* var, double* dvar);
 
 /* ------------------------------------------------------------------------------------------
  * Draws from N(mean, C) on the device: GP.sample_conditional / GP.sample with a caller's random generator (the
@@ -663,7 +682,8 @@ int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n
  * gradient runs there as bgp_hodlr_grad_terms_local_dev on every shard with the solved alpha, the host summing g and
  * assembling the diag slices; with a matching communicator bgp_hodlr_grad_terms does all of it collectively.  The
  * prediction runs there as bgp_hodlr_predict_local_dev on every shard with the solved K^-1 K(x, x*), the host summing
- * the outputs (the prior on one shard); with a matching communicator bgp_hodlr_predict does it collectively.
+ * the outputs (the prior on one shard); with a matching communicator bgp_hodlr_predict does it collectively.  The
+ * variance gradient likewise runs as bgp_hodlr_predict_grad_local_dev, or collectively as bgp_hodlr_predict_grad.
  * bgp_hodlr_log_determinant on a host-exchange shard returns that shard's PARTIAL log-determinant: its own leaves and
  * sub-tree nodes, plus the nodes above the cut on shard 0 only, so the sum over the P shards is log det K.
  *   bgp_hodlr_top_panel(h, &ptr_dev, &row0, &rows, &cols, &ld): device pointer to the (N x cols) column-major panel of

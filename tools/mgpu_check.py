@@ -4,7 +4,10 @@ single-GPU factorisation — same per-node RNG streams, so log-det / solve / gra
 gradient leg runs the collective grad_terms (each rank streams K^-1 over its own columns; all-reduce of g, all-gather of
 the diagonal) against the single-GPU grad_terms on rank 0.  The predict leg runs the collective predictive (each rank
 builds and contracts K(x, x*) over its own rows; the chunks' solves and one all-reduce) for the variance and the
-covariance against the single-GPU bgp_hodlr_predict on rank 0, on the prior's scale."""
+covariance against the single-GPU bgp_hodlr_predict on rank 0, on the prior's scale.  The grad_predict leg runs the
+collective predictive_grad (the same row split for the variance gradient; two all-reduces, var's as predict's) against
+the single-GPU bgp_hodlr_predict_grad on rank 0, and checks on every rank that its var is the collective predictive's
+"var" bit for bit."""
 import os, sys, json
 import numpy as np
 import torch
@@ -38,6 +41,9 @@ for name, kernel, n, ms, exhaust in [
     ga, gg, gd = sh.grad_terms(y, which)  # collective
     xs = np.random.default_rng(7).uniform(x.min() - 0.5, x.max() + 0.5, (300, 1))
     pv, pc = sh.predictive(kernel, xs, "var"), sh.predictive(kernel, xs, "cov")  # collective
+    gv, gdv = sh.predictive_grad(kernel, xs)  # collective
+    var_bits = bool(np.array_equal(gv, pv))
+    ok = ok and var_bits
     if rank == 0:
         s = HODLRSolver(); s.compute(kernel, x[:, None], yerr, min_size=ms, tol=1e-10, seed=42, exhaust=exhaust)
         ld1, ds1 = s.log_determinant, s.dot_solve(y)
@@ -48,15 +54,18 @@ for name, kernel, n, ms, exhaust in [
         pc1 = BasicSolver._predictive_call(s._lib.bgp_hodlr_predict, s._ptr, kernel, xs, "cov")
         kss = np.max(np.abs(kernel.get_value(xs)))
         p_rel = float(max(np.max(np.abs(pv - pv1)), np.max(np.abs(pc - pc1))) / kss)
+        gv1, gdv1 = BasicSolver._predictive_grad_call(s._lib.bgp_hodlr_predict_grad, s._ptr, kernel, xs)
+        pg_rel = float(max(np.max(np.abs(gv - gv1)), np.max(np.abs(gdv - gdv1))) / kss)
         g_rel = float(np.max(np.abs(gg - gg1) / np.maximum(1.0, np.abs(gg1))))
         d_rel = float(np.linalg.norm(gd - gd1) / np.linalg.norm(gd1))
         good = abs(ld - ld1) <= 1e-10 * abs(ld1) and abs(ds - ds1) <= 1e-9 * abs(ds1) and np.linalg.norm(a - a1) <= 1e-9 * np.linalg.norm(a1)
         good = good and g_rel <= 1e-9 and d_rel <= 1e-9 and np.linalg.norm(ga - ga1) <= 1e-9 * np.linalg.norm(ga1)
-        good = good and p_rel <= 1e-9
+        good = good and p_rel <= 1e-9 and pg_rel <= 1e-9 and var_bits
         ok = ok and good
         print(json.dumps({"case": name, "world": world, "logdet_sharded": ld, "logdet_single": ld1, "dot_sharded": ds, "dot_single": ds1,
                           "solve_relerr": float(np.linalg.norm(a - a1) / np.linalg.norm(a1)), "grad_relerr": g_rel,
-                          "grad_diag_relerr": d_rel, "predict_relerr": p_rel, "ok": bool(good)}))
+                          "grad_diag_relerr": d_rel, "predict_relerr": p_rel, "grad_predict_relerr": pg_rel,
+                          "grad_predict_var_is_predict": var_bits, "ok": bool(good)}))
 dist.barrier()
 if rank == 0:
     print("MGPU_CHECK", "PASS" if ok else "FAIL")
