@@ -211,6 +211,8 @@ constexpr size_t LS_SMEM_MAX = 200 * 1024;
 constexpr int LS_MAX_LEAF = (int)(LS_SMEM_MAX / sizeof(double));  // 25600 rows: one column still fits
 
 static bool leaf_solve_fits(int max_leaf, int cols) { return sizeof(double) * (size_t)max_leaf * cols <= LS_SMEM_MAX; }
+// the group plus the kernel's diagonal blocks: at most 225 KB (LS_COLS_WIDE), within the 227 KB a CTA may opt into
+static int ls_smem_limit(int cols) { return (int)(LS_SMEM_MAX + ls_smem_bytes(0, cols)); }
 
 // cudaFuncSetAttribute applies to the current device: the sweep kernels that take more than the default 48 KB of dynamic
 // shared memory get their limits once per device, not at every level of every call.
@@ -220,11 +222,12 @@ static void set_sweep_func_attrs() {
   cudaGetDevice(&dev);
   const uint64_t bit = dev < 64 ? (1ull << dev) : 0;
   if (bit && (done.load(std::memory_order_relaxed) & bit)) return;
-  cudaFuncSetAttribute(leaf_solve_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
-  cudaFuncSetAttribute(leaf_solve_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
-  cudaFuncSetAttribute(leaf_solve_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
-  cudaFuncSetAttribute(leaf_solve_kernel<LS_COLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
-  cudaFuncSetAttribute(leaf_solve_kernel<LS_COLS_WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LS_SMEM_MAX);
+  cudaFuncSetAttribute(leaf_solve_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ls_smem_limit(1));
+  cudaFuncSetAttribute(leaf_solve_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, ls_smem_limit(2));
+  cudaFuncSetAttribute(leaf_solve_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, ls_smem_limit(4));
+  cudaFuncSetAttribute(leaf_solve_kernel<LS_COLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, ls_smem_limit(LS_COLS));
+  cudaFuncSetAttribute(leaf_solve_kernel<LS_COLS_WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                       ls_smem_limit(LS_COLS_WIDE));
   cudaFuncSetAttribute(small_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
   done.fetch_or(bit, std::memory_order_relaxed);
 }
@@ -235,7 +238,7 @@ static int leaf_solve_launch(bgp_hodlr* h, double* X, int64_t ldx, const int* nc
                              int max_cols, cudaStream_t s, int l0, int l1) {
   const int ngroups = (max_cols + COLS - 1) / COLS;
   const dim3 grid((unsigned)((size_t)(l1 - l0) * (size_t)ngroups));
-  const size_t smem = sizeof(double) * (size_t)h->max_leaf * COLS;
+  const size_t smem = ls_smem_bytes(h->max_leaf, COLS);
   leaf_solve_kernel<COLS><<<grid, LS_THREADS, smem, s>>>(h->d_leaves.p + l0, h->d_L.p, X, ldx, ncols_by_depth,
                                                          ncols_fixed, h->max_leaf, ngroups);
   BGP_LAUNCH_CHECK();

@@ -13,6 +13,7 @@
 #include <cooperative_groups.h>
 
 #include "common.cuh"
+#include "gemm_dmma.cuh"
 #include "kernel_eval.cuh"
 
 namespace bgp {
@@ -213,20 +214,35 @@ constexpr int LS_THREADS = 256;
 constexpr int LS_COLS = 8;        // right-hand sides per CTA of the narrow instantiation (a solve: 1 .. 8 columns)
 constexpr int LS_COLS_WIDE = 32;  // ... of the wide one (BGP_LEAF_COLS=32; measured slower than four narrow groups, see hodlr.cu)
 constexpr int LS_NB = 32;         // diagonal block
-constexpr int LS_BATCH = 4;       // rows per lane loaded together in the backward column dots
+constexpr int LS_LDT = LS_NB + 1; // leading dimension of a staged diagonal block
+constexpr int LS_KB = 16;         // factor entries per thread loaded together: k of a half row (forward), rows (backward)
 
-// Blocked substitution: per 32-column block of L, (a) the 32 x 32 diagonal block is staged in shared memory and each
-// warp solves it for its right-hand sides (columns w, w + 8, ...) with shuffles (no block barrier inside), (b) the rows
-// below (forward) / the columns of the block against the rows below (backward) are updated by the whole CTA with
-// coalesced, independent loads.  m / 32 block steps with two barriers each instead of m dependent steps.
+// dynamic shared memory of leaf_solve_kernel<cols> for leaves of up to max_m rows: the right-hand sides
+// (max_m x cols), two diagonal blocks and one 32-row block of cols right-hand sides
+__host__ __device__ inline size_t ls_smem_bytes(int max_m, int cols) {
+  return sizeof(double) * ((size_t)max_m * cols + 2 * LS_NB * LS_LDT + (size_t)LS_NB * cols);
+}
+
+// Blocked substitution.  Per 32-column block step:
+//   forward:  L11 y_blk = x_blk by one warp per right-hand side with shuffles, then x_below -= L21 y_blk, two threads
+//             per row below, 16 entries of L21 each, loaded together and added with one shuffle;
+//   backward: w_blk = y_blk - L21^T z_below for all 32 columns of the block at once (a warp owns 4 columns of L21 and
+//             8 row phases; the partial sums over rows are added by a shuffle butterfly, a fixed order), then
+//             L11^T z_blk = w_blk by one warp per right-hand side.
+// The diagonal block of the next step is copied into shared memory (cp.async, two buffers) while a step computes, and
+// the first batch of a step's L21 entries is issued before the step's first barrier: none of them depends on the
+// right-hand side.
+// Each output sums its terms in a fixed order, so a solve is reproducible bit for bit, and a column's result does not
+// depend on COLS.
 template <int COLS>
 __global__ void __launch_bounds__(LS_THREADS, COLS <= LS_COLS ? 3 : 1) leaf_solve_kernel(const LeafDesc* __restrict__ leaves,
                                                                 const double* __restrict__ Lbuf,
                                                                 double* __restrict__ X, int64_t ldx,
                                                                 const int* __restrict__ ncols_by_depth, int ncols_fixed,
                                                                 int max_m, int ngroups) {
-  extern __shared__ double xs[];  // max_m x COLS, column-major with leading dimension max_m
-  __shared__ double sL[LS_NB][LS_NB + 1];
+  extern __shared__ double xs[];  // max_m x COLS, column-major with leading dimension max_m; then ls_smem_bytes' rest
+  double* const sT = xs + (size_t)max_m * COLS;     // two diagonal blocks, L11(i, k) at [i * LS_LDT + k]
+  double* const sy = sT + 2 * LS_NB * LS_LDT;       // y_blk / w_blk, (i, c) at [c * LS_NB + i]
   const LeafDesc lf = leaves[blockIdx.x / ngroups];
   const int ncols = ncols_by_depth ? ncols_by_depth[lf.depth] : ncols_fixed;
   const int c0 = (blockIdx.x % ngroups) * COLS;
@@ -235,43 +251,66 @@ __global__ void __launch_bounds__(LS_THREADS, COLS <= LS_COLS ? 3 : 1) leaf_solv
   const int m = lf.size;
   const double* A = Lbuf + lf.off;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  constexpr int NW = LS_THREADS / 32;
+  const int nblk = (m + LS_NB - 1) / LS_NB;
   for (int t = threadIdx.x; t < m * COLS; t += LS_THREADS) {  // (columns >= nc: zeros, so that they stay finite)
     const int i = t % m, c = t / m;
     xs[c * max_m + i] = (c < nc) ? X[(int64_t)(c0 + c) * ldx + lf.start + i] : 0.0;
   }
-  // ---- forward: L y = b (unit lower) ----
-  for (int kb = 0; kb < m; kb += LS_NB) {
-    const int nb = min(LS_NB, m - kb);
-    __syncthreads();  // xs updates of the previous block step (and the initial load) are visible; sL is free
-    for (int t = threadIdx.x; t < LS_NB * LS_NB; t += LS_THREADS) {
-      const int i = t % LS_NB, k = t / LS_NB;
-      sL[i][k] = (i < nb && k < nb && i > k) ? A[(int64_t)(kb + k) * m + kb + i] : 0.0;
+  // the strict lower triangle of diagonal block b into its buffer, zeros elsewhere: thread (i = lane, k = warp + 8 j)
+  auto copy_tile = [&](int b) {
+    const int kb = b * LS_NB, nb = min(LS_NB, m - kb);
+    double* T = sT + (b & 1) * LS_NB * LS_LDT;
+    for (int k = warp; k < LS_NB; k += LS_THREADS / 32) {
+      const bool valid = lane > k && lane < nb;
+      cp_async8(T + lane * LS_LDT + k, valid ? A + (int64_t)(kb + k) * m + kb + lane : A, valid);
     }
-    __syncthreads();
-    for (int c = warp; c < nc; c += NW) {
+    cp_async_commit();
+  };
+  double l[LS_KB];
+
+  // ---- forward: L y = b (unit lower) ----
+  // rows below: thread (row p + 16 warp + (lane & 15), k = 16 (lane >> 4) + j)
+  const int fh = lane >> 4, frow = warp * 16 + (lane & 15);
+  auto load_fwd = [&](int kb, int nb, int r) {
+#pragma unroll
+    for (int j = 0; j < LS_KB; ++j) {
+      const int k = fh * LS_KB + j;
+      l[j] = (r < m && k < nb) ? A[(int64_t)(kb + k) * m + r] : 0.0;
+    }
+  };
+  copy_tile(0);
+  for (int b = 0; b < nblk; ++b) {
+    const int kb = b * LS_NB, nb = min(LS_NB, m - kb), r0 = kb + nb;
+    const double* T = sT + (b & 1) * LS_NB * LS_LDT;
+    load_fwd(kb, nb, r0 + frow);
+    cp_async_wait<0>();
+    __syncthreads();  // T, and the updates of the previous step (or the initial load) are visible
+    if (b + 1 < nblk) copy_tile(b + 1);  // into the buffer step b - 1 read before this barrier
+    for (int c = warp; c < nc; c += LS_THREADS / 32) {
       double y = (lane < nb) ? xs[c * max_m + kb + lane] : 0.0;
       for (int k = 0; k < nb; ++k) {
         const double yk = __shfl_sync(0xffffffffu, y, k);
-        if (lane > k) y -= sL[lane][k] * yk;
+        if (lane > k) y -= T[lane * LS_LDT + k] * yk;
       }
-      if (lane < nb) xs[c * max_m + kb + lane] = y;
+      if (lane < nb) { xs[c * max_m + kb + lane] = y; sy[c * LS_NB + lane] = y; }
     }
     __syncthreads();
-    const int r0 = kb + nb;
-    for (int i = r0 + threadIdx.x; i < m; i += LS_THREADS) {
+    for (int p = r0; p < m; p += LS_THREADS / 2) {
+      const int r = p + frow;
+      if (p > r0) load_fwd(kb, nb, r);
       double acc[COLS];
 #pragma unroll
       for (int c = 0; c < COLS; ++c) acc[c] = 0.0;
-      const double* Li = A + (int64_t)kb * m + i;
-#pragma unroll 8
-      for (int k = 0; k < nb; ++k) {
-        const double l = Li[(int64_t)k * m];
 #pragma unroll
-        for (int c = 0; c < COLS; ++c) acc[c] += l * xs[c * max_m + kb + k];
+      for (int j = 0; j < LS_KB; ++j)
+#pragma unroll
+        for (int c = 0; c < COLS; ++c) acc[c] += l[j] * sy[c * LS_NB + fh * LS_KB + j];
+#pragma unroll
+      for (int c = 0; c < COLS; ++c) acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], 16);
+      if (fh == 0 && r < m) {
+#pragma unroll
+        for (int c = 0; c < COLS; ++c) if (c < nc) xs[c * max_m + r] -= acc[c];
       }
-#pragma unroll
-      for (int c = 0; c < COLS; ++c) if (c < nc) xs[c * max_m + i] -= acc[c];
     }
   }
   __syncthreads();
@@ -280,51 +319,53 @@ __global__ void __launch_bounds__(LS_THREADS, COLS <= LS_COLS ? 3 : 1) leaf_solv
     xs[c * max_m + i] /= A[(int64_t)i * m + i];
   }
   // ---- backward: L^T z = y ----
-  const int nblk = (m + LS_NB - 1) / LS_NB;
-  for (int b = nblk - 1; b >= 0; --b) {
-    const int kb = b * LS_NB;
-    const int nb = min(LS_NB, m - kb);
-    const int r0 = kb + nb;
-    __syncthreads();
-    for (int t = threadIdx.x; t < LS_NB * LS_NB; t += LS_THREADS) {
-      const int i = t % LS_NB, k = t / LS_NB;
-      sL[i][k] = (i < nb && k < nb && i > k) ? A[(int64_t)(kb + k) * m + kb + i] : 0.0;
+  // dots: thread (column k = 4 warp + (lane & 3) of the block, rows p + (lane >> 2) + 8 j)
+  const int bk = warp * 4 + (lane & 3), brow = lane >> 2;
+  auto load_bwd = [&](int kb, int nb, int p) {
+#pragma unroll
+    for (int j = 0; j < LS_KB; ++j) {
+      const int r = p + brow + 8 * j;
+      l[j] = (r < m && bk < nb) ? A[(int64_t)(kb + bk) * m + r] : 0.0;
     }
-    // y_k -= sum_{i >= r0} L[i][k] z_i for the columns k of this block: warp w takes k = w, w + 8, ...
-    for (int k = warp; k < nb; k += NW) {
-      double acc[COLS];
+  };
+  copy_tile(nblk - 1);  // (the forward's last reads of this buffer were before the barrier above)
+  for (int b = nblk - 1; b >= 0; --b) {
+    const int kb = b * LS_NB, nb = min(LS_NB, m - kb), r0 = kb + nb;
+    const double* T = sT + (b & 1) * LS_NB * LS_LDT;
+    load_bwd(kb, nb, r0);
+    cp_async_wait<0>();
+    __syncthreads();  // T, and z of the blocks below (or the scaled y) are visible
+    if (b > 0) copy_tile(b - 1);  // into the buffer step b + 1 read before this barrier
+    double acc[COLS];
 #pragma unroll
-      for (int c = 0; c < COLS; ++c) acc[c] = 0.0;
-      const double* Lk = A + (int64_t)(kb + k) * m;
-      // LS_BATCH rows per lane are loaded before they are used: one load latency per batch instead of one per row
-      // (the sums run over the rows in the same order either way)
-      for (int i0 = r0 + lane; i0 < m; i0 += 32 * LS_BATCH) {
-        double l[LS_BATCH];
+    for (int c = 0; c < COLS; ++c) acc[c] = 0.0;
+    for (int p = r0; p < m; p += 8 * LS_KB) {
+      if (p > r0) load_bwd(kb, nb, p);
 #pragma unroll
-        for (int j = 0; j < LS_BATCH; ++j) l[j] = (i0 + 32 * j < m) ? Lk[i0 + 32 * j] : 0.0;
+      for (int j = 0; j < LS_KB; ++j) {
+        const int r = p + brow + 8 * j;
+        if (r < m) {
 #pragma unroll
-        for (int j = 0; j < LS_BATCH; ++j) {
-          const int i = i0 + 32 * j;
-          if (i < m) {
-#pragma unroll
-            for (int c = 0; c < COLS; ++c) acc[c] += l[j] * xs[c * max_m + i];
-          }
+          for (int c = 0; c < COLS; ++c) acc[c] += l[j] * xs[c * max_m + r];
         }
       }
+    }
 #pragma unroll
-      for (int c = 0; c < COLS; ++c) {
-        const double sres = warp_sum(acc[c]);
-        if (lane == 0 && c < nc) xs[c * max_m + kb + k] -= sres;
-      }
+    for (int off = 4; off < 32; off <<= 1)
+#pragma unroll
+      for (int c = 0; c < COLS; ++c) acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], off);
+    if (brow == 0 && bk < nb) {
+#pragma unroll
+      for (int c = 0; c < COLS; ++c) sy[c * LS_NB + bk] = xs[c * max_m + kb + bk] - acc[c];
     }
     __syncthreads();
-    for (int c = warp; c < nc; c += NW) {
-      double y = (lane < nb) ? xs[c * max_m + kb + lane] : 0.0;
+    for (int c = warp; c < nc; c += LS_THREADS / 32) {
+      double z = (lane < nb) ? sy[c * LS_NB + lane] : 0.0;
       for (int k = nb - 1; k >= 0; --k) {
-        const double zk = __shfl_sync(0xffffffffu, y, k);
-        if (lane < k) y -= sL[k][lane] * zk;
+        const double zk = __shfl_sync(0xffffffffu, z, k);
+        if (lane < k) z -= T[k * LS_LDT + lane] * zk;
       }
-      if (lane < nb) xs[c * max_m + kb + lane] = y;
+      if (lane < nb) xs[c * max_m + kb + lane] = z;
     }
   }
   __syncthreads();
