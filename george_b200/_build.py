@@ -21,7 +21,7 @@ LIBDIR = os.path.join(_HERE, "lib")
 LIB = os.path.join(LIBDIR, "libbgp_b200.so")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 
-SOURCES = ["core.cu", "kmat.cu", "kmat_ops.cu", "dense.cu", "hodlr.cu", "comm.cu", "sample.cu"]
+SOURCES = ["core.cu", "kmat.cu", "kmat_ops.cu", "dense.cu", "hodlr.cu", "hodlr_sym.cu", "comm.cu", "sample.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -56,6 +56,14 @@ int comm_rank();
 int comm_world();
 int comm_allreduce_sum_f64(double* buf, size_t count, cudaStream_t s);
 int comm_allgather_f64(const double* send, double* recv, size_t count, cudaStream_t s);
+struct SymFactor;  // hodlr_sym.cu: the symmetric factor K~ = W W^T
+SymFactor* sym_create();
+void sym_destroy(SymFactor* f);
+int sym_build(SymFactor* f, int64_t n, int nlev, const int* lev, const int* nodes, int nleaf, const int64_t* leaves,
+              int max_leaf, const double* dL, const double* V, int64_t ldv, cudaStream_t s, double* logdet_out);
+int sym_apply(SymFactor* f, double* z, int64_t nrhs, int64_t ldz, int transpose, cudaStream_t s);
+int sym_orthogonality(SymFactor* f, double* out, cudaStream_t s);
+void sym_timing(const SymFactor* f, double* ms2);
 }
 using namespace bgp;
 
@@ -159,6 +167,10 @@ struct bgp_hodlr {
   double t_ms[5] = {0, 0, 0, 0, 0};
   double grad_t[4] = {0, 0, 0, 0};  // see bgp_hodlr_last_grad_timing
   double work[6] = {0, 0, 0, 0, 0, 0};
+
+  SymFactor* sym = nullptr;  // the symmetric factor, built on first use after a compute() (bgp_hodlr_sym_factor)
+  bool sym_current = false;  // sym belongs to the current factorisation
+  double sym_log_det = 0.0;
 };
 
 static int ensure_streams(bgp_hodlr* h) {
@@ -624,6 +636,7 @@ static int run_aca2(bgp_hodlr* h, const std::vector<AcaDesc>& descs, std::vector
 static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, const double* x_dev, int64_t n,
                                   int32_t ndim, const double* yerr_dev, const bgp_hodlr_opts_t* opts_in) {
   h->computed = false;
+  h->sym_current = false;
   h->top_pending = false;
   for (uint64_t& c : h->draw_paths) c = 0;  // (rng_mode = reference never runs the speculative draws)
   for (uint64_t& c : h->eval_units) c = 0;
@@ -1206,6 +1219,7 @@ void bgp_hodlr_destroy(bgp_hodlr_t* h) {
   h->d_vpart.release(); h->d_upart.release(); h->d_vmax.release(); h->d_cmax.release(); h->d_stats.release(); h->d_work.release(); h->d_work_count.release();
   for (cudaEvent_t e : h->prof_events) cudaEventDestroy(e);
   h->d_iter.release();
+  if (h->sym) sym_destroy(h->sym);
   if (h->aca_exec) cudaGraphExecDestroy(h->aca_exec);
   if (h->aca_graph) cudaGraphDestroy(h->aca_graph);
   if (h->sC) cudaStreamDestroy(h->sC);
@@ -1227,6 +1241,7 @@ int bgp_hodlr_compute(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
                       const double* yerr, const bgp_hodlr_opts_t* opts) {
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
   h->computed = false;
+  h->sym_current = false;
   h->top_pending = false;  // (hodlr_compute_dev_impl resets these too; this covers the returns before it)
   h->shard_row0.clear(); h->shard_rows.clear();
   BGP_TRY(require_device());
@@ -1788,6 +1803,70 @@ int bgp_hodlr_sample(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double
   BGP_TRY(sample_mark(0, h->sA));
   BGP_TRY(hodlr_predict_cov_dev(h, P, xs, ns, dC));
   return mvn_draw_host_io(dC.p, ns, mean, z, size, jitter, out, h->sA);
+}
+
+// ---- symmetric factor K~ = W W^T (hodlr_sym.cu) ------------------------------------------------------------------
+// Built from the leaves' L D L^T and the raw ACA factors (the V panel), which compute() leaves untouched after it ends,
+// on the first call that needs it after a compute(); compute() marks it stale.  Not on a sharded handle: W's levels
+// above the shard cut would need every shard's rows.
+static int sym_require(bgp_hodlr* h, const char* what) {
+  if (h && h->opts.shard_count > 1) {
+    set_error("%s is not available on a sharded factorisation (shard %d of %d)", what, h->opts.shard_rank,
+              h->opts.shard_count);
+    return BGP_ERR_INVALID;
+  }
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (h->sym_current) return BGP_OK;
+  BGP_TRY(require_device());
+  if (!h->sym && !(h->sym = sym_create())) { set_error("out of host memory"); return BGP_ERR_NOMEM; }
+  const int nlev = (int)h->levels.size();
+  std::vector<int> lev, nodes;
+  for (const LevelInfo& L : h->levels) {
+    lev.insert(lev.end(), {L.r, L.ucol, L.vcol, (int)L.nodes.size()});
+    for (int id : L.nodes) {
+      const HNode& nd = h->nodes[id];
+      nodes.insert(nodes.end(), {nd.start, nd.size, nd.half, nd.rank, id});
+    }
+  }
+  std::vector<int64_t> leaves;
+  int64_t off = 0;
+  for (int id : h->leaves) {  // d_L's layout (hodlr_compute_dev_impl)
+    const HNode& nd = h->nodes[id];
+    const int ncols = nd.depth < nlev ? h->levels[nd.depth].ucol : h->loc.ucols;
+    leaves.insert(leaves.end(), {(int64_t)nd.start, (int64_t)nd.size, (int64_t)ncols, off});
+    off += (int64_t)nd.size * nd.size;
+  }
+  BGP_TRY(sym_build(h->sym, h->n, nlev, lev.data(), nodes.data(), (int)h->leaves.size(), leaves.data(), h->max_leaf,
+                    h->d_L.p, h->loc.vbase(), h->loc.ld, h->sA, &h->sym_log_det));
+  h->sym_current = true;
+  return BGP_OK;
+}
+
+int bgp_hodlr_sym_factor(bgp_hodlr_t* h) { return sym_require(h, "the symmetric factor"); }
+
+int bgp_hodlr_sym_apply(bgp_hodlr_t* h, double* z, int64_t nrhs, int64_t ldz, int32_t transpose) {
+  BGP_TRY(sym_require(h, "the symmetric factor"));
+  if (nrhs <= 0) return BGP_OK;
+  if (ldz < h->n) { set_error("dimension mismatch: ldz < n"); return BGP_ERR_DIM; }
+  return sym_apply(h->sym, z, nrhs, ldz, transpose ? 1 : 0, h->sA);
+}
+
+int bgp_hodlr_sym_log_determinant(bgp_hodlr_t* h, double* out) {
+  BGP_TRY(sym_require(h, "the symmetric factor"));
+  *out = h->sym_log_det;
+  return BGP_OK;
+}
+
+int bgp_hodlr_sym_last_timing(const bgp_hodlr_t* h, double* ms2) {
+  if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  ms2[0] = ms2[1] = 0.0;
+  if (h->sym) sym_timing(h->sym, ms2);
+  return BGP_OK;
+}
+
+int bgp_selftest_hodlr_sym_orthogonality(bgp_hodlr_t* h, double* out) {
+  BGP_TRY(sym_require(h, "the symmetric factor"));
+  return sym_orthogonality(h->sym, out, h->sA);
 }
 
 int bgp_hodlr_num_nodes(const bgp_hodlr_t* h, int64_t* out) {

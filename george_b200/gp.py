@@ -958,7 +958,14 @@ class GP(ModelSet):
         ``K(t, t) + TINY`` on the host).  With ``rng`` (a ``numpy.random.Generator`` or ``RandomState``) the normals are
         ``rng.standard_normal((size, n))``, drawn once after the argument checks: at ``t`` the draws are those of
         :func:`sample_conditional` with ``mu = mean(t)``, ``C = K(t, t)`` and ``jitter = TINY``; with ``t=None`` they
-        are ``solver.apply_sqrt(z) + mean(x)``."""
+        are ``solver.sample_prior(z) + mean(x)`` on a solver with that hook (``HODLRSolver``), else
+        ``solver.apply_sqrt(z) + mean(x)``.
+
+        ``HODLRSolver`` draws through the symmetric factor ``K~ = W W^T`` of its HODLR matrix ``K~`` (built on the
+        device on first use after a ``compute``): the draws ``W z + mean`` are distributed as ``N(mean, K~)``, but they
+        are not the dense solver's draws for the same ``z``, whose square root is the Cholesky factor.  A ``K~`` that
+        is not positive definite raises ``numpy.linalg.LinAlgError`` and leaves the GP as it was.  With ``rng=None``
+        the route stays the reference's, ``apply_sqrt``, which ``HODLRSolver`` does not implement."""
         if rng is None:
             if t is None:
                 self.recompute()
@@ -976,7 +983,10 @@ class GP(ModelSet):
             self._require_computed()
             z = rng.standard_normal((size, self._x.shape[0]))
             self.recompute()
-            draws = self.solver.apply_sqrt(z)
+            hook = getattr(self.solver, "sample_prior", None)
+            draws = hook(z) if hook is not None else None
+            if draws is None:
+                draws = self.solver.apply_sqrt(z)
             draws += self._call_mean(self._x)
         else:
             x = self.parse_samples(t)

@@ -148,6 +148,45 @@ class HODLRSolver(object):
         _lib.check(self._lib.bgp_hodlr_get_inverse(self._ptr, _lib.ptr(out)))
         return out.T
 
+    # ---- symmetric factor K~ = W W^T (not in the reference) -------------------------------------------------------
+    def apply_symmetric_factor(self, z, transpose=False):
+        """``W z`` (or ``W^T z`` with ``transpose``) for the symmetric factor ``K~ = W W^T`` of this factorisation
+        (``include/bgp.h: bgp_hodlr_sym_apply``): ``z`` of shape ``(N,)`` or ``(N, k)``, the result of the same shape.
+        The factor is built on the device on the first call after a ``compute`` and kept until the next one; a
+        ``K~`` that is not positive definite (or not finite) raises ``numpy.linalg.LinAlgError``."""
+        self._require_computed()
+        z = np.asarray(z, dtype=np.float64)
+        if z.ndim not in (1, 2) or z.shape[0] != self._n:
+            raise ValueError("dimension mismatch")
+        b = np.array(z.reshape(self._n, -1), dtype=np.float64, order="F")
+        _lib.check(self._lib.bgp_hodlr_sym_apply(self._ptr, _lib.ptr(b), b.shape[1], self._n, 1 if transpose else 0))
+        return b.reshape(z.shape)
+
+    @property
+    def symmetric_log_determinant(self):
+        """``log|K~|`` from the symmetric factor (``include/bgp.h: bgp_hodlr_sym_log_determinant``): an evaluation
+        independent of :attr:`log_determinant`'s, of the same matrix."""
+        self._require_computed()
+        out = C.c_double()
+        _lib.check(self._lib.bgp_hodlr_sym_log_determinant(self._ptr, C.byref(out)))
+        return out.value
+
+    def symmetric_factor_timing(self):
+        """Device time (ms) of the last symmetric-factor ``build_ms`` and of the last
+        :func:`apply_symmetric_factor`'s products, ``apply_ms``, host transfers excluded
+        (``include/bgp.h: bgp_hodlr_sym_last_timing``)."""
+        t = (C.c_double * 2)()
+        _lib.check(self._lib.bgp_hodlr_sym_last_timing(self._ptr, t))
+        return dict(zip(("build_ms", "apply_ms"), list(t)))
+
+    def symmetric_factor_orthogonality(self):
+        """Test diagnostic: the largest ``|Q^T Q - I|`` entry over the symmetric factor's node bases
+        (``include/bgp.h: bgp_selftest_hodlr_sym_orthogonality``)."""
+        self._require_computed()
+        out = C.c_double()
+        _lib.check(self._lib.bgp_selftest_hodlr_sym_orthogonality(self._ptr, C.byref(out)))
+        return out.value
+
     # ---- introspection (tree / index structure; not in the reference) -------------------------------------------
     def nodes(self):
         n = C.c_int64()

@@ -7,6 +7,8 @@ Drop-in for the reference's shim ``src/george/solvers/hodlr.py:12-76``: same con
 ``NotImplementedError``, pickling drops the native handle and clears ``computed`` so the GP refactorises lazily.
 """
 
+import numpy as np
+
 from .basic import BasicSolver
 from ._hodlr import HODLRSolver as HODLRSolverInterface
 
@@ -86,6 +88,18 @@ class HODLRSolver(BasicSolver):
         if self.solver.shard_count > 1:
             return None
         return self._sample_call(self.solver._lib.bgp_hodlr_sample, self.solver._ptr, kernel, xs, mean, z, jitter)
+
+    def sample_prior(self, z):
+        """Prior draws at the computed coordinates without the mean: ``(W z^T)^T`` for ``z`` of shape ``(size, N)``,
+        ``W`` the symmetric factor ``K~ = W W^T`` of the HODLR matrix (``HODLRSolverInterface.apply_symmetric_factor``);
+        ``None`` on a sharded factorisation."""
+        self._require()
+        if self.solver.shard_count > 1:
+            return None
+        z = np.asarray(z, dtype=np.float64)
+        if z.shape[0] == 0:
+            return np.empty(z.shape, dtype=np.float64)
+        return np.ascontiguousarray(self.solver.apply_symmetric_factor(z.T).T)
 
     def __getstate__(self):
         state = self.__dict__.copy()

@@ -36,7 +36,8 @@ enum {
   BGP_ERR_INVALID = 1,       /* malformed kernel program / argument                              */
   BGP_ERR_DIM = 2,           /* dimension mismatch between x and the kernel                      */
   BGP_ERR_NOT_COMPUTED = 3,  /* solve before compute                                             */
-  BGP_ERR_LINALG = 4,        /* matrix not positive definite (dense path only)                   */
+  BGP_ERR_LINALG = 4,        /* matrix not positive definite (or not finite): dense factorisations, *
+                              * draws, and the HODLR symmetric factor (bgp_hodlr_sym_factor)      */
   BGP_ERR_CUDA = 5,          /* CUDA runtime failure; no CPU fallback exists                     */
   BGP_ERR_NO_DEVICE = 6,     /* no sm_90 device visible: the library refuses to run              */
   BGP_ERR_RANK_CAPACITY = 7, /* ACA rank exceeded the configured capacity (see bgp_hodlr_opts_t) */
@@ -588,6 +589,31 @@ int bgp_hodlr_sample(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double
  * the device for the fused entries, its upload for bgp_mvn_sample) and the upload of mean and z, [1] symmetrisation +
  * Cholesky, [2] the product. */
 int bgp_sample_last_timing(double* ms3);
+
+/* Symmetric factor of a computed (unsharded) HODLR matrix, K~ = W W^T (Ambikasaran, O'Neil & Singh, arXiv:1405.0223):
+ * W = W_leaf W_{k-1} ... W_0, W_leaf = blockdiag(L D^1/2) of the leaves' L D L^T, and W_l block diagonal over the
+ * nodes of level l with blocks I + Q X Q^T (Q orthonormal, from the node's ACA factors).  Built on the device from what
+ * compute() leaves there, on the first of these calls after a compute(), and kept until the next compute(); compute()
+ * and every other entry point do no work for it.  Deterministic: the same factorisation gives the same bits.
+ * Each node's bases come from equilibrated shifted CholeskyQR3, or, where those miss |Q^T Q - I| <= 1e-13 or the Gram
+ * matrix has no Cholesky factor (numerically dependent ACA columns, e.g. a block the ACA returned dense), from
+ * Householder QR: every positive-definite K~ with finite factors is factored.
+ * Device memory, kept on the handle: N * (sum_l r_l + max_l r_l + 64) doubles (the factor panel, the copy of one
+ * level's columns, the apply's 64-column staging), 8 (2r)^2 + 6 r^2 doubles per node, and the products' workspace.
+ * Errors: BGP_ERR_NOT_COMPUTED; BGP_ERR_INVALID on a sharded handle; BGP_ERR_LINALG when K~ is not positive definite,
+ * naming the leaf and row (a pivot D_ii that is not a finite positive number) or the node whose 2r x 2r step
+ * I + M = L L^T has no Cholesky factor, and when a node's factors are not finite. */
+int bgp_hodlr_sym_factor(bgp_hodlr_t* h);
+/* z (n x nrhs, column-major, leading dimension ldz, host) <- W z (transpose = 0) or W^T z, in place.  With z standard
+ * normal, W z is distributed as N(0, K~). */
+int bgp_hodlr_sym_apply(bgp_hodlr_t* h, double* z, int64_t nrhs, int64_t ldz, int32_t transpose);
+/* log|K~| = sum log D_ii + 2 sum_v log|det(I + X_v)|: an independent evaluation of bgp_hodlr_log_determinant's value. */
+int bgp_hodlr_sym_log_determinant(bgp_hodlr_t* h, double* out);
+/* Test diagnostic: max over the nodes and halves of max |Q^T Q - I| of the symmetric factor's orthonormal bases. */
+int bgp_selftest_hodlr_sym_orthogonality(bgp_hodlr_t* h, double* out);
+/* Device-event time (ms) of the last symmetric-factor build ([0]) and of the last bgp_hodlr_sym_apply's products
+ * ([1]: summed over its 64-column groups, host transfers excluded); 0 before the first. */
+int bgp_hodlr_sym_last_timing(const bgp_hodlr_t* h, double* ms2);
 
 /* Tree / index structure introspection (bit-exact parity target; hodlr.h:48-61).
  * Nodes are listed in the reference's PRE-ORDER construction order. */
