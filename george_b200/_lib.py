@@ -117,6 +117,7 @@ SIGNATURES = {
     "bgp_hodlr_sym_apply": (C.c_int, [_p, _p, _i64, _i64, _i32]),
     "bgp_hodlr_sym_log_determinant": (C.c_int, [_p, _dp]),
     "bgp_selftest_hodlr_sym_orthogonality": (C.c_int, [_p, _dp]),
+    "bgp_selftest_hodlr_sym_householder_nodes": (C.c_int, [_p, _p, _i32, _p]),
     "bgp_hodlr_sym_last_timing": (C.c_int, [_p, _dp]),
     "bgp_hodlr_num_nodes": (C.c_int, [_p, C.POINTER(_i64)]),
     "bgp_hodlr_node_info": (C.c_int, [_p, C.POINTER(HodlrNodeInfo)]),

@@ -64,6 +64,7 @@ int sym_build(SymFactor* f, int64_t n, int nlev, const int* lev, const int* node
 int sym_apply(SymFactor* f, double* z, int64_t nrhs, int64_t ldz, int transpose, cudaStream_t s);
 int sym_orthogonality(SymFactor* f, double* out, cudaStream_t s);
 void sym_timing(const SymFactor* f, double* ms2);
+int sym_householder_nodes(const SymFactor* f, int32_t* counts, int32_t cap);
 }
 using namespace bgp;
 
@@ -294,11 +295,20 @@ static int launch_leaf_solve(bgp_hodlr* h, double* X, int64_t ldx, const int* nc
 static int launch_level_big(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t ldx, int ncolsW, int own_off, int factor,
                             int col_lo, int col_hi, cudaStream_t s, int b0, int b1);
 
+// nodes per launch of a level: the products put node * 2 + half on gridDim.y, at most 65535.  A level of 32768 nodes
+// or more (N >= 2^16 min_size) runs in slabs of consecutive nodes; each node's sums are those of a single launch.
+constexpr int LEVEL_SLAB = 32767;
+
 static int launch_level(bgp_hodlr* h, const LevelInfo& L, double* X, int64_t ldx, int ncolsW, int own_off, int factor,
                         int col_lo, int col_hi, cudaStream_t s, int b0 = 0, int b1 = -1) {
   if (b1 < 0) b1 = (int)L.nodes.size();
   const int nn = b1 - b0;
   if (nn <= 0 || L.r == 0) {
+    return BGP_OK;
+  }
+  if (nn > LEVEL_SLAB) {  // the products put node * 2 + half on gridDim.y (at most 65535): slabs of nodes, in order
+    for (int c0 = b0; c0 < b1; c0 += LEVEL_SLAB)
+      BGP_TRY(launch_level(h, L, X, ldx, ncolsW, own_off, factor, col_lo, col_hi, s, c0, std::min(b1, c0 + LEVEL_SLAB)));
     return BGP_OK;
   }
   const int r = L.r;
@@ -1867,6 +1877,12 @@ int bgp_hodlr_sym_last_timing(const bgp_hodlr_t* h, double* ms2) {
 int bgp_selftest_hodlr_sym_orthogonality(bgp_hodlr_t* h, double* out) {
   BGP_TRY(sym_require(h, "the symmetric factor"));
   return sym_orthogonality(h->sym, out, h->sA);
+}
+
+int bgp_selftest_hodlr_sym_householder_nodes(bgp_hodlr_t* h, int32_t* counts, int32_t cap, int32_t* nlev) {
+  BGP_TRY(sym_require(h, "the symmetric factor"));
+  *nlev = sym_householder_nodes(h->sym, counts, cap);
+  return BGP_OK;
 }
 
 int bgp_hodlr_num_nodes(const bgp_hodlr_t* h, int64_t* out) {

@@ -16,6 +16,8 @@
 // transpose runs the reverse order with X^T and D^1/2 L^T.
 #include <algorithm>
 #include <cmath>
+#include <cstdlib>
+#include <cstring>
 #include <vector>
 
 #include "hodlr_sym.cuh"
@@ -39,7 +41,8 @@ struct SymFactor {
   DevBuf<SymNode> d_nodes;
   DevBuf<SymLeaf> d_leaves;
   DevBuf<double> P, XY, QR, part, tbuf, ubuf, z, leaf_logdet, node_logdet, orth, acopy;
-  DevBuf<int> status, bad_row;
+  DevBuf<int> status, bad_row, redone;
+  std::vector<int> householder_nodes;  // per level: nodes whose bases came from sym_householder_kernel
   cudaEvent_t ev[2] = {nullptr, nullptr};
   double build_ms = 0.0, apply_ms = 0.0;  // device time of the last build / of the last apply's products
   ~SymFactor() {
@@ -50,6 +53,12 @@ struct SymFactor {
 
 // |Q^T Q - I| above which CholeskyQR3's bases are redone by Householder QR (the factor identity's 1e-13 target)
 constexpr double SY_ORTH_BAR = 1e-13;
+// The largest level rank the build accepts.  Each node's 2r x 2r Cholesky of I + M, its triangular inverse and the
+// Householder QR of its halves run in one CTA, in time that grows as r^3 (DESIGN.md: 1.9 s at r = 800, 3.9 s at 1024 on
+// one H100); past this the build is rejected before it launches anything.
+constexpr int SY_MAX_RANK = 2048;
+// nodes per launch of the kernels that put the node on gridDim.y (at most 65535; sym_tn / sym_nn use node * 2 + half)
+constexpr int SY_LEVEL_SLAB = 32767;
 
 SymFactor* sym_create() { return new SymFactor(); }
 void sym_destroy(SymFactor* f) { delete f; }
@@ -112,20 +121,34 @@ static int nchunks_of(const SymLevelHost& L) { return std::max(1, (L.max_half + 
 static int launch_tn(SymFactor* f, const SymLevelHost& L, const double* B, int bcol0, int ncols, cudaStream_t s) {
   const int nch = nchunks_of(L);
   BGP_TRY(f->part.reserve((size_t)L.nn * 2 * nch * L.r * ncols, s));
-  const dim3 grid((unsigned)nch, (unsigned)(2 * L.nn), (unsigned)((ncols + SY_TN_TC - 1) / SY_TN_TC));
-  sym_tn_kernel<<<grid, SY_THREADS, 0, s>>>(f->d_nodes.p + L.node0, f->P.p, f->n, B, f->n, bcol0, ncols, f->part.p, nch);
-  BGP_LAUNCH_CHECK();
+  for (int b0 = 0; b0 < L.nn; b0 += SY_LEVEL_SLAB) {
+    const int nb = std::min(SY_LEVEL_SLAB, L.nn - b0);
+    const dim3 grid((unsigned)nch, (unsigned)(2 * nb), (unsigned)((ncols + SY_TN_TC - 1) / SY_TN_TC));
+    sym_tn_kernel<<<grid, SY_THREADS, 0, s>>>(f->d_nodes.p + L.node0, f->P.p, f->n, B, f->n, bcol0, ncols, f->part.p, nch,
+                                              b0);
+    BGP_LAUNCH_CHECK();
+  }
   return BGP_OK;
+}
+
+// sym_nn_kernel's rows per CTA: 32, halved until the staged rows x (r + 1) doubles fit (one row up to r = 25599)
+static int nn_rows(int r) {
+  int rows = SY_NN_ROWS;
+  while (rows > 1 && sizeof(double) * (size_t)rows * (r + 1) > SY_SMEM_MAX) rows /= 2;
+  return rows;
 }
 
 static int launch_nn(SymFactor* f, const SymLevelHost& L, const double* T, int64_t tstride, int64_t thalf, int ldt,
                      double* O, int ocol0, int ncols, int accumulate, cudaStream_t s) {
-  const size_t smem = sizeof(double) * SY_NN_ROWS * (size_t)(L.r + 1);
-  if (smem > SY_SMEM_MAX) { set_error("HODLR rank %d too large for the symmetric factor", L.r); return BGP_ERR_INVALID; }
-  const dim3 grid((unsigned)((L.max_half + 1 + SY_NN_ROWS - 1) / SY_NN_ROWS), (unsigned)(2 * L.nn));
-  sym_nn_kernel<<<grid, SY_THREADS, smem, s>>>(f->d_nodes.p + L.node0, f->P.p, f->n, T, tstride, thalf, ldt, O, f->n,
-                                               ocol0, ncols, accumulate);
-  BGP_LAUNCH_CHECK();
+  const int rows = nn_rows(L.r);
+  const size_t smem = sizeof(double) * rows * (size_t)(L.r + 1);
+  for (int b0 = 0; b0 < L.nn; b0 += SY_LEVEL_SLAB) {
+    const int nb = std::min(SY_LEVEL_SLAB, L.nn - b0);
+    const dim3 grid((unsigned)((L.max_half + 1 + rows - 1) / rows), (unsigned)(2 * nb));
+    sym_nn_kernel<<<grid, SY_THREADS, smem, s>>>(f->d_nodes.p + L.node0, f->P.p, f->n, T, tstride, thalf, ldt, O, f->n,
+                                                 ocol0, ncols, accumulate, rows, b0);
+    BGP_LAUNCH_CHECK();
+  }
   return BGP_OK;
 }
 
@@ -177,6 +200,19 @@ int sym_build(SymFactor* f, int64_t n, int nlev, const int* lev, const int* node
     f->leaves.push_back(lf);
   }
   const int nn = (int)f->nodes.size();
+  for (int l = 0; l < nlev; ++l) {  // before anything is launched
+    const SymLevelHost& L = f->levels[l];
+    if (L.r <= SY_MAX_RANK) continue;
+    int k = L.node0;
+    while (k + 1 < L.node0 + L.nn && f->nodes[k].rank <= SY_MAX_RANK) ++k;
+    const SymNode& d = f->nodes[k];
+    set_error("HODLR node %d (rows [%d, %d), level %d) has rank %d, above the symmetric factor's limit of %d",
+              f->node_id[k], d.start, d.start + d.size, l, d.rank, SY_MAX_RANK);
+    return BGP_ERR_INVALID;
+  }
+  // BGP_SYM_QR=householder (diagnostic): every node through the Householder QR, none through CholeskyQR3
+  const char* qr_env = getenv("BGP_SYM_QR");
+  const bool all_householder = qr_env && !strcmp(qr_env, "householder");
   BGP_TRY(f->d_nodes.reserve(std::max(nn, 1), s));
   BGP_TRY(f->d_leaves.reserve(std::max(nleaf, 1), s));
   BGP_TRY(f->P.reserve((size_t)n * std::max(f->rtot, 1), s));
@@ -185,10 +221,12 @@ int sym_build(SymFactor* f, int64_t n, int nlev, const int* lev, const int* node
   BGP_TRY(f->leaf_logdet.reserve(std::max(nleaf, 1), s));
   BGP_TRY(f->node_logdet.reserve(std::max(nn, 1), s));
   BGP_TRY(f->status.reserve(std::max(nn, 1), s));
+  BGP_TRY(f->redone.reserve(std::max(nn, 1), s));
   BGP_TRY(f->bad_row.reserve(1, s));
   if (nn) BGP_CUDA(cudaMemcpyAsync(f->d_nodes.p, f->nodes.data(), sizeof(SymNode) * nn, cudaMemcpyHostToDevice, s));
   BGP_CUDA(cudaMemcpyAsync(f->d_leaves.p, f->leaves.data(), sizeof(SymLeaf) * nleaf, cudaMemcpyHostToDevice, s));
   BGP_CUDA(cudaMemsetAsync(f->status.p, 0, sizeof(int) * std::max(nn, 1), s));
+  BGP_CUDA(cudaMemsetAsync(f->redone.p, 0, sizeof(int) * std::max(nn, 1), s));
   BGP_CUDA(cudaMemsetAsync(f->node_logdet.p, 0, sizeof(double) * std::max(nn, 1), s));  // levels of rank 0 add nothing
   const int no_row = 0x7fffffff;
   BGP_CUDA(cudaMemcpyAsync(f->bad_row.p, &no_row, sizeof(int), cudaMemcpyHostToDevice, s));
@@ -204,9 +242,12 @@ int sym_build(SymFactor* f, int64_t n, int nlev, const int* lev, const int* node
   // 1. P <- the used V columns
   for (const SymLevelHost& L : f->levels) {
     if (L.r == 0) continue;
-    sym_copy_kernel<<<dim3((unsigned)((L.max_size + SY_THREADS - 1) / SY_THREADS), (unsigned)L.nn), SY_THREADS, 0, s>>>(
-        f->d_nodes.p + L.node0, V, ldv, L.vcol, f->P.p, n);
-    BGP_LAUNCH_CHECK();
+    for (int b0 = 0; b0 < L.nn; b0 += SY_LEVEL_SLAB) {
+      const int nb = std::min(SY_LEVEL_SLAB, L.nn - b0);
+      sym_copy_kernel<<<dim3((unsigned)((L.max_size + SY_THREADS - 1) / SY_THREADS), (unsigned)nb), SY_THREADS, 0, s>>>(
+          f->d_nodes.p + L.node0 + b0, V, ldv, L.vcol, f->P.p, n);
+      BGP_LAUNCH_CHECK();
+    }
   }
   // 2. leaves: D > 0, log|D|, P <- D^-1/2 L^-1 P
   sym_leaf_check_kernel<<<nleaf, SY_THREADS, 0, s>>>(f->d_leaves.p, dL, f->leaf_logdet.p, f->bad_row.p);
@@ -218,7 +259,7 @@ int sym_build(SymFactor* f, int64_t n, int nlev, const int* lev, const int* node
     if (L.r == 0) continue;
     BGP_CUDA(cudaMemcpyAsync(f->acopy.p, f->P.p + (int64_t)L.ucol * n, sizeof(double) * n * L.r,
                              cudaMemcpyDeviceToDevice, s));
-    for (int pass = 0; pass < 3; ++pass) {
+    for (int pass = 0; pass < (all_householder ? 0 : 3); ++pass) {
       BGP_TRY(launch_tn(f, L, f->P.p, L.ucol, L.r, s));
       sym_qr_pass_kernel<<<L.nn, SY_THREADS, sizeof(double) * L.r, s>>>(f->d_nodes.p + L.node0, f->part.p,
                                                                         nchunks_of(L), f->QR.p, pass, f->status.p,
@@ -228,12 +269,14 @@ int sym_build(SymFactor* f, int64_t n, int nlev, const int* lev, const int* node
       BGP_TRY(launch_nn(f, L, f->QR.p + L.q_base + 2 * rr, 6 * rr, rr, L.r, f->P.p, L.ucol, L.r, 0, s));
     }
     BGP_TRY(launch_tn(f, L, f->P.p, L.ucol, L.r, s));
+    // (all_householder: a bar below every |Q^T Q - I| marks every node of nonzero rank)
     sym_orth_kernel<<<L.nn, SY_THREADS, 0, s>>>(f->d_nodes.p + L.node0, f->part.p, nchunks_of(L), nullptr, f->status.p,
-                                                SY_ORTH_BAR, L.node0);
+                                                all_householder ? -1.0 : SY_ORTH_BAR, L.node0);
     BGP_LAUNCH_CHECK();
     // (the copy's column q sits at acopy + q n: shift the base so that the kernel's column ucol + q lands there)
     sym_householder_kernel<<<L.nn, SY_THREADS, sizeof(double) * L.r, s>>>(
-        f->d_nodes.p + L.node0, f->acopy.p - (int64_t)L.ucol * n, n, f->P.p, n, f->QR.p, f->status.p, L.node0);
+        f->d_nodes.p + L.node0, f->acopy.p - (int64_t)L.ucol * n, n, f->P.p, n, f->QR.p, f->status.p, f->redone.p,
+        L.node0);
     BGP_LAUNCH_CHECK();
     sym_node_kernel<<<L.nn, SY_THREADS, 0, s>>>(f->d_nodes.p + L.node0, f->QR.p, f->XY.p, f->node_logdet.p,
                                                 f->status.p, L.node0);
@@ -253,16 +296,20 @@ int sym_build(SymFactor* f, int64_t n, int nlev, const int* lev, const int* node
   BGP_CUDA(cudaEventRecord(f->ev[1], s));
   // errors and the log-determinant
   int bad_row = no_row;
-  std::vector<int> status(nn);
+  std::vector<int> status(nn), redone(nn);
   std::vector<double> ld_leaf(nleaf), ld_node(nn);
   BGP_CUDA(cudaMemcpyAsync(&bad_row, f->bad_row.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   if (nn) BGP_CUDA(cudaMemcpyAsync(status.data(), f->status.p, sizeof(int) * nn, cudaMemcpyDeviceToHost, s));
+  if (nn) BGP_CUDA(cudaMemcpyAsync(redone.data(), f->redone.p, sizeof(int) * nn, cudaMemcpyDeviceToHost, s));
   if (nn) BGP_CUDA(cudaMemcpyAsync(ld_node.data(), f->node_logdet.p, sizeof(double) * nn, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaMemcpyAsync(ld_leaf.data(), f->leaf_logdet.p, sizeof(double) * nleaf, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));
   float ms = 0.f;
   cudaEventElapsedTime(&ms, f->ev[0], f->ev[1]);
   f->build_ms = ms;
+  f->householder_nodes.assign(nlev, 0);
+  for (int l = 0; l < nlev; ++l)
+    for (int b = 0; b < f->levels[l].nn; ++b) f->householder_nodes[l] += redone[f->levels[l].node0 + b];
   if (bad_row != no_row) {
     int li = 0;
     while (li + 1 < nleaf && f->leaves[li].start + f->leaves[li].size <= bad_row) ++li;
@@ -357,6 +404,12 @@ int sym_orthogonality(SymFactor* f, double* out, cudaStream_t s) {
   for (double x : v) m = std::max(m, x);
   *out = m;
   return BGP_OK;
+}
+
+int sym_householder_nodes(const SymFactor* f, int32_t* counts, int32_t cap) {
+  const int nlev = (int)f->householder_nodes.size();
+  for (int l = 0; l < std::min(cap, nlev); ++l) counts[l] = f->householder_nodes[l];
+  return nlev;
 }
 
 void sym_timing(const SymFactor* f, double* ms2) {

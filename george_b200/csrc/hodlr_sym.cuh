@@ -29,7 +29,8 @@ constexpr int SY_TN_ROWS = 64;     // rows per shared-memory slab of sym_tn_kern
 constexpr int SY_TN_TQ = 32;       // Q columns per pass
 constexpr int SY_TN_TC = 32;       // target columns per CTA
 constexpr int SY_TN_CHUNK = 2048;  // rows per CTA: one partial product per chunk, summed in chunk order
-constexpr int SY_NN_ROWS = 32;     // rows per CTA of sym_nn_kernel (staged with all of the node's Q columns)
+constexpr int SY_NN_ROWS = 32;     // rows per CTA of sym_nn_kernel (staged with all of the node's Q columns); fewer,
+                                   // down to 1, where r is too large for 32 rows of it in shared memory
 constexpr int SY_LEAF_COLS = 8;    // right-hand sides per CTA of the leaf kernels
 
 // ---- leaves ------------------------------------------------------------------------------------------------------
@@ -162,14 +163,14 @@ __global__ void __launch_bounds__(SY_THREADS) sym_copy_kernel(const SymNode* __r
 // Partial products  Q_h^T B_h  over one chunk of SY_TN_CHUNK rows of half h of a node: Q_h = the node's own columns of
 // P on the half's rows, B_h = columns [bcol0, bcol0 + ncols) of B on the same rows.  Block (node b, half h, chunk k)
 // of `part` holds the r x ncols partial (leading dimension r) at ((b * 2 + h) * nchunks + k) * r * ncols.
-// grid = (chunk, node * 2 + h, column tile)
+// grid = (chunk, (node - b0) * 2 + h, column tile): a launch covers the nodes [b0, b0 + gridDim.y / 2) of the level
 __global__ void __launch_bounds__(SY_THREADS) sym_tn_kernel(const SymNode* __restrict__ nodes,
                                                             const double* __restrict__ P, int64_t ldp,
                                                             const double* __restrict__ B, int64_t ldb, int bcol0,
-                                                            int ncols, double* __restrict__ part, int nchunks) {
+                                                            int ncols, double* __restrict__ part, int nchunks, int b0) {
   __shared__ double sq[SY_TN_ROWS][SY_TN_TQ + 1];
   __shared__ double sb[SY_TN_ROWS][SY_TN_TC + 1];
-  const SymNode nd = nodes[blockIdx.y >> 1];
+  const SymNode nd = nodes[b0 + (blockIdx.y >> 1)];
   const int h = blockIdx.y & 1;
   const int rs = nd.start + (h ? nd.half : 0), nh = h ? nd.size - nd.half : nd.half;
   const int row_lo = blockIdx.x * SY_TN_CHUNK;
@@ -178,7 +179,7 @@ __global__ void __launch_bounds__(SY_THREADS) sym_tn_kernel(const SymNode* __res
   const int c0 = blockIdx.z * SY_TN_TC;
   if (c0 >= ncols) return;
   const int nc = min(SY_TN_TC, ncols - c0);
-  double* out = part + ((int64_t)blockIdx.y * nchunks + blockIdx.x) * nd.r * ncols;
+  double* out = part + ((int64_t)(2 * b0 + blockIdx.y) * nchunks + blockIdx.x) * nd.r * ncols;
   const int tq = threadIdx.x & 31, tc = threadIdx.x >> 5;
   for (int q0 = 0; q0 < nd.rank; q0 += SY_TN_TQ) {
     const int nq = min(SY_TN_TQ, nd.rank - q0);
@@ -320,30 +321,33 @@ __global__ void __launch_bounds__(SY_THREADS) sym_qr_pass_kernel(const SymNode* 
 
 // O[:, ocol0 + c] (+)= Q_h T_h[:, c] on both halves of every node of a level, c < ncols.  Q_h = the node's own columns
 // of P, T_h(q, c) = T[b * tstride + h * thalf + q + c * ldt].  The CTA stages its rows of Q_h before it writes, and
-// covers all columns of those rows, so O may be Q itself (accumulate = 0: Q_h <- A_h R^-1 in place).
-// grid = (row chunk of SY_NN_ROWS, node * 2 + h); dynamic shared memory SY_NN_ROWS * (r + 1) doubles.
+// covers all columns of those rows, so O may be Q itself (accumulate = 0: Q_h <- A_h R^-1 in place).  Each entry is one
+// sum over q in ascending order, whatever `rows` is.
+// grid = (row chunk of `rows`, (node - b0) * 2 + h); rows a power of two <= SY_NN_ROWS; dynamic shared memory
+// rows * (r + 1) doubles.
 __global__ void __launch_bounds__(SY_THREADS) sym_nn_kernel(const SymNode* __restrict__ nodes, const double* P,
                                                             int64_t ldp, const double* __restrict__ T, int64_t tstride,
                                                             int64_t thalf, int ldt, double* O, int64_t ldo, int ocol0,
-                                                            int ncols, int accumulate) {
+                                                            int ncols, int accumulate, int rows, int b0) {
   extern __shared__ double sa[];  // (row, q) at row * (rank + 1) + q
-  const SymNode nd = nodes[blockIdx.y >> 1];
+  const int b = b0 + (blockIdx.y >> 1);
+  const SymNode nd = nodes[b];
   const int h = blockIdx.y & 1;
   const int rs = nd.start + (h ? nd.half : 0), nh = h ? nd.size - nd.half : nd.half;
-  const int i0 = blockIdx.x * SY_NN_ROWS;
+  const int i0 = blockIdx.x * rows;
   const int n = nd.rank;
   if (i0 >= nh || n == 0) return;
-  const int ni = min(SY_NN_ROWS, nh - i0);
-  for (int t = threadIdx.x; t < SY_NN_ROWS * n; t += SY_THREADS) {
-    const int i = t % SY_NN_ROWS, q = t / SY_NN_ROWS;
+  const int ni = min(rows, nh - i0);
+  for (int t = threadIdx.x; t < rows * n; t += SY_THREADS) {
+    const int i = t % rows, q = t / rows;
     sa[i * (n + 1) + q] = i < ni ? P[(int64_t)(nd.ucol + q) * ldp + rs + i0 + i] : 0.0;
   }
   __syncthreads();
-  const double* Th = T + (int64_t)(blockIdx.y >> 1) * tstride + h * thalf;
-  const int i = threadIdx.x % SY_NN_ROWS;
+  const double* Th = T + (int64_t)b * tstride + h * thalf;
+  const int i = threadIdx.x % rows;
   if (i >= ni) return;
   const int nco = accumulate ? ncols : min(ncols, n);  // in place: the padding columns stay zero
-  for (int c = threadIdx.x / SY_NN_ROWS; c < nco; c += SY_THREADS / SY_NN_ROWS) {
+  for (int c = threadIdx.x / rows; c < nco; c += SY_THREADS / rows) {
     const double* tc = Th + (int64_t)c * ldt;
     double acc = 0.0;
     for (int q = 0; q < n; ++q) acc += sa[i * (n + 1) + q] * tc[q];
@@ -461,7 +465,7 @@ __global__ void __launch_bounds__(SY_THREADS) sym_orth_kernel(const SymNode* __r
     double v = 0.0;
     for (int k = 0; k < SY_THREADS / 32; ++k) v = fmax(v, red[k]);
     if (out) out[node_base + blockIdx.x] = v;
-    if (status && status[node_base + blockIdx.x] == 0 && !(v <= bar)) status[node_base + blockIdx.x] = 3;
+    if (status && n > 0 && status[node_base + blockIdx.x] == 0 && !(v <= bar)) status[node_base + blockIdx.x] = 3;
   }
 }
 
@@ -471,12 +475,12 @@ __global__ void __launch_bounds__(SY_THREADS) sym_orth_kernel(const SymNode* __r
 // to rounding whatever the conditioning, and A = Q R holds to rounding.  The reflectors overwrite A below the diagonal
 // (LAPACK's dgeqr2 / dorg2r conventions), Q goes to the node's own columns of P and R to the node's R slot.  Each dot
 // product is a warp's lanes added with a fixed butterfly, so the result is reproducible.  status <- 0, or 1 when a
-// column is not finite.  Dynamic shared memory: r doubles.
+// column is not finite; redone[node] <- 1 when the node's bases came from here.  Dynamic shared memory: r doubles.
 __global__ void __launch_bounds__(SY_THREADS) sym_householder_kernel(const SymNode* __restrict__ nodes,
                                                                      double* __restrict__ A, int64_t lda,
                                                                      double* __restrict__ P, int64_t ldp,
                                                                      double* __restrict__ QR, int* __restrict__ status,
-                                                                     int node_base) {
+                                                                     int* __restrict__ redone, int node_base) {
   extern __shared__ double stau[];
   __shared__ double red[32];
   const SymNode nd = nodes[blockIdx.x];
@@ -545,7 +549,10 @@ __global__ void __launch_bounds__(SY_THREADS) sym_householder_kernel(const SymNo
       __syncthreads();
     }
   }
-  if (threadIdx.x == 0) status[node_base + blockIdx.x] = finite ? 0 : 1;
+  if (threadIdx.x == 0) {
+    status[node_base + blockIdx.x] = finite ? 0 : 1;
+    redone[node_base + blockIdx.x] = 1;
+  }
 }
 
 }  // namespace bgp

@@ -187,6 +187,17 @@ class HODLRSolver(object):
         _lib.check(self._lib.bgp_selftest_hodlr_sym_orthogonality(self._ptr, C.byref(out)))
         return out.value
 
+    def symmetric_factor_householder_nodes(self):
+        """Test diagnostic: per level (root first), how many nodes the symmetric factor's build orthonormalised by
+        Householder QR instead of CholeskyQR3 (``include/bgp.h: bgp_selftest_hodlr_sym_householder_nodes``)."""
+        self._require_computed()
+        nlev = C.c_int32()
+        _lib.check(self._lib.bgp_selftest_hodlr_sym_householder_nodes(self._ptr, None, 0, C.byref(nlev)))
+        counts = np.zeros(max(nlev.value, 1), dtype=np.int32)
+        _lib.check(self._lib.bgp_selftest_hodlr_sym_householder_nodes(self._ptr, _lib.ptr(counts), nlev.value,
+                                                                          C.byref(nlev)))
+        return [int(c) for c in counts[:nlev.value]]
+
     # ---- introspection (tree / index structure; not in the reference) -------------------------------------------
     def nodes(self):
         n = C.c_int64()

@@ -600,8 +600,13 @@ int bgp_sample_last_timing(double* ms3);
  * Householder QR: every positive-definite K~ with finite factors is factored.
  * Device memory, kept on the handle: N * (sum_l r_l + max_l r_l + 64) doubles (the factor panel, the copy of one
  * level's columns, the apply's 64-column staging), 8 (2r)^2 + 6 r^2 doubles per node, and the products' workspace.
- * Errors: BGP_ERR_NOT_COMPUTED; BGP_ERR_INVALID on a sharded handle; BGP_ERR_LINALG when K~ is not positive definite,
- * naming the leaf and row (a pivot D_ii that is not a finite positive number) or the node whose 2r x 2r step
+ * Limits: a level's rank r at most 2048 (each node's 2r x 2r Cholesky and its Householder QR run in one CTA, whose
+ * time grows as r^3); levels of any width (the level kernels launch in slabs of 32767 nodes).
+ * Diagnostic: BGP_SYM_QR=householder (read when the factor is built) sends every node of nonzero rank through the
+ * Householder QR instead of CholeskyQR3; the two give the same W to rounding.
+ * Errors: BGP_ERR_NOT_COMPUTED; BGP_ERR_INVALID on a sharded handle and, before anything is launched, for a node whose
+ * level rank is above the limit (naming the node, its rank and the limit); BGP_ERR_LINALG when K~ is not positive
+ * definite, naming the leaf and row (a pivot D_ii that is not a finite positive number) or the node whose 2r x 2r step
  * I + M = L L^T has no Cholesky factor, and when a node's factors are not finite. */
 int bgp_hodlr_sym_factor(bgp_hodlr_t* h);
 /* z (n x nrhs, column-major, leading dimension ldz, host) <- W z (transpose = 0) or W^T z, in place.  With z standard
@@ -611,6 +616,9 @@ int bgp_hodlr_sym_apply(bgp_hodlr_t* h, double* z, int64_t nrhs, int64_t ldz, in
 int bgp_hodlr_sym_log_determinant(bgp_hodlr_t* h, double* out);
 /* Test diagnostic: max over the nodes and halves of max |Q^T Q - I| of the symmetric factor's orthonormal bases. */
 int bgp_selftest_hodlr_sym_orthogonality(bgp_hodlr_t* h, double* out);
+/* Test diagnostic: how many nodes of each level (0 = the root) the last symmetric-factor build orthonormalised by
+ * Householder QR rather than CholeskyQR3.  counts[l] for l < min(cap, *nlev); *nlev = the number of internal levels. */
+int bgp_selftest_hodlr_sym_householder_nodes(bgp_hodlr_t* h, int32_t* counts, int32_t cap, int32_t* nlev);
 /* Device-event time (ms) of the last symmetric-factor build ([0]) and of the last bgp_hodlr_sym_apply's products
  * ([1]: summed over its 64-column groups, host transfers excluded); 0 before the first. */
 int bgp_hodlr_sym_last_timing(const bgp_hodlr_t* h, double* ms2);
