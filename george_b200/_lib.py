@@ -116,6 +116,12 @@ SIGNATURES = {
     "bgp_hodlr_sym_factor": (C.c_int, [_p]),
     "bgp_hodlr_sym_apply": (C.c_int, [_p, _p, _i64, _i64, _i32]),
     "bgp_hodlr_sym_log_determinant": (C.c_int, [_p, _dp]),
+    "bgp_hodlr_sym_factor_local": (C.c_int, [_p]),
+    "bgp_hodlr_sym_export_top": (C.c_int, [_p, _p, _i64]),
+    "bgp_hodlr_sym_import_top": (C.c_int, [_p, _p, _i64]),
+    "bgp_hodlr_sym_finish_top": (C.c_int, [_p, _dp]),
+    "bgp_hodlr_sym_apply_local_dev": (C.c_int, [_p, _p, _i64, _i64, _i32]),
+    "bgp_hodlr_sym_apply_top_dev": (C.c_int, [_p, _p, _i64, _i64, _i32]),
     "bgp_selftest_hodlr_sym_orthogonality": (C.c_int, [_p, _dp]),
     "bgp_selftest_hodlr_sym_householder_nodes": (C.c_int, [_p, _p, _i32, _p]),
     "bgp_hodlr_sym_last_timing": (C.c_int, [_p, _dp]),

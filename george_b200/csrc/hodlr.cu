@@ -12,6 +12,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <vector>
 
 #include "common.cuh"
@@ -59,9 +60,15 @@ int comm_allgather_f64(const double* send, double* recv, size_t count, cudaStrea
 struct SymFactor;  // hodlr_sym.cu: the symmetric factor K~ = W W^T
 SymFactor* sym_create();
 void sym_destroy(SymFactor* f);
-int sym_build(SymFactor* f, int64_t n, int nlev, const int* lev, const int* nodes, int nleaf, const int64_t* leaves,
-              int max_leaf, const double* dL, const double* V, int64_t ldv, cudaStream_t s, double* logdet_out);
-int sym_apply(SymFactor* f, double* z, int64_t nrhs, int64_t ldz, int transpose, cudaStream_t s);
+int sym_prepare(SymFactor* f, int64_t n, int64_t row0, int64_t nloc, int cut, int nlev, const int* lev,
+                const int* nodes, int nleaf, const int64_t* leaves, int max_leaf, const double* dL, bool staging,
+                cudaStream_t s);
+int sym_build_local(SymFactor* f, const double* vtop, const double* vloc, int64_t ldvloc, cudaStream_t s);
+int sym_build_top(SymFactor* f, int add_top, cudaStream_t s, double* logdet_out);
+double* sym_top_panel(SymFactor* f, int64_t* cols);
+int sym_apply_dev(SymFactor* f, double* Z, int64_t ldz, int64_t nrhs, int transpose, int part, cudaStream_t s);
+int sym_apply(SymFactor* f, double* z, int64_t nrhs, int64_t ldz, int transpose, cudaStream_t s,
+              const std::function<int(double*, int)>& exchange);
 int sym_orthogonality(SymFactor* f, double* out, cudaStream_t s);
 void sym_timing(const SymFactor* f, double* ms2);
 int sym_householder_nodes(const SymFactor* f, int32_t* counts, int32_t cap);
@@ -171,6 +178,7 @@ struct bgp_hodlr {
 
   SymFactor* sym = nullptr;  // the symmetric factor, built on first use after a compute() (bgp_hodlr_sym_factor)
   bool sym_current = false;  // sym belongs to the current factorisation
+  int sym_stage = 0;         // host-exchange build: 0 none, 1 local part built (finish pending), -1 local part failed
   double sym_log_det = 0.0;
 };
 
@@ -647,6 +655,7 @@ static int hodlr_compute_dev_impl(bgp_hodlr* h, const bgp_kernel_spec_t* spec, c
                                   int32_t ndim, const double* yerr_dev, const bgp_hodlr_opts_t* opts_in) {
   h->computed = false;
   h->sym_current = false;
+  h->sym_stage = 0;
   h->top_pending = false;
   for (uint64_t& c : h->draw_paths) c = 0;  // (rng_mode = reference never runs the speculative draws)
   for (uint64_t& c : h->eval_units) c = 0;
@@ -1252,6 +1261,7 @@ int bgp_hodlr_compute(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const doubl
   if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
   h->computed = false;
   h->sym_current = false;
+  h->sym_stage = 0;
   h->top_pending = false;  // (hodlr_compute_dev_impl resets these too; this covers the returns before it)
   h->shard_row0.clear(); h->shard_rows.clear();
   BGP_TRY(require_device());
@@ -1816,18 +1826,15 @@ int bgp_hodlr_sample(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double
 }
 
 // ---- symmetric factor K~ = W W^T (hodlr_sym.cu) ------------------------------------------------------------------
-// Built from the leaves' L D L^T and the raw ACA factors (the V panel), which compute() leaves untouched after it ends,
-// on the first call that needs it after a compute(); compute() marks it stale.  Not on a sharded handle: W's levels
-// above the shard cut would need every shard's rows.
-static int sym_require(bgp_hodlr* h, const char* what) {
-  if (h && h->opts.shard_count > 1) {
-    set_error("%s is not available on a sharded factorisation (shard %d of %d)", what, h->opts.shard_rank,
-              h->opts.shard_count);
-    return BGP_ERR_INVALID;
-  }
-  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
-  if (h->sym_current) return BGP_OK;
-  BGP_TRY(require_device());
+// Built from the leaves' L D L^T and the raw ACA factors (the V panels), which compute() leaves untouched after it ends,
+// on the first call that needs it after a compute(); compute() marks it stale.  On a shard the factor splits at the
+// shard cut like compute() (DESIGN.md §5): the leaves and owned levels on this shard's rows, one all-gather of this
+// shard's rows of the top levels' columns, then the top levels on every shard.  With a matching communicator
+// bgp_hodlr_sym_factor does all of it collectively; a host-exchange shard runs the steps one by one
+// (bgp_hodlr_sym_factor_local, _export_top, _import_top, _finish_top).
+
+// this handle's levels, nodes and leaves for sym_prepare
+static int sym_prepare_handle(bgp_hodlr* h, bool staging) {
   if (!h->sym && !(h->sym = sym_create())) { set_error("out of host memory"); return BGP_ERR_NOMEM; }
   const int nlev = (int)h->levels.size();
   std::vector<int> lev, nodes;
@@ -1840,25 +1847,110 @@ static int sym_require(bgp_hodlr* h, const char* what) {
   }
   std::vector<int64_t> leaves;
   int64_t off = 0;
-  for (int id : h->leaves) {  // d_L's layout (hodlr_compute_dev_impl)
+  for (int id : h->leaves) {  // d_L's layout (hodlr_compute_dev_impl); ncols: the leaf's local ancestor columns
     const HNode& nd = h->nodes[id];
     const int ncols = nd.depth < nlev ? h->levels[nd.depth].ucol : h->loc.ucols;
     leaves.insert(leaves.end(), {(int64_t)nd.start, (int64_t)nd.size, (int64_t)ncols, off});
     off += (int64_t)nd.size * nd.size;
   }
-  BGP_TRY(sym_build(h->sym, h->n, nlev, lev.data(), nodes.data(), (int)h->leaves.size(), leaves.data(), h->max_leaf,
-                    h->d_L.p, h->loc.vbase(), h->loc.ld, h->sA, &h->sym_log_det));
+  const int cut = h->opts.shard_count > 1 ? std::min(h->cut_depth, nlev) : 0;
+  return sym_prepare(h->sym, h->n, h->row0, h->nloc, cut, nlev, lev.data(), nodes.data(), (int)h->leaves.size(),
+                     leaves.data(), h->max_leaf, h->d_L.p, staging, h->sA);
+}
+
+static int sym_local_handle(bgp_hodlr* h) {
+  return sym_build_local(h->sym, h->top.vbase(), h->loc.vbase(), h->loc.ld, h->sA);
+}
+
+// One all-reduce of one double over the shards: each failing shard adds 2^rank.  *failed_shard = the highest failing
+// shard, or -1 when none failed.
+static int allreduce_failed_shard(bgp_hodlr* h, bool failed, int* failed_shard) {
+  cudaStream_t s = h->sA;
+  double v = failed ? std::ldexp(1.0, h->opts.shard_rank) : 0.0;
+  BGP_CUDA(cudaMemcpyAsync(h->d_scalar.p, &v, sizeof(double), cudaMemcpyHostToDevice, s));
+  BGP_TRY(comm_allreduce_sum_f64(h->d_scalar.p, 1, s));
+  BGP_CUDA(cudaMemcpyAsync(&v, h->d_scalar.p, sizeof(double), cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  *failed_shard = v > 0.0 ? std::ilogb(v) : -1;
+  return BGP_OK;
+}
+
+// bgp_hodlr_sym_factor on a shard with a matching communicator.  Every check and reservation comes first, then an
+// all-reduce of a status; the local build, then a second one, so that a shard whose leaf or node has no factor makes
+// every rank return before the all-gather instead of leaving the others waiting in it; the all-gather of this shard's
+// rows of the top columns, the top levels, and one all-reduce of the partial log-determinants.
+static int sym_build_collective(bgp_hodlr* h) {
+  cudaStream_t s = h->sA;
+  int64_t rows_pad = 0, rtop = 0;
+  for (int64_t r : h->shard_rows) rows_pad = std::max(rows_pad, r);
+  int st = sym_prepare_handle(h, true);
+  if (st == BGP_OK) {  // exchange_rows' staging for the top columns and for the apply's 64-column groups
+    sym_top_panel(h->sym, &rtop);
+    const size_t per = (size_t)std::max<int64_t>(rtop, 64) * rows_pad;
+    st = h->d_xsend.reserve(per, s);
+    if (st == BGP_OK) st = h->d_xrecv.reserve(per * h->opts.shard_count, s);
+  }
+  int failed = -1;
+  BGP_TRY(allreduce_failed_shard(h, st != BGP_OK, &failed));
+  if (st != BGP_OK) return st;
+  if (failed >= 0) {
+    set_error("the symmetric factor: shard %d of %d could not validate or reserve its part", failed,
+              h->opts.shard_count);
+    return BGP_ERR_INVALID;
+  }
+  st = sym_local_handle(h);
+  BGP_TRY(allreduce_failed_shard(h, st != BGP_OK, &failed));
+  if (st != BGP_OK) return st;
+  if (failed >= 0) {
+    set_error("the HODLR matrix has no symmetric factor: the local part failed on shard %d of %d (that shard names the "
+              "leaf or node)", failed, h->opts.shard_count);
+    return BGP_ERR_LINALG;
+  }
+  double* ptop = sym_top_panel(h->sym, &rtop);
+  BGP_TRY(exchange_rows(h, ptop, h->n, rtop, s));
+  double ld = 0.0;
+  BGP_TRY(sym_build_top(h->sym, h->opts.shard_rank == 0, s, &ld));  // the same launches and data on every shard
+  BGP_CUDA(cudaMemcpyAsync(h->d_scalar.p, &ld, sizeof(double), cudaMemcpyHostToDevice, s));
+  BGP_TRY(comm_allreduce_sum_f64(h->d_scalar.p, 1, s));
+  BGP_CUDA(cudaMemcpyAsync(&ld, h->d_scalar.p, sizeof(double), cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  h->sym_log_det = ld;
+  return BGP_OK;
+}
+
+static int sym_require(bgp_hodlr* h, const char* what) {
+  if (h && host_exchange(h)) {
+    set_error("%s is not available on a host-exchange shard of a sharded factorisation (shard %d of %d without a "
+              "matching communicator): use bgp_hodlr_sym_factor_local / _export_top / _import_top / _finish_top and "
+              "bgp_hodlr_sym_apply_local_dev / _top_dev", what, h->opts.shard_rank, h->opts.shard_count);
+    return BGP_ERR_INVALID;
+  }
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (h->sym_current) return BGP_OK;
+  BGP_TRY(require_device());
+  h->sym_stage = 0;
+  if (h->opts.shard_count > 1) {
+    BGP_TRY(sym_build_collective(h));
+  } else {
+    BGP_TRY(sym_prepare_handle(h, false));
+    BGP_TRY(sym_local_handle(h));
+    BGP_TRY(sym_build_top(h->sym, 1, h->sA, &h->sym_log_det));
+  }
   h->sym_current = true;
   return BGP_OK;
 }
 
 int bgp_hodlr_sym_factor(bgp_hodlr_t* h) { return sym_require(h, "the symmetric factor"); }
 
+// On a shard with a matching communicator: collective, z replicated, the result replicated (each 64-column group's own
+// rows all-gathered between the local and the top levels).
 int bgp_hodlr_sym_apply(bgp_hodlr_t* h, double* z, int64_t nrhs, int64_t ldz, int32_t transpose) {
   BGP_TRY(sym_require(h, "the symmetric factor"));
   if (nrhs <= 0) return BGP_OK;
   if (ldz < h->n) { set_error("dimension mismatch: ldz < n"); return BGP_ERR_DIM; }
-  return sym_apply(h->sym, z, nrhs, ldz, transpose ? 1 : 0, h->sA);
+  std::function<int(double*, int)> exchange;
+  if (h->opts.shard_count > 1) exchange = [h](double* Z, int nc) { return exchange_rows(h, Z, h->n, nc, h->sA); };
+  return sym_apply(h->sym, z, nrhs, ldz, transpose ? 1 : 0, h->sA, exchange);
 }
 
 int bgp_hodlr_sym_log_determinant(bgp_hodlr_t* h, double* out) {
@@ -2108,6 +2200,112 @@ int bgp_hodlr_solve_top_dev(bgp_hodlr_t* h, double* b_dev, int64_t nrhs, int64_t
   BGP_TRY(hodlr_solve_dev(h, b_dev, nrhs, ldb, h->sA, 2));
   BGP_CUDA(cudaStreamSynchronize(h->sA));
   return BGP_OK;
+}
+
+
+// ---- the symmetric factor on a host-exchange shard (include/bgp.h) -------------------------------------------------
+// sym_stage: 1 between bgp_hodlr_sym_factor_local and bgp_hodlr_sym_finish_top, -1 after a failed local build.
+static int require_sym_local(const bgp_hodlr* h, const char* what) {
+  if (!h) { set_error("null handle"); return BGP_ERR_INVALID; }
+  if (h->sym_stage == 1) return BGP_OK;
+  if (h->sym_current) {
+    set_error("%s: the symmetric factor is complete (bgp_hodlr_sym_finish_top was already called, or it was built "
+              "whole)", what);
+    return BGP_ERR_INVALID;
+  }
+  if (h->sym_stage < 0) {
+    set_error("%s: the local part of the symmetric factor failed to build (see bgp_hodlr_sym_factor_local's error)",
+              what);
+    return BGP_ERR_NOT_COMPUTED;
+  }
+  set_error("%s: the local part of the symmetric factor has not been built (bgp_hodlr_sym_factor_local)", what);
+  return BGP_ERR_NOT_COMPUTED;
+}
+
+int bgp_hodlr_sym_factor_local(bgp_hodlr_t* h) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  BGP_TRY(require_device());
+  h->sym_current = false;
+  h->sym_stage = -1;
+  BGP_TRY(sym_prepare_handle(h, false));
+  BGP_TRY(sym_local_handle(h));
+  h->sym_stage = 1;
+  return BGP_OK;
+}
+
+int bgp_hodlr_sym_export_top(bgp_hodlr_t* h, double* buf_dev, int64_t rows_pad) {
+  BGP_TRY(require_sym_local(h, "sym_export_top"));
+  if (rows_pad < h->nloc) {
+    set_error("rows_pad %lld smaller than this shard (%lld rows)", (long long)rows_pad, (long long)h->nloc);
+    return BGP_ERR_INVALID;
+  }
+  int64_t cols = 0;
+  double* ptop = sym_top_panel(h->sym, &cols);
+  if (cols == 0 || h->nloc == 0) return BGP_OK;
+  pack_rows_kernel<<<1184, 256, 0, h->sA>>>(ptop, h->n, h->row0, h->nloc, cols, buf_dev, rows_pad);
+  BGP_LAUNCH_CHECK();
+  BGP_CUDA(cudaStreamSynchronize(h->sA));
+  return BGP_OK;
+}
+
+int bgp_hodlr_sym_import_top(bgp_hodlr_t* h, const double* all_buf_dev, int64_t rows_pad) {
+  BGP_TRY(require_sym_local(h, "sym_import_top"));
+  int64_t max_rows = 0;
+  for (int64_t r : h->shard_rows) max_rows = std::max(max_rows, r);
+  if (rows_pad < max_rows) {
+    set_error("rows_pad %lld smaller than the largest shard (%lld rows)", (long long)rows_pad, (long long)max_rows);
+    return BGP_ERR_INVALID;
+  }
+  int64_t cols = 0;
+  double* ptop = sym_top_panel(h->sym, &cols);
+  if (cols == 0) return BGP_OK;
+  for (size_t s = 0; s < h->shard_rows.size(); ++s) {
+    if ((int)s == h->opts.shard_rank) continue;  // own rows are already in place
+    unpack_rows_kernel<<<1184, 256, 0, h->sA>>>(ptop, h->n, h->shard_row0[s], h->shard_rows[s], cols,
+                                                all_buf_dev + (int64_t)s * cols * rows_pad, rows_pad);
+    BGP_LAUNCH_CHECK();
+  }
+  BGP_CUDA(cudaStreamSynchronize(h->sA));
+  return BGP_OK;
+}
+
+int bgp_hodlr_sym_finish_top(bgp_hodlr_t* h, double* partial_logdet) {
+  BGP_TRY(require_sym_local(h, "sym_finish_top"));
+  h->sym_stage = -1;
+  double ld = 0.0;
+  BGP_TRY(sym_build_top(h->sym, h->opts.shard_rank == 0, h->sA, &ld));
+  h->sym_stage = 0;
+  h->sym_log_det = ld;
+  h->sym_current = true;
+  if (partial_logdet) *partial_logdet = ld;
+  return BGP_OK;
+}
+
+// part 1 (local) or 2 (top) of W z / W^T z in place on a device block; an unsharded handle builds the factor on first
+// use (part 1 is all of it there, part 2 nothing), a sharded one needs bgp_hodlr_sym_finish_top (or, with a matching
+// communicator, bgp_hodlr_sym_factor) first
+static int sym_apply_part_dev(bgp_hodlr* h, double* z_dev, int64_t nrhs, int64_t ldz, int32_t transpose, int part) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (h->opts.shard_count == 1) {
+    BGP_TRY(sym_require(h, "the symmetric factor"));
+  } else if (!h->sym_current) {
+    set_error("the symmetric factor of this shard is not complete (bgp_hodlr_sym_finish_top)");
+    return BGP_ERR_NOT_COMPUTED;
+  }
+  if (nrhs <= 0) return BGP_OK;
+  if (ldz < h->n) { set_error("dimension mismatch: ldz < n"); return BGP_ERR_DIM; }
+  if (!z_dev) { set_error("sym_apply: z_dev is null"); return BGP_ERR_INVALID; }
+  BGP_TRY(sym_apply_dev(h->sym, z_dev, ldz, nrhs, transpose ? 1 : 0, part, h->sA));
+  BGP_CUDA(cudaStreamSynchronize(h->sA));
+  return BGP_OK;
+}
+
+int bgp_hodlr_sym_apply_local_dev(bgp_hodlr_t* h, double* z_dev, int64_t nrhs, int64_t ldz, int32_t transpose) {
+  return sym_apply_part_dev(h, z_dev, nrhs, ldz, transpose, 1);
+}
+
+int bgp_hodlr_sym_apply_top_dev(bgp_hodlr_t* h, double* z_dev, int64_t nrhs, int64_t ldz, int32_t transpose) {
+  return sym_apply_part_dev(h, z_dev, nrhs, ldz, transpose, 2);
 }
 
 }  // extern "C"

@@ -197,6 +197,34 @@ class ShardedHODLRSolver(object):
             raise RuntimeError("you must call 'compute' first")
         return BasicSolver._predictive_grad_call(self.solver._lib.bgp_hodlr_predict_grad, self.solver._ptr, kernel, xs)
 
+    def apply_symmetric_factor(self, z, transpose=False):
+        """``W z`` (or ``W^T z`` with ``transpose``) for the symmetric factor ``K~ = W W^T`` of the sharded
+        factorisation, as ``HODLRSolver.apply_symmetric_factor``: ``z`` of shape ``(N,)`` or ``(N, k)``, the result of
+        the same shape.  Collective; ``z`` replicated on every rank, and every rank returns the same result.  The factor
+        is built on the first call after a ``compute``: each rank its own sub-tree's rows, one all-gather of those rows
+        of the top levels' columns, the top nodes on every rank; an apply is the top levels, the rank's own levels and
+        leaves, and one all-gather per 64 columns (``include/bgp.h: bgp_hodlr_sym_apply``).  A ``K~`` that is not
+        positive definite raises ``numpy.linalg.LinAlgError`` on every rank."""
+        if self.solver is None or not self._computed:
+            raise RuntimeError("you must call 'compute' first")
+        z = np.asarray(z, dtype=np.float64)
+        if z.ndim not in (1, 2) or z.shape[0] != self._n:
+            raise ValueError("dimension mismatch")
+        b = np.array(z.reshape(self._n, -1), dtype=np.float64, order="F")
+        _lib.check(self.solver._lib.bgp_hodlr_sym_apply(self.solver._ptr, _lib.ptr(b), b.shape[1], self._n,
+                                                        1 if transpose else 0))
+        return b.reshape(z.shape)
+
+    @property
+    def symmetric_log_determinant(self):
+        """``log|K~|`` from the symmetric factor, the same on every rank (one all-reduce of the ranks' partial sums).
+        Collective (``include/bgp.h: bgp_hodlr_sym_log_determinant``)."""
+        if self.solver is None or not self._computed:
+            raise RuntimeError("you must call 'compute' first")
+        out = C.c_double()
+        _lib.check(self.solver._lib.bgp_hodlr_sym_log_determinant(self.solver._ptr, C.byref(out)))
+        return out.value
+
     def apply_sqrt(self, r):
         raise NotImplementedError("apply_sqrt is not implemented for the HODLRSolver")
 

@@ -171,6 +171,37 @@ class HODLRSolver(object):
         _lib.check(self._lib.bgp_hodlr_sym_log_determinant(self._ptr, C.byref(out)))
         return out.value
 
+    # the symmetric factor on a host-exchange shard, step by step (include/bgp.h: bgp_hodlr_sym_factor_local ...)
+    def symmetric_factor_local(self):
+        """Build the leaves, the owned levels and this shard's rows of the top levels' columns
+        (``bgp_hodlr_sym_factor_local``).  Issues no collective."""
+        self._require_computed()
+        _lib.check(self._lib.bgp_hodlr_sym_factor_local(self._ptr))
+
+    def symmetric_export_top(self, buf_dev, rows_pad):
+        """Pack this shard's rows of the factor's top columns into ``buf_dev`` (``bgp_hodlr_sym_export_top``)."""
+        _lib.check(self._lib.bgp_hodlr_sym_export_top(self._ptr, buf_dev, int(rows_pad)))
+
+    def symmetric_import_top(self, all_buf_dev, rows_pad):
+        """Scatter every other shard's rows from the all-gathered buffer (``bgp_hodlr_sym_import_top``)."""
+        _lib.check(self._lib.bgp_hodlr_sym_import_top(self._ptr, all_buf_dev, int(rows_pad)))
+
+    def symmetric_finish_top(self):
+        """The levels above the shard cut; returns this shard's partial ``log|K~|`` (``bgp_hodlr_sym_finish_top``)."""
+        out = C.c_double()
+        _lib.check(self._lib.bgp_hodlr_sym_finish_top(self._ptr, C.byref(out)))
+        return out.value
+
+    def apply_symmetric_factor_local(self, z_dev, nrhs, ldz, transpose=False):
+        """The local part of ``W z`` / ``W^T z`` in place on a device block (``bgp_hodlr_sym_apply_local_dev``)."""
+        _lib.check(self._lib.bgp_hodlr_sym_apply_local_dev(self._ptr, z_dev, int(nrhs), int(ldz),
+                                                           1 if transpose else 0))
+
+    def apply_symmetric_factor_top(self, z_dev, nrhs, ldz, transpose=False):
+        """The top part of ``W z`` / ``W^T z`` in place on a device block (``bgp_hodlr_sym_apply_top_dev``)."""
+        _lib.check(self._lib.bgp_hodlr_sym_apply_top_dev(self._ptr, z_dev, int(nrhs), int(ldz),
+                                                         1 if transpose else 0))
+
     def symmetric_factor_timing(self):
         """Device time (ms) of the last symmetric-factor ``build_ms`` and of the last
         :func:`apply_symmetric_factor`'s products, ``apply_ms``, host transfers excluded

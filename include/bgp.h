@@ -604,16 +604,57 @@ int bgp_sample_last_timing(double* ms3);
  * time grows as r^3); levels of any width (the level kernels launch in slabs of 32767 nodes).
  * Diagnostic: BGP_SYM_QR=householder (read when the factor is built) sends every node of nonzero rank through the
  * Householder QR instead of CholeskyQR3; the two give the same W to rounding.
- * Errors: BGP_ERR_NOT_COMPUTED; BGP_ERR_INVALID on a sharded handle and, before anything is launched, for a node whose
- * level rank is above the limit (naming the node, its rank and the limit); BGP_ERR_LINALG when K~ is not positive
- * definite, naming the leaf and row (a pivot D_ii that is not a finite positive number) or the node whose 2r x 2r step
- * I + M = L L^T has no Cholesky factor, and when a node's factors are not finite. */
+ * Errors: BGP_ERR_NOT_COMPUTED; BGP_ERR_INVALID on a host-exchange shard (checked first; see the sharded entry points
+ * below) and, before anything is launched, for a node whose level rank is above the limit (naming the node, its rank
+ * and the limit); BGP_ERR_LINALG when K~ is not positive definite, naming the leaf and row (a pivot D_ii that is not a
+ * finite positive number) or the node whose 2r x 2r step I + M = L L^T has no Cholesky factor, and when a node's
+ * factors are not finite.
+ * Sharded (opts.shard_count > 1, DESIGN.md §5): on a shard with a matching communicator these three calls are
+ * COLLECTIVE.  The factor splits at the shard cut: each shard factors its leaves and owned levels on its own rows
+ * (each owned node also updating the top levels' columns there), one all-gather of its rows of those columns, then the
+ * nodes above the cut on every shard; log|K~| is one all-reduce of the shards' partial sums.  Every check and
+ * reservation runs before an all-reduce of a status, and the local build ends with a second one before the all-gather:
+ * a shard whose leaf or node has no factor returns BGP_ERR_LINALG naming it, and every other shard BGP_ERR_LINALG naming
+ * that shard.  bgp_hodlr_sym_apply takes z replicated on every shard and returns the result replicated (W: the top
+ * levels, this shard's levels and leaves on its rows, an all-gather of the rows; W^T the reverse).  After any failure
+ * the factor is not current and the handle stays usable.
+ * Device memory per shard, kept on the handle: N * (R_top + 64) + nloc * R_loc doubles (the top part of the factor
+ * panel, the apply's staging, the local part), the copy of one level's columns (N or nloc rows), the per-node blocks of
+ * the shard's nodes and the nodes above the cut, the products' workspace, and the all-gather's staging
+ * (P + 1) * max(R_top, 64) * rows_pad doubles; R_top and R_loc are the column counts of the top and local U panels. */
 int bgp_hodlr_sym_factor(bgp_hodlr_t* h);
 /* z (n x nrhs, column-major, leading dimension ldz, host) <- W z (transpose = 0) or W^T z, in place.  With z standard
  * normal, W z is distributed as N(0, K~). */
 int bgp_hodlr_sym_apply(bgp_hodlr_t* h, double* z, int64_t nrhs, int64_t ldz, int32_t transpose);
 /* log|K~| = sum log D_ii + 2 sum_v log|det(I + X_v)|: an independent evaluation of bgp_hodlr_log_determinant's value. */
 int bgp_hodlr_sym_log_determinant(bgp_hodlr_t* h, double* out);
+/* The symmetric factor on a host-exchange shard, step by step (the order of export_top / import_top / finish_top /
+ * solve_{local,top}_dev below; the host runs the all-gather):
+ *   1. bgp_hodlr_sym_factor_local on every shard, after its factorisation is finished (bgp_hodlr_finish_top): the
+ *      leaves, the owned levels and this shard's rows of the top levels' columns.  Rebuilds from scratch when called
+ *      again.  Errors as bgp_hodlr_sym_factor's, naming this shard's leaf or node.
+ *   2. bgp_hodlr_sym_export_top into the shard's slot of a (P, cols, rows_pad) device buffer (export_top's layout; cols
+ *      = bgp_hodlr_top_panel's cols), the host all-gathers it, bgp_hodlr_sym_import_top on every shard.
+ *   3. bgp_hodlr_sym_finish_top on every shard, once: the nodes above the cut; marks the factor current and returns
+ *      this shard's PARTIAL log|K~| (its leaves and owned nodes, plus the nodes above the cut on shard 0 only), whose
+ *      sum over the shards is log|K~|.  It is also what bgp_hodlr_sym_log_determinant would hold.
+ *   4. bgp_hodlr_sym_apply_local_dev / bgp_hodlr_sym_apply_top_dev, in place on an (N x nrhs) column-major device block
+ *      with ldz >= N, z replicated: W z is top, then local, then the host assembles rows [row0_s, row0_s + rows_s)
+ *      from shard s; W^T z is local, the host assembles the rows and copies them to every shard, then top.  The local
+ *      part reads and writes this shard's rows only.
+ * On an unsharded handle the local part is the whole factor and the top part does nothing (export / import copy
+ * nothing), and the apply entries build the factor on first use; local + top give bgp_hodlr_sym_apply's bits and the
+ * partial log|K~| is bgp_hodlr_sym_log_determinant's value.  Call-order errors, returned before anything is launched:
+ * BGP_ERR_NOT_COMPUTED for factor_local before the factorisation is finished, for export / import / finish before
+ * factor_local or after it failed, and for the apply entries on a shard before finish; BGP_ERR_INVALID for export /
+ * import / finish once the factor is complete (a second finish) and for a rows_pad below this shard's rows (export) or
+ * the largest shard's rows (import).  Issue no collective. */
+int bgp_hodlr_sym_factor_local(bgp_hodlr_t* h);
+int bgp_hodlr_sym_export_top(bgp_hodlr_t* h, double* buf_dev, int64_t rows_pad);
+int bgp_hodlr_sym_import_top(bgp_hodlr_t* h, const double* all_buf_dev, int64_t rows_pad);
+int bgp_hodlr_sym_finish_top(bgp_hodlr_t* h, double* partial_logdet);
+int bgp_hodlr_sym_apply_local_dev(bgp_hodlr_t* h, double* z_dev, int64_t nrhs, int64_t ldz, int32_t transpose);
+int bgp_hodlr_sym_apply_top_dev(bgp_hodlr_t* h, double* z_dev, int64_t nrhs, int64_t ldz, int32_t transpose);
 /* Test diagnostic: max over the nodes and halves of max |Q^T Q - I| of the symmetric factor's orthonormal bases. */
 int bgp_selftest_hodlr_sym_orthogonality(bgp_hodlr_t* h, double* out);
 /* Test diagnostic: how many nodes of each level (0 = the root) the last symmetric-factor build orthonormalised by

@@ -7,7 +7,9 @@ builds and contracts K(x, x*) over its own rows; the chunks' solves and one all-
 covariance against the single-GPU bgp_hodlr_predict on rank 0, on the prior's scale.  The grad_predict leg runs the
 collective predictive_grad (the same row split for the variance gradient; two all-reduces, var's as predict's) against
 the single-GPU bgp_hodlr_predict_grad on rank 0, and checks on every rank that its var is the collective predictive's
-"var" bit for bit."""
+"var" bit for bit.  The symmetric-factor leg builds K~ = W W^T collectively (each rank its sub-tree's rows, one
+all-gather of the top columns' rows, the top nodes on every rank) and applies W and W^T to replicated columns, against
+the single-GPU factor on rank 0, and checks that every rank returns the same W Z."""
 import os, sys, json
 import numpy as np
 import torch
@@ -44,6 +46,18 @@ for name, kernel, n, ms, exhaust in [
     gv, gdv = sh.predictive_grad(kernel, xs)  # collective
     var_bits = bool(np.array_equal(gv, pv))
     ok = ok and var_bits
+    Z = np.random.default_rng(9).standard_normal((n, 65))
+    try:  # a level rank above the factor's limit is rejected on every rank alike (collective status)
+        wz, wtz, sld = sh.apply_symmetric_factor(Z), sh.apply_symmetric_factor(Z, transpose=True), sh.symmetric_log_determinant
+    except ValueError:
+        wz = None
+    sym_same = True
+    if wz is not None:
+        got = torch.from_numpy(np.ascontiguousarray(wz)).cuda()
+        first = got.clone()
+        dist.broadcast(first, src=0)
+        sym_same = bool(torch.equal(got, first))  # every rank returns the same W Z
+    ok = ok and sym_same
     if rank == 0:
         s = HODLRSolver(); s.compute(kernel, x[:, None], yerr, min_size=ms, tol=1e-10, seed=42, exhaust=exhaust)
         ld1, ds1 = s.log_determinant, s.dot_solve(y)
@@ -61,11 +75,18 @@ for name, kernel, n, ms, exhaust in [
         good = abs(ld - ld1) <= 1e-10 * abs(ld1) and abs(ds - ds1) <= 1e-9 * abs(ds1) and np.linalg.norm(a - a1) <= 1e-9 * np.linalg.norm(a1)
         good = good and g_rel <= 1e-9 and d_rel <= 1e-9 and np.linalg.norm(ga - ga1) <= 1e-9 * np.linalg.norm(ga1)
         good = good and p_rel <= 1e-9 and pg_rel <= 1e-9 and var_bits
+        sym_rel = sym_ld_rel = None
+        if wz is not None:
+            wz1, wtz1, sld1 = s.apply_symmetric_factor(Z), s.apply_symmetric_factor(Z, transpose=True), s.symmetric_log_determinant
+            sym_rel = float(max(np.max(np.abs(wz - wz1)) / np.max(np.abs(wz1)), np.max(np.abs(wtz - wtz1)) / np.max(np.abs(wtz1))))
+            sym_ld_rel = abs(sld - sld1) / abs(sld1)
+            good = good and sym_rel <= 1e-10 and sym_ld_rel <= 1e-10 and sym_same
         ok = ok and good
         print(json.dumps({"case": name, "world": world, "logdet_sharded": ld, "logdet_single": ld1, "dot_sharded": ds, "dot_single": ds1,
                           "solve_relerr": float(np.linalg.norm(a - a1) / np.linalg.norm(a1)), "grad_relerr": g_rel,
                           "grad_diag_relerr": d_rel, "predict_relerr": p_rel, "grad_predict_relerr": pg_rel,
-                          "grad_predict_var_is_predict": var_bits, "ok": bool(good)}))
+                          "grad_predict_var_is_predict": var_bits, "sym_apply_relerr": sym_rel, "sym_logdet_relerr": sym_ld_rel,
+                          "sym_apply_same_on_every_rank": sym_same, "ok": bool(good)}))
 dist.barrier()
 if rank == 0:
     print("MGPU_CHECK", "PASS" if ok else "FAIL")
