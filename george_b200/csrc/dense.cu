@@ -28,6 +28,10 @@ int kmat_grad_contract_members(const DevProgram* dprogs, int np, const unsigned*
                                double ca, double cm, double* g_dev, int64_t gstride, double* diag_dev, int64_t dstride,
                                int members, DevBuf<double>& scratch, cudaStream_t s);
 int fill_identity_launch(double* A, int64_t n, cudaStream_t s);
+int loo_weights_launch(const double* alpha, const double* d, int64_t n, double* q, double* c, cudaStream_t s);
+int scale_rows_launch(double* X, int64_t n, int64_t ncols, int64_t ldx, const double* w, bool sqrt_w, cudaStream_t s);
+int slab_diag_launch(const double* W, int64_t ldw, int64_t j0, int64_t nc, double* d, cudaStream_t s);
+int loo_check_diag(const double* d, int64_t n);
 int fill_identity_members(double* A, int64_t n, int members, cudaStream_t s);
 int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
                              int64_t n2, double* out, int64_t ld, cudaStream_t s);
@@ -449,6 +453,17 @@ __global__ void square2_kernel(const double* __restrict__ yerr, double* __restri
 __global__ void add_into_kernel(const double* __restrict__ a, double* __restrict__ b, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     b[i] = a[i] + b[i];
+}
+// A += 1/2 (beta alpha^T + alpha beta^T) over the whole n x n A (bgp_dense_loo_terms: A = -K^-1 diag(c) K^-1 before).
+// Every rounding is explicit, so A stays exactly symmetric and A_ii = -M_ii + alpha_i beta_i.
+__global__ void loo_form_a_kernel(double* __restrict__ A, int64_t n, const double* __restrict__ alpha,
+                                  const double* __restrict__ beta) {
+  const int64_t total = n * n;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t j = t / n, i = t - j * n;
+    const double sym = __dadd_rn(__dmul_rn(beta[i], alpha[j]), __dmul_rn(alpha[i], beta[j]));
+    A[t] = __dadd_rn(A[t], __dmul_rn(0.5, sym));
+  }
 }
 // out (nr x n, row-major) = r (nr x n, row-major) @ U with U = L^T:  out[a][j] = sum_{i<=j} r[a][i] L[j][i]
 __global__ void apply_sqrt_kernel(const double* __restrict__ L, int64_t n, const double* __restrict__ r, int64_t nr,
@@ -910,6 +925,61 @@ int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r,
   // kernel term of gp.py:457-466 and diag(alpha alpha^T - K^-1) for the white-noise term of gp.py:452-456
   BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, alpha, 1.0, -1.0, dg,
                                     diag_out ? ddiag : nullptr, h->d_gscratch, s));
+  if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
+  if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  return BGP_OK;
+}
+
+int bgp_dense_loo_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* d_out,
+                        double* beta_out, double* g_out, double* diag_out) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (!h->has_inputs) { set_error("the factor was imported: the handle holds no kernel/coordinates"); return BGP_ERR_NOT_COMPUTED; }
+  const int64_t n = h->n;
+  const int np = h->n_params;
+  const bool grad = beta_out || g_out || diag_out;
+  if (grad && np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  cudaStream_t s = h->s;
+  BGP_TRY(h->d_rhs.reserve((size_t)n * 5 + 64, s));
+  double* alpha = h->d_rhs.p;
+  double* dg = h->d_rhs.p + n;  // np <= 64 entries
+  double* ddiag = h->d_rhs.p + n + 64;
+  double* dd = ddiag + n;
+  double* beta = dd + n;        // q = alpha / d, then K^-1 q in place
+  double* cw = beta + n;
+  // pass 1: alpha and d = diag(K^-1), K^-1 resident as in bgp_dense_grad_terms
+  BGP_CUDA(cudaMemcpyAsync(alpha, r, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+  BGP_TRY(dense_potrs_dev(h, alpha, 1, n));
+  BGP_TRY(h->d_inv.reserve((size_t)n * n, s));
+  BGP_TRY(fill_identity_launch(h->d_inv.p, n, s));
+  BGP_TRY(dense_potrs_dev(h, h->d_inv.p, n, n));
+  BGP_TRY(slab_diag_launch(h->d_inv.p, n, 0, n, dd, s));
+  std::vector<double> d_host((size_t)n);
+  if (alpha_out) BGP_CUDA(cudaMemcpyAsync(alpha_out, alpha, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaMemcpyAsync(d_host.data(), dd, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  if (d_out) memcpy(d_out, d_host.data(), sizeof(double) * n);
+  if (!grad) return BGP_OK;
+  BGP_TRY(loo_check_diag(d_host.data(), n));
+  // pass 2: beta = K^-1 (alpha / d); G = diag(sqrt(c)) K^-1 in place; A = -(G^T G) (lower, mirrored) on the tensor pipe,
+  // plus 1/2 (beta alpha^T + alpha beta^T); then the contraction of bgp_kmat_gradient_contract (A given whole)
+  BGP_TRY(loo_weights_launch(alpha, dd, n, beta, cw, s));
+  BGP_TRY(dense_potrs_dev(h, beta, 1, n));
+  BGP_TRY(scale_rows_launch(h->d_inv.p, n, n, n, cw, true, s));
+  DevBuf<double> dA, slices;
+  DevBuf<GemmDesc> descs;
+  BGP_TRY(dA.alloc((size_t)n * n, s));
+  BGP_CUDA(cudaMemsetAsync(dA.p, 0, sizeof(double) * n * n, s));
+  BGP_TRY(predict_gemm_sub(h->d_inv.p, n, h->d_inv.p, n, n, n, n, true, dA.p, n, slices, descs, s));
+  slices.release();
+  loo_form_a_kernel<<<(unsigned)std::min<int64_t>((n * n + 255) / 256, 16 * (int64_t)num_sms()), 256, 0, s>>>(
+      dA.p, n, alpha, beta);
+  BGP_LAUNCH_CHECK();
+  BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
+  if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
+  BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, dA.p, n, nullptr, 0.0, 1.0, dg,
+                                    diag_out ? ddiag : nullptr, h->d_gscratch, s));
+  if (beta_out) BGP_CUDA(cudaMemcpyAsync(beta_out, beta, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
   if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
   if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));

@@ -29,11 +29,15 @@ int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const uns
                               int64_t n, const double* M, int64_t ldm, const double* alpha, double ca, double cm,
                               double* g_dev, double* diag_dev, DevBuf<double>& scratch, cudaStream_t s);
 int fill_identity_launch(double* A, int64_t n, cudaStream_t s);
+int loo_weights_launch(const double* alpha, const double* d, int64_t n, double* q, double* c, cudaStream_t s);
+int scale_rows_launch(double* X, int64_t n, int64_t ncols, int64_t ldx, const double* w, bool sqrt_w, cudaStream_t s);
+int slab_diag_launch(const double* W, int64_t ldw, int64_t j0, int64_t nc, double* d, cudaStream_t s);
+int loo_check_diag(const double* d, int64_t n);
 int64_t grad_slab_partial_size(int64_t n, int64_t c, int np);
 int64_t grad_slab_tile_size(int64_t n, int np);
 int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigned* which_dev, const double* x, int64_t n,
-                          const double* W, int64_t j0, int64_t nc, int64_t jlo, int64_t jhi, const double* alpha,
-                          double* partial, double* tile_part, double* diag_dev, cudaStream_t s);
+                          const double* W, int64_t j0, int64_t nc, int64_t jlo, int64_t jhi, const double* u,
+                          const double* v, double* partial, double* tile_part, double* diag_dev, cudaStream_t s);
 int kmat_grad_slab_finish(int np, int64_t jlo, int64_t jhi, const double* tile_part, double* g_dev, cudaStream_t s);
 int kmat_symmetric_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x, int64_t n,
                                const double* diag_add, double* out, int64_t ld, cudaStream_t s);
@@ -1402,7 +1406,7 @@ static int grad_stream_own_columns(bgp_hodlr* h, int np, const double* alpha, in
     BGP_TRY(hodlr_solve_dev(h, W, nc, n, s, 0, j0));
     if (prof) BGP_CUDA(cudaEventRecord(h->ev[5], s));
     BGP_TRY(kmat_grad_slab_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, W, j0, nc, jlo, jhi, alpha,
-                                  partial, tile_part, ddiag, s));
+                                  alpha, partial, tile_part, ddiag, s));
     if (prof) {
       BGP_CUDA(cudaEventRecord(h->ev[7], s));
       BGP_CUDA(cudaEventSynchronize(h->ev[7]));
@@ -1487,6 +1491,80 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
   BGP_CUDA(cudaStreamSynchronize(s));
   h->grad_t[0] = t_solve;
   h->grad_t[1] = t_contract;
+  return BGP_OK;
+}
+
+// Leave-one-out terms of the HODLR matrix (include/bgp.h), always streamed in the slabs of grad_stream_own_columns:
+// pass 1 takes d_j = (K^-1)_jj from each restricted slab solve S = K^-1 E_J; pass 2 (a gradient asked for) solves
+// beta = K^-1 (alpha / d), and per slab recomputes S, scales its rows by c and solves T = K^-1 diag(c) S unrestricted
+// (diag(c) S is dense), then contracts beta_i alpha_j - T_ij over i in [0, n), j in J (kmat_grad_slab_launch with
+// u = beta, v = alpha) and writes diagA_j = alpha_j beta_j - T_jj.
+int bgp_hodlr_loo_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* d_out,
+                        double* beta_out, double* g_out, double* diag_out) {
+  if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
+  if (host_exchange(h) || h->opts.shard_count > 1) {
+    set_error("loo_terms is not available on a sharded factorisation");
+    return BGP_ERR_INVALID;
+  }
+  const int64_t n = h->n;
+  const int np = h->prog.n_params_total;
+  if (!rows_ordered(h)) { set_error("internal: HODLR rows are not ordered by level"); return BGP_ERR_CUDA; }
+  const bool grad = beta_out || g_out || diag_out;
+  if (grad && np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  cudaStream_t s = h->sA;
+  bool forced = false;
+  const int64_t c = grad_slab_cols(n, &forced);
+  BGP_TRY(h->d_rhs.reserve((size_t)n * 5 + 64, s));
+  double* alpha = h->d_rhs.p;
+  double* dg = h->d_rhs.p + n;
+  double* ddiag = h->d_rhs.p + n + 64;
+  double* dd = ddiag + n;
+  double* beta = dd + n;  // q = alpha / d, then K^-1 q in place
+  double* cw = beta + n;
+  BGP_CUDA(cudaMemcpyAsync(alpha, r, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+  BGP_TRY(hodlr_solve_dev(h, alpha, 1, n, s, 0));
+  BGP_TRY(h->d_inv.reserve((size_t)n * c, s));
+  double* W = h->d_inv.p;
+  // S = K^-1 E_J for the slab J = [j0, j0 + nc), by the row-restricted solve
+  auto slab_solve = [&](int64_t j0, int64_t nc) -> int {
+    BGP_CUDA(cudaMemsetAsync(W, 0, sizeof(double) * n * nc, s));
+    eye_slab_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, n, j0, nc, 0, n);
+    BGP_LAUNCH_CHECK();
+    return hodlr_solve_dev(h, W, nc, n, s, 0, j0);
+  };
+  for (int64_t j0 = 0; j0 < n; j0 += c) {
+    const int64_t nc = std::min(c, n - j0);
+    BGP_TRY(slab_solve(j0, nc));
+    BGP_TRY(slab_diag_launch(W, n, j0, nc, dd, s));
+  }
+  std::vector<double> d_host((size_t)n);
+  if (alpha_out) BGP_CUDA(cudaMemcpyAsync(alpha_out, alpha, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaMemcpyAsync(d_host.data(), dd, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  if (d_out) memcpy(d_out, d_host.data(), sizeof(double) * n);
+  if (!grad) return BGP_OK;
+  BGP_TRY(loo_check_diag(d_host.data(), n));
+  BGP_TRY(loo_weights_launch(alpha, dd, n, beta, cw, s));
+  BGP_TRY(hodlr_solve_dev(h, beta, 1, n, s, 0));
+  const int64_t tsize = grad_slab_tile_size(n, np), psize = grad_slab_partial_size(n, c, np);
+  BGP_TRY(h->d_gscratch.reserve((size_t)(tsize + psize), s));
+  double* tile_part = h->d_gscratch.p;
+  double* partial = h->d_gscratch.p + tsize;
+  BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
+  if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
+  for (int64_t j0 = 0; j0 < n; j0 += c) {
+    const int64_t nc = std::min(c, n - j0);
+    BGP_TRY(slab_solve(j0, nc));
+    BGP_TRY(scale_rows_launch(W, n, nc, n, cw, false, s));
+    BGP_TRY(hodlr_solve_dev(h, W, nc, n, s, 0));
+    BGP_TRY(kmat_grad_slab_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, W, j0, nc, 0, n, beta, alpha,
+                                  partial, tile_part, diag_out ? ddiag : nullptr, s));
+  }
+  BGP_TRY(kmat_grad_slab_finish(np, 0, n, tile_part, dg, s));
+  if (beta_out) BGP_CUDA(cudaMemcpyAsync(beta_out, beta, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
+  if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;
 }
 

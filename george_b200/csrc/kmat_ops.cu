@@ -19,6 +19,7 @@
 // expensive ones.  Partial sums are written per CTA and reduced by a second tiny kernel in a fixed order, so results
 // are run-to-run deterministic (no atomics).
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <vector>
 
@@ -573,7 +574,10 @@ int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const uns
 // ---------------------------------------------------------------------------------------------------------------
 // Slab gradient contraction (bgp_hodlr_grad_terms at large n, which never holds all of K^-1): for a slab
 // W = K^-1 E_J of columns J = [j0, j0 + nc) (n x nc, column-major, W[(j - j0) n + i] = (K^-1)_ij),
-//     g_p += sum_{i, j in J} (alpha_i alpha_j - W_ij) dK_ij/dtheta_p.
+//     g_p += sum_{i, j in J} (u_i v_j - W_ij) dK_ij/dtheta_p,
+// u = v = alpha for grad_log_likelihood.  bgp_hodlr_loo_terms passes u = beta, v = alpha and W = K^-1 diag(c) K^-1 E_J:
+// summed over every ordered pair against a symmetric dK, u_i v_j gives what the symmetrised 1/2 (u_i v_j + v_i u_j)
+// gives.
 // Every ordered pair is evaluated (george's einsum over all (i, j)): the symmetric weighting of
 // kmat_grad_contract_kernel would need rows of K^-1 from two slabs.  One thread per row i; the coordinates and alpha of
 // a 32-column j-tile are staged in shared memory and W is read coalesced along i.  CTA (tile t, split s) covers rows
@@ -600,7 +604,8 @@ __global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevPro
                                                                     const double* __restrict__ x, int64_t n,
                                                                     const double* __restrict__ W, int64_t j0,
                                                                     int64_t nc, int64_t jlo, int64_t jhi,
-                                                                    const double* __restrict__ alpha, int stage_x,
+                                                                    const double* __restrict__ u,
+                                                                    const double* __restrict__ v, int stage_x,
                                                                     double* __restrict__ partial) {
   extern __shared__ double sxj[];  // GS_TJ x nd coordinates of the tile's columns (stage_x)
   __shared__ DevProgram P;
@@ -613,11 +618,11 @@ __global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevPro
   const int64_t r0 = (int64_t)blockIdx.y * GS_ROWS, r1 = min(n, r0 + GS_ROWS);
   stage_program(&P, gprog);
   for (int q = threadIdx.x; q < np; q += blockDim.x) sw[q] = which[q];
-  // a column outside the window gets weight 0 (alpha_j staged as 0, and its W column is zero: the identity is placed in
+  // a column outside the window gets weight 0 (v_j staged as 0, and its W column is zero: the identity is placed in
   // the window only), so it adds exactly nothing, and the loop below carries no window bounds
   if (threadIdx.x < nj) {
     const int64_t j = jt + threadIdx.x;
-    saj[threadIdx.x] = (j >= jlo && j < jhi) ? alpha[j] : 0.0;
+    saj[threadIdx.x] = (j >= jlo && j < jhi) ? v[j] : 0.0;
   }
   if (stage_x)
     for (int t = threadIdx.x; t < nj * nd; t += GS_THREADS) sxj[t] = x[jt * nd + t];
@@ -627,7 +632,7 @@ __global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevPro
 #pragma unroll
   for (int q = 0; q < NPMAX; ++q) acc[q] = 0.0;
   for (int64_t i = r0 + threadIdx.x; i < r1; i += GS_THREADS) {
-    const double ai = alpha[i];
+    const double ai = u[i];
     const double* xi = x + i * nd;
     for (int c = 0; c < nj; ++c) {
       const double w = ai * saj[c] - Wt[(int64_t)c * n + i];
@@ -659,13 +664,14 @@ __global__ void grad_slab_reduce_kernel(const double* __restrict__ partial, int6
   }
 }
 
-// diag[j] = alpha_j^2 - W_jj for j in [j0, j0 + nc) inside the window [jlo, jhi) (no other entry is written): the
-// square and the difference rounded separately (no contraction into an FMA), as alpha**2 - diag(K^-1) is on the host
+// diag[j] = u_j v_j - W_jj for j in [j0, j0 + nc) inside the window [jlo, jhi) (no other entry is written): the
+// product and the difference rounded separately (no contraction into an FMA), as alpha**2 - diag(K^-1) is on the host
 __global__ void grad_slab_diag_kernel(const double* __restrict__ W, int64_t n, int64_t j0, int64_t nc, int64_t jlo,
-                                      int64_t jhi, const double* __restrict__ alpha, double* __restrict__ diag) {
+                                      int64_t jhi, const double* __restrict__ u, const double* __restrict__ v,
+                                      double* __restrict__ diag) {
   for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nc; k += (int64_t)gridDim.x * blockDim.x) {
     const int64_t j = j0 + k;
-    if (j >= jlo && j < jhi) diag[j] = __dsub_rn(__dmul_rn(alpha[j], alpha[j]), W[k * n + j]);
+    if (j >= jlo && j < jhi) diag[j] = __dsub_rn(__dmul_rn(u[j], v[j]), W[k * n + j]);
   }
 }
 
@@ -677,11 +683,12 @@ int64_t grad_slab_partial_size(int64_t n, int64_t c, int np) {
 int64_t grad_slab_tile_size(int64_t n, int np) { return ((n + GS_TJ - 1) / GS_TJ) * std::max(np, 1); }
 
 // One slab (j0 a multiple of 32) restricted to the columns [jlo, jhi): its tiles' partials into
-// tile_part + (j0 / 32) * np, and diag[j] for j in [j0, j0 + nc) and in the window when diag_dev is set.
+// tile_part + (j0 / 32) * np, and diag[j] for j in [j0, j0 + nc) and in the window when diag_dev is set.  Passing
+// u = v = alpha is the contraction of grad_log_likelihood, bit for bit.
 // partial: grad_slab_partial_size(n, nc, np) doubles.
 int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigned* which_dev, const double* x, int64_t n,
-                          const double* W, int64_t j0, int64_t nc, int64_t jlo, int64_t jhi, const double* alpha,
-                          double* partial, double* tile_part, double* diag_dev, cudaStream_t s) {
+                          const double* W, int64_t j0, int64_t nc, int64_t jlo, int64_t jhi, const double* u,
+                          const double* v, double* partial, double* tile_part, double* diag_dev, cudaStream_t s) {
   if (nc <= 0) return BGP_OK;
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
   if (j0 % GS_TJ) { set_error("internal: slab start %lld is not a multiple of %d", (long long)j0, GS_TJ); return BGP_ERR_INVALID; }
@@ -693,10 +700,10 @@ int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigne
     const size_t smem = stage_x ? sbytes : 0;
     const dim3 grid((unsigned)ntile, (unsigned)nsplit);
     if (np <= 8)
-      kmat_grad_slab_kernel<8><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, jlo, jhi, alpha,
+      kmat_grad_slab_kernel<8><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, jlo, jhi, u, v,
                                                                stage_x, partial);
     else
-      kmat_grad_slab_kernel<64><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, jlo, jhi, alpha,
+      kmat_grad_slab_kernel<64><<<grid, GS_THREADS, smem, s>>>(dprog, which_dev, x, n, W, j0, nc, jlo, jhi, u, v,
                                                                 stage_x, partial);
     BGP_LAUNCH_CHECK();
     const int64_t total = ntile * np;
@@ -706,7 +713,7 @@ int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigne
   }
   if (diag_dev) {
     grad_slab_diag_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, n, j0, nc, jlo, jhi,
-                                                                                              alpha, diag_dev);
+                                                                                              u, v, diag_dev);
     BGP_LAUNCH_CHECK();
   }
   return BGP_OK;
@@ -737,6 +744,68 @@ int fill_identity_members(double* A, int64_t n, int members, cudaStream_t s) {
   return BGP_OK;
 }
 int fill_identity_launch(double* A, int64_t n, cudaStream_t s) { return fill_identity_members(A, n, 1, s); }
+
+// ---------------------------------------------------------------------------------------------------------------
+// Leave-one-out cross-validation (bgp_dense_loo_terms, bgp_hodlr_loo_terms; Rasmussen & Williams, GPML eqs. 5.10-5.13):
+// with alpha = K^-1 r and d = diag(K^-1), the gradient of L_loo = sum_i [1/2 log d_i - alpha_i^2 / (2 d_i)] + const
+// contracts A = 1/2 (beta alpha^T + alpha beta^T) - K^-1 diag(c) K^-1 with dK, where
+//     q_i = alpha_i / d_i,   beta = K^-1 q,   c_i = (1 + alpha_i q_i) / (2 d_i).
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void loo_weights_kernel(const double* __restrict__ alpha, const double* __restrict__ d, int64_t n,
+                                   double* __restrict__ q, double* __restrict__ c) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const double qi = alpha[i] / d[i];
+    q[i] = qi;
+    c[i] = (1.0 + alpha[i] * qi) / (2.0 * d[i]);
+  }
+}
+int loo_weights_launch(const double* alpha, const double* d, int64_t n, double* q, double* c, cudaStream_t s) {
+  loo_weights_kernel<<<(unsigned)std::min<int64_t>((n + 255) / 256, 1184), 256, 0, s>>>(alpha, d, n, q, c);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
+// X (n x ncols, column-major ldx): row i scaled by w_i, or by sqrt(w_i) with `sqrt_w`
+__global__ void scale_rows_kernel(double* __restrict__ X, int64_t n, int64_t ncols, int64_t ldx,
+                                  const double* __restrict__ w, int sqrt_w) {
+  const int64_t total = n * ncols;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t j = t / n, i = t - j * n;
+    X[j * ldx + i] *= sqrt_w ? sqrt(w[i]) : w[i];
+  }
+}
+int scale_rows_launch(double* X, int64_t n, int64_t ncols, int64_t ldx, const double* w, bool sqrt_w, cudaStream_t s) {
+  const int64_t total = n * ncols;
+  if (total <= 0) return BGP_OK;
+  scale_rows_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 16 * (int64_t)num_sms()), 256, 0, s>>>(
+      X, n, ncols, ldx, w, sqrt_w ? 1 : 0);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
+// The gradient needs every d_j > 0 (c and sqrt(c) are formed from it); a loose-tolerance HODLR matrix, or rounding of
+// a nearly singular K, can break that.  BGP_ERR_INVALID names the first offending point.
+int loo_check_diag(const double* d, int64_t n) {
+  for (int64_t j = 0; j < n; ++j)
+    if (!(d[j] > 0.0) || !std::isfinite(d[j])) {
+      set_error("leave-one-out: diag(K^-1) at point %lld is %g, not a finite positive number", (long long)j, d[j]);
+      return BGP_ERR_INVALID;
+    }
+  return BGP_OK;
+}
+
+// d[j0 + k] = W[k * ldw + j0 + k] for k < nc: the diagonal entries of the slab W = K^-1 E_J, J = [j0, j0 + nc)
+__global__ void slab_diag_kernel(const double* __restrict__ W, int64_t ldw, int64_t j0, int64_t nc,
+                                 double* __restrict__ d) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nc; k += (int64_t)gridDim.x * blockDim.x)
+    d[j0 + k] = W[k * ldw + j0 + k];
+}
+int slab_diag_launch(const double* W, int64_t ldw, int64_t j0, int64_t nc, double* d, cudaStream_t s) {
+  if (nc <= 0) return BGP_OK;
+  slab_diag_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, ldw, j0, nc, d);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // Predictive variance / covariance (GP.predict with return_var / return_cov; bgp_dense_predict, bgp_hodlr_predict).

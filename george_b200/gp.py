@@ -601,6 +601,121 @@ class GP(ModelSet):
                 grad[pos:pos + n_k] = 0.5 * self.kernel.kernel.gradient_contract(mask.astype(np.uint32), self._x, A)[mask]
         return grad
 
+    # -- leave-one-out cross-validation (Rasmussen & Williams, GPML §5.4.2, eqs. 5.10-5.13) ---------------------------
+    def loo_predict(self, y):
+        """The leave-one-out predictive of each observation at the computed coordinates: ``(mu, var)``, each of shape
+        ``(N,)``, the mean and variance of ``y_i`` given all the other points, from one factorisation:
+        ``mu_i = y_i - alpha_i / d_i`` and ``var_i = 1 / d_i`` with ``alpha = K^-1 (y - mean)`` and ``d = diag(K^-1)``.
+        ``var`` includes the white noise and ``yerr``.  ``(y - mu) / sqrt(var)`` are the standardised LOO residuals.
+
+        The HODLR solvers give the LOO quantities of their HODLR matrix ``K~``, not of the dense ``K``."""
+        self.recompute(quiet=False)
+        y = np.asarray(self._check_dimensions(y), dtype=np.float64)
+        alpha, d = self._loo_terms(self._residual_of(y), None)
+        return y - alpha / d, 1.0 / d
+
+    def loo_log_likelihood(self, y, quiet=False):
+        """The leave-one-out log predictive probability ``sum_i log p(y_i | y_-i)`` (GPML eq. 5.11), a model-selection
+        score that is less sensitive to a mis-specified model than :func:`log_likelihood`:
+        ``sum_i [-1/2 log(2 pi) + 1/2 log d_i - alpha_i^2 / (2 d_i)]`` with ``alpha`` and ``d`` as in
+        :func:`loo_predict`.  Semantics follow :func:`log_likelihood`: ``-inf`` on a factorisation or mean-function
+        failure when ``quiet``, and for a non-finite result (including a ``d_i`` that is not finite and positive, which
+        a loose-tolerance HODLR matrix can give).
+
+        The HODLR solvers give the LOO quantities of their HODLR matrix ``K~``, not of the dense ``K``."""
+        if not self.recompute(quiet=quiet):
+            return -np.inf
+        try:
+            r = self._residual_of(y)
+        except ValueError as exc:
+            if quiet and "mean function" in str(exc):
+                return -np.inf
+            raise
+        alpha, d = self._loo_terms(r, None)
+        return self._loo_value(alpha, d)
+
+    def grad_loo_log_likelihood(self, y, quiet=False, return_value=False):
+        """Gradient of :func:`loo_log_likelihood` w.r.t. the active parameter vector, in :func:`grad_log_likelihood`'s
+        layout (mean, white noise, kernel; frozen parameters left out), from one factorisation (GPML eqs. 5.12-5.13):
+        with ``beta = K^-1 (alpha / d)``, ``c = (1 + alpha**2 / d) / (2 d)`` and
+        ``A = 1/2 (beta alpha^T + alpha beta^T) - K^-1 diag(c) K^-1``, the kernel part is ``sum_ij A_ij dK_ij/dtheta``,
+        the white-noise part ``sum_i A_ii exp(wn_i) dwn_i/dtheta`` and the mean part ``dmu/dtheta . beta``.  Use it as
+        ``scipy.optimize.minimize(..., jac=True)``'s objective with ``return_value``, which returns
+        ``(loo_log_likelihood, grad)`` from the same pass, the value bit for bit what :func:`loo_log_likelihood` returns.
+
+        A ``d_i`` that is not finite and positive raises ``ValueError`` naming the point.  With ``quiet`` any failure
+        that :func:`grad_log_likelihood` absorbs gives a zero gradient (and ``-inf`` for the value).
+
+        Solvers with a ``loo_terms`` hook (``BasicSolver``, ``HODLRSolver``) run on the device and never form K^-1 on
+        the host; any other solver forms ``K^-1`` with ``apply_inverse`` on the host.  The HODLR solvers give the LOO
+        quantities of their HODLR matrix ``K~``, not of the dense ``K``."""
+        nothing = np.zeros(len(self), dtype=np.float64)
+        fail = (-np.inf, nothing) if return_value else nothing
+        if not self.recompute(quiet=quiet):
+            return fail
+        n_wn, n_k, n_mean = len(self.white_noise), len(self.kernel), len(self.mean)
+        mask = self.kernel.unfrozen_mask
+        try:
+            r = self._residual_of(y)
+            alpha, d, beta, gk, diagA = self._loo_terms(r, mask.astype(np.uint32))
+            dmu = self._call_mean_gradient(self._x) if n_mean else None
+        except ValueError:
+            if quiet:
+                return fail
+            raise
+
+        grad = np.empty(len(self))
+        pos = 0
+        if n_mean:
+            grad[pos:pos + n_mean] = np.dot(dmu, beta)
+            pos += n_mean
+        if n_wn:
+            wn = self._call_white_noise(self._x)
+            dwn = self._call_white_noise_gradient(self._x)
+            grad[pos:pos + n_wn] = np.sum((np.exp(wn) * diagA)[None, :] * dwn, axis=1)
+            pos += n_wn
+        if n_k:
+            grad[pos:pos + n_k] = gk[mask]
+        return (self._loo_value(alpha, d), grad) if return_value else grad
+
+    @staticmethod
+    def _loo_value(alpha, d):
+        """``sum_i [-1/2 log(2 pi) + 1/2 log d_i - alpha_i^2 / (2 d_i)]``; ``-inf`` unless every ``d_i`` is finite and
+        positive and the sum is finite."""
+        if not np.all(np.isfinite(d) & (d > 0)):
+            return -np.inf
+        v = float(np.sum(-0.5 * np.log(2 * np.pi) + 0.5 * np.log(d) - alpha ** 2 / (2 * d)))
+        return v if np.isfinite(v) else -np.inf
+
+    def _loo_terms(self, r, which):
+        """``(alpha, d)``, or with ``which`` (0/1 over all kernel parameters) ``(alpha, d, beta, g, diagA)``, as
+        ``BasicSolver.loo_terms`` returns them: from the solver's ``loo_terms`` hook, or on the host from
+        ``K^-1 = solver.apply_inverse(eye(N))`` and ``KernelInterface.gradient_contract`` (``TrivialSolver``, plug-in
+        solvers and a dense solver restored from a pickle)."""
+        hook = getattr(self.solver, "loo_terms", None)
+        if hook is not None:
+            terms = hook(r, which)
+            if terms is not None:
+                return terms
+        n = len(r)
+        kinv = np.asarray(self.solver.apply_inverse(np.eye(n), in_place=True), dtype=np.float64).reshape(n, n)
+        alpha = kinv.dot(r)
+        d = np.diag(kinv).copy()
+        if which is None:
+            return alpha, d
+        bad = np.flatnonzero(~(np.isfinite(d) & (d > 0)))
+        if bad.size:
+            raise ValueError("leave-one-out: diag(K^-1) at point {0} is {1:g}, not a finite positive number".format(
+                bad[0], d[bad[0]]))
+        q = alpha / d
+        beta = kinv.dot(q)
+        c = (1.0 + alpha * q) / (2.0 * d)
+        A = 0.5 * (np.outer(beta, alpha) + np.outer(alpha, beta)) - kinv.dot(c[:, None] * kinv)
+        g = np.zeros(len(which), dtype=np.float64)
+        if len(which):
+            g = self.kernel.kernel.gradient_contract(which, self._x, A)
+        return alpha, d, beta, g, np.diag(A).copy()
+
     def batch_grad_log_likelihood(self, vectors, y, quiet=False, return_log_likelihood=False):
         """:func:`grad_log_likelihood` at many parameter vectors: row ``b`` of the ``(B, len(gp))`` result is bit for
         bit what ``gp.set_parameter_vector(vectors[b]); gp.grad_log_likelihood(y, quiet=quiet)`` returns on the

@@ -178,6 +178,12 @@ class ShardedHODLRSolver(object):
                                             _lib.ptr(g), _lib.ptr(diag)))
         return alpha, g[:which.size], diag
 
+    def loo_terms(self, r, which=None):
+        """Leave-one-out cross-validation is not available on a sharded factorisation: its gradient would need a
+        collective full solve per slab.  Raises ``NotImplementedError`` on every rank before any collective, so no rank
+        is left waiting."""
+        raise NotImplementedError("leave-one-out cross-validation is not implemented for the ShardedHODLRSolver")
+
     def predictive(self, kernel, xs, what):
         """``BasicSolver.predictive`` on the sharded factorisation: the variance (``what="var"``, ``(ns,)``) or
         covariance (``"cov"``, ``(ns, ns)``) of ``GP.predict``.  Collective; ``xs`` replicated on every rank, and every

@@ -230,6 +230,38 @@ class BasicSolver(object):
     def _grad_terms_call(self, which, r, alpha, g, diag):
         return self._handle.lib.bgp_dense_grad_terms(self._handle.ptr, which, r, alpha, g, diag)
 
+    def loo_terms(self, r, which=None):
+        """The leave-one-out cross-validation terms of ``GP.loo_*`` on the device from the stored factor
+        (``include/bgp.h: bgp_dense_loo_terms``): ``(alpha, d)`` with ``alpha = K^-1 r`` and ``d = diag(K^-1)``; with
+        ``which`` (a 0/1 mask over ALL kernel parameters) also ``beta = K^-1 (alpha / d)``, ``g[p] = sum_ij A_ij
+        dK_ij/dtheta_p`` (zeros where ``which`` is 0) and ``diagA = diag(A)``, where ``A = 1/2 (beta alpha^T + alpha
+        beta^T) - K^-1 diag(c) K^-1`` and ``c = (1 + alpha**2 / d) / (2 d)``.  A gradient with a ``d_i`` that is not
+        finite and positive raises ``ValueError`` naming the point.  Returns ``None`` for a solver restored from a pickle,
+        as :func:`grad_terms` does."""
+        self._require()
+        if not getattr(self, "_has_inputs", True):
+            return None
+        r = np.ascontiguousarray(r, dtype=np.float64)
+        if r.shape != (self._n,):
+            raise ValueError("dimension mismatch")
+        _check_finite(r)
+        n = self._n
+        alpha = np.empty(n, dtype=np.float64)
+        d = np.empty(n, dtype=np.float64)
+        if which is None:
+            _lib.check(self._loo_terms_call(None, _lib.ptr(r), _lib.ptr(alpha), _lib.ptr(d), None, None, None))
+            return alpha, d
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        beta = np.empty(n, dtype=np.float64)
+        g = np.zeros(max(which.size, 1), dtype=np.float64)
+        diag = np.empty(n, dtype=np.float64)
+        _lib.check(self._loo_terms_call(_lib.ptr(which), _lib.ptr(r), _lib.ptr(alpha), _lib.ptr(d), _lib.ptr(beta),
+                                        _lib.ptr(g), _lib.ptr(diag)))
+        return alpha, d, beta, g[:which.size], diag
+
+    def _loo_terms_call(self, which, r, alpha, d, beta, g, diag):
+        return self._handle.lib.bgp_dense_loo_terms(self._handle.ptr, which, r, alpha, d, beta, g, diag)
+
     def predictive(self, kernel, xs, what):
         """The predictive variance (``what="var"``, shape ``(ns,)``) or covariance (``what="cov"``, ``(ns, ns)``) of
         ``GP.predict`` (gp.py:534-545) at ``xs`` (``(ns, ndim)``), computed on the device from the stored factor with

@@ -65,6 +65,9 @@ class HODLRSolver(BasicSolver):
     def _grad_terms_call(self, which, r, alpha, g, diag):
         return self.solver._lib.bgp_hodlr_grad_terms(self.solver._ptr, which, r, alpha, g, diag)
 
+    def _loo_terms_call(self, which, r, alpha, d, beta, g, diag):
+        return self.solver._lib.bgp_hodlr_loo_terms(self.solver._ptr, which, r, alpha, d, beta, g, diag)
+
     def predictive(self, kernel, xs, what):
         """``BasicSolver.predictive`` on the HODLR factorisation (``include/bgp.h: bgp_hodlr_predict``); ``None`` on a
         sharded factorisation."""

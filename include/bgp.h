@@ -71,8 +71,8 @@ uint64_t bgp_launch_count(void);
  *   - an expression depth of at most 8: the operand stack of the postfix program, e.g. 8 leaves nested to the right,
  *     k1 + (k2 + (... + k8)), while any number of left-nested operators keep it at 2;
  *   - hyper-parameter gradients (bgp_kmat_gradient_*, bgp_kmat_gradient_contract, bgp_dense_grad_terms,
- *     bgp_dense_batch_grad_terms, bgp_hodlr_grad_terms) take at most 64 hyper-parameters, checked before anything
- *     is solved;
+ *     bgp_dense_batch_grad_terms, bgp_hodlr_grad_terms, bgp_*_loo_terms) take at most 64 hyper-parameters, checked
+ *     before anything is solved;
  *   - input-coordinate gradients (bgp_kmat_x1/x2_gradient_general) take at most BGP_MAX_DIM = 8 input dimensions;
  *   - the HODLR solver takes at most 32 input dimensions.
  * The kernel-matrix builds, the matvec, the dense solver, the batched paths and predictions have no input-dimension
@@ -227,6 +227,24 @@ int bgp_dense_import_factor(bgp_dense_t* h, const double* factor, int64_t n, dou
  * bgp_dense_import_factor (it holds no kernel / coordinates). */
 int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
                          double* diag_out);
+/* Leave-one-out cross-validation terms (GP.loo_predict, GP.loo_log_likelihood, GP.grad_loo_log_likelihood; Rasmussen &
+ * Williams, GPML eqs. 5.10-5.13), computed on the device from the stored factor, kernel and coordinates:
+ *   alpha_out = K^-1 r (n),  d_out = diag(K^-1) (n)                                        (pass 1)
+ *   beta_out  = K^-1 (alpha / d) (n),
+ *   g_out[p]  = sum_ij A_ij dK_ij/dtheta_p (n_params; 0 where which[p] = 0; no factor 1/2: it is inside A),
+ *   diag_out  = diag(A) = alpha o beta - diag(K^-1 diag(c) K^-1) (n, for the white-noise term)   (pass 2)
+ * with c_i = (1 + alpha_i^2 / d_i) / (2 d_i) and A = 1/2 (beta alpha^T + alpha beta^T) - K^-1 diag(c) K^-1.  The LOO
+ * predictive of y_i is mean y_i - alpha_i / d_i and variance 1 / d_i.  Any output pointer may be NULL; when beta_out,
+ * g_out and diag_out are all NULL only pass 1 runs.  K^-1 is formed whole and K^-1 diag(c) K^-1 = G^T G, G =
+ * diag(sqrt(c)) K^-1, runs on the FP64 tensor pipe.  Device workspace (doubles): n^2 (K^-1, kept by the handle as
+ * bgp_dense_grad_terms keeps it) in pass 1; pass 2 adds n^2 for A and the product's split-K slices, n^2 each: one slice
+ * from n = 2176 (3 n^2 in all: about 26 GB at n = 32768), at most four below (6 n^2), plus ceil(n / 32)^2 P for the
+ * contraction and 5 n + 64.  Errors: BGP_ERR_NOT_COMPUTED before compute and on a handle restored by
+ * bgp_dense_import_factor; BGP_ERR_INVALID, when pass 2 is asked for, for more than 64 kernel parameters (before
+ * anything is launched) and for a d_j that is not finite and positive (the message names j; alpha_out and d_out are
+ * written, pass 2 does not run). */
+int bgp_dense_loo_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* d_out,
+                        double* beta_out, double* g_out, double* diag_out);
 /* timing of the last compute: [0]=kernel-matrix build ms, [1]=potrf ms (device events). */
 int bgp_dense_last_timing(const bgp_dense_t* h, double* ms2);
 
@@ -502,6 +520,17 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
  * than 64 kernel parameters and for a NULL alpha_dev (both before anything is launched). */
 int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const double* alpha_dev, double* g_part_out,
                                    double* diag_dev);
+/* The HODLR counterpart of bgp_dense_loo_terms: the same outputs and errors, for the HODLR matrix K~ (not the dense K).
+ * Always streamed, at every n, in the column slabs of bgp_hodlr_grad_terms (c columns, BGP_GRAD_CHUNK included):
+ *   pass 1: per slab S = K~^-1 E_J by the row-restricted solve, d_j = S_jj for j in J;
+ *   pass 2: beta by one solve, then per slab S again, its rows scaled by c, T = K~^-1 diag(c) S by a full c-column
+ *           solve, and the contraction of beta_i alpha_j - T_ij over i in [0, n), j in J (every ordered pair, so this is
+ *           the symmetrised A's sum) with diagA_j = alpha_j beta_j - T_jj.
+ * Device workspace (doubles): n c + ceil(n / 32) P + ceil(n / 1024) (c / 32) P, plus 5 n + 64.  The sum order depends
+ * only on n; where the solve has no atomics two identical calls return the same bits.  BGP_ERR_INVALID also on a
+ * sharded factorisation (host-exchange shard or not), before anything is launched. */
+int bgp_hodlr_loo_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* d_out,
+                        double* beta_out, double* g_out, double* diag_out);
 /* The HODLR counterpart of bgp_dense_predict (see there for the outputs, workspace and errors).
  * On a sharded factorisation with a matching communicator (see the multi-GPU block below) the call is COLLECTIVE, with
  * spec, xs and ns replicated: per test-point chunk each shard builds its own rows J of K(x, x*) into an N x c chunk, the
