@@ -2,21 +2,24 @@
 // Replaces get_exact_matrix + Eigen LDLT (hodlr.h:122-133, 225-227, 87-89).  (A 32-column blocked leaf SOLVE was tried
 // and measured slower than leaf_solve_kernel for the 1..160 right-hand sides of this path, so it was dropped.)
 //
-// The leaf is factorised in 32-column panels, left to right.  A panel (rows k0.., columns k0..k0+31) is built in shared
-// memory, brought up to date there and written to global memory once, final:
-//   (1) build: the panel's kernel entries on and below the diagonal, evaluated by the whole CTA, LF_BUILD_ILP
-//       independent entries per thread in flight (the 1-D shapes through ShapeEval, the same arithmetic as the
-//       interpreter);
-//   (2) update: panel -= L(k0:, 0:k0) D L(k0:k0+32, 0:k0)^T on the tensor pipe (mma.sync.m8n8k4.f64): 16 x 32 output
-//       tiles dealt to the 8 warps, both operands read straight from the finished columns in global memory (this CTA
-//       wrote them, so they come from L1 / L2), the D scaling applied to the B fragment on the fly, no barrier inside;
+// The leaf is factorised in 32-column panels, left to right.  A panel (rows k0.., columns k0..k0+31) is brought up to
+// date in shared memory and written to global memory once, final:
+//   (1) build: the panel's kernel entries on and below the diagonal, LF_BUILD_ILP independent entries per thread in
+//       flight (the 1-D shapes through ShapeEval, the same arithmetic as the interpreter), parked in the panel's own
+//       slots of the factor (the diagonal in shared memory) until its turn;
+//   (2) update: panel -= L(k0:, 0:k0) D L(k0:k0+32, 0:k0)^T on the tensor pipe (mma.sync.m8n8k4.f64) in 16 x 32 output
+//       tiles, both operands read straight from the finished columns in global memory (this CTA wrote them, so they
+//       come from L1 / L2), the D scaling applied to the B fragment on the fly;
 //   (3) the 32 x 32 diagonal block: right-looking LDL^T by one warp in shared memory, lane = row, with a rolled loop
 //       (a fully unrolled register version is ~7k instructions run once per panel by one warp: it streamed through the
 //       instruction cache and cost more than the rest of the panel).  The same warp eliminates the identity alongside,
 //       which leaves W = L11^-T D^-1 in shared memory;
 //   (4) the rows below it: L21 = A21 W on the tensor pipe, 16 x 32 tiles dealt to the 8 warps, written to global memory
 //       from the accumulators.
-// No entry of the leaf is read back and rewritten in global memory.
+// Warps 1..7 look one panel ahead: while warp 0 runs (3) for panel p they build panel p + 1 and accumulate its update
+// over the columns before panel p, none of which depends on panel p.  The accumulators are parked unsubtracted; at
+// panel p + 1's turn all warps continue them with panel p's 32 columns and subtract once, so each entry sums its terms
+// in the order of a single pass and the factor is bit for bit that of the panel-by-panel schedule (DESIGN.md §6).
 #pragma once
 
 #include "gemm_dmma.cuh"
@@ -62,6 +65,7 @@ __global__ void __launch_bounds__(LF_THREADS, 2) leaf_factor_kernel(const DevPro
   double* w11 = dall + ldp;
   DevProgram* P = reinterpret_cast<DevProgram*>(w11 + LF_NB * LF_LDW);
   __shared__ double red[32];
+  __shared__ double draw[LF_NB];  // the diagonal kernel entries (+ diag) of the next panel
   if constexpr (SHAPE == BGP_SHAPE_GENERIC) stage_program(P, gprog);
   __syncthreads();
   const auto fn = ShapeEval<SHAPE>::make(P, gprog);
@@ -74,71 +78,105 @@ __global__ void __launch_bounds__(LF_THREADS, 2) leaf_factor_kernel(const DevPro
 
   // independent kernel evaluations per thread in flight in the build (the interpreter keeps one: its stack is large)
   constexpr int LF_BUILD_ILP = SHAPE == BGP_SHAPE_GENERIC ? 1 : 4;
-  double logdet = 0.0;
-  for (int k0 = 0; k0 < m; k0 += LF_NB) {
-    const int nb = min(LF_NB, m - k0), rem = m - k0;
-    // (1) build
-    for (int t0 = threadIdx.x; t0 < nb * rem; t0 += LF_BUILD_ILP * LF_THREADS) {
+  // (1) build of the panel at leaf row kp by threads t_first.. (nthreads of them): its kernel entries on and below the
+  // diagonal, parked until the panel's turn: off the diagonal in their own slots of the factor, the diagonal in draw
+  auto build = [&](int kp, int t_first, int nthreads) {
+    const int nb = min(LF_NB, m - kp), rem = m - kp;
+    for (int t0 = t_first; t0 < nb * rem; t0 += LF_BUILD_ILP * nthreads) {
       double v[LF_BUILD_ILP];
 #pragma unroll
       for (int u = 0; u < LF_BUILD_ILP; ++u) {
-        const int t = t0 + u * LF_THREADS, c = t / rem, i = t - c * rem;
-        v[u] = (t < nb * rem && i >= c) ? fn(xs + (int64_t)(k0 + i) * nd, xs + (int64_t)(k0 + c) * nd) : 0.0;
+        const int t = t0 + u * nthreads, c = t / rem, i = t - c * rem;
+        v[u] = (t < nb * rem && i >= c) ? fn(xs + (int64_t)(kp + i) * nd, xs + (int64_t)(kp + c) * nd) : 0.0;
       }
 #pragma unroll
       for (int u = 0; u < LF_BUILD_ILP; ++u) {
-        const int t = t0 + u * LF_THREADS, c = t / rem, i = t - c * rem;
-        if (t < nb * rem && i >= c) pn[c * ldp + i] = (i == c) ? v[u] + diag[lf.start + k0 + i] : v[u];
+        const int t = t0 + u * nthreads, c = t / rem, i = t - c * rem;
+        if (t < nb * rem && i > c) A[(int64_t)(kp + c) * m + kp + i] = v[u];
+        if (t < nb * rem && i == c) draw[c] = v[u] + diag[lf.start + kp + i];
       }
+    }
+  };
+  // (2) update: acc += L(kp + r0.., q) D(q) L(kp + 0..31, q)^T over the finished columns q in [q_lo, q_hi), a 16 x 32
+  // tile of the panel at leaf row kp on the tensor pipe (mma.sync.m8n8k4.f64), both operands read straight from the
+  // finished columns in global memory (this CTA wrote them, so they come from L1 / L2), the D scaling applied to the
+  // B fragment on the fly
+  auto update = [&](double (&acc)[2][4][2], int kp, int r0, int q_lo, int q_hi) {
+    const int nb = min(LF_NB, m - kp), rem = m - kp;
+    bool aok[2], bok[4];
+#pragma unroll
+    for (int a = 0; a < 2; ++a) aok[a] = r0 + a * 8 + lr < rem;
+#pragma unroll
+    for (int b = 0; b < 4; ++b) bok[b] = b * 8 + lr < nb;
+#pragma unroll 4
+    for (int q0 = q_lo; q0 < q_hi; q0 += 4) {
+      const int q = q0 + lc;
+      const double* Lq = A + (int64_t)q * m + kp;
+      const double dq = dall[q];
+      double af[2], bf[4];
+#pragma unroll
+      for (int a = 0; a < 2; ++a) af[a] = aok[a] ? Lq[r0 + a * 8 + lr] : 0.0;
+#pragma unroll
+      for (int b = 0; b < 4; ++b) bf[b] = bok[b] ? Lq[b * 8 + lr] * dq : 0.0;
+#pragma unroll
+      for (int a = 0; a < 2; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b) dmma884(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
+    }
+  };
+  // a panel's update accumulators are parked unsubtracted in rows 0..31 of columns 32.. of the leaf, in its strict
+  // upper triangle, which no consumer of the factor reads: element f = 8 a + 2 b + e of lane `lane` of tile t at row
+  // `lane` of column 32 + 16 t + f, so that a warp stores and loads 256 contiguous bytes.  Only panels from row 64 on
+  // park, so their tiles end at column m - 18 or before.
+  auto parked = [&](int t, int a, int b, int e) -> double& {
+    return A[(int64_t)(LF_NB + 16 * t + 8 * a + 2 * b + e) * m + lane];
+  };
+
+  double logdet = 0.0;
+  build(0, threadIdx.x, LF_THREADS);
+  __syncthreads();
+  for (int k0 = 0; k0 < m; k0 += LF_NB) {
+    const int nb = min(LF_NB, m - k0), rem = m - k0, k1 = k0 + LF_NB;
+    // (2) into shared memory: the panel's kernel entries minus its update, the parked accumulators of the columns
+    // before the previous panel continued with the previous panel's 32 columns, so that every entry sums its terms in
+    // the order of one pass over the columns 0..k0-1
+    for (int t = warp; t < (rem + 15) / 16; t += LF_THREADS / 32) {
+      const int r0 = t * 16;
+      double acc[2][4][2];
+#pragma unroll
+      for (int a = 0; a < 2; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) acc[a][b][e] = k0 > LF_NB ? parked(t, a, b, e) : 0.0;
+      update(acc, k0, r0, max(k0 - LF_NB, 0), k0);
+      // all loads of the kernel entries before the first store (a shared-memory store would hold back the loads after
+      // it: the compiler cannot tell pn from draw)
+#pragma unroll
+      for (int a = 0; a < 2; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int i = r0 + a * 8 + lr, c = b * 8 + 2 * lc + e;
+            if (i < rem && c < nb && i >= c)
+              acc[a][b][e] = (i == c ? draw[c] : A[(int64_t)(k0 + c) * m + k0 + i]) - acc[a][b][e];
+          }
+#pragma unroll
+      for (int a = 0; a < 2; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int i = r0 + a * 8 + lr, c = b * 8 + 2 * lc + e;
+            if (i < rem && c < nb && i >= c) pn[c * ldp + i] = acc[a][b][e];
+          }
     }
     __syncthreads();
-    // (2) update from the finished columns 0..k0-1
-    if (k0 > 0) {
-      const int n_tiles = (rem + 15) / 16;
-      bool bok[4];
-#pragma unroll
-      for (int b = 0; b < 4; ++b) bok[b] = b * 8 + lr < nb;
-      for (int t = warp; t < n_tiles; t += LF_THREADS / 32) {
-        const int r0 = t * 16;
-        bool aok[2];
-#pragma unroll
-        for (int a = 0; a < 2; ++a) aok[a] = r0 + a * 8 + lr < rem;
-        double acc[2][4][2];
-#pragma unroll
-        for (int a = 0; a < 2; ++a)
-#pragma unroll
-          for (int b = 0; b < 4; ++b) { acc[a][b][0] = 0.0; acc[a][b][1] = 0.0; }
-#pragma unroll 4
-        for (int q0 = 0; q0 < k0; q0 += 4) {
-          const int q = q0 + lc;
-          const double* Lq = A + (int64_t)q * m + k0;
-          const double dq = dall[q];
-          double af[2], bf[4];
-#pragma unroll
-          for (int a = 0; a < 2; ++a) af[a] = aok[a] ? Lq[r0 + a * 8 + lr] : 0.0;
-#pragma unroll
-          for (int b = 0; b < 4; ++b) bf[b] = bok[b] ? Lq[b * 8 + lr] * dq : 0.0;
-#pragma unroll
-          for (int a = 0; a < 2; ++a)
-#pragma unroll
-            for (int b = 0; b < 4; ++b) dmma884(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
-        }
-#pragma unroll
-        for (int a = 0; a < 2; ++a) {
-          const int i = r0 + a * 8 + lr;
-#pragma unroll
-          for (int b = 0; b < 4; ++b)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int c = b * 8 + 2 * lc + e;
-              if (i < rem && c < nb && i >= c) pn[c * ldp + i] -= acc[a][b][e];
-            }
-        }
-      }
-      __syncthreads();
-    }
     // (3) warp 0: LDL^T of the diagonal block, lane = row i, and T = L11^-1 (starting from the identity, row i of T
-    // takes the same eliminations as row i of the block); then W = T^T D^-1
+    // takes the same eliminations as row i of the block); then W = T^T D^-1.  Meanwhile warps 1..7 look one panel
+    // ahead: they build the next panel and accumulate its update from the columns before this one, none of which
+    // depends on this panel.
     if (warp == 0) {
       double* t11 = w11;  // T(i, j) at t11[j * LF_LDW + i]
       for (int j = 0; j < LF_NB; ++j) t11[j * LF_LDW + lane] = (j == lane) ? 1.0 : 0.0;
@@ -165,6 +203,25 @@ __global__ void __launch_bounds__(LF_THREADS, 2) leaf_factor_kernel(const DevPro
         dall[k0 + lane] = d;
         logdet += log(fabs(d));
         for (int j = 0; j <= lane; ++j) t11[j * LF_LDW + lane] *= dinv;
+      }
+    } else if (k1 < m) {
+      build(k1, threadIdx.x - 32, LF_THREADS - 32);
+      if (k0 > 0) {
+        for (int t = warp - 1; t < (m - k1 + 15) / 16; t += LF_THREADS / 32 - 1) {
+          const int r0 = t * 16;
+          double acc[2][4][2];
+#pragma unroll
+          for (int a = 0; a < 2; ++a)
+#pragma unroll
+            for (int b = 0; b < 4; ++b) { acc[a][b][0] = 0.0; acc[a][b][1] = 0.0; }
+          update(acc, k1, r0, 0, k0);
+#pragma unroll
+          for (int a = 0; a < 2; ++a)
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) parked(t, a, b, e) = acc[a][b][e];
+        }
       }
     }
     __syncthreads();
