@@ -1641,10 +1641,12 @@ static int predict_own_prepare(bgp_hodlr* h, const bgp_kernel_spec_t* spec, int6
   } else {
     BGP_TRY(w->dB.reserve((size_t)nloc * ns, s));
     BGP_TRY(w->dout.reserve((size_t)ns * ns, s));
-    int64_t nsplit_c, nsplit_t, klen;  // predict_gemm_sub's split-K slices of a full chunk and of the tail
+    // predict_gemm_sub's split-K slices of a full chunk and of the tail; none when the product has one slice
+    int64_t nsplit_c, nsplit_t, klen;
     predict_gemm_plan(c, ns, nloc, &nsplit_c, &klen);
     predict_gemm_plan(tail, ns, nloc, &nsplit_t, &klen);
-    BGP_TRY(w->scratch.reserve((size_t)std::max(nsplit_c * c, nsplit_t * tail) * ns, s));
+    const int64_t sc = std::max(nsplit_c > 1 ? nsplit_c * c : 0, nsplit_t > 1 ? nsplit_t * tail : 0) * ns;
+    if (sc > 0) BGP_TRY(w->scratch.reserve((size_t)sc, s));
     BGP_TRY(w->ddesc.reserve((size_t)std::max(nsplit_c, nsplit_t), s));
   }
   return BGP_OK;

@@ -923,6 +923,17 @@ __global__ void predict_slices_add_kernel(const double* __restrict__ slices, int
   }
 }
 
+// C[i*ldc + j] = C[j*ldc + i] for i > j: the upper triangle of the n x n C from its lower one (member blockIdx.y:
+// C + y * cstride)
+__global__ void mirror_lower_kernel(double* __restrict__ C, int64_t n, int64_t ldc, int64_t cstride) {
+  const int64_t total = n * n;
+  C += blockIdx.y * cstride;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t j = t / n, i = t - j * n;
+    if (i > j) C[i * ldc + j] = C[j * ldc + i];
+  }
+}
+
 // The split-K plan of the covariance product (m x nn, K deep): nsplit slices of klen (a multiple of GD_BK) each
 void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, int64_t* klen_out) {
   const int64_t tiles = ((m + GD_BM - 1) / GD_BM) * ((nn + GD_BN - 1) / GD_BN);
@@ -936,7 +947,9 @@ void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, in
 }
 
 // C (m x nn, column-major ldc) -= A'B' with A'(i, k) = A[i*lda + k], B'(k, j) = B[j*ldb + k], k < K: the (1, 1) DMMA
-// variant split over K into nsplit zeroed slices (each one GD_SUB target), then added into C in a fixed order.
+// variant split over K into nsplit zeroed slices (each one GD_SUB target), then added into C in a fixed order.  With
+// one slice the product is subtracted from C directly, with no slice buffer: C - x is the value C + (0 - x) that the
+// slice path gives (up to the sign of an exact zero).
 // `lower` (m == nn, A == B): only the lower triangle is computed and the result is mirrored, so C stays exactly symmetric.
 // `members` > 1: member b uses A and B + b * abstride and C + b * cstride; all members' slices go through one DMMA
 // launch (nsplit * members descriptors, member-major) and one add, so the launch count does not depend on members
@@ -949,10 +962,13 @@ int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int6
   if (members > 65535) { set_error("predict: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
   int64_t nsplit, klen;
   predict_gemm_plan(m, nn, K, &nsplit, &klen);
+  const bool direct = nsplit == 1;
   const int64_t slice = m * nn;
   const int64_t nslices = nsplit * members;
-  BGP_TRY(slices.reserve((size_t)(slice * nslices), s));
-  BGP_CUDA(cudaMemsetAsync(slices.p, 0, sizeof(double) * slice * nslices, s));
+  if (!direct) {
+    BGP_TRY(slices.reserve((size_t)(slice * nslices), s));
+    BGP_CUDA(cudaMemsetAsync(slices.p, 0, sizeof(double) * slice * nslices, s));
+  }
   std::vector<GemmDesc> hd((size_t)nslices);
   for (int64_t mb = 0; mb < members; ++mb)
     for (int64_t sp = 0; sp < nsplit; ++sp) {
@@ -960,13 +976,22 @@ int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int6
       GemmDesc& d = hd[(size_t)(mb * nsplit + sp)];
       d.A = A + mb * abstride + k0; d.lda = lda;
       d.B = B + mb * abstride + k0; d.ldb = ldb;
-      d.C = slices.p + (mb * nsplit + sp) * slice; d.ldc = m;
+      if (direct) { d.C = C + mb * cstride; d.ldc = ldc; }
+      else { d.C = slices.p + (mb * nsplit + sp) * slice; d.ldc = m; }
       d.M = (int)m; d.N = (int)nn; d.K = (int)std::max<int64_t>(0, std::min(klen, K - k0));
       d.mode = GD_SUB | (lower ? GD_LOWER : 0);
     }
   BGP_TRY(descs.reserve((size_t)nslices, s));
   BGP_CUDA(cudaMemcpyAsync(descs.p, hd.data(), sizeof(GemmDesc) * nslices, cudaMemcpyHostToDevice, s));
   BGP_TRY((gemm_dmma_launch<true, true>(descs.p, (int)nslices, (int)m, (int)nn, nullptr, s)));
+  if (direct) {
+    if (lower) {
+      mirror_lower_kernel<<<dim3((unsigned)std::min<int64_t>((slice + 255) / 256, 8 * (int64_t)num_sms()), (unsigned)members),
+                            256, 0, s>>>(C, m, ldc, cstride);
+      BGP_LAUNCH_CHECK();
+    }
+    return BGP_OK;
+  }
   predict_slices_add_kernel<<<dim3((unsigned)std::min<int64_t>((slice + 255) / 256, 8 * (int64_t)num_sms()), (unsigned)members),
                               256, 0, s>>>(slices.p, (int)nsplit, m, nn, C, ldc, lower ? 1 : 0, cstride);
   BGP_LAUNCH_CHECK();

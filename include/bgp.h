@@ -237,8 +237,9 @@ int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r,
  * predictive of y_i is mean y_i - alpha_i / d_i and variance 1 / d_i.  Any output pointer may be NULL; when beta_out,
  * g_out and diag_out are all NULL only pass 1 runs.  K^-1 is formed whole and K^-1 diag(c) K^-1 = G^T G, G =
  * diag(sqrt(c)) K^-1, runs on the FP64 tensor pipe.  Device workspace (doubles): n^2 (K^-1, kept by the handle as
- * bgp_dense_grad_terms keeps it) in pass 1; pass 2 adds n^2 for A and the product's split-K slices, n^2 each: one slice
- * from n = 2176 (3 n^2 in all: about 26 GB at n = 32768), at most four below (6 n^2), plus ceil(n / 32)^2 P for the
+ * bgp_dense_grad_terms keeps it) in pass 1; pass 2 adds n^2 for A and the product's split-K slices, n^2 each: none once
+ * the product has one slice, ceil(n / 128)^2 >= 2 x the SM count (from n = 2049 on a 132-SM H100 SXM; 2 n^2 in all:
+ * about 34.5 GB at n = 46411, beside the n^2 of the factor), at most four below (6 n^2), plus ceil(n / 32)^2 P for the
  * contraction and 5 n + 64.  Errors: BGP_ERR_NOT_COMPUTED before compute and on a handle restored by
  * bgp_dense_import_factor; BGP_ERR_INVALID, when pass 2 is asked for, for more than 64 kernel parameters (before
  * anything is launched) and for a d_j that is not finite and positive (the message names j; alpha_out and d_out are
@@ -264,8 +265,10 @@ int bgp_dense_last_timing(const bgp_dense_t* h, double* ms2);
  * accumulates a node's Gram product with atomics once a half has more than 512 rows.  Negative variances are returned
  * as computed.
  * Device workspace (doubles), besides the result (ns or ns^2) and xs:
- *   dense VAR  N*c + O(c)                 dense COV  N*ns + split-K slices (ns^2 each, at most max(ns^2, 2^27) in all)
- *   HODLR VAR  2*N*c + O(c)               HODLR COV  N*ns + N*c + split-K slices (c*ns each, at most max(c*ns, 2^27))
+ *   dense VAR  N*c + O(c)                 dense COV  N*ns + split-K slices (ns^2 each, at most 2^27 in all)
+ *   HODLR VAR  2*N*c + O(c)               HODLR COV  N*ns + N*c + split-K slices (c*ns each, at most 2^27 in all)
+ * A product of one split-K slice (at least two 128 x 128 tiles per SM, N <= 256, or more than 2^26 entries) has no
+ * slice buffer: it is subtracted from the result in place.
  * Errors: BGP_ERR_NOT_COMPUTED before compute and on a dense handle restored by bgp_dense_import_factor (no
  * coordinates); BGP_ERR_DIM when the spec's ndim differs from the handle's; BGP_ERR_INVALID on a host-exchange HODLR
  * shard, an unknown `what` or ns < 0; BGP_ERR_NOMEM when the workspace cannot be allocated.  ns == 0 writes nothing.
@@ -540,7 +543,7 @@ int bgp_hodlr_loo_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, 
  * the first collective, and one all-reduce of a status value makes a failure on any rank an error on every rank.  The
  * number of chunks depends only on N, ns and BGP_PREDICT_CHUNK, which must therefore be the same on every rank.
  * Device workspace per shard (doubles), besides the result and xs, with nloc = the shard's rows:
- *   VAR  N*c + nloc*c + O(c)             COV  N*c + nloc*ns + split-K slices (c*ns each, at most max(c*ns, 2^27))
+ *   VAR  N*c + nloc*c + O(c)             COV  N*c + nloc*ns + split-K slices (c*ns each, at most 2^27; none with one)
  * A host-exchange shard returns BGP_ERR_INVALID, as before; it computes its part with bgp_hodlr_predict_local_dev. */
 int bgp_hodlr_predict(bgp_hodlr_t* h, const bgp_kernel_spec_t* spec, const double* xs, int64_t ns, int32_t what,
                       double* out);

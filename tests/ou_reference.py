@@ -27,7 +27,9 @@ Everything else follows in O(n):
   (``d sqrt(r^2) / dlog m = -sqrt(r^2) / 2``).  The gradient terms of ``grad_terms``,
   ``g_p = sum_ij (alpha alpha^T - K^-1)_ij dK_ij/dtheta_p`` with ``alpha = K^-1 r``, are therefore
   ``g_c = r . alpha - n`` and ``g_m = alpha^T D alpha / 2 - tr(K^-1 D) / 2``.  D is semi-separable: ``D a`` takes one
-  forward and one backward sweep, and ``tr(K^-1 D)`` needs only the first off-diagonal of K^-1 (D's diagonal is 0).
+  forward and one backward sweep, and ``tr(K^-1 D)`` needs only the first off-diagonal of K^-1 (D's diagonal is 0);
+* the leave-one-out terms of ``loo_terms`` (``loo_terms`` has the derivation): ``K^-1 diag(w) K^-1`` is pentadiagonal,
+  and each contraction with K or D is a dot with one ``K a`` / ``D a`` sweep plus five bands.
 
 Every recursion runs on the ratios ``rho_j`` and the scaled gaps ``(x_j - x_{j-1}) / l``, never on ``exp(+-x / l)``,
 so nothing overflows however long the interval.  All arithmetic is ``np.longdouble`` (x87 80-bit on x86-64, eps
@@ -123,29 +125,39 @@ class OU(object):
         return out.reshape(z.shape)
 
     # ---- the log-likelihood gradient ------------------------------------------------------------------------------
-    def apply_d(self, a):
-        """``D a`` for a vector ``a``, ``D_ij = K_ij |x_i - x_j| / l``, in one forward and one backward sweep.
+    def _sweeps(self, a):
+        """``(K a, D a)`` for a vector ``a``, ``D_ij = K_ij |x_i - x_j| / l``, in one forward and one backward sweep.
 
         Forward: ``P_i = sum_{j<i} exp(-(x_i - x_j)/l) a_j`` and ``Q_i = sum_{j<i} exp(-(x_i - x_j)/l) (x_i - x_j)/l a_j``
         obey ``P_i = rho_i (P_{i-1} + a_{i-1})`` and ``Q_i = rho_i (Q_{i-1} + delta_i (P_{i-1} + a_{i-1}))``; the
-        backward sweep is the mirror image.  ``(D a)_i = c (Q_i + Q'_i)``."""
+        backward sweep is the mirror image.  ``(K a)_i = c (a_i + P_i + P'_i)`` and ``(D a)_i = c (Q_i + Q'_i)``."""
         a = np.asarray(a, dtype=LD).tolist()
         rho, dl = self.rho.tolist(), self.delta.tolist()
         n = self.n
-        out = [LD(0)] * n
+        ka, da = list(a), [LD(0)] * n
         P = Q = LD(0)
         for i in range(1, n):
             t = P + a[i - 1]
             Q = rho[i] * (Q + dl[i] * t)
             P = rho[i] * t
-            out[i] = Q
+            ka[i] += P
+            da[i] = Q
         P = Q = LD(0)
         for i in range(n - 2, -1, -1):
             t = P + a[i + 1]
             Q = rho[i + 1] * (Q + dl[i + 1] * t)
             P = rho[i + 1] * t
-            out[i] += Q
-        return self.c * np.array(out, dtype=LD)
+            ka[i] += P
+            da[i] += Q
+        return self.c * np.array(ka, dtype=LD), self.c * np.array(da, dtype=LD)
+
+    def apply_d(self, a):
+        """``D a`` for a vector ``a`` (see ``_sweeps``)."""
+        return self._sweeps(a)[1]
+
+    def apply_k(self, a):
+        """``K a`` for a vector ``a`` (see ``_sweeps``)."""
+        return self._sweeps(a)[0]
 
     def trace_kinv_d(self):
         """``tr(K^-1 D) = 2 sum_j K^-1_{j,j+1} D_{j,j+1}``, with ``D_{j,j+1} = c rho_{j+1} delta_{j+1}``."""
@@ -161,6 +173,56 @@ class OU(object):
         g_m = (alpha @ self.apply_d(alpha) - self.trace_kinv_d()) / 2
         d, _ = self.inv_tridiag()
         return alpha, np.array([g_c, g_m], dtype=LD), alpha ** 2 - d
+
+    # ---- leave-one-out cross-validation -------------------------------------------------------------------------------
+    def loo_terms(self, r):
+        """The leave-one-out terms of ``loo_terms`` for theta = (log c, log m), as a dict:
+
+        * ``alpha = K^-1 r``, ``d = diag(K^-1) = t`` (the diagonal of the tridiagonal ``T = K^-1``, off-diagonal ``e``);
+        * ``beta = K^-1 q`` with ``q = alpha / d``, and the weights ``w_i = (1 + alpha_i q_i) / (2 d_i)``;
+        * ``M = T diag(w) T`` is pentadiagonal: ``M_jj = w_{j-1} e_{j-1}^2 + w_j t_j^2 + w_{j+1} e_j^2``,
+          ``M_{j,j+1} = e_j (w_j t_j + w_{j+1} t_{j+1})`` and ``M_{j,j+2} = e_j w_{j+1} e_{j+1}``;
+        * ``A = 1/2 (beta alpha^T + alpha beta^T) - M``, so ``diagA = alpha beta - diag(M)``;
+        * ``g_logc = sum_ij K_ij A_ij = beta . r - sum_j w_j t_j``: ``K alpha = r``, and
+          ``tr(K T W T) = tr(W T K T) = tr(W T)``;
+        * ``g_logm = sum_ij (D / 2)_ij A_ij = (beta^T D alpha - sum_ij D_ij M_ij) / 2``.  D's diagonal is 0, so the
+          second term needs only the bands ``D_{j,j+1} = c rho_{j+1} delta_{j+1}`` and
+          ``D_{j,j+2} = c rho_{j+1} rho_{j+2} (delta_{j+1} + delta_{j+2})`` (c the kernel amplitude);
+        * ``value = sum_i [-1/2 log 2 pi + 1/2 log d_i - alpha_i^2 / (2 d_i)]``; the LOO predictive of ``r_i`` is
+          ``r_i - alpha_i / d_i`` with variance ``1 / d_i``.
+
+        ``gscale`` bounds ``sum_ij |dK_p|_ij |A_ij|`` from above in O(n): K and D have non-negative entries and
+        ``|M| <= |T| W |T|`` (five bands, W > 0), so it is ``|beta|^T K |alpha| + sum_ij K_ij (|T| W |T|)_ij`` for log c
+        and half of the same with D for log m."""
+        r = np.asarray(r, dtype=LD)
+        t, e = self.inv_tridiag()
+        alpha = self.solve(r)
+        d = t.copy()
+        q = alpha / d
+        beta = self.solve(q)
+        w = (1 + alpha * q) / (2 * d)
+        # the bands of M = T W T (M1, M2: first and second super-diagonals) and of |T| W |T|
+        M0 = w * t * t
+        M0[1:] += w[:-1] * e * e
+        M0[:-1] += w[1:] * e * e
+        M1 = e * (w[:-1] * t[:-1] + w[1:] * t[1:])
+        M2 = e[:-1] * w[1:-1] * e[1:]
+        # the bands of K / c and of D / c (D0 = 0)
+        K1 = self.rho[1:]
+        K2 = self.rho[1:-1] * self.rho[2:]
+        D1 = self.rho[1:] * self.delta[1:]
+        D2 = K2 * (self.delta[1:-1] + self.delta[2:])
+        Db = self._sweeps(beta)[1]
+        g_c = beta @ r - np.sum(w * t)
+        g_m = (Db @ alpha - 2 * self.c * (np.sum(D1 * M1) + np.sum(D2 * M2))) / 2
+        value = np.sum(-np.log(2 * LD(np.pi)) / 2 + np.log(d) / 2 - alpha ** 2 / (2 * d))
+        aa, ab = np.abs(alpha), np.abs(beta)
+        Kab, Dab = self._sweeps(ab)
+        band_k = self.c * (np.sum(M0) + 2 * np.sum(K1 * np.abs(M1)) + 2 * np.sum(K2 * np.abs(M2)))
+        band_d = 2 * self.c * (np.sum(D1 * np.abs(M1)) + np.sum(D2 * np.abs(M2)))
+        gscale = np.array([Kab @ aa + band_k, (Dab @ aa + band_d) / 2], dtype=LD)
+        return dict(alpha=alpha, d=d, beta=beta, g=np.array([g_c, g_m], dtype=LD), diagA=alpha * beta - M0,
+                    value=value, gscale=gscale)
 
     # ---- prediction -------------------------------------------------------------------------------------------------
     def predict(self, t, alpha):

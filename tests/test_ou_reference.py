@@ -4,9 +4,11 @@
 The closed forms are what the large-index GPU tests (``test_gpu_zz_large_index.py``) compare the solvers with at sizes
 where no O(n^3) reference runs, so each quantity they use is pinned here at n <= 500: the factor's columns, log det,
 solves, the tridiagonal K^-1, ``z L^T``, ``D a``, the gradient terms (against ``einsum`` over the oracle's gradient
-tensor, which also fixes the factor 1/2 and the sign of the ``log m`` derivative) and the predictive mean and variance.
-The differences are the float64 rounding of K's entries carried through cond(K) <= 10 (largest measured: 7.7e-16, in
-K^-1 and the gradient's diagonal; bar 1e-14).
+tensor, which also fixes the factor 1/2 and the sign of the ``log m`` derivative), the predictive mean and variance,
+and the leave-one-out terms of ``test_gpu_zz_loo_closed_form.py`` (``K a``, alpha, d, beta, diag(A), g and its scale
+against the brute-force formula, the value and LOO predictive against refits without the point).
+The differences are the float64 rounding of K's entries carried through cond(K) <= 10 (largest measured: 1.5e-15, in
+the LOO diag(A); bar 1e-14).
 """
 import numpy as np
 import pytest
@@ -98,6 +100,56 @@ def test_gradient_terms_match_the_oracle_gradient_tensor(oracle, n, c, m, gap):
     assert _rel(alpha, alpha_ref) <= TOL
     assert np.all(np.abs(g - g_ref) <= TOL * scale), (g, g_ref, scale)
     assert _rel(diag, np.diag(A)) <= TOL
+
+
+@pytest.mark.parametrize("n,c,m,gap", CASES)
+def test_loo_terms_match_the_longdouble_formula(oracle, n, c, m, gap):
+    """``loo_terms`` against the brute-force formula on the oracle's K (``_ld_formula`` of test_gpu_loo.py), g against
+    ``einsum`` over the oracle's gradient tensor, and the value and predictive against N - 1-point refits."""
+    x, kernel, spec, K, ou = _case(n, c, m, gap)
+    L = hiprec.chol_ld(K)
+    Kinv = hiprec.solve_ld(L, np.eye(n))
+    Kinv = (Kinv + Kinv.T) / 2
+    dK = oracle.gradient_general(spec, [1, 1], x[:, None], x[:, None]).astype(LD)
+    a = np.random.default_rng(n + 4).standard_normal(n)
+    assert _rel(ou.apply_k(a), K.astype(LD) @ a.astype(LD)) <= TOL
+    assert _rel(ou.apply_k(a), dK[:, :, 0] @ a.astype(LD)) <= TOL  # dK/dlog c = K
+
+    r = np.sin(x / np.sqrt(m)) + 0.1 * np.random.default_rng(n + 5).standard_normal(n)
+    alpha_ref = Kinv @ r.astype(LD)
+    d_ref = np.diag(Kinv).copy()
+    q = alpha_ref / d_ref
+    beta_ref = Kinv @ q
+    w = (1 + alpha_ref * q) / (2 * d_ref)
+    A = (np.outer(beta_ref, alpha_ref) + np.outer(alpha_ref, beta_ref)) / 2 - Kinv @ (w[:, None] * Kinv)
+    g_ref = np.einsum("ijk,ij->k", dK, A)
+    scale = np.einsum("ijk,ij->k", np.abs(dK), np.abs(A))
+    value_ref = np.sum(-np.log(2 * LD(np.pi)) / 2 + np.log(d_ref) / 2 - alpha_ref ** 2 / (2 * d_ref))
+
+    t = ou.loo_terms(r)
+    assert _rel(t["alpha"], alpha_ref) <= TOL
+    assert _rel(t["d"], d_ref) <= TOL
+    assert _rel(t["beta"], beta_ref) <= TOL
+    assert _rel(t["diagA"], np.diag(A)) <= TOL
+    assert np.all(np.abs(t["g"] - g_ref) <= TOL * scale), (t["g"], g_ref, scale)
+    assert np.all(t["gscale"] >= scale * (1 - TOL)), (t["gscale"], scale)  # an upper bound
+    assert np.all(t["gscale"] <= 4 * scale), (t["gscale"], scale)          # and not a loose one
+    assert abs(float(t["value"] - value_ref)) <= TOL * float(np.sum(np.abs(np.log(d_ref)) + alpha_ref ** 2 / d_ref) + n)
+
+    # the LOO predictive and each point's term of the value against refits without the point
+    for i in sorted({0, n // 2, n - 1}):
+        k = np.delete(np.arange(n), i)
+        if k.size:
+            Li = hiprec.chol_ld(K[np.ix_(k, k)])
+            mu = K[i, k].astype(LD) @ hiprec.solve_ld(Li, r[k].astype(LD))
+            var = LD(K[i, i]) - K[i, k].astype(LD) @ hiprec.solve_ld(Li, K[k, i].astype(LD))
+        else:
+            mu, var = LD(0), LD(K[i, i])
+        assert abs(float(r[i] - t["alpha"][i] / t["d"][i] - mu)) <= TOL * max(1.0, float(np.max(np.abs(r))))
+        assert abs(float(1 / t["d"][i] - var)) <= TOL * c
+        term = -np.log(2 * LD(np.pi) * var) / 2 - (r[i] - mu) ** 2 / (2 * var)
+        own = -np.log(2 * LD(np.pi)) / 2 + np.log(t["d"][i]) / 2 - t["alpha"][i] ** 2 / (2 * t["d"][i])
+        assert abs(float(own - term)) <= TOL * max(1.0, abs(float(term)))
 
 
 @pytest.mark.parametrize("n,c,m,gap", CASES)
