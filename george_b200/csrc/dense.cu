@@ -32,6 +32,12 @@ int loo_weights_launch(const double* alpha, const double* d, int64_t n, double* 
 int scale_rows_launch(double* X, int64_t n, int64_t ncols, int64_t ldx, const double* w, bool sqrt_w, cudaStream_t s);
 int slab_diag_launch(const double* W, int64_t ldw, int64_t j0, int64_t nc, double* d, cudaStream_t s);
 int loo_check_diag(const double* d, int64_t n);
+int loo_weights_members(const double* alpha, const double* d, int64_t n, double* q, double* c, int members,
+                        cudaStream_t s);
+int scale_rows_members(double* X, int64_t n, int64_t ncols, int64_t ldx, const double* w, bool sqrt_w, int members,
+                       int64_t xstride, int64_t wstride, cudaStream_t s);
+int slab_diag_members(const double* W, int64_t ldw, int64_t j0, int64_t nc, double* d, int members, int64_t wstride,
+                      int64_t dstride, cudaStream_t s);
 int fill_identity_members(double* A, int64_t n, int members, cudaStream_t s);
 int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
                              int64_t n2, double* out, int64_t ld, cudaStream_t s);
@@ -456,14 +462,26 @@ __global__ void add_into_kernel(const double* __restrict__ a, double* __restrict
 }
 // A += 1/2 (beta alpha^T + alpha beta^T) over the whole n x n A (bgp_dense_loo_terms: A = -K^-1 diag(c) K^-1 before).
 // Every rounding is explicit, so A stays exactly symmetric and A_ii = -M_ii + alpha_i beta_i.
+// (member blockIdx.y of a batch: A + y * n^2, alpha and beta + y * n)
 __global__ void loo_form_a_kernel(double* __restrict__ A, int64_t n, const double* __restrict__ alpha,
                                   const double* __restrict__ beta) {
   const int64_t total = n * n;
+  A += blockIdx.y * total;
+  alpha += blockIdx.y * n;
+  beta += blockIdx.y * n;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t j = t / n, i = t - j * n;
     const double sym = __dadd_rn(__dmul_rn(beta[i], alpha[j]), __dmul_rn(alpha[i], beta[j]));
     A[t] = __dadd_rn(A[t], __dmul_rn(0.5, sym));
   }
+}
+// `members` matrices of order n back to back; a single call passes one member
+static int loo_form_a_members(double* A, int64_t n, const double* alpha, const double* beta, int members,
+                              cudaStream_t s) {
+  loo_form_a_kernel<<<dim3((unsigned)std::min<int64_t>((n * n + 255) / 256, 16 * (int64_t)num_sms()), (unsigned)members),
+                      256, 0, s>>>(A, n, alpha, beta);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
 }
 // out (nr x n, row-major) = r (nr x n, row-major) @ U with U = L^T:  out[a][j] = sum_{i<=j} r[a][i] L[j][i]
 __global__ void apply_sqrt_kernel(const double* __restrict__ L, int64_t n, const double* __restrict__ r, int64_t nr,
@@ -972,9 +990,7 @@ int bgp_dense_loo_terms(bgp_dense_t* h, const uint32_t* which, const double* r, 
   BGP_CUDA(cudaMemsetAsync(dA.p, 0, sizeof(double) * n * n, s));
   BGP_TRY(predict_gemm_sub(h->d_inv.p, n, h->d_inv.p, n, n, n, n, true, dA.p, n, slices, descs, s));
   slices.release();
-  loo_form_a_kernel<<<(unsigned)std::min<int64_t>((n * n + 255) / 256, 16 * (int64_t)num_sms()), 256, 0, s>>>(
-      dA.p, n, alpha, beta);
-  BGP_LAUNCH_CHECK();
+  BGP_TRY(loo_form_a_members(dA.p, n, alpha, beta, 1, s));
   BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
   if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
   BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, dA.p, n, nullptr, 0.0, 1.0, dg,
@@ -1151,6 +1167,8 @@ struct bgp_dense_batch : BatchStream {
   DevBuf<unsigned> d_which;
   // bgp_dense_batch_predict_grad: dmu, a test-point chunk of dvar and the input-gradient contraction's partials
   DevBuf<double> d_dmu, d_dvar, d_xgp;
+  // bgp_dense_batch_loo_terms (besides d_inv, d_gp, d_g and d_which): A, beta (q, then K^-1 q) and c
+  DevBuf<double> d_loo_a, d_beta, d_cw;
 };
 
 // members per chunk: as many members of per_member doubles as fit in 4 GiB, at least one; BGP_BATCH_CHUNK=<members>
@@ -1456,6 +1474,71 @@ int bgp_dense_batch_grad_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* sp
   return batch_run(h, bp, x, n, ndim, yerr, r, per_member, 65535, tmp_cols,
                    {{&h->d_A, nn}, {&h->d_inv, nn}, {&h->d_gp, nt * nt * P}, {&h->d_g, P}}, setup, step, info,
                    {{log_det, 1}, {quad, 1}, {alpha, n}, {diag, n}, {g, P}});
+}
+
+int bgp_dense_batch_loo_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
+                              int64_t P, const double* x, int64_t n, int32_t ndim, const double* yerr, const double* r,
+                              const uint32_t* which, double* alpha, double* d, double* beta, double* g, double* diag,
+                              int32_t* info) {
+  const bool grad = which != nullptr;
+  if (grad && P > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  BatchPrograms bp;
+  BGP_TRY(batch_begin(h, spec, params, B, P, x, n, ndim, &bp));
+  if (B == 0) return BGP_OK;
+  cudaStream_t s = h->s;
+  const int64_t nn = n * n;
+  // n <= DS_MAX_RHS: K^-1 goes through the few-column solve, as bgp_dense_loo_terms sends it, with n x n of scratch
+  const int64_t tmp_cols = n <= DS_MAX_RHS ? n : 1;
+  const int64_t nt = (n + 31) / 32;  // the contraction's 32 x 32 tiles
+  // the G^T G product's split-K plan, bgp_dense_loo_terms' (no slice buffer with one slice)
+  int64_t gsplit = 1, gklen = 0;
+  if (grad) predict_gemm_plan(n, n, n, &gsplit, &gklen);
+  const int64_t slices = gsplit > 1 ? gsplit * nn : 0;
+  // doubles per member (see include/bgp.h): factor, K^-1 and the vectors of batch_reserve_common; pass 2 adds A, the
+  // product's slices, beta, c, the contraction partials and g
+  int64_t per_member = 2 * nn + (4 + tmp_cols) * n;
+  std::vector<ChunkBuf> bufs = {{&h->d_A, nn}, {&h->d_inv, nn}};
+  if (grad) {
+    per_member += nn + slices + 2 * n + nt * nt * P + P;
+    bufs.insert(bufs.end(), {{&h->d_loo_a, nn}, {&h->d_slices, slices}, {&h->d_beta, n}, {&h->d_cw, n},
+                             {&h->d_gp, nt * nt * P}, {&h->d_g, P}});
+  }
+  auto setup = [&](int64_t) -> int {
+    if (!grad) return BGP_OK;
+    BGP_TRY(h->d_which.reserve((size_t)std::max<int64_t>(1, P), s));
+    if (P > 0) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * P, cudaMemcpyHostToDevice, s));
+    return BGP_OK;
+  };
+  // the steps of bgp_dense_loo_terms after bgp_dense_compute, member-indexed, with no host check of d in between: a
+  // member whose d is not finite and positive runs pass 2 on its own slabs
+  auto step = [&](int64_t c0, int mc, const DevProgram*, const DevProgram* dprogs) -> int {
+    double* dd = h->d_yerr.p;  // d = diag(K_b^-1), in d_yerr: the build in batch_factor_chunk consumed yerr^2
+    BGP_TRY(fill_identity_members(h->d_inv.p, n, mc, s));
+    BGP_TRY(potrs_members(h->d_A.p, n, nn, h->d_inv.p, n, n, nn, mc, h->d_tmp.p, s));
+    BGP_TRY(slab_diag_members(h->d_inv.p, n, 0, n, dd, mc, nn, n, s));
+    if (alpha) BGP_CUDA(cudaMemcpyAsync(alpha + c0 * n, h->d_sol.p, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
+    if (d) BGP_CUDA(cudaMemcpyAsync(d + c0 * n, dd, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
+    if (!grad) return BGP_OK;
+    // pass 2: q and c; beta_b = K_b^-1 q_b (the one-column solve, as for alpha); G_b = diag(sqrt(c_b)) K_b^-1 in place;
+    // A_b = -(G_b^T G_b) (lower, mirrored) on the tensor pipe plus 1/2 (beta_b alpha_b^T + alpha_b beta_b^T); then the
+    // contraction with A_b given whole, its diagonal into d_diag (whose yerr^2 the build consumed)
+    BGP_TRY(loo_weights_members(h->d_sol.p, dd, n, h->d_beta.p, h->d_cw.p, mc, s));
+    BGP_TRY(potrs_small_members(h->d_A.p, n, h->d_beta.p, 1, n, h->d_tmp.p, mc, nn, n, s));
+    BGP_TRY(scale_rows_members(h->d_inv.p, n, n, n, h->d_cw.p, true, mc, nn, n, s));
+    BGP_CUDA(cudaMemsetAsync(h->d_loo_a.p, 0, sizeof(double) * mc * nn, s));
+    BGP_TRY(predict_gemm_sub_members(h->d_inv.p, n, h->d_inv.p, n, n, n, n, true, h->d_loo_a.p, n, mc, nn, nn,
+                                     h->d_slices, h->d_pdesc, s));
+    BGP_TRY(loo_form_a_members(h->d_loo_a.p, n, h->d_sol.p, h->d_beta.p, mc, s));
+    BGP_TRY(kmat_grad_contract_members(dprogs, (int)P, h->d_which.p, h->d_x.p, n, h->d_loo_a.p, n, nn, nullptr, 0,
+                                       0.0, 1.0, h->d_g.p, P, diag ? h->d_diag.p : nullptr, n, mc, h->d_gp, s));
+    if (beta) BGP_CUDA(cudaMemcpyAsync(beta + c0 * n, h->d_beta.p, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
+    if (g && P > 0) BGP_CUDA(cudaMemcpyAsync(g + c0 * P, h->d_g.p, sizeof(double) * mc * P, cudaMemcpyDeviceToHost, s));
+    if (diag) BGP_CUDA(cudaMemcpyAsync(diag + c0 * n, h->d_diag.p, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
+    return BGP_OK;
+  };
+  // one launch per step for the chunk: the split-K product takes one descriptor per member and slice
+  return batch_run(h, bp, x, n, ndim, yerr, r, per_member, 65535 / gsplit, tmp_cols, bufs, setup, step, info,
+                   {{alpha, n}, {d, n}, {beta, grad ? n : 0}, {g, grad ? P : 0}, {diag, grad ? n : 0}});
 }
 
 int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,

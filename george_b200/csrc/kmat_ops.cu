@@ -751,36 +751,53 @@ int fill_identity_launch(double* A, int64_t n, cudaStream_t s) { return fill_ide
 // contracts A = 1/2 (beta alpha^T + alpha beta^T) - K^-1 diag(c) K^-1 with dK, where
 //     q_i = alpha_i / d_i,   beta = K^-1 q,   c_i = (1 + alpha_i q_i) / (2 d_i).
 // ---------------------------------------------------------------------------------------------------------------
+// (member blockIdx.y of a batch: every vector + y * n)
 __global__ void loo_weights_kernel(const double* __restrict__ alpha, const double* __restrict__ d, int64_t n,
                                    double* __restrict__ q, double* __restrict__ c) {
+  const int64_t m = (int64_t)blockIdx.y * n;
+  alpha += m; d += m; q += m; c += m;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const double qi = alpha[i] / d[i];
     q[i] = qi;
     c[i] = (1.0 + alpha[i] * qi) / (2.0 * d[i]);
   }
 }
-int loo_weights_launch(const double* alpha, const double* d, int64_t n, double* q, double* c, cudaStream_t s) {
-  loo_weights_kernel<<<(unsigned)std::min<int64_t>((n + 255) / 256, 1184), 256, 0, s>>>(alpha, d, n, q, c);
+// `members` vectors of n back to back (member stride n); a single call passes one member
+int loo_weights_members(const double* alpha, const double* d, int64_t n, double* q, double* c, int members,
+                        cudaStream_t s) {
+  if (n <= 0 || members <= 0) return BGP_OK;
+  loo_weights_kernel<<<dim3((unsigned)std::min<int64_t>((n + 255) / 256, 1184), (unsigned)members), 256, 0, s>>>(
+      alpha, d, n, q, c);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
+int loo_weights_launch(const double* alpha, const double* d, int64_t n, double* q, double* c, cudaStream_t s) {
+  return loo_weights_members(alpha, d, n, q, c, 1, s);
+}
 
-// X (n x ncols, column-major ldx): row i scaled by w_i, or by sqrt(w_i) with `sqrt_w`
+// X (n x ncols, column-major ldx): row i scaled by w_i, or by sqrt(w_i) with `sqrt_w` (member blockIdx.y of a batch:
+// X + y * xstride, w + y * wstride)
 __global__ void scale_rows_kernel(double* __restrict__ X, int64_t n, int64_t ncols, int64_t ldx,
-                                  const double* __restrict__ w, int sqrt_w) {
+                                  const double* __restrict__ w, int sqrt_w, int64_t xstride, int64_t wstride) {
+  X += blockIdx.y * xstride;
+  w += blockIdx.y * wstride;
   const int64_t total = n * ncols;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t j = t / n, i = t - j * n;
     X[j * ldx + i] *= sqrt_w ? sqrt(w[i]) : w[i];
   }
 }
-int scale_rows_launch(double* X, int64_t n, int64_t ncols, int64_t ldx, const double* w, bool sqrt_w, cudaStream_t s) {
+int scale_rows_members(double* X, int64_t n, int64_t ncols, int64_t ldx, const double* w, bool sqrt_w, int members,
+                       int64_t xstride, int64_t wstride, cudaStream_t s) {
   const int64_t total = n * ncols;
-  if (total <= 0) return BGP_OK;
-  scale_rows_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 16 * (int64_t)num_sms()), 256, 0, s>>>(
-      X, n, ncols, ldx, w, sqrt_w ? 1 : 0);
+  if (total <= 0 || members <= 0) return BGP_OK;
+  scale_rows_kernel<<<dim3((unsigned)std::min<int64_t>((total + 255) / 256, 16 * (int64_t)num_sms()), (unsigned)members),
+                      256, 0, s>>>(X, n, ncols, ldx, w, sqrt_w ? 1 : 0, xstride, wstride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
+}
+int scale_rows_launch(double* X, int64_t n, int64_t ncols, int64_t ldx, const double* w, bool sqrt_w, cudaStream_t s) {
+  return scale_rows_members(X, n, ncols, ldx, w, sqrt_w, 1, 0, 0, s);
 }
 
 // The gradient needs every d_j > 0 (c and sqrt(c) are formed from it); a loose-tolerance HODLR matrix, or rounding of
@@ -795,16 +812,24 @@ int loo_check_diag(const double* d, int64_t n) {
 }
 
 // d[j0 + k] = W[k * ldw + j0 + k] for k < nc: the diagonal entries of the slab W = K^-1 E_J, J = [j0, j0 + nc)
+// (member blockIdx.y of a batch: W + y * wstride, d + y * dstride)
 __global__ void slab_diag_kernel(const double* __restrict__ W, int64_t ldw, int64_t j0, int64_t nc,
-                                 double* __restrict__ d) {
+                                 double* __restrict__ d, int64_t wstride, int64_t dstride) {
+  W += blockIdx.y * wstride;
+  d += blockIdx.y * dstride;
   for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nc; k += (int64_t)gridDim.x * blockDim.x)
     d[j0 + k] = W[k * ldw + j0 + k];
 }
-int slab_diag_launch(const double* W, int64_t ldw, int64_t j0, int64_t nc, double* d, cudaStream_t s) {
-  if (nc <= 0) return BGP_OK;
-  slab_diag_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, ldw, j0, nc, d);
+int slab_diag_members(const double* W, int64_t ldw, int64_t j0, int64_t nc, double* d, int members, int64_t wstride,
+                      int64_t dstride, cudaStream_t s) {
+  if (nc <= 0 || members <= 0) return BGP_OK;
+  slab_diag_kernel<<<dim3((unsigned)std::min<int64_t>((nc + 255) / 256, 1184), (unsigned)members), 256, 0, s>>>(
+      W, ldw, j0, nc, d, wstride, dstride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
+}
+int slab_diag_launch(const double* W, int64_t ldw, int64_t j0, int64_t nc, double* d, cudaStream_t s) {
+  return slab_diag_members(W, ldw, j0, nc, d, 1, 0, 0, s);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -716,6 +716,144 @@ class GP(ModelSet):
             g = self.kernel.kernel.gradient_contract(which, self._x, A)
         return alpha, d, beta, g, np.diag(A).copy()
 
+    def batch_loo_predict(self, vectors, y):
+        """:func:`loo_predict` at many parameter vectors: ``(mu, var)``, each ``(B, N)``, row ``b`` bit for bit what
+        ``gp.set_parameter_vector(vectors[b]); gp.loo_predict(y)`` returns on the computed ``x`` and ``yerr``: the
+        standardised LOO residuals ``(y - mu) / sqrt(var)`` of every sample of a posterior chain in one call, for
+        calibration and outlier checks.  See :func:`batch_grad_loo_log_likelihood` for the errors, the GP's state and
+        which solvers run batched.
+
+        :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
+        """
+        return self._batch_loo("predict", vectors, y, False, False)
+
+    def batch_loo_log_likelihood(self, vectors, y, quiet=False):
+        """:func:`loo_log_likelihood` at many parameter vectors: entry ``b`` of the ``(B,)`` result is bit for bit what
+        ``gp.set_parameter_vector(vectors[b]); gp.loo_log_likelihood(y, quiet=quiet)`` returns on the computed ``x``
+        and ``yerr``.  See :func:`batch_grad_loo_log_likelihood` for the errors, the GP's state and which solvers run
+        batched.
+
+        :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
+        """
+        return self._batch_loo("value", vectors, y, quiet, False)
+
+    def batch_grad_loo_log_likelihood(self, vectors, y, quiet=False, return_value=False):
+        """:func:`grad_loo_log_likelihood` at many parameter vectors: row ``b`` of the ``(B, len(gp))`` result is bit
+        for bit what ``gp.set_parameter_vector(vectors[b]); gp.grad_loo_log_likelihood(y, quiet=quiet,
+        return_value=return_value)`` returns on the computed ``x`` and ``yerr``; with ``return_value`` the result is
+        ``(value, grad)``, ``value`` of shape ``(B,)``.  The values and gradients of every start of a multi-start LOO
+        fit (an objective more multimodal than the marginal likelihood) in one call.
+
+        With ``quiet`` a failing member gets the loop's ``-inf`` and zero gradient and the others are unaffected;
+        otherwise the exception that loop raises first is raised, with its type and message (white noise or
+        factorisation, then the residual, then a ``d_i`` that is not finite and positive, then the mean gradient),
+        with one difference: the checks that do not depend on the member (the shape of ``vectors``, ``y``'s length)
+        come first.  The GP is left as it was: parameter vector, factorisation, cached solve and dirty flags.
+
+        Solvers with a ``batch_loo_terms`` hook (``BasicSolver``) factorise all members, form their ``K^-1`` and
+        contract the kernel gradients in one batched pass on the device.  Any other solver (``HODLRSolver``,
+        ``TrivialSolver``, ``ShardedHODLRSolver``, plug-ins) takes that loop, and so do a kernel without a valid device
+        program and, for the gradient, one with more than 64 parameters (the device contraction's limit: every
+        member's gradient then fails as it does in the loop).
+
+        :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
+        """
+        return self._batch_loo("grad", vectors, y, quiet, return_value)
+
+    def _batch_loo(self, kind, vectors, y, quiet, return_value):
+        """The three ``batch_*loo*`` methods: ``kind`` is ``"predict"``, ``"value"`` or ``"grad"``."""
+        vectors = self._batch_vectors(vectors)
+        self._check_dimensions(y)
+        nb, n = len(vectors), len(self._x)
+        if nb == 0:
+            if kind == "predict":
+                return np.empty((0, n), dtype=np.float64), np.empty((0, n), dtype=np.float64)
+            value, grad = np.empty(0, dtype=np.float64), np.empty((0, len(self)), dtype=np.float64)
+            return value if kind == "value" else ((value, grad) if return_value else grad)
+        batch = getattr(self.solver_type, "batch_loo_terms", None)
+        if batch is not None:
+            out = self._batch_loo_device(batch, kind, vectors, y, quiet, return_value)
+            if out is not None:
+                return out
+        if kind == "predict":
+            res = self._batch_loop(vectors, lambda: self.loo_predict(y))
+            return np.stack([r[0] for r in res]), np.stack([r[1] for r in res])
+        if kind == "value":
+            return np.array(self._batch_loop(vectors, lambda: self.loo_log_likelihood(y, quiet=quiet)),
+                            dtype=np.float64)
+        res = self._batch_loop(vectors, lambda: self.grad_loo_log_likelihood(y, quiet=quiet, return_value=True))
+        value, grad = np.array([r[0] for r in res], dtype=np.float64), np.stack([r[1] for r in res])
+        return (value, grad) if return_value else grad
+
+    def _batch_loo_device(self, batch, kind, vectors, y, quiet, return_value):
+        """The batched dense path of :func:`_batch_loo`; ``None`` when the kernel has no valid device program or, for
+        the gradient, more than ``_MAX_GRAD_PARAMS`` parameters."""
+        members = self._batch_members(vectors, y, self._residual_of,
+                                      lambda y, c: y if c == 0.0 else y - c)  # the operations of GP._residual_of
+        if members is None or (kind == "grad" and members[2].shape[1] > _MAX_GRAD_PARAMS):
+            return None
+        spec, full, kpar, sigma, resid, fact_err, mean_err = members
+        nb = len(vectors)
+        if kind == "predict":
+            alpha, d, info = batch(spec, kpar, self._x, sigma, resid)
+            self._raise_member_error(spec, kpar, info, fact_err, mean_err)
+            y = np.asarray(self._check_dimensions(y), dtype=np.float64)
+            return y - alpha / d, 1.0 / d
+        grad = kind == "grad"
+        if grad:
+            mask = self.kernel.unfrozen_mask
+            alpha, d, beta, g, diag, info = batch(spec, kpar, self._x, sigma, resid, mask.astype(np.uint32))
+        else:
+            alpha, d, info = batch(spec, kpar, self._x, sigma, resid)
+        # GP.loo_log_likelihood / GP.grad_loo_log_likelihood member by member, with their operations
+        n_mean, n_wn, n_k = len(self.mean), len(self.white_noise), len(self.kernel)
+        full_mean, full_wn = self.mean.full_size, self.white_noise.full_size
+        value = np.full(nb, -np.inf)
+        out = np.zeros((nb, len(self)), dtype=np.float64)
+        for b in range(nb):  # the loop's order: factorisation (white noise included), residual, d, mean gradient
+            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
+            if exc is not None:
+                if not (quiet and isinstance(exc, (ValueError, LinAlgError))):
+                    raise exc
+                continue
+            exc = mean_err[b]
+            if exc is not None:
+                # loo_log_likelihood swallows only the mean's own ValueError under quiet, the gradient any ValueError
+                if not (quiet and isinstance(exc, ValueError) and (grad or "mean function" in str(exc))):
+                    raise exc
+                continue
+            if not grad:
+                value[b] = self._loo_value(alpha[b], d[b])
+                continue
+            bad = np.flatnonzero(~(np.isfinite(d[b]) & (d[b] > 0)))
+            try:
+                if bad.size:  # the single call's check, raised there by the solver
+                    raise ValueError("leave-one-out: diag(K^-1) at point {0} is {1:g}, not a finite positive "
+                                     "number".format(bad[0], d[b, bad[0]]))
+                dmu = None
+                if n_mean:
+                    dmu = self._swap_eval(self.mean, full[b, :full_mean], lambda: self._call_mean_gradient(self._x))
+            except ValueError:
+                if quiet:
+                    continue
+                raise
+            pos = 0
+            if n_mean:
+                out[b, pos:pos + n_mean] = np.dot(dmu, beta[b])
+                pos += n_mean
+            if n_wn:
+                wn, dwn = self._swap_eval(self.white_noise, full[b, full_mean:full_mean + full_wn],
+                                          lambda: (self._call_white_noise(self._x),
+                                                   self._call_white_noise_gradient(self._x)))
+                out[b, pos:pos + n_wn] = np.sum((np.exp(wn) * diag[b])[None, :] * dwn, axis=1)
+                pos += n_wn
+            if n_k:
+                out[b, pos:pos + n_k] = g[b][mask]
+            value[b] = self._loo_value(alpha[b], d[b])
+        if not grad:
+            return value
+        return (value, out) if return_value else out
+
     def batch_grad_log_likelihood(self, vectors, y, quiet=False, return_log_likelihood=False):
         """:func:`grad_log_likelihood` at many parameter vectors: row ``b`` of the ``(B, len(gp))`` result is bit for
         bit what ``gp.set_parameter_vector(vectors[b]); gp.grad_log_likelihood(y, quiet=quiet)`` returns on the

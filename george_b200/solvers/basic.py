@@ -369,6 +369,33 @@ class BasicSolver(object):
         return log_det, quad, alpha, g, diag, info
 
     @staticmethod
+    def batch_loo_terms(spec, params, x, yerr, r, which=None):
+        """``(alpha, d, info)``, or with ``which`` (``(P,)``, shared by all members) ``(alpha, d, beta, g, diag,
+        info)``, for ``B`` parameter vectors of one kernel program on the same ``x``: member ``b`` factorises as in
+        :func:`batch_log_likelihood` and returns what :func:`loo_terms` returns for it, every array but ``g`` (``(B,
+        P)``) ``(B, n)`` (``include/bgp.h: bgp_dense_batch_loo_terms``).  ``info`` is that of
+        :func:`batch_log_likelihood`; a failed member's rows are NaN.  A member's outputs are bit-identical to
+        :func:`compute` with its spec and yerr followed by :func:`loo_terms`, with one difference: a ``d`` that is not
+        finite and positive raises nothing here (the member's gradient rows are what that arithmetic gives), so the
+        caller checks it.  With ``which``, more than 64 kernel parameters raise ``ValueError`` before anything is
+        solved."""
+        x, _, params, yerr, r, which = _batch_inputs(spec, params, x, yerr, r, which=which)
+        nb, n, npar = params.shape[0], x.shape[0], params.shape[1]
+        alpha = np.empty((nb, n), dtype=np.float64)
+        d = np.empty((nb, n), dtype=np.float64)
+        info = np.zeros(nb, dtype=np.int32)
+        if which is None:
+            _batch_call("bgp_dense_batch_loo_terms", spec, params, x, yerr, r, None, _lib.ptr(alpha), _lib.ptr(d), None,
+                        None, None, _lib.ptr(info))
+            return alpha, d, info
+        beta = np.empty((nb, n), dtype=np.float64)
+        g = np.empty((nb, npar), dtype=np.float64)
+        diag = np.empty((nb, n), dtype=np.float64)
+        _batch_call("bgp_dense_batch_loo_terms", spec, params, x, yerr, r, _lib.ptr(which), _lib.ptr(alpha),
+                    _lib.ptr(d), _lib.ptr(beta), _lib.ptr(g), _lib.ptr(diag), _lib.ptr(info))
+        return alpha, d, beta, g, diag, info
+
+    @staticmethod
     def batch_predict(spec, params, x, yerr, r, xs, what):
         """``(mean, out, info)`` for ``B`` parameter vectors of one kernel program on the same ``x``: member ``b``
         factorises as in :func:`batch_log_likelihood`, ``mean[b] = K_b(xs, x) K_b^-1 r[b]`` (``(B, ns)``, the kernel

@@ -18,12 +18,13 @@ __all__ = ["HODLRSolver"]
 class HODLRSolver(BasicSolver):
 
     # no batched HODLR factorisation: GP.batch_log_likelihood, GP.batch_predict, GP.batch_grad_log_likelihood,
-    # GP.batch_sample_conditional and GP.batch_grad_predict take their per-vector loops
+    # GP.batch_sample_conditional, GP.batch_grad_predict and the GP.batch_*loo* methods take their per-vector loops
     batch_log_likelihood = None
     batch_predict = None
     batch_grad_terms = None
     batch_sample = None
     batch_predict_grad = None
+    batch_loo_terms = None
 
     def __init__(self, kernel, min_size=100, tol=0.1, seed=42, rng_mode=None, rank_capacity=0,
                  exhaust="dense"):

@@ -339,6 +339,37 @@ int bgp_dense_batch_grad_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* sp
                                double* alpha, double* diag,              /* B x n, may be NULL       */
                                double* g,                                /* B x P, may be NULL       */
                                int32_t* info);                           /* B                        */
+/* Batched leave-one-out terms (GP.batch_loo_predict, GP.batch_loo_log_likelihood, GP.batch_grad_loo_log_likelihood):
+ * for the same B members as bgp_dense_batch_log_likelihood (spec, params, x, yerr; r = y - mean(x) per member, B x n
+ * row-major), what bgp_dense_loo_terms returns for each member:
+ *   alpha[b*n + i]   (K_b^-1 r_b)_i                    d[b*n + i]      (K_b^-1)_ii                         (pass 1)
+ *   beta[b*n + i]    (K_b^-1 (alpha_b / d_b))_i        g[b*P + p]      sum_ij A_b,ij dK_b,ij/dtheta_p      (pass 2)
+ *   diag[b*n + i]    A_b,ii
+ * with A_b and c_b as in bgp_dense_loo_terms.  which == NULL runs pass 1 only, with no parameter limit; beta, g and
+ * diag may then be NULL.  which != NULL (P entries, shared by all members) runs pass 2 for every member; any output
+ * but info may be NULL.  Each member's outputs are bit-identical to bgp_dense_compute followed by bgp_dense_loo_terms
+ * on member b's spec and yerr: the same kernels run with a member index (K_b^-1 by solving against the identity,
+ * through the few-column solve when n <= 8; the G^T G product with the single call's split-K plan; the same contraction
+ * tiles and fixed reduction order), so a member's results do not depend on B, its position or the chunking.
+ * info[b] as in bgp_dense_batch_log_likelihood (0, the leading-minor index, or -1 for an invalid member program); a
+ * failed member's outputs are NaN and do not disturb the other members.  Unlike bgp_dense_loo_terms nothing checks d on
+ * the host between the passes: a member whose d is not finite and positive is not an error, its pass-2 rows are what
+ * that arithmetic gives, and the caller checks d (GP does, raising the single call's ValueError).
+ * Members run in chunks that fit in 4 GiB of device memory (BGP_BATCH_CHUNK=<members> overrides it), capped so that
+ * the split-K product is one launch; every step of a chunk is one launch for all its members, with no host work in
+ * between, so the launch count depends on n and the number of chunks, never on B within a chunk.
+ * Device workspace per member (doubles): 2 n^2 (factor and K^-1) + (4 + t) n (t = n for n <= 8, else 1); pass 2 adds
+ * n^2 (A) + nsplit n^2 (the product's split-K slices, none when nsplit = 1: 2 n^2 at n = 512, none from n = 2049 on a
+ * 132-SM H100 SXM) + 2 n (beta, c) + ceil(n / 32)^2 P contraction partials + P.  Shared: B programs, x, which.
+ * Errors: those of bgp_dense_batch_log_likelihood; BGP_ERR_INVALID for P > 64 when which != NULL, before anything is
+ * launched; BGP_ERR_NOMEM when a single member does not fit.  B == 0 writes nothing. */
+int bgp_dense_batch_loo_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params,
+                              int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
+                              const double* yerr, const double* r,     /* B x n row-major             */
+                              const uint32_t* which,                   /* P, or NULL for pass 1 only  */
+                              double* alpha, double* d,                /* B x n, may be NULL          */
+                              double* beta, double* g, double* diag,   /* B x n, B x P, B x n, or NULL */
+                              int32_t* info);                          /* B                           */
 /* Batched predictions (GP.batch_predict): for the same B members as bgp_dense_batch_log_likelihood (spec, params, x,
  * yerr; r = y - mean(x) per member, B x n row-major) and the test points xs (ns x ndim row-major, host):
  *   mean[b*ns + j]        = (K_b(x*, x) K_b^-1 r_b)_j            (the kernel part of GP.predict's mean)

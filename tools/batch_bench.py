@@ -1,7 +1,8 @@
 # -*- coding: utf-8 -*-
 """The GP.batch_* methods against the per-vector loops they replace (set_parameter_vector, then the one-vector method).
 
-    python tools/batch_bench.py --entry {log_likelihood,grad,predict,grad_predict,sample} [--workload co2|matern52_3d]
+    python tools/batch_bench.py --entry {log_likelihood,grad,predict,grad_predict,sample,loo}
+        [--workload co2|matern52_3d]
         [--min-seconds 1.0] [--cpu-members 4] [--kind mean|var|cov] [--rounds 7] [--reps 5]
 
 One JSON line per shape.  Every line has
@@ -24,6 +25,11 @@ and the fields of its entry:
   sample          GP.batch_sample_conditional(rng=g) against sample_conditional(rng=g): loop_ms / batch_ms (median
                   host-clock time of one call over --reps alternating repetitions), loop_spread / batch_spread (min,
                   max), speedup and bit_equal (the draws and the generators' final states are equal)
+  loo             GP.batch_loo_predict, batch_loo_log_likelihood(quiet=True) and
+                  batch_grad_loo_log_likelihood(quiet=True, return_value=True) against loo_predict,
+                  loo_log_likelihood and grad_loo_log_likelihood, per method: loop_ms_per_member and
+                  batch_ms_per_member (host-clock medians over --rounds alternating rounds), loop_spread / batch_spread
+                  (min, max per member), speedup and equal (the outputs are bit-identical in every round)
 Workloads: the CO2 GP of the hyper-parameter tutorial (a sum of four kernel products, fitted mean and white noise) and
 Matern-5/2 3-D (the Bayesian-optimisation case), at the sizes listed in each entry's table below: the sizes a sampler's
 step, a posterior-predictive pass or an acquisition optimiser's step uses.  Every shape is warmed up first, through
@@ -142,7 +148,8 @@ def _timed_hook(name):
     return staticmethod(hook)
 
 
-for _name in ("batch_log_likelihood", "batch_grad_terms", "batch_predict", "batch_predict_grad", "batch_sample"):
+for _name in ("batch_log_likelihood", "batch_grad_terms", "batch_predict", "batch_predict_grad", "batch_sample",
+              "batch_loo_terms"):
     setattr(TimedSolver, _name, _timed_hook(_name))
 
 
@@ -349,8 +356,54 @@ def bench_sample(args, emit):
                   "speedup": round(med["loop"] / med["batch"], 2), "bit_equal": equal})
 
 
+def bench_loo(args, emit):
+    """CO2 at n = 512 with B in {8, 64}; Matern-5/2 3-D at n = 1024 and n = 4096 with B = 32."""
+    methods = [
+        ("predict", lambda gp, v, y: gp.batch_loo_predict(v, y), lambda gp, y: gp.loo_predict(y)),
+        ("value", lambda gp, v, y: gp.batch_loo_log_likelihood(v, y, quiet=True),
+         lambda gp, y: gp.loo_log_likelihood(y, quiet=True)),
+        ("grad", lambda gp, v, y: gp.batch_grad_loo_log_likelihood(v, y, quiet=True, return_value=True),
+         lambda gp, y: gp.grad_loo_log_likelihood(y, quiet=True, return_value=True)),
+    ]
+    work = [("co2", 512, [8, 64]), ("matern52_3d", 1024, [32]), ("matern52_3d", 4096, [32])]
+    for name, n, sizes in work:
+        if args.workload not in (None, name):
+            continue
+        gp, y, scale, _ = MODELS[name](n)
+        gp.log_likelihood(y)
+        rng = np.random.default_rng(n)
+        for nb in sizes:
+            vecs = vectors(gp, scale, nb, rng)
+            for method, batch_fn, one_fn in methods:
+                def one():
+                    res = loop(gp, vecs, lambda: one_fn(gp, y))
+                    if isinstance(res[0], tuple):
+                        return tuple(np.stack([r[k] for r in res]) for k in range(len(res[0])))
+                    return np.array(res)
+                batch = lambda: batch_fn(gp, vecs, y)  # noqa: E731
+
+                def same(a, b):
+                    a, b = (a, b) if isinstance(a, tuple) else ((a,), (b,))
+                    return all(np.array_equal(u, w) for u, w in zip(a, b))
+                want = one()  # warm-up of this shape (workspace, code paths) for both routes
+                equal = same(batch(), want)
+                t_loop, t_batch = [], []
+                for _ in range(args.rounds):  # alternate the two routes
+                    for fn, ts in ((one, t_loop), (batch, t_batch)):
+                        dt, out = timed(fn)
+                        ts.append(dt * 1e3 / nb)
+                        equal = equal and same(out, want)
+                ml, mb = float(np.median(t_loop)), float(np.median(t_batch))
+                emit({"workload": name, "n": n, "B": nb, "method": method,
+                      "loop_ms_per_member": round(ml, 4), "batch_ms_per_member": round(mb, 4),
+                      "loop_spread": [round(min(t_loop), 4), round(max(t_loop), 4)],
+                      "batch_spread": [round(min(t_batch), 4), round(max(t_batch), 4)],
+                      "batch_device_ms_per_member": round(device_ms(gp, batch) / nb, 4),
+                      "speedup": round(ml / mb, 2), "equal": bool(equal)})
+
+
 ENTRIES = {"log_likelihood": bench_log_likelihood, "grad": bench_grad, "predict": bench_predict,
-           "grad_predict": bench_grad_predict, "sample": bench_sample}
+           "grad_predict": bench_grad_predict, "sample": bench_sample, "loo": bench_loo}
 
 
 def main():
@@ -360,7 +413,7 @@ def main():
     ap.add_argument("--min-seconds", type=float, default=1.0, help="log_likelihood, grad, predict: per timing")
     ap.add_argument("--cpu-members", type=int, default=4, help="log_likelihood: members of the CPU route")
     ap.add_argument("--kind", choices=["mean", "var", "cov"], default=None, help="predict: only this kind")
-    ap.add_argument("--rounds", type=int, default=7, help="grad_predict: alternating rounds")
+    ap.add_argument("--rounds", type=int, default=7, help="grad_predict, loo: alternating rounds")
     ap.add_argument("--reps", type=int, default=5, help="sample: alternating repetitions")
     args = ap.parse_args()
     assert george._lib.load().bgp_device_count() > 0, "no device: this benchmark measures the H100 path"
