@@ -414,31 +414,50 @@ class GP(ModelSet):
         return spec, full, kpar, sigma, resid, fact_err, mean_err
 
     @staticmethod
-    def _batch_factor_error(spec, kpar, b, err, info):
-        """The exception member ``b``'s factorisation raises on the per-vector path (``err``: the white-noise one),
-        from the batch's ``info``; ``None`` when it succeeds."""
-        if err is not None or info == 0:
-            return err
-        if info > 0:
-            return LinAlgError("%d-th leading minor of the array is not positive definite" % info)
-        member = patch_specs(spec, kpar[b:b + 1])[0]
-        try:
-            _lib.check(_lib.load().bgp_spec_validate(C.byref(member)))
-        except Exception as e:
-            return e
-        return ValueError("invalid kernel")
+    def _member_error(spec, kpar, b, info, fact_err, *later):
+        """The exception member ``b`` meets first on the per-vector path, or ``None``: the white noise
+        (``fact_err[b]``) or the factorisation (from the batch's ``info[b]``), then the first of ``later`` (per-member
+        lists of an exception or ``None``, in the loop's order)."""
+        exc = fact_err[b]
+        if exc is None and info[b] > 0:
+            exc = LinAlgError("%d-th leading minor of the array is not positive definite" % info[b])
+        elif exc is None and info[b] < 0:
+            member = patch_specs(spec, kpar[b:b + 1])[0]
+            try:
+                _lib.check(_lib.load().bgp_spec_validate(C.byref(member)))
+            except Exception as e:
+                exc = e
+            else:
+                exc = ValueError("invalid kernel")
+        for errs in later:
+            if exc is None:
+                exc = errs[b]
+        return exc
 
     def _raise_member_error(self, spec, kpar, info, fact_err, *later):
-        """Raise the exception the per-vector loop meets first, member by member: the white noise or the
-        factorisation (``fact_err``, ``info``), then the first of ``later`` (per-member lists of an exception or
-        ``None``, in the loop's order)."""
+        """Raise the exception the per-vector loop meets first, member by member (:func:`_member_error`)."""
         for b in range(len(info)):
-            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
-            for errs in later:
-                if exc is None:
-                    exc = errs[b]
+            exc = self._member_error(spec, kpar, b, info, fact_err, *later)
             if exc is not None:
                 raise exc
+
+    def _member_failed(self, spec, kpar, b, info, fact_err, mean_err, quiet, any_value_error):
+        """Whether member ``b`` fails in the white noise, the factorisation or the residual, the first stages of the
+        value and gradient paths.  The failure is raised unless ``quiet`` absorbs it as the single calls do: a
+        ``ValueError`` or ``LinAlgError`` of the white noise or the factorisation (``recompute``), and a ``ValueError``
+        of the residual, any one when ``any_value_error`` (the gradients) or only the mean function's own (the values,
+        which let the solver's non-finite right-hand side through)."""
+        exc = self._member_error(spec, kpar, b, info, fact_err)
+        if exc is not None:
+            absorbed = quiet and isinstance(exc, (ValueError, LinAlgError))
+        else:
+            exc = mean_err[b]
+            if exc is None:
+                return False
+            absorbed = quiet and isinstance(exc, ValueError) and (any_value_error or "mean function" in str(exc))
+        if absorbed:
+            return True
+        raise exc
 
     def _batch_ll(self, log_det, quad):
         """GP.compute / GP.log_likelihood over the members, in the same order of operations."""
@@ -458,17 +477,8 @@ class GP(ModelSet):
         log_det, quad, info = batch(spec, kpar, self._x, sigma, resid)
         ll = self._batch_ll(log_det, quad)
         for b in range(len(vectors)):
-            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
-            if exc is not None:
+            if self._member_failed(spec, kpar, b, info, fact_err, mean_err, quiet, False):
                 ll[b] = -np.inf
-                if not (quiet and isinstance(exc, (ValueError, LinAlgError))):
-                    raise exc
-                continue
-            exc = mean_err[b]
-            if exc is not None:
-                ll[b] = -np.inf
-                if not (quiet and isinstance(exc, ValueError) and "mean function" in str(exc)):
-                    raise exc
         return ll
 
     def batch_predict(self, vectors, y, t, return_cov=True, return_var=False, kernel=None):
@@ -552,13 +562,14 @@ class GP(ModelSet):
         nothing = np.zeros(len(self), dtype=np.float64)
         if not self.recompute(quiet=quiet):
             return nothing
-        n_wn, n_k, n_mean = len(self.white_noise), len(self.kernel), len(self.mean)
+        layout = n_mean, n_wn, n_k = self._grad_layout()
+        mask = self.kernel.unfrozen_mask
+        gk = diagA = dmu = None
         fused = getattr(self.solver, "grad_terms", None) if (n_wn or n_k) else None
         try:
             if fused is not None:
                 # alpha, the kernel-gradient contraction and diag(alpha alpha^T - K^-1) in one device pass: neither
                 # K^-1 nor the (N, N, P) gradient tensor visits the host (reference gp.py:437-466 forms both)
-                mask = self.kernel.unfrozen_mask
                 terms = fused(self._residual(y), mask.astype(np.uint32))
                 if terms is None:
                     fused = None
@@ -574,9 +585,6 @@ class GP(ModelSet):
         if fused is None and (n_wn or n_k):
             A = np.outer(alpha, alpha) - self.solver.get_inverse()
             diagA = np.diag(A)
-
-        grad = np.empty(len(self))
-        pos = 0
         if n_mean:
             try:
                 dmu = self._call_mean_gradient(self._x)
@@ -584,22 +592,49 @@ class GP(ModelSet):
                 if quiet:
                     return nothing
                 raise
-            grad[pos:pos + n_mean] = np.dot(dmu, alpha)
+        if fused is None and n_k:
+            # plug-in solvers without grad_terms: K^-1 comes from the solver, the contraction still runs on the
+            # device without the (N, N, P) tensor
+            gk = self.kernel.kernel.gradient_contract(mask.astype(np.uint32), self._x, A)
+        return self._grad_row(np.empty(len(self)), layout, dmu, alpha, self._white_noise_terms, diagA, gk, mask, 0.5)
+
+    def _white_noise_terms(self):
+        """``(wn, dwn)``: the white-noise model and its gradient at the computed coordinates."""
+        return self._call_white_noise(self._x), self._call_white_noise_gradient(self._x)
+
+    def _grad_layout(self):
+        """``(n_mean, n_wn, n_k)``, the active parameters of each part of a gradient; once per call, outside the
+        batches' member loops, as a kernel's size takes tens of microseconds to count."""
+        return len(self.mean), len(self.white_noise), len(self.kernel)
+
+    def _grad_row(self, grad, layout, dmu, w, noise, diagA, gk, mask, scale):
+        """Fill and return ``grad`` (``(len(gp),)``) in :func:`grad_log_likelihood`'s layout (mean, white noise,
+        kernel; frozen parameters left out, ``layout`` from :func:`_grad_layout`): ``dmu . w``,
+        ``scale * sum_i exp(wn_i) diagA_i dwn_i`` and ``scale * gk[mask]``, with ``(wn, dwn) = noise()`` called only
+        when white-noise parameters are active.  ``scale`` is 1/2 for the marginal likelihood and 1 for the
+        leave-one-out log-likelihood (``1.0 * x`` is ``x`` bit for bit)."""
+        n_mean, n_wn, n_k = layout
+        pos = 0
+        if n_mean:
+            grad[pos:pos + n_mean] = np.dot(dmu, w)
             pos += n_mean
         if n_wn:
-            wn = self._call_white_noise(self._x)
-            dwn = self._call_white_noise_gradient(self._x)
-            grad[pos:pos + n_wn] = 0.5 * np.sum((np.exp(wn) * diagA)[None, :] * dwn, axis=1)
+            wn, dwn = noise()
+            grad[pos:pos + n_wn] = np.sum((np.exp(wn) * diagA)[None, :] * dwn, axis=1)
             pos += n_wn
         if n_k:
-            if fused is not None:
-                grad[pos:pos + n_k] = 0.5 * gk[mask]
-            else:
-                # plug-in solvers without grad_terms: K^-1 comes from the solver, the contraction still runs on the
-                # device without the (N, N, P) tensor
-                mask = self.kernel.unfrozen_mask
-                grad[pos:pos + n_k] = 0.5 * self.kernel.kernel.gradient_contract(mask.astype(np.uint32), self._x, A)[mask]
+            grad[pos:pos + n_k] = gk[mask]
+        grad[n_mean:] *= scale
         return grad
+
+    def _member_gradients(self, layout, full):
+        """The mean gradient (``None`` without active mean parameters) of the member whose full parameter vector is
+        ``full``, and the ``noise`` of :func:`_grad_row` for that member; both evaluate the models with ``full`` set."""
+        n_mean, n_wn = self.mean.full_size, self.white_noise.full_size
+        dmu = None
+        if layout[0]:
+            dmu = self._swap_eval(self.mean, full[:n_mean], lambda: self._call_mean_gradient(self._x))
+        return dmu, lambda: self._swap_eval(self.white_noise, full[n_mean:n_mean + n_wn], self._white_noise_terms)
 
     # -- leave-one-out cross-validation (Rasmussen & Williams, GPML §5.4.2, eqs. 5.10-5.13) ---------------------------
     def loo_predict(self, y):
@@ -653,29 +688,17 @@ class GP(ModelSet):
         fail = (-np.inf, nothing) if return_value else nothing
         if not self.recompute(quiet=quiet):
             return fail
-        n_wn, n_k, n_mean = len(self.white_noise), len(self.kernel), len(self.mean)
+        layout = self._grad_layout()
         mask = self.kernel.unfrozen_mask
         try:
             r = self._residual_of(y)
             alpha, d, beta, gk, diagA = self._loo_terms(r, mask.astype(np.uint32))
-            dmu = self._call_mean_gradient(self._x) if n_mean else None
+            dmu = self._call_mean_gradient(self._x) if layout[0] else None
         except ValueError:
             if quiet:
                 return fail
             raise
-
-        grad = np.empty(len(self))
-        pos = 0
-        if n_mean:
-            grad[pos:pos + n_mean] = np.dot(dmu, beta)
-            pos += n_mean
-        if n_wn:
-            wn = self._call_white_noise(self._x)
-            dwn = self._call_white_noise_gradient(self._x)
-            grad[pos:pos + n_wn] = np.sum((np.exp(wn) * diagA)[None, :] * dwn, axis=1)
-            pos += n_wn
-        if n_k:
-            grad[pos:pos + n_k] = gk[mask]
+        grad = self._grad_row(np.empty(len(self)), layout, dmu, beta, self._white_noise_terms, diagA, gk, mask, 1.0)
         return (self._loo_value(alpha, d), grad) if return_value else grad
 
     @staticmethod
@@ -806,21 +829,11 @@ class GP(ModelSet):
         else:
             alpha, d, info = batch(spec, kpar, self._x, sigma, resid)
         # GP.loo_log_likelihood / GP.grad_loo_log_likelihood member by member, with their operations
-        n_mean, n_wn, n_k = len(self.mean), len(self.white_noise), len(self.kernel)
-        full_mean, full_wn = self.mean.full_size, self.white_noise.full_size
+        layout = self._grad_layout()
         value = np.full(nb, -np.inf)
         out = np.zeros((nb, len(self)), dtype=np.float64)
         for b in range(nb):  # the loop's order: factorisation (white noise included), residual, d, mean gradient
-            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
-            if exc is not None:
-                if not (quiet and isinstance(exc, (ValueError, LinAlgError))):
-                    raise exc
-                continue
-            exc = mean_err[b]
-            if exc is not None:
-                # loo_log_likelihood swallows only the mean's own ValueError under quiet, the gradient any ValueError
-                if not (quiet and isinstance(exc, ValueError) and (grad or "mean function" in str(exc))):
-                    raise exc
+            if self._member_failed(spec, kpar, b, info, fact_err, mean_err, quiet, grad):
                 continue
             if not grad:
                 value[b] = self._loo_value(alpha[b], d[b])
@@ -830,25 +843,12 @@ class GP(ModelSet):
                 if bad.size:  # the single call's check, raised there by the solver
                     raise ValueError("leave-one-out: diag(K^-1) at point {0} is {1:g}, not a finite positive "
                                      "number".format(bad[0], d[b, bad[0]]))
-                dmu = None
-                if n_mean:
-                    dmu = self._swap_eval(self.mean, full[b, :full_mean], lambda: self._call_mean_gradient(self._x))
+                dmu, noise = self._member_gradients(layout, full[b])
             except ValueError:
                 if quiet:
                     continue
                 raise
-            pos = 0
-            if n_mean:
-                out[b, pos:pos + n_mean] = np.dot(dmu, beta[b])
-                pos += n_mean
-            if n_wn:
-                wn, dwn = self._swap_eval(self.white_noise, full[b, full_mean:full_mean + full_wn],
-                                          lambda: (self._call_white_noise(self._x),
-                                                   self._call_white_noise_gradient(self._x)))
-                out[b, pos:pos + n_wn] = np.sum((np.exp(wn) * diag[b])[None, :] * dwn, axis=1)
-                pos += n_wn
-            if n_k:
-                out[b, pos:pos + n_k] = g[b][mask]
+            self._grad_row(out[b], layout, dmu, beta[b], noise, diag[b], g[b], mask, 1.0)
             value[b] = self._loo_value(alpha[b], d[b])
         if not grad:
             return value
@@ -902,41 +902,20 @@ class GP(ModelSet):
         log_det, quad, alpha, g, diag, info = batch(spec, kpar, self._x, sigma, resid, mask.astype(np.uint32))
         ll = self._batch_ll(log_det, quad)
         # GP.grad_log_likelihood member by member, with its operations
-        n_mean, n_wn, n_k = len(self.mean), len(self.white_noise), len(self.kernel)
-        full_mean, full_wn = self.mean.full_size, self.white_noise.full_size
+        layout = self._grad_layout()
         grad = np.zeros((nb, len(self)), dtype=np.float64)
         for b in range(nb):  # the loop's order: factorisation (white noise included), residual, mean gradient
-            exc = self._batch_factor_error(spec, kpar, b, fact_err[b], info[b])
-            if exc is not None:
-                if not (quiet and isinstance(exc, (ValueError, LinAlgError))):
-                    raise exc
+            # (with the value, the loop's log_likelihood comes first and lets a residual ValueError through)
+            if self._member_failed(spec, kpar, b, info, fact_err, mean_err, quiet, not return_ll):
                 ll[b] = -np.inf
                 continue
-            exc = mean_err[b]
-            if exc is not None:
-                # log_likelihood swallows only the mean's own ValueError under quiet, grad_log_likelihood any ValueError
-                if not (quiet and isinstance(exc, ValueError) and (not return_ll or "mean function" in str(exc))):
-                    raise exc
-                ll[b] = -np.inf
-                continue
-            pos = 0
-            if n_mean:
-                try:
-                    dmu = self._swap_eval(self.mean, full[b, :full_mean], lambda: self._call_mean_gradient(self._x))
-                except ValueError:
-                    if quiet:
-                        continue
-                    raise
-                grad[b, pos:pos + n_mean] = np.dot(dmu, alpha[b])
-                pos += n_mean
-            if n_wn:
-                wn, dwn = self._swap_eval(self.white_noise, full[b, full_mean:full_mean + full_wn],
-                                          lambda: (self._call_white_noise(self._x),
-                                                   self._call_white_noise_gradient(self._x)))
-                grad[b, pos:pos + n_wn] = 0.5 * np.sum((np.exp(wn) * diag[b])[None, :] * dwn, axis=1)
-                pos += n_wn
-            if n_k:
-                grad[b, pos:pos + n_k] = 0.5 * g[b][mask]
+            try:
+                dmu, noise = self._member_gradients(layout, full[b])
+            except ValueError:
+                if quiet:
+                    continue
+                raise
+            self._grad_row(grad[b], layout, dmu, alpha[b], noise, diag[b], g[b], mask, 0.5)
         return ll, grad
 
     def grad_lnlikelihood(self, y, quiet=False):
