@@ -69,6 +69,9 @@ SIGNATURES = {
     "bgp_dense_grad_terms": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_grad_terms": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_grad_terms_local_dev": (C.c_int, [_p, _p, _p, _p, _p]),
+    "bgp_dense_grad_x_terms": (C.c_int, [_p, _p, _p, _p, _p, _p, _p]),
+    "bgp_hodlr_grad_x_terms": (C.c_int, [_p, _p, _p, _p, _p, _p, _p]),
+    "bgp_hodlr_grad_x_terms_local_dev": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "bgp_dense_loo_terms": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_loo_terms": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p]),
     "bgp_dense_predict": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),

@@ -28,6 +28,8 @@ int kmat_grad_contract_members(const DevProgram* dprogs, int np, const unsigned*
                                double ca, double cm, double* g_dev, int64_t gstride, double* diag_dev, int64_t dstride,
                                int members, DevBuf<double>& scratch, cudaStream_t s);
 int fill_identity_launch(double* A, int64_t n, cudaStream_t s);
+int grad_x_resident_launch(const DevProgram& P, const DevProgram* dprog, const double* x, int64_t n, double* Kinv,
+                           const double* alpha, double* dx_dev, DevBuf<double>& scratch, cudaStream_t s);
 int loo_weights_launch(const double* alpha, const double* d, int64_t n, double* q, double* c, cudaStream_t s);
 int scale_rows_launch(double* X, int64_t n, int64_t ncols, int64_t ldx, const double* w, bool sqrt_w, cudaStream_t s);
 int slab_diag_launch(const double* W, int64_t ldw, int64_t j0, int64_t nc, double* d, cudaStream_t s);
@@ -511,6 +513,7 @@ struct bgp_dense {
   DevBuf<unsigned> d_which;
   bool has_inputs = false;           // d_x / d_prog describe the factor in d_A (false after import_factor)
   int ndim = 0, n_params = 0;
+  DevProgram prog;                   // host copy of d_prog (its shape selects the x-gradient evaluator)
   DevBuf<int> d_info;
   DevBuf<GemmDesc> d_gdesc;
   double t_ms[2] = {0, 0};
@@ -811,6 +814,7 @@ int bgp_dense_compute(bgp_dense_t* h, const bgp_kernel_spec_t* spec, const doubl
   h->has_inputs = false;
   h->ndim = ndim;
   h->n_params = P.n_params_total;
+  h->prog = P;
   BGP_TRY(upload_program(P, h->d_prog, s));
   BGP_TRY(h->d_x.reserve((size_t)n * ndim, s));
   BGP_TRY(h->d_yerr.reserve((size_t)n, s));
@@ -920,13 +924,18 @@ int bgp_dense_get_inverse(bgp_dense_t* h, double* out) {
   return bgp_dense_apply_inverse(h, out, n, n);
 }
 
-int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
-                         double* diag_out) {
+// With xgrad (bgp_dense_grad_x_terms) the call also forms dx (n x ndim, row-major) from the resident K^-1 after the
+// contraction: grad_x_resident_launch turns it into alpha alpha^T - K^-1 and runs the x-gradient matvec over it.  A NULL
+// `which` then skips the parameter contraction.
+static int dense_grad_terms_impl(bgp_dense* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
+                                 double* diag_out, bool xgrad, double* dx_out) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
   if (!h->has_inputs) { set_error("the factor was imported: the handle holds no kernel/coordinates"); return BGP_ERR_NOT_COMPUTED; }
   const int64_t n = h->n;
-  const int np = h->n_params;
+  const int np = (xgrad && !which) ? 0 : h->n_params;
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  const int nd = h->ndim;
+  if (xgrad && nd > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, nd); return BGP_ERR_INVALID; }
   cudaStream_t s = h->s;
   BGP_TRY(h->d_rhs.reserve((size_t)n * 2 + 64, s));
   double* alpha = h->d_rhs.p;
@@ -943,10 +952,26 @@ int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r,
   // kernel term of gp.py:457-466 and diag(alpha alpha^T - K^-1) for the white-noise term of gp.py:452-456
   BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, alpha, 1.0, -1.0, dg,
                                     diag_out ? ddiag : nullptr, h->d_gscratch, s));
+  DevBuf<double> ddx;
+  if (xgrad) {
+    BGP_TRY(ddx.alloc((size_t)n * nd, s));
+    BGP_TRY(grad_x_resident_launch(h->prog, h->d_prog.p, h->d_x.p, n, h->d_inv.p, alpha, ddx.p, h->d_gscratch, s));
+  }
   if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
   if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  if (xgrad && dx_out) BGP_CUDA(cudaMemcpyAsync(dx_out, ddx.p, sizeof(double) * n * nd, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));
   return BGP_OK;
+}
+
+int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
+                         double* diag_out) {
+  return dense_grad_terms_impl(h, which, r, alpha_out, g_out, diag_out, false, nullptr);
+}
+
+int bgp_dense_grad_x_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
+                           double* diag_out, double* dx_out) {
+  return dense_grad_terms_impl(h, which, r, alpha_out, g_out, diag_out, true, dx_out);
 }
 
 int bgp_dense_loo_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* d_out,

@@ -39,6 +39,13 @@ int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigne
                           const double* W, int64_t j0, int64_t nc, int64_t jlo, int64_t jhi, const double* u,
                           const double* v, double* partial, double* tile_part, double* diag_dev, cudaStream_t s);
 int kmat_grad_slab_finish(int np, int64_t jlo, int64_t jhi, const double* tile_part, double* g_dev, cudaStream_t s);
+int64_t grad_slab_x_partial_size(int64_t n, int64_t c, int nd);
+int kmat_grad_x_slab_launch(const DevProgram* dprog, int shape, int nd, int np, const unsigned* which_dev,
+                            const double* x, int64_t n, const double* W, int64_t j0, int64_t nc, int64_t jlo,
+                            int64_t jhi, const double* alpha, double* partial, double* tile_part, double* xpart,
+                            double* diag_dev, double* dx_dev, cudaStream_t s);
+int grad_x_resident_launch(const DevProgram& P, const DevProgram* dprog, const double* x, int64_t n, double* Kinv,
+                           const double* alpha, double* dx_dev, DevBuf<double>& scratch, cudaStream_t s);
 int kmat_symmetric_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x, int64_t n,
                                const double* diag_add, double* out, int64_t ld, cudaStream_t s);
 int kmat_general_launch_auto(const DevProgram& P, const DevProgram* dprog, const double* x1, int64_t n1, const double* x2,
@@ -1066,6 +1073,28 @@ static int exchange_rows(bgp_hodlr* h, double* P, int64_t ld, int64_t cols, cuda
   return BGP_OK;
 }
 
+// exchange_rows for an n x cols ROW-major matrix P (dx of bgp_hodlr_grad_x_terms): through a column-major copy
+__global__ void transpose_rows_kernel(const double* __restrict__ src, int64_t rows, int64_t cols, double* __restrict__ dst) {
+  const int64_t total = rows * cols;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t i = t / cols, q = t - i * cols;
+    dst[q * rows + i] = src[t];
+  }
+}
+static int exchange_rows_wide(bgp_hodlr* h, double* P, int64_t cols, cudaStream_t s) {
+  if (cols == 1) return exchange_rows(h, P, h->n, 1, s);
+  const int64_t n = h->n, total = n * cols;
+  const unsigned blocks = (unsigned)std::min<int64_t>((total + 255) / 256, 1184);
+  DevBuf<double> colmajor;
+  BGP_TRY(colmajor.alloc((size_t)total, s));
+  transpose_rows_kernel<<<blocks, 256, 0, s>>>(P, n, cols, colmajor.p);
+  BGP_LAUNCH_CHECK();
+  BGP_TRY(exchange_rows(h, colmajor.p, n, cols, s));
+  transpose_rows_kernel<<<blocks, 256, 0, s>>>(colmajor.p, cols, n, P);  // column-major n x cols = row-major cols x n
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
 // [*first, *last): the items 0 .. count-1, whose row intervals [start(k), start(k) + size(k)) are disjoint and ordered
 // by start, that meet rows [lo, hi)
 template <class StartSize>
@@ -1384,18 +1413,23 @@ static float event_ms(cudaEvent_t a, cudaEvent_t b) {
 // Slabs of c columns start at the global multiple of 64 at or below row0; the identity is placed in J only, each slab is
 // solved with the row-restricted solve and contracted over the window J, and the per-tile partials of the tiles meeting
 // J are summed in order.  alpha: the full n-vector K^-1 r; d_which holds which[0 .. np).  Issues no collective.
+// ddx (may be NULL): each slab also contracts the input gradient of its columns in the same pass
+// (kmat_grad_x_slab_launch), ddx[j * ndim + q] for j in J only; g and ddiag keep their bits.
 static int grad_stream_own_columns(bgp_hodlr* h, int np, const double* alpha, int64_t c, double* dg, double* ddiag,
-                                   double* t_solve, double* t_contract) {
+                                   double* t_solve, double* t_contract, double* ddx = nullptr) {
   cudaStream_t s = h->sA;
   const int64_t n = h->n, jlo = h->row0, jhi = h->row0 + h->nloc;
   const bool prof = h->profile;
-  // slab W (n x c), then the per-tile partials and one slab's per-split partials in d_gscratch
+  // slab W (n x c), then the per-tile partials, one slab's per-split partials and (ddx) its input-gradient partials in
+  // d_gscratch
   const int64_t tsize = grad_slab_tile_size(n, np), psize = grad_slab_partial_size(n, c, np);
+  const int64_t xsize = ddx ? grad_slab_x_partial_size(n, c, h->ndim) : 0;
   BGP_TRY(h->d_inv.reserve((size_t)n * c, s));
-  BGP_TRY(h->d_gscratch.reserve((size_t)(tsize + psize), s));
+  BGP_TRY(h->d_gscratch.reserve((size_t)(tsize + psize + xsize), s));
   double* W = h->d_inv.p;
   double* tile_part = h->d_gscratch.p;
   double* partial = h->d_gscratch.p + tsize;
+  double* xpart = partial + psize;
   int64_t slabs = 0;
   for (int64_t j0 = jlo / 64 * 64; j0 < jhi; j0 += c, ++slabs) {
     const int64_t nc = std::min(c, jhi - j0);
@@ -1405,8 +1439,12 @@ static int grad_stream_own_columns(bgp_hodlr* h, int np, const double* alpha, in
     BGP_LAUNCH_CHECK();
     BGP_TRY(hodlr_solve_dev(h, W, nc, n, s, 0, j0));
     if (prof) BGP_CUDA(cudaEventRecord(h->ev[5], s));
-    BGP_TRY(kmat_grad_slab_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, W, j0, nc, jlo, jhi, alpha,
-                                  alpha, partial, tile_part, ddiag, s));
+    if (ddx)
+      BGP_TRY(kmat_grad_x_slab_launch(h->d_prog.p, h->prog.shape, h->ndim, np, h->d_which.p, h->d_x.p, n, W, j0, nc, jlo,
+                                      jhi, alpha, partial, tile_part, xpart, ddiag, ddx, s));
+    else
+      BGP_TRY(kmat_grad_slab_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, W, j0, nc, jlo, jhi, alpha,
+                                    alpha, partial, tile_part, ddiag, s));
     if (prof) {
       BGP_CUDA(cudaEventRecord(h->ev[7], s));
       BGP_CUDA(cudaEventSynchronize(h->ev[7]));
@@ -1435,13 +1473,18 @@ static int grad_stream_own_columns(bgp_hodlr* h, int np, const double* alpha, in
 // On a shard with a matching communicator the call is collective and always streamed, composed of the existing pieces:
 // alpha by the collective solve, grad_stream_own_columns on this shard's columns, an all-reduce of g and an all-gather
 // of the diag slices.  Every rank issues the same collectives in the same order; none sits inside the slab loop.
-int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
-                         double* diag_out) {
+// With xgrad (bgp_hodlr_grad_x_terms) the same call also forms dx (n x ndim, row-major): resident, by the x-gradient
+// matvec over alpha alpha^T - K^-1 after the contraction; streamed, in the slabs' own pass; sharded, one more all-gather
+// of the dx row slices.  A NULL `which` then skips the parameter contraction.
+static int hodlr_grad_terms_impl(bgp_hodlr* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
+                                 double* diag_out, bool xgrad, double* dx_out, const char* what) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
-  if (host_exchange(h)) { set_error("grad_terms is not available on a sharded factorisation"); return BGP_ERR_INVALID; }
+  if (host_exchange(h)) { set_error("%s is not available on a sharded factorisation", what); return BGP_ERR_INVALID; }
   const int64_t n = h->n;
-  const int np = h->prog.n_params_total;
+  const int np = (xgrad && !which) ? 0 : h->prog.n_params_total;
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  const int nd = h->ndim;
+  if (xgrad && nd > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, nd); return BGP_ERR_INVALID; }
   const bool sharded = h->opts.shard_count > 1;
   if (sharded && !rows_ordered(h)) { set_error("internal: HODLR rows are not ordered by level"); return BGP_ERR_CUDA; }
   cudaStream_t s = h->sA;
@@ -1460,6 +1503,8 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
   BGP_TRY(hodlr_solve_dev(h, alpha, 1, n, s, 0));
   if (prof) { BGP_CUDA(cudaEventRecord(h->ev[5], s)); BGP_CUDA(cudaEventSynchronize(h->ev[5])); t_solve += event_ms(h->ev[4], h->ev[5]); }
   if (alpha_out) BGP_CUDA(cudaMemcpyAsync(alpha_out, alpha, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  DevBuf<double> ddx;
+  if (xgrad) BGP_TRY(ddx.alloc((size_t)n * nd, s));
   if (resident) {
     if (prof) BGP_CUDA(cudaEventRecord(h->ev[4], s));
     BGP_TRY(h->d_inv.reserve((size_t)n * n, s));
@@ -1470,6 +1515,7 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
     if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
     BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, alpha, 1.0, -1.0, dg,
                                       diag_out ? ddiag : nullptr, h->d_gscratch, s));
+    if (xgrad) BGP_TRY(grad_x_resident_launch(h->prog, h->d_prog.p, h->d_x.p, n, h->d_inv.p, alpha, ddx.p, h->d_gscratch, s));
     if (prof) {
       BGP_CUDA(cudaEventRecord(h->ev[7], s));
       BGP_CUDA(cudaEventSynchronize(h->ev[7]));
@@ -1480,18 +1526,30 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
     if (!rows_ordered(h)) { set_error("internal: HODLR rows are not ordered by level"); return BGP_ERR_CUDA; }
     BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
     if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
-    BGP_TRY(grad_stream_own_columns(h, np, alpha, c, dg, diag_out ? ddiag : nullptr, &t_solve, &t_contract));
-    if (sharded) {  // every shard's partial g, and its rows of diag to every shard
+    BGP_TRY(grad_stream_own_columns(h, np, alpha, c, dg, diag_out ? ddiag : nullptr, &t_solve, &t_contract, ddx.p));
+    if (sharded) {  // every shard's partial g, and its rows of diag (and of dx) to every shard
       if (np) BGP_TRY(comm_allreduce_sum_f64(dg, (size_t)np, s));
       if (diag_out) BGP_TRY(exchange_rows(h, ddiag, n, 1, s));
+      if (xgrad) BGP_TRY(exchange_rows_wide(h, ddx.p, nd, s));
     }
   }
   if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
   if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  if (xgrad && dx_out) BGP_CUDA(cudaMemcpyAsync(dx_out, ddx.p, sizeof(double) * n * nd, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));
   h->grad_t[0] = t_solve;
   h->grad_t[1] = t_contract;
   return BGP_OK;
+}
+
+int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
+                         double* diag_out) {
+  return hodlr_grad_terms_impl(h, which, r, alpha_out, g_out, diag_out, false, nullptr, "grad_terms");
+}
+
+int bgp_hodlr_grad_x_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
+                           double* diag_out, double* dx_out) {
+  return hodlr_grad_terms_impl(h, which, r, alpha_out, g_out, diag_out, true, dx_out, "grad_x_terms");
 }
 
 // Leave-one-out terms of the HODLR matrix (include/bgp.h), always streamed in the slabs of grad_stream_own_columns:
@@ -1568,13 +1626,17 @@ int bgp_hodlr_loo_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, 
   return BGP_OK;
 }
 
-// One shard's part of the streamed gradient (include/bgp.h): grad_stream_own_columns with the caller's alpha and diag.
-int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const double* alpha_dev, double* g_part_out,
-                                   double* diag_dev) {
+// One shard's part of the streamed gradient (include/bgp.h): grad_stream_own_columns with the caller's alpha and diag
+// (and, with xgrad, its dx rows; a NULL `which` then skips the parameter contraction).
+static int hodlr_grad_terms_local_impl(bgp_hodlr* h, const uint32_t* which, const double* alpha_dev,
+                                       double* g_part_out, double* diag_dev, bool xgrad, double* dx_dev,
+                                       const char* what) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
-  const int np = h->prog.n_params_total;
+  const int np = (xgrad && !which) ? 0 : h->prog.n_params_total;
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
-  if (!alpha_dev) { set_error("grad_terms_local: alpha_dev is null"); return BGP_ERR_INVALID; }
+  if (xgrad && h->ndim > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, h->ndim); return BGP_ERR_INVALID; }
+  if (!alpha_dev) { set_error("%s: alpha_dev is null", what); return BGP_ERR_INVALID; }
+  if (xgrad && !dx_dev) { set_error("%s: dx_dev is null", what); return BGP_ERR_INVALID; }
   if (!rows_ordered(h)) { set_error("internal: HODLR rows are not ordered by level"); return BGP_ERR_CUDA; }
   cudaStream_t s = h->sA;
   bool forced = false;
@@ -1585,12 +1647,22 @@ int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const 
   double* dg = h->d_rhs.p;
   BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
   if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
-  BGP_TRY(grad_stream_own_columns(h, np, alpha_dev, c, dg, diag_dev, &t_solve, &t_contract));
+  BGP_TRY(grad_stream_own_columns(h, np, alpha_dev, c, dg, diag_dev, &t_solve, &t_contract, xgrad ? dx_dev : nullptr));
   if (np && g_part_out) BGP_CUDA(cudaMemcpyAsync(g_part_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
   BGP_CUDA(cudaStreamSynchronize(s));
   h->grad_t[0] = t_solve;
   h->grad_t[1] = t_contract;
   return BGP_OK;
+}
+
+int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const double* alpha_dev, double* g_part_out,
+                                   double* diag_dev) {
+  return hodlr_grad_terms_local_impl(h, which, alpha_dev, g_part_out, diag_dev, false, nullptr, "grad_terms_local");
+}
+
+int bgp_hodlr_grad_x_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const double* alpha_dev,
+                                     double* g_part_out, double* diag_dev, double* dx_dev) {
+  return hodlr_grad_terms_local_impl(h, which, alpha_dev, g_part_out, diag_dev, true, dx_dev, "grad_x_terms_local");
 }
 
 // One handle's part of GP.predict's variance / covariance, over its own rows J = [row0, row0 + nloc) ([0, n) unsharded):

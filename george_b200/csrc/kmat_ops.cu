@@ -597,8 +597,16 @@ constexpr int64_t GS_ROWS = 1024;  // rows per i-split
 // x_j staging (inputs of up to 128 dimensions): with the ~12 KB of static shared memory it stays under the default
 // 48 KB per CTA; wider inputs read x_j from global memory
 constexpr size_t GS_SMEM_CAP = 32 * 1024;
+constexpr int GS_WARPS = GS_THREADS / 32;
 
-template <int NPMAX>
+// XSHAPE >= 0 (GP.grad_log_likelihood_x, bgp_hodlr_grad_x_terms): the same pass also contracts the input gradient of
+// each of the tile's columns j,
+//     xpart[((tile * nsplit + split) * GS_TJ + c) * nd + q] = sum_{i in split} w_ij d k(x_j, x_i) / d x_jq,
+// with w_ij = u_i v_j - W_ij the weight of the parameter contraction and the evaluator of kmat_x1_grad_matvec_kernel for
+// shape XSHAPE (the arguments swapped, x_j first, so a non-stationary kernel is differentiated in x_j).  Each warp sums
+// its 32 rows of a column with warp_sum and adds the sum to its own slot in shared memory; the CTA then adds the warps'
+// slots in warp order.  A NULL `which` skips the parameter contraction.  Needs nd <= BGP_MAX_DIM and staged x_j.
+template <int NPMAX, int XSHAPE = -1>
 __global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevProgram* __restrict__ gprog,
                                                                     const unsigned* __restrict__ which,
                                                                     const double* __restrict__ x, int64_t n,
@@ -606,13 +614,14 @@ __global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevPro
                                                                     int64_t nc, int64_t jlo, int64_t jhi,
                                                                     const double* __restrict__ u,
                                                                     const double* __restrict__ v, int stage_x,
-                                                                    double* __restrict__ partial) {
+                                                                    double* __restrict__ partial,
+                                                                    double* __restrict__ xpart = nullptr) {
   extern __shared__ double sxj[];  // GS_TJ x nd coordinates of the tile's columns (stage_x)
   __shared__ DevProgram P;
   __shared__ unsigned sw[BGP_MAX_LEAVES * (4 + BGP_MAX_METRIC)];
   __shared__ double saj[GS_TJ];
   __shared__ double red[32];
-  const int np = gprog->n_params_total, nd = gprog->ndim;
+  const int np = (XSHAPE >= 0 && !which) ? 0 : gprog->n_params_total, nd = gprog->ndim;
   const int64_t jt = j0 + (int64_t)blockIdx.x * GS_TJ;  // first column of the tile
   const int nj = (int)min((int64_t)GS_TJ, j0 + nc - jt);
   const int64_t r0 = (int64_t)blockIdx.y * GS_ROWS, r1 = min(n, r0 + GS_ROWS);
@@ -631,15 +640,57 @@ __global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevPro
   double acc[NPMAX], g[NPMAX];
 #pragma unroll
   for (int q = 0; q < NPMAX; ++q) acc[q] = 0.0;
-  for (int64_t i = r0 + threadIdx.x; i < r1; i += GS_THREADS) {
-    const double ai = u[i];
-    const double* xi = x + i * nd;
-    for (int c = 0; c < nj; ++c) {
-      const double w = ai * saj[c] - Wt[(int64_t)c * n + i];
-      kernel_value_grad(P, xi, stage_x ? sxj + c * nd : x + (jt + c) * nd, sw, g);
+  if constexpr (XSHAPE < 0) {
+    for (int64_t i = r0 + threadIdx.x; i < r1; i += GS_THREADS) {
+      const double ai = u[i];
+      const double* xi = x + i * nd;
+      for (int c = 0; c < nj; ++c) {
+        const double w = ai * saj[c] - Wt[(int64_t)c * n + i];
+        kernel_value_grad(P, xi, stage_x ? sxj + c * nd : x + (jt + c) * nd, sw, g);
 #pragma unroll
-      for (int q = 0; q < NPMAX; ++q)
-        if (q < np) acc[q] = fma(w, g[q], acc[q]);
+        for (int q = 0; q < NPMAX; ++q)
+          if (q < np) acc[q] = fma(w, g[q], acc[q]);
+      }
+    }
+  } else {
+    using Eval = X1GradEval<XSHAPE>;
+    constexpr int NDMAX = Eval::type::NDMAX;
+    const typename Eval::type fx = Eval::make(&P);
+    double* wdx = sxj + GS_TJ * nd;  // GS_WARPS x GS_TJ x nd: warp w's sums of column c
+    for (int t = threadIdx.x; t < GS_WARPS * GS_TJ * nd; t += GS_THREADS) wdx[t] = 0.0;
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // every lane runs every row step (a lane past r1 adds zeros) so that the warp sums see the whole warp; the
+    // parameter sums of a live row run in the order of the unflagged kernel, so they keep its bits
+    for (int64_t ib = r0; ib < r1; ib += GS_THREADS) {
+      const int64_t i = ib + threadIdx.x;
+      const bool live = i < r1;
+      const double ai = live ? u[i] : 0.0;
+      const double* xi = x + (live ? i : r0) * nd;
+      for (int c = 0; c < nj; ++c) {
+        double gx[NDMAX];
+        double w = 0.0;
+        if (live) {
+          w = ai * saj[c] - Wt[(int64_t)c * n + i];
+          if (np) {
+            kernel_value_grad(P, xi, sxj + c * nd, sw, g);
+#pragma unroll
+            for (int q = 0; q < NPMAX; ++q)
+              if (q < np) acc[q] = fma(w, g[q], acc[q]);
+          }
+          fx(sxj + c * nd, xi, gx);
+        } else {
+#pragma unroll
+          for (int q = 0; q < NDMAX; ++q) gx[q] = 0.0;
+        }
+#pragma unroll
+        for (int q = 0; q < NDMAX; ++q) {
+          if (q < nd) {  // uniform across the warp
+            const double s = warp_sum(w * gx[q]);
+            if (lane == 0) wdx[(warp * GS_TJ + c) * nd + q] += s;
+          }
+        }
+      }
     }
   }
   // one partial per (tile, split, parameter)
@@ -649,6 +700,31 @@ __global__ void __launch_bounds__(GS_THREADS) kmat_grad_slab_kernel(const DevPro
       const double s = block_sum(acc[q], red);
       if (threadIdx.x == 0) partial[((int64_t)blockIdx.x * gridDim.y + blockIdx.y) * np + q] = s;
     }
+  }
+  if constexpr (XSHAPE >= 0) {
+    __syncthreads();
+    const double* wdx = sxj + GS_TJ * nd;
+    double* out = xpart + ((int64_t)blockIdx.x * gridDim.y + blockIdx.y) * GS_TJ * nd;
+    for (int t = threadIdx.x; t < nj * nd; t += GS_THREADS) {
+      double s = wdx[t];
+      for (int w = 1; w < GS_WARPS; ++w) s += wdx[w * GS_TJ * nd + t];
+      out[t] = s;
+    }
+  }
+}
+
+// dx[j * nd + q] = sum_s xpart[((tile * nsplit + s) * GS_TJ + c) * nd + q], s ascending, for the columns
+// j = j0 + tile * GS_TJ + c of one slab that lie in the window [jlo, jhi) (no other row is written)
+__global__ void grad_slab_x_reduce_kernel(const double* __restrict__ xpart, int64_t nsplit, int64_t j0, int64_t nc,
+                                          int64_t jlo, int64_t jhi, int nd, double* __restrict__ dx) {
+  const int64_t total = nc * nd;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t k = t / nd, q = t - k * nd, j = j0 + k;
+    if (j < jlo || j >= jhi) continue;
+    const int64_t tile = k / GS_TJ, c = k - tile * GS_TJ;
+    double s = 0.0;
+    for (int64_t sp = 0; sp < nsplit; ++sp) s += xpart[((tile * nsplit + sp) * GS_TJ + c) * nd + q];
+    dx[j * nd + q] = s;
   }
 }
 
@@ -717,6 +793,90 @@ int kmat_grad_slab_launch(const DevProgram* dprog, int nd, int np, const unsigne
     BGP_LAUNCH_CHECK();
   }
   return BGP_OK;
+}
+
+// doubles of per-slab input-gradient partials for slabs of up to c columns of an n-row K^-1, nd-dimensional inputs
+int64_t grad_slab_x_partial_size(int64_t n, int64_t c, int nd) {
+  return ((n + GS_ROWS - 1) / GS_ROWS) * ((c + GS_TJ - 1) / GS_TJ) * GS_TJ * std::max(nd, 1);
+}
+
+// kmat_grad_slab_launch with the input gradient of the slab's columns in the same pass (bgp_hodlr_grad_x_terms):
+// the parameter partials, tile_part and diag exactly as kmat_grad_slab_launch writes them with u = v = alpha (the same
+// kernel body, bit for bit), and dx_dev[j * nd + q] = sum_i (alpha_i alpha_j - W_ij) d k(x_j, x_i) / d x_jq for the
+// columns j of the slab in [jlo, jhi), summed over the row splits in order: dx_j depends on n alone, not on the slab
+// width.  which_dev NULL (np 0) skips the parameter contraction.  shape: the program's shape (it selects the evaluator,
+// as in kmat_x1_grad_matvec_members); nd <= BGP_MAX_DIM.  xpart: grad_slab_x_partial_size(n, nc, nd) doubles.
+int kmat_grad_x_slab_launch(const DevProgram* dprog, int shape, int nd, int np, const unsigned* which_dev,
+                            const double* x, int64_t n, const double* W, int64_t j0, int64_t nc, int64_t jlo,
+                            int64_t jhi, const double* alpha, double* partial, double* tile_part, double* xpart,
+                            double* diag_dev, double* dx_dev, cudaStream_t s) {
+  if (nc <= 0) return BGP_OK;
+  if (!which_dev) np = 0;
+  if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  if (nd > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, nd); return BGP_ERR_INVALID; }
+  if (j0 % GS_TJ) { set_error("internal: slab start %lld is not a multiple of %d", (long long)j0, GS_TJ); return BGP_ERR_INVALID; }
+  const int64_t nsplit = (n + GS_ROWS - 1) / GS_ROWS, ntile = (nc + GS_TJ - 1) / GS_TJ;
+  if (nsplit > 65535 || ntile > 0x7fffffffLL) { set_error("kmat_grad_slab: n too large for one launch"); return BGP_ERR_INVALID; }
+  const size_t smem = sizeof(double) * (size_t)(1 + GS_WARPS) * GS_TJ * nd;  // x_j staged, then the warps' sums
+  const dim3 grid((unsigned)ntile, (unsigned)nsplit);
+  const unsigned* which = np ? which_dev : nullptr;
+#define BGP_GXS_LAUNCH(NPM, SH)                                                                                  \
+  kmat_grad_slab_kernel<NPM, SH><<<grid, GS_THREADS, smem, s>>>(dprog, which, x, n, W, j0, nc, jlo, jhi, alpha, alpha, \
+                                                                1, partial, xpart)
+#define BGP_GXS_SHAPES(NPM)                                                   \
+  switch (shape) {                                                            \
+    case BGP_SHAPE_EXPSQ: BGP_GXS_LAUNCH(NPM, BGP_SHAPE_EXPSQ); break;        \
+    case BGP_SHAPE_M32: BGP_GXS_LAUNCH(NPM, BGP_SHAPE_M32); break;            \
+    case BGP_SHAPE_M52: BGP_GXS_LAUNCH(NPM, BGP_SHAPE_M52); break;            \
+    case BGP_SHAPE_EXP: BGP_GXS_LAUNCH(NPM, BGP_SHAPE_EXP); break;            \
+    default: BGP_GXS_LAUNCH(NPM, BGP_SHAPE_GENERIC); break;                   \
+  }
+  if (np <= 8) {
+    BGP_GXS_SHAPES(8)
+  } else {
+    BGP_GXS_SHAPES(64)
+  }
+#undef BGP_GXS_SHAPES
+#undef BGP_GXS_LAUNCH
+  BGP_LAUNCH_CHECK();
+  if (np > 0) {
+    const int64_t total = ntile * np;
+    grad_slab_reduce_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 8 * (int64_t)num_sms()), 256, 0, s>>>(
+        partial, nsplit, ntile, np, tile_part + (j0 / GS_TJ) * np);
+    BGP_LAUNCH_CHECK();
+  }
+  grad_slab_x_reduce_kernel<<<(unsigned)std::min<int64_t>((nc * nd + 255) / 256, 8 * (int64_t)num_sms()), 256, 0, s>>>(
+      xpart, nsplit, j0, nc, jlo, jhi, nd, dx_dev);
+  BGP_LAUNCH_CHECK();
+  if (diag_dev) {
+    grad_slab_diag_kernel<<<(unsigned)std::min<int64_t>((nc + 255) / 256, 1184), 256, 0, s>>>(W, n, j0, nc, jlo, jhi,
+                                                                                              alpha, alpha, diag_dev);
+    BGP_LAUNCH_CHECK();
+  }
+  return BGP_OK;
+}
+
+// A (n x n, in place) = alpha alpha^T - A: K^-1 becomes the weight of the log-likelihood's gradient, the product and the
+// difference rounded separately, as np.outer(alpha, alpha) - K^-1 on the host
+__global__ void grad_x_form_a_kernel(double* __restrict__ A, int64_t n, const double* __restrict__ alpha) {
+  const int64_t total = n * n;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t j = t / n, i = t - j * n;
+    A[t] = __dsub_rn(__dmul_rn(alpha[i], alpha[j]), A[t]);
+  }
+}
+
+// The resident input gradient of bgp_dense_grad_x_terms and bgp_hodlr_grad_x_terms: with Kinv (n x n) = K^-1,
+//     dx[i * nd + q] = sum_j (alpha_i alpha_j - K^-1_ji) d k(x_i, x_j) / d x_iq,
+// Kinv overwritten by alpha alpha^T - K^-1, then contracted by the x-gradient matvec of GP.grad_predict with V = that
+// matrix (column i holds the weights of point i).  P: the host program (its shape selects the evaluator).
+int grad_x_resident_launch(const DevProgram& P, const DevProgram* dprog, const double* x, int64_t n, double* Kinv,
+                           const double* alpha, double* dx_dev, DevBuf<double>& scratch, cudaStream_t s) {
+  if (n <= 0) return BGP_OK;
+  grad_x_form_a_kernel<<<(unsigned)std::min<int64_t>((n * n + 255) / 256, 16 * (int64_t)num_sms()), 256, 0, s>>>(Kinv, n,
+                                                                                                             alpha);
+  BGP_LAUNCH_CHECK();
+  return kmat_x1_grad_matvec_launch(P, dprog, x, n, x, n, Kinv, n, 1.0, 0, dx_dev, scratch, s);
 }
 
 // g_dev[q] = sum_t tile_part[t * np + q] over the tiles that meet the columns [jlo, jhi) (all ceil(n / 32) tiles for

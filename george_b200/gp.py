@@ -59,10 +59,10 @@ def _sampling_jitter(rng, jitter):
     return jitter
 
 
-def _check_grad_predict_mean(mean):
+def _check_grad_predict_mean(mean, method="grad_predict", model="mean"):
     if type(mean) is not ConstantModel:
-        raise NotImplementedError("grad_predict needs the mean model's gradient with respect to the inputs, which "
-                                  "the modeling protocol does not provide; only a constant mean is supported")
+        raise NotImplementedError("{0} needs the {1} model's gradient with respect to the inputs, which the modeling "
+                                  "protocol does not provide; only a constant {1} is supported".format(method, model))
 
 
 def _check_grad_predict_dim(xs):
@@ -635,6 +635,71 @@ class GP(ModelSet):
         if layout[0]:
             dmu = self._swap_eval(self.mean, full[:n_mean], lambda: self._call_mean_gradient(self._x))
         return dmu, lambda: self._swap_eval(self.white_noise, full[n_mean:n_mean + n_wn], self._white_noise_terms)
+
+    def grad_log_likelihood_x(self, y, quiet=False, return_gradient=False):
+        """Gradient of :func:`log_likelihood` with respect to the training inputs: ``dx[i, q] = d log_likelihood(y) /
+        d x[i, q]`` at the computed coordinates, of shape ``(N, ndim)`` (also for 1-D input).  With
+        ``return_gradient`` the result is ``(grad, dx)``, ``grad`` from the same pass and the same launches as
+        :func:`grad_log_likelihood`: its bits wherever that method is reproducible (dense; HODLR up to N = 1024, whose
+        solve adds with atomics above).  This is what fits any parameter that enters through the coordinates, by the chain rule: a
+        time delay between two light curves, a warping or drift of one input axis, latent inputs.
+
+        With ``A = alpha alpha^T - K^-1``, ``dx_i = sum_j A_ij d k(x_i, x_j) / d x_i``, the true derivative for every
+        metric (each ``x_i`` enters row i and column i of ``K``; the 1/2 of the log-likelihood cancels the factor 2).
+        ``yerr`` is data and contributes nothing.  The mean and the white-noise model must be ``ConstantModel`` s (fitted
+        or not); anything else raises ``NotImplementedError``, as inputs of more than 8 dimensions raise ``ValueError``,
+        before any device work.  ``quiet`` follows :func:`grad_log_likelihood`: a failure it absorbs gives zeros for
+        ``dx`` (and ``grad``).
+
+        Solvers with a ``grad_x_terms`` hook (``BasicSolver``, ``HODLRSolver``, ``ShardedHODLRSolver``, collective)
+        contract on the device; the HODLR solvers stream ``K^-1`` in column slabs above N = 65536 and contract the input
+        gradient in the same pass as the hyper-parameter gradient.  Like their :func:`grad_log_likelihood`, the HODLR
+        solvers return the hybrid of ``K~^-1`` (the inverse of the HODLR matrix) with the exact kernel derivative.  Any
+        other solver (``TrivialSolver``, plug-ins, a dense solver restored from a pickle) forms ``A`` on the host from
+        ``solver.get_inverse()`` and contracts it on the device with ``KernelInterface.x1_gradient_matvec``.
+        """
+        _check_grad_predict_mean(self.mean, "grad_log_likelihood_x")
+        _check_grad_predict_mean(self.white_noise, "grad_log_likelihood_x", "white-noise")
+        self._require_computed()
+        _check_grad_predict_dim(self._x)
+        n, nd = self._x.shape
+        fail = (np.zeros(len(self), dtype=np.float64), np.zeros((n, nd), dtype=np.float64))
+        if not return_gradient:
+            fail = fail[1]
+        if not self.recompute(quiet=quiet):
+            return fail
+        layout = n_mean, n_wn, n_k = self._grad_layout()
+        mask = self.kernel.unfrozen_mask
+        # grad_log_likelihood's route for each part of grad: the fused terms when white-noise or kernel parameters
+        # are active, otherwise alpha from the solve alone
+        fused = return_gradient and bool(n_wn or n_k)
+        hook = getattr(self.solver, "grad_x_terms", None)
+        terms = gk = diagA = dmu = None
+        try:
+            r = self._residual(y)
+            if hook is not None:
+                terms = hook(r, mask.astype(np.uint32) if fused else None)
+            if terms is None:
+                alpha = self._compute_alpha(y, False)
+                A = np.outer(alpha, alpha) - self.solver.get_inverse()
+                diagA = np.diag(A)
+                if fused and n_k:
+                    gk = self.kernel.kernel.gradient_contract(mask.astype(np.uint32), self._x, A)
+                dx = self.kernel.kernel.x1_gradient_matvec(self._x, self._x, A, scale=1.0)
+            else:
+                alpha, gk, diagA, dx = terms
+            if return_gradient and not fused:
+                alpha = self._compute_alpha(y, False)
+            if return_gradient and n_mean:
+                dmu = self._call_mean_gradient(self._x)
+        except ValueError:
+            if quiet:
+                return fail
+            raise
+        if not return_gradient:
+            return dx
+        grad = self._grad_row(np.empty(len(self)), layout, dmu, alpha, self._white_noise_terms, diagA, gk, mask, 0.5)
+        return grad, dx
 
     # -- leave-one-out cross-validation (Rasmussen & Williams, GPML §5.4.2, eqs. 5.10-5.13) ---------------------------
     def loo_predict(self, y):

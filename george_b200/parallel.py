@@ -31,7 +31,7 @@ import numpy as np
 
 from . import _lib
 from ._spec import flatten
-from .solvers.basic import BasicSolver
+from .solvers.basic import BasicSolver, _grad_x_terms_call
 
 __all__ = ["ShardedHODLRSolver", "shard_ranges", "allgather_padded"]
 
@@ -177,6 +177,18 @@ class ShardedHODLRSolver(object):
         _lib.check(lib.bgp_hodlr_grad_terms(self.solver._ptr, _lib.ptr(which), _lib.ptr(r), _lib.ptr(alpha),
                                             _lib.ptr(g), _lib.ptr(diag)))
         return alpha, g[:which.size], diag
+
+    def grad_x_terms(self, r, which):
+        """``(alpha, g, diagA, dx)`` for ``GP.grad_log_likelihood_x``, as ``BasicSolver.grad_x_terms`` returns them.
+        Collective; ``r`` replicated on every rank, and every rank returns the same result.  Each rank streams K^-1 over
+        the columns of its own rows and contracts their input gradient in the same pass; the collectives are those of
+        :func:`grad_terms` and one all-gather of the ``dx`` row slices (``include/bgp.h: bgp_hodlr_grad_x_terms``).
+        The argument checks run on every rank before any collective, so a bad call leaves no rank waiting."""
+        if self.solver is None or not self._computed:
+            raise RuntimeError("you must call 'compute' first")
+        lib, ptr = self.solver._lib, self.solver._ptr
+        return _grad_x_terms_call(lambda *args: lib.bgp_hodlr_grad_x_terms(ptr, *args), self._n, self.solver._ndim,
+                                  r, which)
 
     def loo_terms(self, r, which=None):
         """Leave-one-out cross-validation is not available on a sharded factorisation: its gradient would need a

@@ -48,6 +48,7 @@ class HODLRSolver(object):
             self._ptr = C.c_void_p()
             _lib.check(self._lib.bgp_hodlr_create(C.byref(self._ptr)))
         self._n = 0
+        self._ndim = 0
         self.shard_count = 1
         self._fresh = True  # nothing computed through THIS object yet (a parked handle still holds its previous state)
 
@@ -104,7 +105,7 @@ class HODLRSolver(object):
             raise ValueError("dimension mismatch")
         spec = flatten(kernel_spec)
         o = self._opts(min_size, tol, seed, rng_mode, rank_capacity, shard_rank, shard_count, exhaust)
-        self._n = x.shape[0]
+        self._n, self._ndim = x.shape
         self.shard_count = int(shard_count)
         self._fresh = False
         _lib.check(self._lib.bgp_hodlr_compute(self._ptr, C.byref(spec), _lib.ptr(x), x.shape[0], x.shape[1],
@@ -297,6 +298,21 @@ class HODLRSolver(object):
         g = np.zeros(max(which.size, 1), dtype=np.float64)
         _lib.check(self._lib.bgp_hodlr_grad_terms_local_dev(self._ptr, _lib.ptr(which), alpha_dev, _lib.ptr(g),
                                                             diag_dev))
+        return g[:which.size]
+
+    def grad_x_terms_local(self, alpha_dev, which, dx_dev, diag_dev=None):
+        """:func:`grad_terms_local` with the input gradient of the log-likelihood for this handle's own rows
+        (``include/bgp.h: bgp_hodlr_grad_x_terms_local_dev``): ``dx_dev``, a device pointer to ``n * ndim`` doubles,
+        receives ``dx[j * ndim + q]`` for those rows only.  ``which`` ``None`` skips the parameter contraction (the
+        returned ``g`` is then empty).  Returns the partial ``g``; issues no collective."""
+        self._require_computed()
+        if which is None:
+            _lib.check(self._lib.bgp_hodlr_grad_x_terms_local_dev(self._ptr, None, alpha_dev, None, diag_dev, dx_dev))
+            return np.zeros(0, dtype=np.float64)
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        g = np.zeros(max(which.size, 1), dtype=np.float64)
+        _lib.check(self._lib.bgp_hodlr_grad_x_terms_local_dev(self._ptr, _lib.ptr(which), alpha_dev, _lib.ptr(g),
+                                                              diag_dev, dx_dev))
         return g[:which.size]
 
     def predict_local(self, kernel, xs, what, w_dev, ldw, add_prior):

@@ -112,6 +112,25 @@ def _batch_call(name, spec, params, x, yerr, r, *rest):
                                     _lib.ptr(yerr), _lib.ptr(r), *rest))
 
 
+def _grad_x_terms_call(call, n, ndim, r, which):
+    """``(alpha, g, diagA, dx)`` from a ``bgp_*_grad_x_terms`` entry point ``call(which, r, alpha, g, diag, dx)``
+    (the handle bound), after the checks of ``BasicSolver.grad_terms``; ``which`` ``None`` passes NULL."""
+    r = np.ascontiguousarray(r, dtype=np.float64)
+    if r.shape != (n,):
+        raise ValueError("dimension mismatch")
+    _check_finite(r)
+    alpha = np.empty(n, dtype=np.float64)
+    diag = np.empty(n, dtype=np.float64)
+    dx = np.empty((n, ndim), dtype=np.float64)
+    if which is None:
+        _lib.check(call(None, _lib.ptr(r), _lib.ptr(alpha), None, _lib.ptr(diag), _lib.ptr(dx)))
+        return alpha, np.zeros(0, dtype=np.float64), diag, dx
+    which = np.ascontiguousarray(which, dtype=np.uint32)
+    g = np.zeros(max(which.size, 1), dtype=np.float64)
+    _lib.check(call(_lib.ptr(which), _lib.ptr(r), _lib.ptr(alpha), _lib.ptr(g), _lib.ptr(diag), _lib.ptr(dx)))
+    return alpha, g[:which.size], diag, dx
+
+
 class BasicSolver(object):
 
     def __init__(self, kernel):
@@ -152,7 +171,7 @@ class BasicSolver(object):
         _lib.check(lib.bgp_dense_compute(self._handle.ptr, C.byref(spec), _lib.ptr(x), n, ndim, _lib.ptr(yerr)))
         ld = C.c_double()
         _lib.check(lib.bgp_dense_log_determinant(self._handle.ptr, C.byref(ld)))
-        self._n = n
+        self._n, self._ndim = n, ndim
         self._has_inputs = True
         self.log_determinant = ld.value
         self.computed = True
@@ -229,6 +248,20 @@ class BasicSolver(object):
 
     def _grad_terms_call(self, which, r, alpha, g, diag):
         return self._handle.lib.bgp_dense_grad_terms(self._handle.ptr, which, r, alpha, g, diag)
+
+    def grad_x_terms(self, r, which):
+        """:func:`grad_terms` with the gradient of the log-likelihood with respect to the training inputs, from the
+        same pass (``include/bgp.h: bgp_dense_grad_x_terms``): ``(alpha, g, diagA, dx)``, ``alpha``, ``g`` and ``diagA``
+        bit for bit what :func:`grad_terms` returns and ``dx[i, q] = sum_j (alpha alpha^T - K^-1)_ij dk(x_i, x_j) /
+        dx_iq`` (``(n, ndim)``).  ``which`` ``None`` skips the parameter contraction (``g`` is then empty).  Returns
+        ``None`` for a solver restored from a pickle, as :func:`grad_terms` does."""
+        self._require()
+        if not getattr(self, "_has_inputs", True):
+            return None
+        return _grad_x_terms_call(self._grad_x_terms_lib, self._n, self._ndim, r, which)
+
+    def _grad_x_terms_lib(self, *args):
+        return self._handle.lib.bgp_dense_grad_x_terms(self._handle.ptr, *args)
 
     def loo_terms(self, r, which=None):
         """The leave-one-out cross-validation terms of ``GP.loo_*`` on the device from the stored factor

@@ -61,10 +61,13 @@ class HODLRSolver(BasicSolver):
     def _require(self):
         if getattr(self, "solver", None) is None or not self._computed:
             raise RuntimeError("you must call 'compute' first")
-        self._n = self.solver._n
+        self._n, self._ndim = self.solver._n, self.solver._ndim
 
     def _grad_terms_call(self, which, r, alpha, g, diag):
         return self.solver._lib.bgp_hodlr_grad_terms(self.solver._ptr, which, r, alpha, g, diag)
+
+    def _grad_x_terms_lib(self, *args):
+        return self.solver._lib.bgp_hodlr_grad_x_terms(self.solver._ptr, *args)
 
     def _loo_terms_call(self, which, r, alpha, d, beta, g, diag):
         return self.solver._lib.bgp_hodlr_loo_terms(self.solver._ptr, which, r, alpha, d, beta, g, diag)

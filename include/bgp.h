@@ -227,6 +227,19 @@ int bgp_dense_import_factor(bgp_dense_t* h, const double* factor, int64_t n, dou
  * bgp_dense_import_factor (it holds no kernel / coordinates). */
 int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
                          double* diag_out);
+/* bgp_dense_grad_terms plus the log-likelihood's gradient with respect to the training inputs (GP.grad_log_likelihood_x):
+ *   dx_out[i * ndim + q] = sum_j (alpha alpha^T - K^-1)_ij d k(x_i, x_j) / d x_iq     (n * ndim, host)
+ * the true derivative for every metric (the evaluator of bgp_kmat_x1_gradient_matvec).  Each x_i enters row i and
+ * column i of K, and the 1/2 of the log-likelihood cancels the factor 2 of the symmetric pair, so dx_out is
+ * d log L / d x with no further factor.  alpha_out, g_out and diag_out are bgp_dense_grad_terms' and its bits (the same
+ * launches); a NULL `which` skips the parameter contraction (g_out is then not written).  K^-1 stays resident, as in
+ * bgp_dense_grad_terms; after the contraction it is overwritten by alpha alpha^T - K^-1 (rounded as on the host) and
+ * contracted by the x-gradient matvec with V = that matrix.  Extra device workspace: n * ndim + the matvec's partials.
+ * Errors (before anything is launched): BGP_ERR_NOT_COMPUTED before compute and on a handle restored by
+ * bgp_dense_import_factor; BGP_ERR_INVALID for more than BGP_MAX_DIM input dimensions and for more than 64 kernel
+ * parameters with a non-NULL which. */
+int bgp_dense_grad_x_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
+                           double* diag_out, double* dx_out);
 /* Leave-one-out cross-validation terms (GP.loo_predict, GP.loo_log_likelihood, GP.grad_loo_log_likelihood; Rasmussen &
  * Williams, GPML eqs. 5.10-5.13), computed on the device from the stored factor, kernel and coordinates:
  *   alpha_out = K^-1 r (n),  d_out = diag(K^-1) (n)                                        (pass 1)
@@ -554,6 +567,31 @@ int bgp_hodlr_grad_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r,
  * than 64 kernel parameters and for a NULL alpha_dev (both before anything is launched). */
 int bgp_hodlr_grad_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const double* alpha_dev, double* g_part_out,
                                    double* diag_dev);
+/* bgp_dense_grad_x_terms on the HODLR matrix: alpha_out, g_out, diag_out are bgp_hodlr_grad_terms' and its bits, and
+ *   dx_out[i * ndim + q] = sum_j (alpha alpha^T - K~^-1)_ij d k(x_i, x_j) / d x_iq
+ * with K~^-1 the inverse of the HODLR matrix and the exact kernel derivative (the hybrid that bgp_hodlr_grad_terms
+ * returns for the hyper-parameters).  Resident regime (n <= 65536, BGP_GRAD_CHUNK unset): as bgp_dense_grad_x_terms.
+ * Streamed regime: each slab W = K~^-1 E_J contracts, in the same kernel pass as g, the input gradient of its own
+ * columns, dx_j = sum_i (alpha_i alpha_j - W_ij) d k(x_j, x_i) / d x_j (the kernel differentiated in x_j, so
+ * non-stationary kernels are exact); the per-row-split partials are summed in an order that depends only on n, so dx
+ * does not depend on the slab width and two identical calls return the same bits.  Extra device workspace: n * ndim +
+ * ceil(n / 1024) * c * ndim.  The resident and streamed dx agree to rounding (their sums run in different orders).
+ * On a sharded factorisation with a matching communicator the call is COLLECTIVE, as bgp_hodlr_grad_terms is: the
+ * collective alpha solve, each shard's slabs over its own columns, the all-reduce of g, the all-gather of the diag
+ * slices when diag_out is set, and one all-gather of the dx row slices; no collective sits inside the slab loop.
+ * Errors (before anything is launched): BGP_ERR_NOT_COMPUTED before compute; BGP_ERR_INVALID for more than BGP_MAX_DIM
+ * input dimensions, for more than 64 kernel parameters with a non-NULL which, and on a host-exchange shard (which
+ * computes its part with bgp_hodlr_grad_x_terms_local_dev). */
+int bgp_hodlr_grad_x_terms(bgp_hodlr_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
+                           double* diag_out, double* dx_out);
+/* One shard's part of bgp_hodlr_grad_x_terms: bgp_hodlr_grad_terms_local_dev's g_part_out and diag_dev (its bits) and
+ * dx_dev[j * ndim + q] (device, n * ndim) for the rows j of this handle only (no other row is written).  Issues no
+ * collective.  On an unsharded handle it returns bit for bit what bgp_hodlr_grad_x_terms returns on the streamed path.
+ * A NULL which skips the parameter contraction.  Errors (before anything is launched): BGP_ERR_NOT_COMPUTED as
+ * bgp_hodlr_grad_terms_local_dev; BGP_ERR_INVALID for more than BGP_MAX_DIM input dimensions, more than 64 kernel
+ * parameters with a non-NULL which, a NULL alpha_dev and a NULL dx_dev. */
+int bgp_hodlr_grad_x_terms_local_dev(bgp_hodlr_t* h, const uint32_t* which, const double* alpha_dev, double* g_part_out,
+                                     double* diag_dev, double* dx_dev);
 /* The HODLR counterpart of bgp_dense_loo_terms: the same outputs and errors, for the HODLR matrix K~ (not the dense K).
  * Always streamed, at every n, in the column slabs of bgp_hodlr_grad_terms (c columns, BGP_GRAD_CHUNK included):
  *   pass 1: per slab S = K~^-1 E_J by the row-restricted solve, d_j = S_jj for j in J;
