@@ -70,6 +70,7 @@ SIGNATURES = {
     "bgp_hodlr_grad_terms": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_grad_terms_local_dev": (C.c_int, [_p, _p, _p, _p, _p]),
     "bgp_dense_grad_x_terms": (C.c_int, [_p, _p, _p, _p, _p, _p, _p]),
+    "bgp_dense_fisher_terms": (C.c_int, [_p, _p, _p, _p, _i32, _p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_grad_x_terms": (C.c_int, [_p, _p, _p, _p, _p, _p, _p]),
     "bgp_hodlr_grad_x_terms_local_dev": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "bgp_dense_loo_terms": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p]),

@@ -76,6 +76,11 @@ int predict_var_launch(const double* B, int64_t ldb, const double* W, int64_t ld
                        const double* kdiag, double* var, DevBuf<double>& scratch, cudaStream_t s);
 int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
                      bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
+int predict_gemm_sub_bt(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
+                        bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs,
+                        cudaStream_t s);
+int kmat_gradient_plane_launch(const DevProgram* dprog, int np, int p, const double* x, int64_t n, double* out,
+                               int64_t ldo, cudaStream_t s);
 
 constexpr int DN_NB = 64;   // inner panel width (diagonal block in shared memory)
 constexpr int DN_MB = 256;  // middle block of the delayed-update hierarchy (see dense_potrf)
@@ -924,11 +929,78 @@ int bgp_dense_get_inverse(bgp_dense_t* h, double* out) {
   return bgp_dense_apply_inverse(h, out, n, n);
 }
 
+// GP.fisher_information's rows (bgp_dense_fisher_terms): nv white-noise vectors (host, nv x n) and the outputs
+struct FisherArgs {
+  const double* v;
+  int nv;
+  double* rows_out;     // nrow x np
+  double* rdiag_out;    // nrow x n
+  double* prod_ms_out;  // nrow (may be NULL): device time of each row's products
+};
+
+// The Fisher rows from the resident K^-1 (see bgp_dense_fisher_terms).  Row by row, one n x n plane / product buffer P and
+// one n x n T: a kernel row p builds dK_p into P, T = -K^-T dK_p and P = K^-T dK_p K^-1 (two GD_SUB products into zeroed
+// targets, the second one lower-triangular and mirrored, with T consumed as stored); a white-noise row scales the rows of
+// a copy of K^-1 in T by v and forms P = -K^-T diag(v) K^-1 (one lower product).  The contraction of bgp_dense_grad_terms
+// then gives the row's kernel entries (cm = +1 or -1 for the sign of P) and diag(P), each row in its own fixed order.
+static int dense_fisher_rows(bgp_dense* h, const uint32_t* which, int np, const FisherArgs& f) {
+  const int64_t n = h->n;
+  const int nd = h->ndim;
+  cudaStream_t s = h->s;
+  std::vector<int> krow;
+  for (int q = 0; q < np; ++q)
+    if (which[q]) krow.push_back(q);
+  const int nk = (int)krow.size(), nrow = nk + f.nv;
+  if (nrow == 0) return BGP_OK;
+  DevBuf<double> dP, dT, dv, drows, drd, slices;
+  DevBuf<GemmDesc> descs;
+  BGP_TRY(dP.alloc((size_t)n * n, s));
+  BGP_TRY(dT.alloc((size_t)n * n, s));
+  if (f.nv) {
+    BGP_TRY(dv.alloc((size_t)f.nv * n, s));
+    BGP_CUDA(cudaMemcpyAsync(dv.p, f.v, sizeof(double) * f.nv * n, cudaMemcpyHostToDevice, s));
+  }
+  BGP_TRY(drows.alloc((size_t)std::max(nrow * np, 1), s));
+  BGP_TRY(drd.alloc((size_t)nrow * n, s));
+  const size_t bytes = sizeof(double) * (size_t)n * (size_t)n;
+  for (int row = 0; row < nrow; ++row) {
+    if (f.prod_ms_out) BGP_CUDA(cudaEventRecord(h->ev[0], s));
+    double cm = 1.0;
+    if (row < nk) {
+      BGP_TRY(kmat_gradient_plane_launch(h->d_prog.p, np, krow[row], h->d_x.p, n, dP.p, n, s));
+      BGP_CUDA(cudaMemsetAsync(dT.p, 0, bytes, s));
+      BGP_TRY(predict_gemm_sub(h->d_inv.p, n, dP.p, n, n, n, n, false, dT.p, n, slices, descs, s));
+      BGP_CUDA(cudaMemsetAsync(dP.p, 0, bytes, s));
+      BGP_TRY(predict_gemm_sub_bt(h->d_inv.p, n, dT.p, n, n, n, n, true, dP.p, n, slices, descs, s));
+    } else {
+      BGP_CUDA(cudaMemcpyAsync(dT.p, h->d_inv.p, bytes, cudaMemcpyDeviceToDevice, s));
+      BGP_TRY(scale_rows_launch(dT.p, n, n, n, dv.p + (int64_t)(row - nk) * n, false, s));
+      BGP_CUDA(cudaMemsetAsync(dP.p, 0, bytes, s));
+      BGP_TRY(predict_gemm_sub(h->d_inv.p, n, dT.p, n, n, n, n, true, dP.p, n, slices, descs, s));
+      cm = -1.0;
+    }
+    if (f.prod_ms_out) {
+      BGP_CUDA(cudaEventRecord(h->ev[1], s));
+      BGP_CUDA(cudaEventSynchronize(h->ev[1]));
+      float ms = 0.0f;
+      BGP_CUDA(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
+      f.prod_ms_out[row] = ms;
+    }
+    BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, nd, np, h->d_which.p, h->d_x.p, n, dP.p, n, nullptr, 0.0, cm,
+                                      drows.p + (int64_t)row * np, drd.p + (int64_t)row * n, h->d_gscratch, s));
+  }
+  if (np) BGP_CUDA(cudaMemcpyAsync(f.rows_out, drows.p, sizeof(double) * nrow * np, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaMemcpyAsync(f.rdiag_out, drd.p, sizeof(double) * nrow * n, cudaMemcpyDeviceToHost, s));
+  BGP_CUDA(cudaStreamSynchronize(s));
+  return BGP_OK;
+}
+
 // With xgrad (bgp_dense_grad_x_terms) the call also forms dx (n x ndim, row-major) from the resident K^-1 after the
 // contraction: grad_x_resident_launch turns it into alpha alpha^T - K^-1 and runs the x-gradient matvec over it.  A NULL
-// `which` then skips the parameter contraction.
+// `which` then skips the parameter contraction.  With fisher (bgp_dense_fisher_terms) it forms the Fisher rows from the
+// resident K^-1 after the contraction; a NULL `r` then skips alpha and the contraction.
 static int dense_grad_terms_impl(bgp_dense* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
-                                 double* diag_out, bool xgrad, double* dx_out) {
+                                 double* diag_out, bool xgrad, double* dx_out, const FisherArgs* fisher = nullptr) {
   if (!h || !h->computed) { set_error("the solver has not been computed"); return BGP_ERR_NOT_COMPUTED; }
   if (!h->has_inputs) { set_error("the factor was imported: the handle holds no kernel/coordinates"); return BGP_ERR_NOT_COMPUTED; }
   const int64_t n = h->n;
@@ -936,22 +1008,39 @@ static int dense_grad_terms_impl(bgp_dense* h, const uint32_t* which, const doub
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
   const int nd = h->ndim;
   if (xgrad && nd > BGP_MAX_DIM) { set_error("input-coordinate gradients support at most %d dimensions (got %d)", BGP_MAX_DIM, nd); return BGP_ERR_INVALID; }
+  if (fisher) {
+    if (np && !which) { set_error("fisher_terms: which is required for a kernel with parameters"); return BGP_ERR_INVALID; }
+    if (fisher->nv < 0 || (fisher->nv && !fisher->v)) { set_error("fisher_terms: invalid white-noise vectors"); return BGP_ERR_INVALID; }
+    if (!fisher->rows_out || !fisher->rdiag_out) { set_error("fisher_terms: NULL output"); return BGP_ERR_INVALID; }
+  } else if (!r) {
+    set_error("r is NULL"); return BGP_ERR_INVALID;
+  }
   cudaStream_t s = h->s;
   BGP_TRY(h->d_rhs.reserve((size_t)n * 2 + 64, s));
   double* alpha = h->d_rhs.p;
   double* dg = h->d_rhs.p + n;       // np <= 64 entries
   double* ddiag = h->d_rhs.p + n + 64;
-  BGP_CUDA(cudaMemcpyAsync(alpha, r, sizeof(double) * n, cudaMemcpyHostToDevice, s));
-  BGP_TRY(dense_potrs_dev(h, alpha, 1, n));
-  if (alpha_out) BGP_CUDA(cudaMemcpyAsync(alpha_out, alpha, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  if (r) {
+    BGP_CUDA(cudaMemcpyAsync(alpha, r, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+    BGP_TRY(dense_potrs_dev(h, alpha, 1, n));
+    if (alpha_out) BGP_CUDA(cudaMemcpyAsync(alpha_out, alpha, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  }
   BGP_TRY(h->d_inv.reserve((size_t)n * n, s));
   BGP_TRY(fill_identity_launch(h->d_inv.p, n, s));
   BGP_TRY(dense_potrs_dev(h, h->d_inv.p, n, n));
   BGP_TRY(h->d_which.reserve(std::max(np, 1), s));
   if (np) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * np, cudaMemcpyHostToDevice, s));
   // kernel term of gp.py:457-466 and diag(alpha alpha^T - K^-1) for the white-noise term of gp.py:452-456
-  BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, alpha, 1.0, -1.0, dg,
-                                    diag_out ? ddiag : nullptr, h->d_gscratch, s));
+  if (r)
+    BGP_TRY(kmat_grad_contract_launch(h->d_prog.p, h->ndim, np, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, alpha, 1.0, -1.0,
+                                      dg, diag_out ? ddiag : nullptr, h->d_gscratch, s));
+  if (fisher) {
+    if (r) {  // bgp_dense_grad_terms' outputs, queued before the rows
+      if (np && g_out) BGP_CUDA(cudaMemcpyAsync(g_out, dg, sizeof(double) * np, cudaMemcpyDeviceToHost, s));
+      if (diag_out) BGP_CUDA(cudaMemcpyAsync(diag_out, ddiag, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+    }
+    return dense_fisher_rows(h, which, np, *fisher);
+  }
   DevBuf<double> ddx;
   if (xgrad) {
     BGP_TRY(ddx.alloc((size_t)n * nd, s));
@@ -972,6 +1061,13 @@ int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r,
 int bgp_dense_grad_x_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
                            double* diag_out, double* dx_out) {
   return dense_grad_terms_impl(h, which, r, alpha_out, g_out, diag_out, true, dx_out);
+}
+
+int bgp_dense_fisher_terms(bgp_dense_t* h, const uint32_t* which, const double* r, const double* v, int32_t nv,
+                           double* alpha_out, double* g_out, double* diag_out, double* rows_out, double* rdiag_out,
+                           double* prod_ms_out) {
+  const FisherArgs f{v, nv, rows_out, rdiag_out, prod_ms_out};
+  return dense_grad_terms_impl(h, which, r, alpha_out, g_out, diag_out, false, nullptr, &f);
 }
 
 int bgp_dense_loo_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* d_out,

@@ -571,6 +571,48 @@ int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const uns
                                     scratch, s);
 }
 
+// One hyper-parameter's plane of the kernel gradient, out[i * ldo + j] = d k(x_i, x_j) / d theta_p (n x n), for
+// GP.fisher_information's kernel rows: kmat_gradient_kernel interleaves all P planes, which would make the Fisher pass's
+// memory grow with P.  Every entry evaluates the pair as (x_min(i,j), x_max(i,j)), so the plane is exactly symmetric, with
+// parameter p the only active one.  One thread per entry along j: the stores are coalesced, and the ~2x evaluations are
+// noise beside the O(n^3) products that consume the plane.
+template <int NPMAX>
+__global__ void __launch_bounds__(256) kmat_gradient_plane_kernel(const DevProgram* __restrict__ gprog, int p,
+                                                                  const double* __restrict__ x, int64_t n,
+                                                                  double* __restrict__ out, int64_t ldo) {
+  __shared__ DevProgram P;
+  __shared__ unsigned sw[BGP_MAX_LEAVES * (4 + BGP_MAX_METRIC)];
+  stage_program(&P, gprog);
+  const int np = gprog->n_params_total;
+  for (int q = threadIdx.x; q < np; q += blockDim.x) sw[q] = (q == p) ? 1u : 0u;
+  __syncthreads();
+  const int nd = P.ndim;
+  double g[NPMAX];
+  const int64_t total = n * n;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t i = t / n, j = t - i * n;
+    const int64_t a = i < j ? i : j, b = i < j ? j : i;
+    kernel_value_grad(P, x + a * nd, x + b * nd, sw, g);
+    double v = 0.0;
+#pragma unroll
+    for (int q = 0; q < NPMAX; ++q)
+      if (q == p) v = g[q];
+    out[i * ldo + j] = v;
+  }
+}
+
+int kmat_gradient_plane_launch(const DevProgram* dprog, int np, int p, const double* x, int64_t n, double* out,
+                               int64_t ldo, cudaStream_t s) {
+  if (n <= 0) return BGP_OK;
+  if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  if (p < 0 || p >= np) { set_error("gradient plane %d out of range (%d parameters)", p, np); return BGP_ERR_INVALID; }
+  const unsigned blocks = (unsigned)std::min<int64_t>((n * n + 255) / 256, 16 * (int64_t)num_sms());
+  if (np <= 8) kmat_gradient_plane_kernel<8><<<blocks, 256, 0, s>>>(dprog, p, x, n, out, ldo);
+  else kmat_gradient_plane_kernel<64><<<blocks, 256, 0, s>>>(dprog, p, x, n, out, ldo);
+  BGP_LAUNCH_CHECK();
+  return BGP_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Slab gradient contraction (bgp_hodlr_grad_terms at large n, which never holds all of K^-1): for a slab
 // W = K^-1 E_J of columns J = [j0, j0 + nc) (n x nc, column-major, W[(j - j0) n + i] = (K^-1)_ij),
@@ -1139,9 +1181,10 @@ void predict_gemm_plan(int64_t m, int64_t nn, int64_t K, int64_t* nsplit_out, in
 // `members` > 1: member b uses A and B + b * abstride and C + b * cstride; all members' slices go through one DMMA
 // launch (nsplit * members descriptors, member-major) and one add, so the launch count does not depend on members
 // while nsplit * members <= 65535.
-int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn,
-                             int64_t K, bool lower, double* C, int64_t ldc, int members, int64_t abstride,
-                             int64_t cstride, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s) {
+// `b_kcontig` false (gemm_sub_split_bt): B'(k, j) = B[k*ldb + j] instead, the (1, 0) DMMA variant.
+static int gemm_sub_split(const double* A, int64_t lda, const double* B, int64_t ldb, bool b_kcontig, int64_t m,
+                          int64_t nn, int64_t K, bool lower, double* C, int64_t ldc, int members, int64_t abstride,
+                          int64_t cstride, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s) {
   if (m <= 0 || nn <= 0 || members <= 0) return BGP_OK;
   if (m > 0x7fffffffLL || nn > 0x7fffffffLL || K > 0x7fffffffLL) { set_error("predict: GEMM too large"); return BGP_ERR_INVALID; }
   if (members > 65535) { set_error("predict: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
@@ -1160,7 +1203,7 @@ int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int6
       const int64_t k0 = sp * klen;
       GemmDesc& d = hd[(size_t)(mb * nsplit + sp)];
       d.A = A + mb * abstride + k0; d.lda = lda;
-      d.B = B + mb * abstride + k0; d.ldb = ldb;
+      d.B = B + mb * abstride + (b_kcontig ? k0 : k0 * ldb); d.ldb = ldb;
       if (direct) { d.C = C + mb * cstride; d.ldc = ldc; }
       else { d.C = slices.p + (mb * nsplit + sp) * slice; d.ldc = m; }
       d.M = (int)m; d.N = (int)nn; d.K = (int)std::max<int64_t>(0, std::min(klen, K - k0));
@@ -1168,7 +1211,8 @@ int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int6
     }
   BGP_TRY(descs.reserve((size_t)nslices, s));
   BGP_CUDA(cudaMemcpyAsync(descs.p, hd.data(), sizeof(GemmDesc) * nslices, cudaMemcpyHostToDevice, s));
-  BGP_TRY((gemm_dmma_launch<true, true>(descs.p, (int)nslices, (int)m, (int)nn, nullptr, s)));
+  if (b_kcontig) BGP_TRY((gemm_dmma_launch<true, true>(descs.p, (int)nslices, (int)m, (int)nn, nullptr, s)));
+  else BGP_TRY((gemm_dmma_launch<true, false>(descs.p, (int)nslices, (int)m, (int)nn, nullptr, s)));
   if (direct) {
     if (lower) {
       mirror_lower_kernel<<<dim3((unsigned)std::min<int64_t>((slice + 255) / 256, 8 * (int64_t)num_sms()), (unsigned)members),
@@ -1182,9 +1226,20 @@ int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int6
   BGP_LAUNCH_CHECK();
   return BGP_OK;
 }
+int predict_gemm_sub_members(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn,
+                             int64_t K, bool lower, double* C, int64_t ldc, int members, int64_t abstride,
+                             int64_t cstride, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s) {
+  return gemm_sub_split(A, lda, B, ldb, true, m, nn, K, lower, C, ldc, members, abstride, cstride, slices, descs, s);
+}
 int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
                      bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s) {
   return predict_gemm_sub_members(A, lda, B, ldb, m, nn, K, lower, C, ldc, 1, 0, 0, slices, descs, s);
+}
+// predict_gemm_sub with B'(k, j) = B[k*ldb + j]: C -= A' B^T for a column-major B (n x K), consumed as stored
+int predict_gemm_sub_bt(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
+                        bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs,
+                        cudaStream_t s) {
+  return gemm_sub_split(A, lda, B, ldb, false, m, nn, K, lower, C, ldc, 1, 0, 0, slices, descs, s);
 }
 
 }  // namespace bgp

@@ -18,8 +18,10 @@ from numpy.linalg import LinAlgError
 from . import _lib, kernels
 from ._spec import BGP_MAX_DIM, flatten, num_params, patch_specs
 from .modeling import ConstantModel, ModelSet
-from .solvers import BasicSolver, TrivialSolver
+from .parallel import ShardedHODLRSolver
+from .solvers import BasicSolver, HODLRSolver, TrivialSolver
 from .solvers.basic import NONFINITE_RHS
+from .solvers.hodlr import FISHER_HODLR
 from .utils import device_gaussian_samples, multivariate_gaussian_samples
 
 __all__ = ["GP"]
@@ -700,6 +702,106 @@ class GP(ModelSet):
             return dx
         grad = self._grad_row(np.empty(len(self)), layout, dmu, alpha, self._white_noise_terms, diagA, gk, mask, 0.5)
         return grad, dx
+
+    # -- second order ------------------------------------------------------------------------------------------------
+    def fisher_information(self, y=None, quiet=False):
+        """The expected Fisher information of the active parameter vector, ``F`` of shape ``(len(gp), len(gp))`` in
+        :func:`grad_log_likelihood`'s layout (mean, white noise, kernel; frozen parameters left out; kernel parameters
+        in the log units of :func:`get_parameter_vector`):
+
+            F_pq = dmu_p^T K^-1 dmu_q + 1/2 tr(K^-1 dK_p K^-1 dK_q)
+
+        with ``dK = diag(exp(wn) dwn)`` for a white-noise parameter, and zero between mean and covariance parameters.
+        It needs first derivatives only, does not depend on ``y`` and is positive semi-definite by construction, so
+        after a fit ``inv(F)`` gives the parameters' Cramér-Rao / Laplace covariance (their standard errors), a
+        sampler's mass matrix or start ball, and ``p + solve(F, grad)`` a Fisher-scoring step.  ``F`` is exactly
+        symmetric, and two calls return the same bits.
+
+        With ``y`` the result is ``(grad, F)``: ``grad`` comes from the same pass and, on ``BasicSolver``, is bit for bit
+        :func:`grad_log_likelihood`, so a scoring step costs one ``K^-1``.  ``quiet`` follows
+        :func:`grad_log_likelihood`: a failure it absorbs (a failed factorisation, a model returning NaN, more than 64
+        kernel parameters) gives zeros for ``F`` (and ``grad``).
+
+        ``BasicSolver`` forms ``K^-1 dK_p K^-1`` for each kernel and white-noise parameter on the FP64 tensor pipe from
+        the resident ``K^-1`` (``include/bgp.h: bgp_dense_fisher_terms``), in device memory that does not grow with
+        the number of parameters.  ``TrivialSolver``, plug-ins and a dense solver restored from a pickle compute the
+        formula on the host from ``solver.apply_inverse(eye(N))`` and ``kernel.get_gradient``.  ``HODLRSolver`` and
+        ``ShardedHODLRSolver`` raise ``NotImplementedError`` before any device work.
+        """
+        if isinstance(self.solver_type, type) and issubclass(self.solver_type, (HODLRSolver, ShardedHODLRSolver)):
+            raise NotImplementedError(FISHER_HODLR)
+        size = len(self)
+        fail = np.zeros((size, size), dtype=np.float64)
+        if y is not None:
+            fail = (np.zeros(size, dtype=np.float64), fail)
+        if not self.recompute(quiet=quiet):
+            return fail
+        layout = n_mean, n_wn, n_k = self._grad_layout()
+        mask = self.kernel.unfrozen_mask
+        # grad_log_likelihood's route for alpha: the fused terms when white-noise or kernel parameters are active
+        fused = y is not None and bool(n_wn or n_k)
+        noise = dmu = gk = diagA = alpha = None
+        try:
+            r = self._residual(y) if fused else None
+            v = np.zeros((0, len(self._x)), dtype=np.float64)
+            if n_wn:
+                noise = self._white_noise_terms()
+                v = np.exp(noise[0])[None, :] * noise[1]
+            rows = rdiag = None
+            if n_wn or n_k:
+                hook = getattr(self.solver, "fisher_terms", None)
+                terms = None if hook is None else hook(r, mask.astype(np.uint32), v)
+                if terms is None:
+                    rows, rdiag = self._fisher_rows_host(v, n_k)
+                    if fused:
+                        alpha = self._compute_alpha(y, False)
+                        A = np.outer(alpha, alpha) - self.solver.get_inverse()
+                        diagA = np.diag(A)
+                        if n_k:
+                            gk = self.kernel.kernel.gradient_contract(mask.astype(np.uint32), self._x, A)
+                else:
+                    gterms, rows, rdiag = terms
+                    rows = rows[:, mask]
+                    if fused:
+                        alpha, gk, diagA = gterms
+            if y is not None and not fused:
+                alpha = self._compute_alpha(y, False)
+            if n_mean:
+                dmu = self._call_mean_gradient(self._x)
+                kinv_dmu = np.asarray(self.solver.apply_inverse(np.array(dmu.T, dtype=np.float64, order="F")),
+                                      dtype=np.float64).reshape(len(self._x), n_mean)
+        except ValueError:
+            if quiet:
+                return fail
+            raise
+        F = np.zeros((size, size), dtype=np.float64)
+        if n_mean:
+            M = np.dot(dmu, kinv_dmu)
+            F[:n_mean, :n_mean] = 0.5 * (M + M.T)
+        if n_wn or n_k:
+            # R in F's order (white noise, then kernel) from the rows in the solver's order (kernel, then white noise)
+            order = np.concatenate([np.arange(n_k, n_k + n_wn), np.arange(n_k)])
+            R = np.empty((n_wn + n_k, n_wn + n_k), dtype=np.float64)
+            R[:, :n_wn] = 0.5 * np.dot(rdiag[order], v.T)
+            R[:, n_wn:] = 0.5 * rows[order]
+            F[n_mean:, n_mean:] = 0.5 * (R + R.T)
+        if y is None:
+            return F
+        grad = self._grad_row(np.empty(size), layout, dmu, alpha, lambda: noise, diagA, gk, mask, 0.5)
+        return grad, F
+
+    def _fisher_rows_host(self, v, n_k):
+        """``(rows, rdiag)`` as ``BasicSolver.fisher_terms`` returns them (active kernel columns only), on the host:
+        ``B = K^-1 dK K^-1`` for each active kernel parameter, then each white-noise vector (``dK = diag(v_k)``), with
+        ``K^-1 = solver.apply_inverse(eye(N))`` and ``dK_p`` from ``kernel.get_gradient``."""
+        n = len(self._x)
+        kinv = np.asarray(self.solver.apply_inverse(np.eye(n), in_place=True), dtype=np.float64).reshape(n, n)
+        dK = self.kernel.get_gradient(self._x) if n_k else np.zeros((n, n, 0))
+        planes = [kinv.dot(dK[:, :, p]).dot(kinv) for p in range(n_k)]
+        planes += [kinv.T.dot(vk[:, None] * kinv) for vk in v]
+        rows = np.array([np.einsum("ij,ijq->q", B, dK) for B in planes]).reshape(len(planes), n_k)
+        rdiag = np.array([np.diag(B) for B in planes]).reshape(len(planes), n)
+        return rows, rdiag
 
     # -- leave-one-out cross-validation (Rasmussen & Williams, GPML §5.4.2, eqs. 5.10-5.13) ---------------------------
     def loo_predict(self, y):

@@ -32,6 +32,7 @@ import numpy as np
 from . import _lib
 from ._spec import flatten
 from .solvers.basic import BasicSolver, _grad_x_terms_call
+from .solvers.hodlr import FISHER_HODLR
 
 __all__ = ["ShardedHODLRSolver", "shard_ranges", "allgather_padded"]
 
@@ -195,6 +196,11 @@ class ShardedHODLRSolver(object):
         collective full solve per slab.  Raises ``NotImplementedError`` on every rank before any collective, so no rank
         is left waiting."""
         raise NotImplementedError("leave-one-out cross-validation is not implemented for the ShardedHODLRSolver")
+
+    def fisher_terms(self, r, which, v, prod_ms=None):
+        """The Fisher information is not available on a sharded factorisation, as on ``HODLRSolver``.  Raises
+        ``NotImplementedError`` on every rank before any collective, so no rank is left waiting."""
+        raise NotImplementedError(FISHER_HODLR)
 
     def predictive(self, kernel, xs, what):
         """``BasicSolver.predictive`` on the sharded factorisation: the variance (``what="var"``, ``(ns,)``) or

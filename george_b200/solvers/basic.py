@@ -263,6 +263,45 @@ class BasicSolver(object):
     def _grad_x_terms_lib(self, *args):
         return self._handle.lib.bgp_dense_grad_x_terms(self._handle.ptr, *args)
 
+    def fisher_terms(self, r, which, v, prod_ms=None):
+        """The rows of ``GP.fisher_information`` on the device from the stored factor and the resident ``K^-1``
+        (``include/bgp.h: bgp_dense_fisher_terms``): ``(grad_terms, rows, rdiag)``.  ``rows`` is ``(nrow, P)`` and
+        ``rdiag`` ``(nrow, n)``, one row for each kernel parameter where ``which`` (a 0/1 mask over ALL kernel
+        parameters) is set, then one per white-noise vector of ``v`` (``(nv, n)``); with ``B = K^-1 dK K^-1`` for that
+        row's ``dK`` (``diag(v_k)`` for a white-noise row), ``rows[., q] = sum_ij B_ij dK_q,ij`` and ``rdiag = diag(B)``.
+        ``grad_terms`` is what :func:`grad_terms` returns, bit for bit, when ``r`` is given and ``None`` when ``r`` is
+        ``None``.  ``prod_ms`` (an ``(nrow,)`` float64 array) receives each row's product time in ms.  Returns ``None``
+        for a solver restored from a pickle, as :func:`grad_terms` does."""
+        self._require()
+        if not getattr(self, "_has_inputs", True):
+            return None
+        n = self._n
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        v = np.ascontiguousarray(v, dtype=np.float64).reshape(-1, n)
+        nrow = int(np.count_nonzero(which)) + v.shape[0]
+        rows = np.zeros((nrow, max(which.size, 1)), dtype=np.float64)
+        rdiag = np.empty((nrow, n), dtype=np.float64)
+        if prod_ms is not None and (prod_ms.shape != (nrow,) or prod_ms.dtype != np.float64):
+            raise ValueError("prod_ms must be a float64 array of shape ({0},)".format(nrow))
+        terms = None
+        rp = alpha = g = diag = None
+        if r is not None:
+            r = np.ascontiguousarray(r, dtype=np.float64)
+            if r.shape != (n,):
+                raise ValueError("dimension mismatch")
+            _check_finite(r)
+            alpha = np.empty(n, dtype=np.float64)
+            g = np.zeros(max(which.size, 1), dtype=np.float64)
+            diag = np.empty(n, dtype=np.float64)
+            rp = _lib.ptr(r)
+            terms = alpha, g[:which.size], diag
+        _lib.check(self._handle.lib.bgp_dense_fisher_terms(
+            self._handle.ptr, _lib.ptr(which), rp, _lib.ptr(v) if v.shape[0] else None, v.shape[0],
+            None if alpha is None else _lib.ptr(alpha), None if g is None else _lib.ptr(g),
+            None if diag is None else _lib.ptr(diag), _lib.ptr(rows), _lib.ptr(rdiag),
+            None if prod_ms is None else _lib.ptr(prod_ms)))
+        return terms, rows[:, :which.size], rdiag
+
     def loo_terms(self, r, which=None):
         """The leave-one-out cross-validation terms of ``GP.loo_*`` on the device from the stored factor
         (``include/bgp.h: bgp_dense_loo_terms``): ``(alpha, d)`` with ``alpha = K^-1 r`` and ``d = diag(K^-1)``; with

@@ -14,6 +14,9 @@ from ._hodlr import HODLRSolver as HODLRSolverInterface
 
 __all__ = ["HODLRSolver"]
 
+FISHER_HODLR = ("the Fisher information is not implemented for the HODLR solvers: its exact trace is O(P N^3) at HODLR "
+                "sizes; use the dense BasicSolver")
+
 
 class HODLRSolver(BasicSolver):
 
@@ -68,6 +71,11 @@ class HODLRSolver(BasicSolver):
 
     def _grad_x_terms_lib(self, *args):
         return self.solver._lib.bgp_hodlr_grad_x_terms(self.solver._ptr, *args)
+
+    def fisher_terms(self, r, which, v, prod_ms=None):
+        """The Fisher information is not available on a HODLR factorisation: its exact trace needs N^2 products, O(P N^3)
+        at HODLR sizes.  Raises ``NotImplementedError`` (``GP.fisher_information`` raises it before any device work)."""
+        raise NotImplementedError(FISHER_HODLR)
 
     def _loo_terms_call(self, which, r, alpha, d, beta, g, diag):
         return self.solver._lib.bgp_hodlr_loo_terms(self.solver._ptr, which, r, alpha, d, beta, g, diag)

@@ -240,6 +240,27 @@ int bgp_dense_grad_terms(bgp_dense_t* h, const uint32_t* which, const double* r,
  * parameters with a non-NULL which. */
 int bgp_dense_grad_x_terms(bgp_dense_t* h, const uint32_t* which, const double* r, double* alpha_out, double* g_out,
                            double* diag_out, double* dx_out);
+/* The rows of the expected Fisher information of the hyper-parameters (GP.fisher_information), from the resident K^-1:
+ * row p for each kernel parameter with which[p] != 0 (ascending p), then one row per white-noise vector v_k
+ * (v: nv x n, host, row-major; dK = diag(v_k)).  With B = K^-1 dK_row K^-1 (dK_p the device program's derivative):
+ *   rows_out[row * np + q] = sum_ij B_ij dK_q,ij  (np = all kernel parameters, 0 where which[q] == 0)     (nrow x np)
+ *   rdiag_out[row * n + i] = B_ii                                                                        (nrow x n)
+ * so F = 1/2 tr(K^-1 dK_a K^-1 dK_b) is 1/2 rows_out for kernel columns and 1/2 rdiag_out . v_l for white-noise
+ * columns; the caller applies the 1/2 and symmetrises.  B runs on the FP64 tensor pipe: a kernel row materialises
+ * dK_p, then T = K^-1 dK_p and B = K^-1 T^T (lower triangle, mirrored, so B is exactly symmetric); a white-noise row forms
+ * K^-1 diag(v_k) K^-1 from a row-scaled copy of K^-1 in one lower product.  Each row is contracted by the parameter
+ * contraction of bgp_dense_grad_terms, in a fixed order (no atomics): identical calls return identical bits.
+ * With r, alpha_out / g_out / diag_out are bgp_dense_grad_terms' outputs and its bits (the same launches, first); a NULL r
+ * skips alpha and the contraction of alpha alpha^T - K^-1 (those outputs are then not written).  prod_ms_out (may be
+ * NULL; nrow entries) receives the device time of each row's products (the call then synchronises once per row).
+ * Device workspace: K^-1 (as bgp_dense_grad_terms keeps it) + 2 n^2 (one dK_p / B buffer, one T buffer) + the products'
+ * split-K slices (at most 1 GiB) + nrow * (n + np): it does not grow with the number of parameters.
+ * Errors (before anything is launched): BGP_ERR_NOT_COMPUTED as bgp_dense_grad_terms; BGP_ERR_INVALID for more than
+ * 64 kernel parameters, a NULL which with kernel parameters, nv < 0, a NULL v with nv > 0 and a NULL rows_out or
+ * rdiag_out. */
+int bgp_dense_fisher_terms(bgp_dense_t* h, const uint32_t* which, const double* r, const double* v, int32_t nv,
+                           double* alpha_out, double* g_out, double* diag_out, double* rows_out, double* rdiag_out,
+                           double* prod_ms_out);
 /* Leave-one-out cross-validation terms (GP.loo_predict, GP.loo_log_likelihood, GP.grad_loo_log_likelihood; Rasmussen &
  * Williams, GPML eqs. 5.10-5.13), computed on the device from the stored factor, kernel and coordinates:
  *   alpha_out = K^-1 r (n),  d_out = diag(K^-1) (n)                                        (pass 1)
