@@ -98,6 +98,8 @@ SIGNATURES = {
                                              _p, _p]),
     "bgp_dense_batch_loo_terms": (C.c_int, [_p, _specp, _p, _i64, _i64, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p,
                                             _p, _p]),
+    "bgp_dense_batch_fisher_terms": (C.c_int, [_p, _specp, _p, _i64, _i64, _p, _i64, _i32, _p, _p, _p, _p, _i32, _p,
+                                               _i32, _p, _p, _p, _p, _p, _p, _p]),
     "bgp_dense_create": (C.c_int, [C.POINTER(_p)]),
     "bgp_dense_destroy": (None, [_p]),
     "bgp_dense_compute": (C.c_int, [_p, _specp, _p, _i64, _i32, _p]),

@@ -79,8 +79,13 @@ int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb,
 int predict_gemm_sub_bt(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
                         bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs,
                         cudaStream_t s);
+int predict_gemm_sub_bt_members(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn,
+                                int64_t K, bool lower, double* C, int64_t ldc, int members, int64_t abstride,
+                                int64_t cstride, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s);
 int kmat_gradient_plane_launch(const DevProgram* dprog, int np, int p, const double* x, int64_t n, double* out,
                                int64_t ldo, cudaStream_t s);
+int kmat_gradient_plane_members(const DevProgram* dprogs, int np, int p, const double* x, int64_t n, double* out,
+                                int64_t ldo, int64_t ostride, int members, cudaStream_t s);
 
 constexpr int DN_NB = 64;   // inner panel width (diagonal block in shared memory)
 constexpr int DN_MB = 256;  // middle block of the delayed-update hierarchy (see dense_potrf)
@@ -1290,6 +1295,9 @@ struct bgp_dense_batch : BatchStream {
   DevBuf<double> d_dmu, d_dvar, d_xgp;
   // bgp_dense_batch_loo_terms (besides d_inv, d_gp, d_g and d_which): A, beta (q, then K^-1 q) and c
   DevBuf<double> d_loo_a, d_beta, d_cw;
+  // bgp_dense_batch_fisher_terms (besides d_inv, d_gp, d_g, d_which and d_slices): the plane / product buffer P, T,
+  // the rows and their diagonals, the white-noise vectors and the mean gradients (K^-1 dmu^T after the solve)
+  DevBuf<double> d_fp, d_ft, d_frows, d_frd, d_fv, d_fdmu;
 };
 
 // members per chunk: as many members of per_member doubles as fit in 4 GiB, at least one; BGP_BATCH_CHUNK=<members>
@@ -1378,14 +1386,15 @@ static int batch_upload_xs(bgp_dense_batch* h, const double* xs, int64_t ns, int
 
 // members [c0, c0 + mc): K_b + diag(yerr_b^2) built and factorised in place (d_A, member stride n^2, info in d_info) and
 // alpha_b = K_b^-1 r_b in d_sol (member stride n): the steps of bgp_dense_compute and of the few-right-hand-side solve
-// of bgp_dense_apply_inverse / bgp_dense_dot_solve, member-indexed, one launch per step for the whole chunk
+// of bgp_dense_apply_inverse / bgp_dense_dot_solve, member-indexed, one launch per step for the whole chunk.  A NULL r
+// (bgp_dense_batch_fisher_terms without residuals) skips the residual upload and the alpha solve.
 static int batch_factor_chunk(bgp_dense_batch* h, const BatchPrograms& bp, int64_t c0, int mc, int64_t n,
                               const double* yerr, const double* r) {
   cudaStream_t s = h->s;
   const int64_t len = (int64_t)mc * n;
   const int64_t mstride = n * n;
   BGP_CUDA(cudaMemcpyAsync(h->d_yerr.p, yerr + c0 * n, sizeof(double) * len, cudaMemcpyHostToDevice, s));
-  BGP_CUDA(cudaMemcpyAsync(h->d_r.p, r + c0 * n, sizeof(double) * len, cudaMemcpyHostToDevice, s));
+  if (r) BGP_CUDA(cudaMemcpyAsync(h->d_r.p, r + c0 * n, sizeof(double) * len, cudaMemcpyHostToDevice, s));
   BGP_CUDA(cudaMemsetAsync(h->d_info.p, 0, sizeof(int) * mc, s));
   // yerr^2 exactly as bgp_dense_compute squares it (an elementwise product: the layout does not matter)
   square2_kernel<<<(unsigned)std::min<int64_t>((len + 255) / 256, 1184), 256, 0, s>>>(h->d_yerr.p, h->d_diag.p, len);
@@ -1393,6 +1402,7 @@ static int batch_factor_chunk(bgp_dense_batch* h, const BatchPrograms& bp, int64
   BGP_TRY(kmat_symmetric_batch_launch_auto(bp.progs.data() + c0, h->d_prog.p + c0, mc, h->d_x.p, n, h->d_diag.p,
                                            h->d_A.p, mstride, h->d_fn, s));
   BGP_TRY(dense_potrf_members(h->d_A.p, n, mstride, mc, h->d_info.p, nullptr, h->d_gdesc, s));
+  if (!r) return BGP_OK;
   BGP_CUDA(cudaMemcpyAsync(h->d_sol.p, h->d_r.p, sizeof(double) * len, cudaMemcpyDeviceToDevice, s));
   return potrs_small_members(h->d_A.p, n, h->d_sol.p, 1, n, h->d_tmp.p, mc, mstride, n, s);
 }
@@ -1660,6 +1670,103 @@ int bgp_dense_batch_loo_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spe
   // one launch per step for the chunk: the split-K product takes one descriptor per member and slice
   return batch_run(h, bp, x, n, ndim, yerr, r, per_member, 65535 / gsplit, tmp_cols, bufs, setup, step, info,
                    {{alpha, n}, {d, n}, {beta, grad ? n : 0}, {g, grad ? P : 0}, {diag, grad ? n : 0}});
+}
+
+int bgp_dense_batch_fisher_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,
+                                 int64_t P, const double* x, int64_t n, int32_t ndim, const double* yerr,
+                                 const double* r, const uint32_t* which, const double* v, int32_t nv, const double* dmu,
+                                 int32_t nm, double* alpha, double* g, double* diag, double* rows, double* rdiag,
+                                 double* kdmu, int32_t* info) {
+  if (P > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
+  if (P > 0 && !which) { set_error("fisher_terms: which is required for a kernel with parameters"); return BGP_ERR_INVALID; }
+  if (nv < 0 || (nv > 0 && !v)) { set_error("fisher_terms: invalid white-noise vectors"); return BGP_ERR_INVALID; }
+  if (nm < 0 || (nm > 0 && !dmu)) { set_error("fisher_terms: invalid mean gradients"); return BGP_ERR_INVALID; }
+  BatchPrograms bp;
+  BGP_TRY(batch_begin(h, spec, params, B, P, x, n, ndim, &bp));
+  if (B == 0) return BGP_OK;
+  cudaStream_t s = h->s;
+  const int64_t nn = n * n;
+  std::vector<int> krow;  // the kernel rows, then nv white-noise rows, as bgp_dense_fisher_terms orders them
+  for (int64_t q = 0; q < P; ++q)
+    if (which[q]) krow.push_back((int)q);
+  const int64_t nk = (int64_t)krow.size(), nrow = nk + nv;
+  // the few-column solve's scratch: K^-1 when n <= 8 (as bgp_dense_fisher_terms sends it), dmu when nm <= 8
+  const int64_t tmp_cols = std::max<int64_t>(n <= DS_MAX_RHS ? n : 1, nm <= DS_MAX_RHS ? nm : 1);
+  const int64_t nt = (n + 31) / 32;  // the contraction's 32 x 32 tiles
+  // the products' split-K plan, bgp_dense_fisher_terms' (no slice buffer with one slice)
+  int64_t gsplit = 1, gklen = 0;
+  if (nrow) predict_gemm_plan(n, n, n, &gsplit, &gklen);
+  const int64_t slices = gsplit > 1 ? gsplit * nn : 0;
+  const int64_t planes = nrow ? nn : 0;
+  // doubles per member (see include/bgp.h): factor, K^-1, P, T, the split-K slices, the vectors of
+  // batch_reserve_common, partials, g, the rows and their diagonals, v and dmu
+  const int64_t per_member = 2 * nn + 2 * planes + slices + (4 + tmp_cols) * n + nt * nt * P + P + nrow * (P + n) +
+                             (int64_t)(nv + nm) * n;
+  const std::vector<ChunkBuf> bufs = {{&h->d_A, nn}, {&h->d_inv, nn}, {&h->d_fp, planes}, {&h->d_ft, planes},
+                                      {&h->d_slices, slices}, {&h->d_gp, nt * nt * P}, {&h->d_g, P},
+                                      {&h->d_frows, nrow * P}, {&h->d_frd, nrow * n}, {&h->d_fv, (int64_t)nv * n},
+                                      {&h->d_fdmu, (int64_t)nm * n}};
+  auto setup = [&](int64_t) -> int {
+    BGP_TRY(h->d_which.reserve((size_t)std::max<int64_t>(1, P), s));
+    if (P > 0) BGP_CUDA(cudaMemcpyAsync(h->d_which.p, which, sizeof(unsigned) * P, cudaMemcpyHostToDevice, s));
+    return BGP_OK;
+  };
+  // the steps of bgp_dense_fisher_terms after bgp_dense_compute, member-indexed, each row one set of launches for the
+  // whole chunk; then the mean block's solve, the nm-column bgp_dense_apply_inverse
+  auto step = [&](int64_t c0, int mc, const DevProgram*, const DevProgram* dprogs) -> int {
+    BGP_TRY(fill_identity_members(h->d_inv.p, n, mc, s));
+    BGP_TRY(potrs_members(h->d_A.p, n, nn, h->d_inv.p, n, n, nn, mc, h->d_tmp.p, s));
+    if (r) {  // bgp_dense_batch_grad_terms' contraction; the diagonal goes to d_diag, whose yerr^2 the build consumed
+      BGP_TRY(kmat_grad_contract_members(dprogs, (int)P, h->d_which.p, h->d_x.p, n, h->d_inv.p, n, nn, h->d_sol.p, n,
+                                         1.0, -1.0, h->d_g.p, P, diag ? h->d_diag.p : nullptr, n, mc, h->d_gp, s));
+      if (alpha) BGP_CUDA(cudaMemcpyAsync(alpha + c0 * n, h->d_sol.p, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
+      if (diag) BGP_CUDA(cudaMemcpyAsync(diag + c0 * n, h->d_diag.p, sizeof(double) * mc * n, cudaMemcpyDeviceToHost, s));
+      if (g && P > 0) BGP_CUDA(cudaMemcpyAsync(g + c0 * P, h->d_g.p, sizeof(double) * mc * P, cudaMemcpyDeviceToHost, s));
+    }
+    if (nv)
+      BGP_CUDA(cudaMemcpyAsync(h->d_fv.p, v + c0 * nv * n, sizeof(double) * mc * nv * n, cudaMemcpyHostToDevice, s));
+    const size_t bytes = sizeof(double) * (size_t)mc * (size_t)nn;
+    for (int64_t row = 0; row < nrow; ++row) {
+      double cm = 1.0;
+      if (row < nk) {
+        BGP_TRY(kmat_gradient_plane_members(dprogs, (int)P, krow[(size_t)row], h->d_x.p, n, h->d_fp.p, n, nn, mc, s));
+        BGP_CUDA(cudaMemsetAsync(h->d_ft.p, 0, bytes, s));
+        BGP_TRY(predict_gemm_sub_members(h->d_inv.p, n, h->d_fp.p, n, n, n, n, false, h->d_ft.p, n, mc, nn, nn,
+                                         h->d_slices, h->d_pdesc, s));
+        BGP_CUDA(cudaMemsetAsync(h->d_fp.p, 0, bytes, s));
+        BGP_TRY(predict_gemm_sub_bt_members(h->d_inv.p, n, h->d_ft.p, n, n, n, n, true, h->d_fp.p, n, mc, nn, nn,
+                                            h->d_slices, h->d_pdesc, s));
+      } else {
+        BGP_CUDA(cudaMemcpyAsync(h->d_ft.p, h->d_inv.p, bytes, cudaMemcpyDeviceToDevice, s));
+        BGP_TRY(scale_rows_members(h->d_ft.p, n, n, n, h->d_fv.p + (row - nk) * n, false, mc, nn, (int64_t)nv * n, s));
+        BGP_CUDA(cudaMemsetAsync(h->d_fp.p, 0, bytes, s));
+        BGP_TRY(predict_gemm_sub_members(h->d_inv.p, n, h->d_ft.p, n, n, n, n, true, h->d_fp.p, n, mc, nn, nn,
+                                         h->d_slices, h->d_pdesc, s));
+        cm = -1.0;
+      }
+      BGP_TRY(kmat_grad_contract_members(dprogs, (int)P, h->d_which.p, h->d_x.p, n, h->d_fp.p, n, nn, nullptr, 0, 0.0,
+                                         cm, h->d_frows.p + row * P, nrow * P, h->d_frd.p + row * n, nrow * n, mc,
+                                         h->d_gp, s));
+    }
+    if (rows && nrow * P > 0)
+      BGP_CUDA(cudaMemcpyAsync(rows + c0 * nrow * P, h->d_frows.p, sizeof(double) * mc * nrow * P,
+                               cudaMemcpyDeviceToHost, s));
+    if (rdiag && nrow > 0)
+      BGP_CUDA(cudaMemcpyAsync(rdiag + c0 * nrow * n, h->d_frd.p, sizeof(double) * mc * nrow * n,
+                               cudaMemcpyDeviceToHost, s));
+    if (nm) {
+      const int64_t len = (int64_t)nm * n;
+      BGP_CUDA(cudaMemcpyAsync(h->d_fdmu.p, dmu + c0 * len, sizeof(double) * mc * len, cudaMemcpyHostToDevice, s));
+      BGP_TRY(potrs_members(h->d_A.p, n, nn, h->d_fdmu.p, nm, n, len, mc, h->d_tmp.p, s));
+      if (kdmu) BGP_CUDA(cudaMemcpyAsync(kdmu + c0 * len, h->d_fdmu.p, sizeof(double) * mc * len, cudaMemcpyDeviceToHost, s));
+    }
+    return BGP_OK;
+  };
+  // one launch per step for the chunk: the split-K products take one descriptor per member and slice
+  const int64_t rl = r ? 1 : 0;
+  return batch_run(h, bp, x, n, ndim, yerr, r, per_member, 65535 / gsplit, tmp_cols, bufs, setup, step, info,
+                   {{alpha, rl * n}, {g, rl * P}, {diag, rl * n}, {rows, nrow * P}, {rdiag, nrow * n},
+                    {kdmu, (int64_t)nm * n}});
 }
 
 int bgp_dense_batch_predict(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params, int64_t B,

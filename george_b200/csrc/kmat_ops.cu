@@ -576,10 +576,14 @@ int kmat_grad_contract_launch(const DevProgram* dprog, int nd, int np, const uns
 // memory grow with P.  Every entry evaluates the pair as (x_min(i,j), x_max(i,j)), so the plane is exactly symmetric, with
 // parameter p the only active one.  One thread per entry along j: the stores are coalesced, and the ~2x evaluations are
 // noise beside the O(n^3) products that consume the plane.
+// Member blockIdx.y of a batch evaluates with gprog + y and writes its plane at out + y * ostride.
 template <int NPMAX>
 __global__ void __launch_bounds__(256) kmat_gradient_plane_kernel(const DevProgram* __restrict__ gprog, int p,
                                                                   const double* __restrict__ x, int64_t n,
-                                                                  double* __restrict__ out, int64_t ldo) {
+                                                                  double* __restrict__ out, int64_t ldo,
+                                                                  int64_t ostride) {
+  gprog += blockIdx.y;
+  out += blockIdx.y * ostride;
   __shared__ DevProgram P;
   __shared__ unsigned sw[BGP_MAX_LEAVES * (4 + BGP_MAX_METRIC)];
   stage_program(&P, gprog);
@@ -601,16 +605,23 @@ __global__ void __launch_bounds__(256) kmat_gradient_plane_kernel(const DevProgr
   }
 }
 
-int kmat_gradient_plane_launch(const DevProgram* dprog, int np, int p, const double* x, int64_t n, double* out,
-                               int64_t ldo, cudaStream_t s) {
-  if (n <= 0) return BGP_OK;
+// `members` planes of one x in one launch: member b evaluates with dprogs[b] and writes out + b * ostride, each entry
+// exactly as a one-member call computes it.  All members share np and p.
+int kmat_gradient_plane_members(const DevProgram* dprogs, int np, int p, const double* x, int64_t n, double* out,
+                                int64_t ldo, int64_t ostride, int members, cudaStream_t s) {
+  if (n <= 0 || members <= 0) return BGP_OK;
   if (np > 64) { set_error("gradient supports at most 64 hyper-parameters"); return BGP_ERR_INVALID; }
   if (p < 0 || p >= np) { set_error("gradient plane %d out of range (%d parameters)", p, np); return BGP_ERR_INVALID; }
-  const unsigned blocks = (unsigned)std::min<int64_t>((n * n + 255) / 256, 16 * (int64_t)num_sms());
-  if (np <= 8) kmat_gradient_plane_kernel<8><<<blocks, 256, 0, s>>>(dprog, p, x, n, out, ldo);
-  else kmat_gradient_plane_kernel<64><<<blocks, 256, 0, s>>>(dprog, p, x, n, out, ldo);
+  if (members > 65535) { set_error("gradient plane: more than 65535 members in one launch"); return BGP_ERR_INVALID; }
+  const dim3 grid((unsigned)std::min<int64_t>((n * n + 255) / 256, 16 * (int64_t)num_sms()), (unsigned)members);
+  if (np <= 8) kmat_gradient_plane_kernel<8><<<grid, 256, 0, s>>>(dprogs, p, x, n, out, ldo, ostride);
+  else kmat_gradient_plane_kernel<64><<<grid, 256, 0, s>>>(dprogs, p, x, n, out, ldo, ostride);
   BGP_LAUNCH_CHECK();
   return BGP_OK;
+}
+int kmat_gradient_plane_launch(const DevProgram* dprog, int np, int p, const double* x, int64_t n, double* out,
+                               int64_t ldo, cudaStream_t s) {
+  return kmat_gradient_plane_members(dprog, np, p, x, n, out, ldo, 0, 1, s);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1236,10 +1247,15 @@ int predict_gemm_sub(const double* A, int64_t lda, const double* B, int64_t ldb,
   return predict_gemm_sub_members(A, lda, B, ldb, m, nn, K, lower, C, ldc, 1, 0, 0, slices, descs, s);
 }
 // predict_gemm_sub with B'(k, j) = B[k*ldb + j]: C -= A' B^T for a column-major B (n x K), consumed as stored
+int predict_gemm_sub_bt_members(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn,
+                                int64_t K, bool lower, double* C, int64_t ldc, int members, int64_t abstride,
+                                int64_t cstride, DevBuf<double>& slices, DevBuf<GemmDesc>& descs, cudaStream_t s) {
+  return gemm_sub_split(A, lda, B, ldb, false, m, nn, K, lower, C, ldc, members, abstride, cstride, slices, descs, s);
+}
 int predict_gemm_sub_bt(const double* A, int64_t lda, const double* B, int64_t ldb, int64_t m, int64_t nn, int64_t K,
                         bool lower, double* C, int64_t ldc, DevBuf<double>& slices, DevBuf<GemmDesc>& descs,
                         cudaStream_t s) {
-  return gemm_sub_split(A, lda, B, ldb, false, m, nn, K, lower, C, ldc, 1, 0, 0, slices, descs, s);
+  return predict_gemm_sub_bt_members(A, lda, B, ldb, m, nn, K, lower, C, ldc, 1, 0, 0, slices, descs, s);
 }
 
 }  // namespace bgp

@@ -20,7 +20,7 @@ from ._spec import BGP_MAX_DIM, flatten, num_params, patch_specs
 from .modeling import ConstantModel, ModelSet
 from .parallel import ShardedHODLRSolver
 from .solvers import BasicSolver, HODLRSolver, TrivialSolver
-from .solvers.basic import NONFINITE_RHS
+from .solvers.basic import NONFINITE_RHS, _check_finite
 from .solvers.hodlr import FISHER_HODLR
 from .utils import device_gaussian_samples, multivariate_gaussian_samples
 
@@ -360,7 +360,8 @@ class GP(ModelSet):
         ``sigma`` and ``resid`` (``(B, n)``) are built with the elementwise operations of :func:`_sigma` and of
         ``residual`` (the method the single path forms its residual with), ``const_residual(c)`` being that residual
         for a constant mean ``c``.  ``fact_err[b]`` / ``mean_err[b]`` is the exception the per-vector path meets while
-        factorising (white noise) and while forming the residual (mean), or ``None``."""
+        factorising (white noise) and while forming the residual (mean), or ``None``.  With ``y`` ``None`` no residual
+        is formed: ``resid`` is ``None`` and ``mean_err`` all ``None``."""
         try:
             spec = flatten(self.kernel)
         except Exception:
@@ -374,7 +375,8 @@ class GP(ModelSet):
         kpar = np.ascontiguousarray(full[:, n_mean + n_wn:])
         if kpar.shape[1] != num_params(spec):
             return None
-        y = self._check_dimensions(y)
+        if y is not None:
+            y = self._check_dimensions(y)
 
         fact_err, mean_err = [None] * nb, [None] * nb
         sigma = np.empty((nb, n), dtype=np.float64)
@@ -390,6 +392,8 @@ class GP(ModelSet):
                 except Exception as exc:
                     fact_err[b] = exc
                     sigma[b] = 1.0
+        if y is None:
+            return spec, full, kpar, sigma, None, fact_err, mean_err
         resid = np.empty((nb, n), dtype=np.float64)
         if type(self.mean) is ConstantModel:
             for b in range(nb):
@@ -728,8 +732,7 @@ class GP(ModelSet):
         formula on the host from ``solver.apply_inverse(eye(N))`` and ``kernel.get_gradient``.  ``HODLRSolver`` and
         ``ShardedHODLRSolver`` raise ``NotImplementedError`` before any device work.
         """
-        if isinstance(self.solver_type, type) and issubclass(self.solver_type, (HODLRSolver, ShardedHODLRSolver)):
-            raise NotImplementedError(FISHER_HODLR)
+        self._check_fisher_solver()
         size = len(self)
         fail = np.zeros((size, size), dtype=np.float64)
         if y is not None:
@@ -740,7 +743,7 @@ class GP(ModelSet):
         mask = self.kernel.unfrozen_mask
         # grad_log_likelihood's route for alpha: the fused terms when white-noise or kernel parameters are active
         fused = y is not None and bool(n_wn or n_k)
-        noise = dmu = gk = diagA = alpha = None
+        noise = dmu = kinv_dmu = gk = diagA = alpha = None
         try:
             r = self._residual(y) if fused else None
             v = np.zeros((0, len(self._x)), dtype=np.float64)
@@ -774,7 +777,25 @@ class GP(ModelSet):
             if quiet:
                 return fail
             raise
-        F = np.zeros((size, size), dtype=np.float64)
+        F = self._fisher_matrix(np.zeros((size, size), dtype=np.float64), layout, dmu, kinv_dmu, rows, rdiag, v)
+        if y is None:
+            return F
+        grad = self._grad_row(np.empty(size), layout, dmu, alpha, lambda: noise, diagA, gk, mask, 0.5)
+        return grad, F
+
+    def _check_fisher_solver(self):
+        """The Fisher information's first check: ``NotImplementedError`` on a HODLR-typed GP, before any work."""
+        if isinstance(self.solver_type, type) and issubclass(self.solver_type, (HODLRSolver, ShardedHODLRSolver)):
+            raise NotImplementedError(FISHER_HODLR)
+
+    @staticmethod
+    def _fisher_matrix(F, layout, dmu, kinv_dmu, rows, rdiag, v):
+        """Fill and return the zeroed ``F`` (``(len(gp), len(gp))``) of :func:`fisher_information` from its blocks, for
+        the single and the batched paths alike: the mean block ``1/2 (M + M^T)`` with ``M = dmu . K^-1 dmu^T``
+        (``kinv_dmu``, ``(N, n_mean)``), and the covariance block ``1/2 (R + R^T)`` with ``R`` the white-noise dots
+        ``1/2 rdiag . v^T`` and the kernel entries ``1/2 rows`` (active kernel columns only), ``rows`` and ``rdiag``
+        in the solver's row order (kernel, then white noise) and ``v`` the white-noise vectors (``(n_wn, N)``)."""
+        n_mean, n_wn, n_k = layout
         if n_mean:
             M = np.dot(dmu, kinv_dmu)
             F[:n_mean, :n_mean] = 0.5 * (M + M.T)
@@ -785,9 +806,91 @@ class GP(ModelSet):
             R[:, :n_wn] = 0.5 * np.dot(rdiag[order], v.T)
             R[:, n_wn:] = 0.5 * rows[order]
             F[n_mean:, n_mean:] = 0.5 * (R + R.T)
-        if y is None:
-            return F
-        grad = self._grad_row(np.empty(size), layout, dmu, alpha, lambda: noise, diagA, gk, mask, 0.5)
+        return F
+
+    def batch_fisher_information(self, vectors, y=None, quiet=False):
+        """:func:`fisher_information` at many parameter vectors: ``F`` of shape ``(B, len(gp), len(gp))``, or with ``y``
+        ``(grad, F)`` with ``grad`` ``(B, len(gp))``.  Member ``b`` is bit for bit what
+        ``gp.set_parameter_vector(vectors[b]); gp.fisher_information(y, quiet=quiet)`` returns on the computed ``x`` and
+        ``yerr``: a Jeffreys prior ``1/2 log det F`` for every walker of an ensemble sampler's step, the metric of
+        Riemannian-manifold HMC chains in lock-step, or the Laplace standard errors and Fisher-scoring steps of every
+        start of a multi-start fit, in one call.
+
+        With ``quiet`` a failing member gets the loop's zeros and the others are unaffected; otherwise the exception
+        that loop raises first is raised, with its type and message (white noise or factorisation, then the residual,
+        then the white-noise terms, then the mean gradient), with one difference: the checks that do not depend on the
+        member (the shape of ``vectors``, ``y``'s length) come first.  The GP is left as it was: parameter vector,
+        factorisation, cached solve and dirty flags.  A HODLR-typed GP raises ``NotImplementedError`` before any work,
+        as :func:`fisher_information` does.
+
+        Solvers with a ``batch_fisher_terms`` hook (``BasicSolver``) factorise all members, form their ``K^-1`` and
+        every row's ``K^-1 dK K^-1`` in one batched pass on the device, each launch covering all the members of a chunk
+        (``include/bgp.h: bgp_dense_batch_fisher_terms``).  Any other solver (``TrivialSolver``, plug-ins) takes that
+        loop, and so do a kernel without a valid device program, one with more than 64 parameters (every member then
+        fails as it does in the loop) and a GP whose only active parameters are the mean's.
+
+        :param vectors: ``(B, len(gp))`` active-parameter vectors, as :func:`set_parameter_vector` takes them
+        """
+        self._check_fisher_solver()
+        vectors = self._batch_vectors(vectors)
+        if y is not None:
+            self._check_dimensions(y)
+        size = len(self)
+        out = None
+        if len(vectors) == 0:
+            out = np.empty((0, size), dtype=np.float64), np.empty((0, size, size), dtype=np.float64)
+        batch = getattr(self.solver_type, "batch_fisher_terms", None)
+        if out is None and batch is not None and (len(self.white_noise) or len(self.kernel)):
+            out = self._batch_fisher_device(batch, vectors, y, quiet)
+        if out is None:
+            res = self._batch_loop(vectors, lambda: self.fisher_information(y, quiet=quiet))
+            if y is None:
+                return np.stack(res)
+            out = np.stack([r[0] for r in res]), np.stack([r[1] for r in res])
+        return out if y is not None else out[1]
+
+    def _batch_fisher_device(self, batch, vectors, y, quiet):
+        """The batched dense path of :func:`batch_fisher_information`: ``(grad, F)``, or ``None`` when the kernel has
+        no valid device program or more than ``_MAX_GRAD_PARAMS`` parameters."""
+        members = self._batch_predict_members(vectors, y)  # GP._residual, the single call's residual
+        if members is None or members[2].shape[1] > _MAX_GRAD_PARAMS:
+            return None
+        spec, full, kpar, sigma, resid, fact_err, mean_err = members
+        nb, n, size = len(vectors), len(self._x), len(self)
+        layout = n_mean, n_wn, n_k = self._grad_layout()
+        mask = self.kernel.unfrozen_mask
+        # each member's white-noise vectors and mean gradient, the device's inputs, with the single call's operations;
+        # a member's first failure here is kept for the loop over the members below
+        wn_full = slice(self.mean.full_size, self.mean.full_size + self.white_noise.full_size)
+        noise, dmu, late_err = [None] * nb, [None] * nb, [None] * nb
+        v = np.zeros((nb, n_wn, n), dtype=np.float64)
+        dmu_in = np.zeros((nb, n_mean, n), dtype=np.float64)
+        for b in range(nb):
+            try:
+                if n_wn:
+                    noise[b] = self._swap_eval(self.white_noise, full[b, wn_full], self._white_noise_terms)
+                    v[b] = np.exp(noise[b][0])[None, :] * noise[b][1]
+                dmu[b] = self._member_gradients(layout, full[b])[0]
+                if n_mean:
+                    d = np.array(dmu[b].T, dtype=np.float64, order="F")
+                    _check_finite(d)  # BasicSolver.apply_inverse's check, which the single call's solve meets
+                    dmu_in[b] = d.T
+            except Exception as exc:
+                late_err[b] = exc
+        gterms, rows, rdiag, kdmu, info = batch(spec, kpar, self._x, sigma, resid, mask.astype(np.uint32), v, dmu_in)
+        grad = np.zeros((nb, size), dtype=np.float64)
+        F = np.zeros((nb, size, size), dtype=np.float64)
+        for b in range(nb):  # the loop's order: factorisation (white noise included), residual, white noise, mean
+            if self._member_failed(spec, kpar, b, info, fact_err, mean_err, quiet, True):
+                continue
+            if late_err[b] is not None:
+                if quiet and isinstance(late_err[b], ValueError):
+                    continue
+                raise late_err[b]
+            self._fisher_matrix(F[b], layout, dmu[b], kdmu[b].T, rows[b][:, mask], rdiag[b], v[b])
+            if y is not None:
+                alpha, g, diag = gterms
+                self._grad_row(grad[b], layout, dmu[b], alpha[b], lambda: noise[b], diag[b], g[b], mask, 0.5)
         return grad, F
 
     def _fisher_rows_host(self, v, n_k):

@@ -75,14 +75,15 @@ def _test_points(kernel, xs):
 
 def _batch_inputs(spec, params, x, yerr, r, xs=None, which=None):
     """``(x, xs, params, yerr, r, which)`` normalised and checked for the ``batch_*`` statics: ``x`` ``(n, ndim)``,
-    ``params`` ``(B, num_params(spec))``, ``yerr`` and ``r`` ``(B, n)``, ``which`` (when given) ``(P,)``, then the
-    dimension of the program, ``x`` and ``xs`` (when given, ``(ns, ndim)``)."""
+    ``params`` ``(B, num_params(spec))``, ``yerr`` and ``r`` (``None`` allowed) ``(B, n)``, ``which`` (when given)
+    ``(P,)``, then the dimension of the program, ``x`` and ``xs`` (when given, ``(ns, ndim)``)."""
     x = _points(x)
     if xs is not None:
         xs = _points(xs)
     params = np.ascontiguousarray(params, dtype=np.float64)
     yerr = np.ascontiguousarray(yerr, dtype=np.float64)
-    r = np.ascontiguousarray(r, dtype=np.float64)
+    if r is not None:
+        r = np.ascontiguousarray(r, dtype=np.float64)
     if which is not None:
         which = np.ascontiguousarray(which, dtype=np.uint32)
     if x.ndim != 2 or x.shape[0] == 0:
@@ -92,7 +93,7 @@ def _batch_inputs(spec, params, x, yerr, r, xs=None, which=None):
     if params.ndim != 2 or params.shape[1] != npar:
         raise ValueError("params must have shape (B, {0})".format(npar))
     nb = params.shape[0]
-    if yerr.shape != (nb, n) or r.shape != (nb, n):
+    if yerr.shape != (nb, n) or (r is not None and r.shape != (nb, n)):
         raise ValueError("yerr and r must have shape ({0}, {1})".format(nb, n))
     if which is not None and which.shape != (npar,):
         raise ValueError("which must have shape ({0},)".format(npar))
@@ -103,13 +104,13 @@ def _batch_inputs(spec, params, x, yerr, r, xs=None, which=None):
 
 def _batch_call(name, spec, params, x, yerr, r, *rest):
     """The library's batched entry point ``name`` on the shared workspace, with the members' common arguments followed
-    by ``rest``; nothing for no members."""
+    by ``rest`` (``r`` ``None`` passes NULL); nothing for no members."""
     nb, (n, ndim) = params.shape[0], x.shape
     if nb == 0:
         return
     h = _get_batch_handle()
     _lib.check(getattr(h.lib, name)(h.ptr, C.byref(spec), _lib.ptr(params), nb, params.shape[1], _lib.ptr(x), n, ndim,
-                                    _lib.ptr(yerr), _lib.ptr(r), *rest))
+                                    _lib.ptr(yerr), None if r is None else _lib.ptr(r), *rest))
 
 
 def _grad_x_terms_call(call, n, ndim, r, which):
@@ -466,6 +467,41 @@ class BasicSolver(object):
         _batch_call("bgp_dense_batch_loo_terms", spec, params, x, yerr, r, _lib.ptr(which), _lib.ptr(alpha),
                     _lib.ptr(d), _lib.ptr(beta), _lib.ptr(g), _lib.ptr(diag), _lib.ptr(info))
         return alpha, d, beta, g, diag, info
+
+    @staticmethod
+    def batch_fisher_terms(spec, params, x, yerr, r, which, v, dmu):
+        """``(grad_terms, rows, rdiag, kdmu, info)`` for ``B`` parameter vectors of one kernel program on the same
+        ``x``: member ``b`` factorises as in :func:`batch_log_likelihood` and returns what :func:`fisher_terms` returns
+        for it with ``which`` (``(P,)``, shared by all members) and its white-noise vectors ``v[b]`` (``v`` ``(B, nv,
+        n)``), ``rows`` ``(B, nrow, P)`` and ``rdiag`` ``(B, nrow, n)``, plus ``kdmu[b] = K_b^-1 dmu[b]^T`` stored as
+        ``(nm, n)`` for its mean gradients ``dmu[b]`` (``dmu`` ``(B, nm, n)``), the solve of ``apply_inverse``
+        (``include/bgp.h: bgp_dense_batch_fisher_terms``).  ``grad_terms`` is ``(alpha, g, diag)`` as
+        :func:`batch_grad_terms` returns them when ``r`` (``(B, n)``) is given and ``None`` when ``r`` is ``None``.
+        ``info`` is that of :func:`batch_log_likelihood`; a failed member's rows are NaN.  A member's outputs are
+        bit-identical to :func:`compute` with its spec and yerr followed by :func:`fisher_terms` and
+        ``apply_inverse(dmu[b].T)``.  More than 64 kernel parameters raise ``ValueError`` before anything is solved."""
+        x, _, params, yerr, r, which = _batch_inputs(spec, params, x, yerr, r, which=which)
+        nb, n, npar = params.shape[0], x.shape[0], params.shape[1]
+        v = np.ascontiguousarray(v, dtype=np.float64)
+        dmu = np.ascontiguousarray(dmu, dtype=np.float64)
+        if v.ndim != 3 or v.shape[0] != nb or v.shape[2] != n or dmu.ndim != 3 or dmu.shape[0] != nb or \
+                dmu.shape[2] != n:
+            raise ValueError("v and dmu must have shape ({0}, nv, {1}) and ({0}, nm, {1})".format(nb, n))
+        nv, nm = v.shape[1], dmu.shape[1]
+        nrow = int(np.count_nonzero(which)) + nv
+        rows = np.empty((nb, nrow, npar), dtype=np.float64)
+        rdiag = np.empty((nb, nrow, n), dtype=np.float64)
+        kdmu = np.empty((nb, nm, n), dtype=np.float64)
+        info = np.zeros(nb, dtype=np.int32)
+        terms = (None, None, None)
+        if r is not None:
+            terms = (np.empty((nb, n), dtype=np.float64), np.empty((nb, npar), dtype=np.float64),
+                     np.empty((nb, n), dtype=np.float64))
+        _batch_call("bgp_dense_batch_fisher_terms", spec, params, x, yerr, r, _lib.ptr(which),
+                    _lib.ptr(v) if nv else None, nv, _lib.ptr(dmu) if nm else None, nm,
+                    *[None if t is None else _lib.ptr(t) for t in terms], _lib.ptr(rows), _lib.ptr(rdiag),
+                    _lib.ptr(kdmu), _lib.ptr(info))
+        return (None if r is None else terms), rows, rdiag, kdmu, info
 
     @staticmethod
     def batch_predict(spec, params, x, yerr, r, xs, what):

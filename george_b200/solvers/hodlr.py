@@ -21,13 +21,15 @@ FISHER_HODLR = ("the Fisher information is not implemented for the HODLR solvers
 class HODLRSolver(BasicSolver):
 
     # no batched HODLR factorisation: GP.batch_log_likelihood, GP.batch_predict, GP.batch_grad_log_likelihood,
-    # GP.batch_sample_conditional, GP.batch_grad_predict and the GP.batch_*loo* methods take their per-vector loops
+    # GP.batch_sample_conditional, GP.batch_grad_predict and the GP.batch_*loo* methods take their per-vector loops;
+    # GP.batch_fisher_information raises NotImplementedError, as GP.fisher_information does
     batch_log_likelihood = None
     batch_predict = None
     batch_grad_terms = None
     batch_sample = None
     batch_predict_grad = None
     batch_loo_terms = None
+    batch_fisher_terms = None
 
     def __init__(self, kernel, min_size=100, tol=0.1, seed=42, rng_mode=None, rank_capacity=0,
                  exhaust="dense"):

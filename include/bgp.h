@@ -71,8 +71,8 @@ uint64_t bgp_launch_count(void);
  *   - an expression depth of at most 8: the operand stack of the postfix program, e.g. 8 leaves nested to the right,
  *     k1 + (k2 + (... + k8)), while any number of left-nested operators keep it at 2;
  *   - hyper-parameter gradients (bgp_kmat_gradient_*, bgp_kmat_gradient_contract, bgp_dense_grad_terms,
- *     bgp_dense_batch_grad_terms, bgp_hodlr_grad_terms, bgp_*_loo_terms) take at most 64 hyper-parameters, checked
- *     before anything is solved;
+ *     bgp_dense_batch_grad_terms, bgp_hodlr_grad_terms, bgp_*_loo_terms, bgp_dense_batch_fisher_terms) take at most 64
+ *     hyper-parameters, checked before anything is solved;
  *   - input-coordinate gradients (bgp_kmat_x1/x2_gradient_general) take at most BGP_MAX_DIM = 8 input dimensions;
  *   - the HODLR solver takes at most 32 input dimensions.
  * The kernel-matrix builds, the matvec, the dense solver, the batched paths and predictions have no input-dimension
@@ -404,6 +404,45 @@ int bgp_dense_batch_loo_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spe
                               double* alpha, double* d,                /* B x n, may be NULL          */
                               double* beta, double* g, double* diag,   /* B x n, B x P, B x n, or NULL */
                               int32_t* info);                          /* B                           */
+/* Batched Fisher information rows (GP.batch_fisher_information): for the same B members as
+ * bgp_dense_batch_log_likelihood (spec, params, x, yerr) and one selection `which` (P entries, shared by all members),
+ * what bgp_dense_fisher_terms returns for each member, plus the mean block's solve:
+ *   alpha[b*n + i], g[b*P + p], diag[b*n + i]   bgp_dense_batch_grad_terms' outputs, with r (B x n row-major)
+ *   rows[(b*nrow + k)*P + q]                      sum_ij B_b,k,ij dK_b,ij/dtheta_q                        (B x nrow x P)
+ *   rdiag[(b*nrow + k)*n + i]                     B_b,k,ii                                                (B x nrow x n)
+ *   kdmu[(b*nm + m)*n + i]                        (K_b^-1 dmu_b,m)_i                                      (B x nm x n)
+ * with nrow = (number of which[q] != 0) + nv and B_b,k = K_b^-1 dK K_b^-1 for row k's dK, in bgp_dense_fisher_terms'
+ * order: the kernel rows (ascending q), then one row per white-noise vector v[(b*nv + k)*n + i] (B x nv x n: the vectors
+ * depend on the member's white-noise parameters; dK = diag(v_b,k)).  dmu (B x nm x n) holds each member's nm mean
+ * gradients; kdmu is the nm-column bgp_dense_apply_inverse of them.  A NULL r skips the residual upload, alpha and the
+ * contraction of alpha alpha^T - K^-1 (alpha, g and diag are then not written).  Any output but info may be NULL.
+ * Each member's outputs are bit-identical to bgp_dense_compute followed by bgp_dense_fisher_terms and
+ * bgp_dense_apply_inverse(dmu_b) on member b's spec and yerr: the same kernels run with a member index (K_b^-1 by
+ * solving against the identity; the gradient planes with the same evaluator and one-hot mask; both products with the
+ * single call's split-K plan; the same contraction tiles and fixed reduction order), so a member's results do not depend
+ * on B, its position or the chunking.  info[b] as in bgp_dense_batch_log_likelihood (0, the leading-minor index, or -1
+ * for an invalid member program); a failed member's outputs are NaN and do not disturb the other members.
+ * Members run in chunks that fit in 4 GiB of device memory (BGP_BATCH_CHUNK=<members> overrides it), capped so that
+ * each split-K product is one launch; every launch of a row covers the whole chunk, so the launch count depends on n,
+ * nrow and the number of chunks, never on B within a chunk.
+ * Device workspace per member (doubles): 2 n^2 (factor and K^-1) + 2 n^2 (P and T, none when nrow = 0) + nsplit n^2
+ * (the products' split-K slices, none when nsplit = 1: 2 n^2 at n = 512, none from n = 2049 on a 132-SM H100 SXM) +
+ * (4 + t) n (the vectors of batch_reserve_common; t = the larger of n for n <= 8 and nm for nm <= 8, else 1) +
+ * ceil(n / 32)^2 P contraction partials + P (g) + nrow (P + n) (rows, rdiag) + nv n (v) + nm n (dmu).  Shared: B
+ * programs, x, which.
+ * Errors: those of bgp_dense_batch_log_likelihood; BGP_ERR_INVALID for P > 64, a NULL which with P > 0, nv < 0 or nm < 0,
+ * and a NULL v or dmu with nv > 0 or nm > 0, before anything is solved; BGP_ERR_NOMEM when a single member does not
+ * fit.  B == 0 writes nothing. */
+int bgp_dense_batch_fisher_terms(bgp_dense_batch_t* h, const bgp_kernel_spec_t* spec, const double* params,
+                                 int64_t B, int64_t P, const double* x, int64_t n, int32_t ndim,
+                                 const double* yerr, const double* r,   /* B x n row-major; r may be NULL */
+                                 const uint32_t* which,                 /* P, shared by all members       */
+                                 const double* v, int32_t nv,           /* B x nv x n                     */
+                                 const double* dmu, int32_t nm,         /* B x nm x n                     */
+                                 double* alpha, double* g, double* diag, /* B x n, B x P, B x n, or NULL  */
+                                 double* rows, double* rdiag,           /* B x nrow x P, B x nrow x n     */
+                                 double* kdmu,                          /* B x nm x n, may be NULL        */
+                                 int32_t* info);                        /* B                              */
 /* Batched predictions (GP.batch_predict): for the same B members as bgp_dense_batch_log_likelihood (spec, params, x,
  * yerr; r = y - mean(x) per member, B x n row-major) and the test points xs (ns x ndim row-major, host):
  *   mean[b*ns + j]        = (K_b(x*, x) K_b^-1 r_b)_j            (the kernel part of GP.predict's mean)

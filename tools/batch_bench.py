@@ -1,8 +1,8 @@
 # -*- coding: utf-8 -*-
 """The GP.batch_* methods against the per-vector loops they replace (set_parameter_vector, then the one-vector method).
 
-    python tools/batch_bench.py --entry {log_likelihood,grad,predict,grad_predict,sample,loo}
-        [--workload co2|matern52_3d]
+    python tools/batch_bench.py --entry {log_likelihood,grad,predict,grad_predict,sample,loo,fisher}
+        [--workload co2|matern52_3d|matern32_1d]
         [--min-seconds 1.0] [--cpu-members 4] [--kind mean|var|cov] [--rounds 7] [--reps 5]
 
 One JSON line per shape.  Every line has
@@ -30,9 +30,12 @@ and the fields of its entry:
                   loo_log_likelihood and grad_loo_log_likelihood, per method: loop_ms_per_member and
                   batch_ms_per_member (host-clock medians over --rounds alternating rounds), loop_spread / batch_spread
                   (min, max per member), speedup and equal (the outputs are bit-identical in every round)
-Workloads: the CO2 GP of the hyper-parameter tutorial (a sum of four kernel products, fitted mean and white noise) and
-Matern-5/2 3-D (the Bayesian-optimisation case), at the sizes listed in each entry's table below: the sizes a sampler's
-step, a posterior-predictive pass or an acquisition optimiser's step uses.  Every shape is warmed up first, through
+  fisher          GP.batch_fisher_information(quiet=True), without and with y, against fisher_information: the fields
+                  of loo
+Workloads: the CO2 GP of the hyper-parameter tutorial (a sum of four kernel products, fitted mean and white noise),
+Matern-5/2 3-D (the Bayesian-optimisation case) and Matern-3/2 1-D (a light curve with a fitted mean and white noise,
+the Fisher information's large case), at the sizes listed in each entry's table below: the sizes a sampler's step, a
+posterior-predictive pass or an acquisition optimiser's step uses.  Every shape is warmed up first, through
 both routes.
 """
 import argparse
@@ -93,7 +96,18 @@ def matern_gp(n, seed=0):
     return gp, y, 0.05, lambda ns: np.random.default_rng(seed + 1).uniform(-3, 3, (ns, 3))
 
 
-MODELS = {"co2": co2_gp, "matern52_3d": matern_gp}
+def matern32_gp(n, seed=0):
+    """As :func:`co2_gp`."""
+    rng = np.random.default_rng(seed)
+    t = np.sort(rng.uniform(0, 100, n))
+    y = np.sin(t / 3) + 0.1 * rng.standard_normal(n)
+    gp = george.GP(1.3 * kernels.Matern32Kernel(4.0), mean=0.1, fit_mean=True, white_noise=np.log(0.05),
+                   fit_white_noise=True)
+    gp.compute(t, 0.3)
+    return gp, y, 0.05, lambda ns: np.linspace(0, 100, ns)
+
+
+MODELS = {"co2": co2_gp, "matern52_3d": matern_gp, "matern32_1d": matern32_gp}
 
 
 def repeat(fn, min_seconds):
@@ -149,7 +163,7 @@ def _timed_hook(name):
 
 
 for _name in ("batch_log_likelihood", "batch_grad_terms", "batch_predict", "batch_predict_grad", "batch_sample",
-              "batch_loo_terms"):
+              "batch_loo_terms", "batch_fisher_terms"):
     setattr(TimedSolver, _name, _timed_hook(_name))
 
 
@@ -402,8 +416,46 @@ def bench_loo(args, emit):
                       "speedup": round(ml / mb, 2), "equal": bool(equal)})
 
 
+def bench_fisher(args, emit):
+    """CO2 at n = 512 with B = 64, where a single call's rows are launch-bound; Matern-3/2 1-D at n = 4096 with
+    B = 16, where they run near the tensor pipe's rate."""
+    work = [("co2", 512, 64), ("matern32_1d", 4096, 16)]
+    for name, n, nb in work:
+        if args.workload not in (None, name):
+            continue
+        gp, y, scale, _ = MODELS[name](n)
+        gp.log_likelihood(y)
+        vecs = vectors(gp, scale, nb, np.random.default_rng(n))
+        for method, yy in (("F", None), ("grad_F", y)):
+            def one():
+                res = loop(gp, vecs, lambda: gp.fisher_information(yy, quiet=True))
+                if yy is None:
+                    return np.stack(res)
+                return np.stack([r[0] for r in res]), np.stack([r[1] for r in res])
+            batch = lambda: gp.batch_fisher_information(vecs, yy, quiet=True)  # noqa: E731
+
+            def same(a, b):
+                a, b = (a, b) if isinstance(a, tuple) else ((a,), (b,))
+                return all(np.array_equal(u, w) for u, w in zip(a, b))
+            want = one()  # warm-up of this shape (workspace, code paths) for both routes
+            equal = same(batch(), want)
+            t_loop, t_batch = [], []
+            for _ in range(args.rounds):  # alternate the two routes
+                for fn, ts in ((one, t_loop), (batch, t_batch)):
+                    dt, out = timed(fn)
+                    ts.append(dt * 1e3 / nb)
+                    equal = equal and same(out, want)
+            ml, mb = float(np.median(t_loop)), float(np.median(t_batch))
+            emit({"workload": name, "n": n, "B": nb, "method": method,
+                  "loop_ms_per_member": round(ml, 4), "batch_ms_per_member": round(mb, 4),
+                  "loop_spread": [round(min(t_loop), 4), round(max(t_loop), 4)],
+                  "batch_spread": [round(min(t_batch), 4), round(max(t_batch), 4)],
+                  "batch_device_ms_per_member": round(device_ms(gp, batch) / nb, 4),
+                  "speedup": round(ml / mb, 2), "equal": bool(equal)})
+
+
 ENTRIES = {"log_likelihood": bench_log_likelihood, "grad": bench_grad, "predict": bench_predict,
-           "grad_predict": bench_grad_predict, "sample": bench_sample, "loo": bench_loo}
+           "grad_predict": bench_grad_predict, "sample": bench_sample, "loo": bench_loo, "fisher": bench_fisher}
 
 
 def main():
@@ -413,7 +465,7 @@ def main():
     ap.add_argument("--min-seconds", type=float, default=1.0, help="log_likelihood, grad, predict: per timing")
     ap.add_argument("--cpu-members", type=int, default=4, help="log_likelihood: members of the CPU route")
     ap.add_argument("--kind", choices=["mean", "var", "cov"], default=None, help="predict: only this kind")
-    ap.add_argument("--rounds", type=int, default=7, help="grad_predict, loo: alternating rounds")
+    ap.add_argument("--rounds", type=int, default=7, help="grad_predict, loo, fisher: alternating rounds")
     ap.add_argument("--reps", type=int, default=5, help="sample: alternating repetitions")
     args = ap.parse_args()
     assert george._lib.load().bgp_device_count() > 0, "no device: this benchmark measures the H100 path"
