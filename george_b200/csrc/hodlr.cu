@@ -2246,7 +2246,6 @@ int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n
   BGP_TRY(require_device());
   if (m <= 0 || n <= 0 || k <= 0) { set_error("bgp_selftest_gemm: bad sizes"); return BGP_ERR_INVALID; }
   if (mode & ~(GD_ATOMIC_ADD | GD_LOWER)) { set_error("bgp_selftest_gemm: bad mode %d", mode); return BGP_ERR_INVALID; }
-  if (a_kcontig && !b_kcontig) { set_error("bgp_selftest_gemm: the (A K-contiguous) x (B N-contiguous) variant is not built"); return BGP_ERR_INVALID; }
   cudaStream_t s = 0;
   const size_t na = (size_t)(a_kcontig ? m : k) * lda, nb = (size_t)(b_kcontig ? n : k) * ldb, nc = (size_t)n * ldc;
   DevBuf<double> dA, dB, dC;
@@ -2259,7 +2258,8 @@ int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n
   g.A = dA.p; g.B = dB.p; g.C = dC.p; g.M = m; g.N = n; g.K = k; g.mode = mode;
   g.lda = lda; g.ldb = ldb; g.ldc = ldc;
   BGP_CUDA(cudaMemcpyAsync(dd.p, &g, sizeof(g), cudaMemcpyHostToDevice, s));
-  if (a_kcontig) BGP_TRY((gemm_dmma_launch<true, true>(dd.p, 1, m, n, nullptr, s)));
+  if (a_kcontig && b_kcontig) BGP_TRY((gemm_dmma_launch<true, true>(dd.p, 1, m, n, nullptr, s)));
+  else if (a_kcontig) BGP_TRY((gemm_dmma_launch<true, false>(dd.p, 1, m, n, nullptr, s)));
   else if (b_kcontig) BGP_TRY((gemm_dmma_launch<false, true>(dd.p, 1, m, n, nullptr, s)));
   else BGP_TRY((gemm_dmma_launch<false, false>(dd.p, 1, m, n, nullptr, s)));
   BGP_CUDA(cudaMemcpyAsync(C_host, dC.p, sizeof(double) * nc, cudaMemcpyDeviceToHost, s));

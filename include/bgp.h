@@ -889,9 +889,10 @@ int bgp_hodlr_last_aca_profile(const bgp_hodlr_t* h, double* p12);
  *     column-major, ld n) is overwritten by S^-1 R, *logdet = log|det S|      (stands in for Eigen::FullPivLU,
  *     hodlr.h:228-234, :90-93, :250).
  *   bgp_selftest_gemm: C (m x n, column-major ldc) -= A' B'; A' (m,k) = a_kcontig ? A[m*lda+k] : A[k*lda+m];
- *     B' (k,n) = b_kcontig ? B[n*ldb+k] : B[k*ldb+n].  Built variants: (a_kcontig, b_kcontig) = (1,1), (0,1) and (0,0)
- *     (the last is the one the dense Cholesky's trailing updates use).  mode: bit 0 (1) C += A'B' with atomics instead,
- *     bit 8 (256) only entries with row >= column are written (the Cholesky's lower-triangular output). */
+ *     B' (k,n) = b_kcontig ? B[n*ldb+k] : B[k*ldb+n].  All four (a_kcontig, b_kcontig) variants are built: (0,0) is the
+ *     one the dense Cholesky's trailing updates use, (1,0) the Fisher rows' second product.  mode: bit 0 (1) C += A'B'
+ *     with atomics instead, bit 8 (256) only entries with row >= column are written (the Cholesky's lower-triangular
+ *     output). */
 int bgp_selftest_lu(int32_t n, int32_t nrhs, const double* S_host, double* R_host, double* logdet);
 int bgp_selftest_gemm(int32_t a_kcontig, int32_t b_kcontig, int32_t m, int32_t n, int32_t k, const double* A_host,
                       int64_t lda, const double* B_host, int64_t ldb, double* C_host, int64_t ldc, int32_t mode);

@@ -29,7 +29,9 @@ Everything else follows in O(n):
   ``g_c = r . alpha - n`` and ``g_m = alpha^T D alpha / 2 - tr(K^-1 D) / 2``.  D is semi-separable: ``D a`` takes one
   forward and one backward sweep, and ``tr(K^-1 D)`` needs only the first off-diagonal of K^-1 (D's diagonal is 0);
 * the leave-one-out terms of ``loo_terms`` (``loo_terms`` has the derivation): ``K^-1 diag(w) K^-1`` is pentadiagonal,
-  and each contraction with K or D is a dot with one ``K a`` / ``D a`` sweep plus five bands.
+  and each contraction with K or D is a dot with one ``K a`` / ``D a`` sweep plus five bands;
+* the likelihood factors over the points, ``p(r) = prod_j N(r_j; rho_j r_{j-1}, c s_j^2)`` (``factor_terms``), and the
+  expected Fisher information (``fisher``) and the gradient in the inputs (``grad_x``) are sums over those factors.
 
 Every recursion runs on the ratios ``rho_j`` and the scaled gaps ``(x_j - x_{j-1}) / l``, never on ``exp(+-x / l)``,
 so nothing overflows however long the interval.  All arithmetic is ``np.longdouble`` (x87 80-bit on x86-64, eps
@@ -223,6 +225,85 @@ class OU(object):
         gscale = np.array([Kab @ aa + band_k, (Dab @ aa + band_d) / 2], dtype=LD)
         return dict(alpha=alpha, d=d, beta=beta, g=np.array([g_c, g_m], dtype=LD), diagA=alpha * beta - M0,
                     value=value, gscale=gscale)
+
+    # ---- the factors of the likelihood: Fisher information and input gradient -------------------------------------
+    def factor_terms(self, r, delta=None):
+        """``t_j = log N(r_j; rho_j r_{j-1}, v_j)`` with ``v_0 = c`` and ``v_j = c s_j^2``, so that ``sum_j t_j`` is the
+        log-likelihood of ``r`` (``(n,)``).  ``K = L L^T`` with ``L = sqrt(c) A diag(s)`` makes ``L^-1 r`` the scaled
+        innovations ``u_j / (sqrt(c) s_j)``, ``u_j = r_j - rho_j r_{j-1}``, and ``log det K`` the sum of ``log v_j``.
+        ``delta`` (``(n,)``, entry 0 unused) replaces the scaled gaps: t_j depends on the inputs through delta_j alone."""
+        r = np.asarray(r, dtype=LD)
+        dl = self.delta if delta is None else np.asarray(delta, dtype=LD)
+        rho = np.exp(-dl)
+        rho[0] = 0
+        v = -self.c * np.expm1(-2 * dl)
+        v[0] = self.c
+        u = r.copy()
+        u[1:] -= rho[1:] * r[:-1]
+        return -np.log(2 * LD(np.pi) * v) / 2 - u * u / (2 * v)
+
+    def fisher(self, mean=True):
+        """The expected Fisher information for theta = (log c, log m), led by a constant mean's row with ``mean``:
+        ``(3, 3)`` in the order (mean, log c, log m), or ``(2, 2)``.
+
+        The factors of ``factor_terms`` have scores of zero conditional mean given the earlier points, so scores of
+        different factors are uncorrelated and F sums over the factors.  For ``N(r; rho r', v)`` with ``E[r'^2] = c``
+        a factor adds ``c drho_p drho_q / v + dv_p dv_q / (2 v^2)``.  With ``drho_j/dlog m = rho_j delta_j / 2``
+        (``delta_j = gap / sqrt(m)``), ``dv_j/dlog m = -c rho_j^2 delta_j``, ``dv_j/dlog c = v_j``, ``drho/dlog c = 0``
+        and nothing for factor 0 but its ``log c`` term:
+
+            F_cc = n / 2,   F_cm = -sum_j rho_j^2 delta_j / (2 s_j^2) = tr(K^-1 D) / 4,
+            F_mm = sum_j [rho_j^2 delta_j^2 / (4 s_j^2) + rho_j^4 delta_j^2 / (2 s_j^4)].
+
+        The mean enters the mean of r only: ``F_mumu = 1^T K^-1 1``, the sum of the tridiagonal K^-1's entries, and
+        its cross terms with the kernel parameters are 0."""
+        rho2, dl, s2 = self.rho[1:] ** 2, self.delta[1:], self.s2[1:]
+        F = np.zeros((2, 2), dtype=LD)
+        F[0, 0] = LD(self.n) / 2
+        F[0, 1] = F[1, 0] = -np.sum(rho2 * dl / (2 * s2))
+        F[1, 1] = np.sum(rho2 * dl * dl / (4 * s2) + rho2 * rho2 * dl * dl / (2 * s2 * s2))
+        if not mean:
+            return F
+        d, e = self.inv_tridiag()
+        out = np.zeros((3, 3), dtype=LD)
+        out[0, 0] = np.sum(d) + 2 * np.sum(e)
+        out[1:, 1:] = F
+        return out
+
+    def grad_x(self, r):
+        """``(dx, scale)``: ``dx_i = d log p(r) / d x_i`` (``(n,)``), which is ``sum_j (alpha alpha^T - K^-1)_ij
+        dk(x_i, x_j)/dx_i``, and a per-entry bound of what that contraction sums.
+
+        Factor j of ``factor_terms`` depends on the inputs through the gap ``x_j - x_{j-1}`` alone.  With
+        ``rho' = -rho_j / l`` and ``v' = 2 c rho_j^2 / l`` its derivatives in the gap, the factor's derivative is
+
+            G_j = -v' / (2 v_j) + u_j r_{j-1} rho' / v_j + u_j^2 v' / (2 v_j^2),
+
+        and x_i is the upper end of gap i and the lower end of gap i + 1: ``dx_i = G_i - G_{i+1}`` (G_0 = G_n = 0),
+        which telescopes to ``sum_i dx_i = 0``.
+
+        ``scale_i >= sum_j |A_ij| |dk_ij/dx_i|`` (A = alpha alpha^T - K^-1): ``|dk_ij/dx_i| = k_ij / l`` off the
+        diagonal and 0 on it, and K^-1 is tridiagonal, so it is ``|alpha_i| ((K |alpha|)_i - c |alpha_i|) / l`` plus
+        ``|K^-1_{i,i+-1}| k_{i,i+-1} / l`` for the two neighbours."""
+        r = np.asarray(r, dtype=LD)
+        rho, s2, ell, n = self.rho[1:], self.s2[1:], self.ell, self.n
+        v = self.c * s2
+        u = r[1:] - rho * r[:-1]
+        drho = -rho / ell
+        dv = 2 * self.c * rho * rho / ell
+        G = -dv / (2 * v) + u * r[:-1] * drho / v + u * u * dv / (2 * v * v)
+        dx = np.zeros(n, dtype=LD)
+        dx[1:] += G
+        dx[:-1] -= G
+        alpha = self.solve(r)
+        aa = np.abs(alpha)
+        ka = self.apply_k(aa)
+        _, e = self.inv_tridiag()
+        nb = np.abs(e) * self.c * rho / ell  # |K^-1_{j,j+1}| |dk_{j,j+1}|
+        scale = aa * (ka - self.c * aa) / ell
+        scale[1:] += nb
+        scale[:-1] += nb
+        return dx, scale
 
     # ---- prediction -------------------------------------------------------------------------------------------------
     def predict(self, t, alpha):

@@ -9,8 +9,11 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 
-def _gemm(lib, a_k, A, B, Cm, atomic):
-    """A: stored array (column-major semantics handled by the caller), returns updated C (m x n)."""
+GD_ATOMIC_ADD, GD_LOWER = 1, 256
+
+
+def _gemm(lib, a_k, b_k, A, B, Cm, mode):
+    """A, B: stored arrays (column-major semantics handled by the caller), returns updated C (m x n)."""
     from george_b200 import _lib
     m, n = Cm.shape
     k = A.shape[1] if a_k == 0 else A.shape[0]
@@ -18,8 +21,8 @@ def _gemm(lib, a_k, A, B, Cm, atomic):
     Af = np.asfortranarray(A)
     Bf = np.asfortranarray(B)
     Cf = np.asfortranarray(Cm.copy())
-    _lib.check(lib.bgp_selftest_gemm(a_k, 1, m, n, k, _lib.ptr(Af), Af.shape[0], _lib.ptr(Bf), Bf.shape[0],
-                                     _lib.ptr(Cf), Cf.shape[0], int(atomic)))
+    _lib.check(lib.bgp_selftest_gemm(a_k, b_k, m, n, k, _lib.ptr(Af), Af.shape[0], _lib.ptr(Bf), Bf.shape[0],
+                                     _lib.ptr(Cf), Cf.shape[0], mode))
     return Cf
 
 
@@ -27,20 +30,25 @@ def _gemm(lib, a_k, A, B, Cm, atomic):
                                    (513, 129, 33)])
 @pytest.mark.parametrize("a_k", [0, 1])
 def test_dmma_gemm_variants(gpu, m, n, k, a_k):
+    """Every (a_kcontig, b_kcontig) variant in the subtracting, atomic-adding and lower-only modes; the lower-only
+    mode leaves the entries above the diagonal untouched."""
     from george_b200 import _lib
     lib = _lib.load()
     rng = np.random.default_rng(m * 7 + n * 3 + k)
     Ap = rng.normal(size=(m, k))          # A' (m x k)
-    Bp = rng.normal(size=(k, n))          # B' (k x n), stored K x N column-major  (b_kcontig)
+    Bp = rng.normal(size=(k, n))          # B' (k x n)
     C0 = rng.normal(size=(m, n))
     A_store = Ap if a_k == 0 else Ap.T.copy()   # a_k=0: M x K column-major; a_k=1: K x M column-major
-    for atomic in (0, 1):
-        got = _gemm(lib, a_k, A_store, Bp, C0, atomic)
-        want = C0 + Ap @ Bp if atomic else C0 - Ap @ Bp
-        np.testing.assert_allclose(got, want, rtol=0, atol=1e-11 * max(1.0, np.sqrt(k)))
-
-
-GD_LOWER = 256
+    lower = np.tril(np.ones((m, n), dtype=bool))
+    for b_k in (0, 1):
+        B_store = Bp if b_k == 1 else Bp.T.copy()  # b_k=1: K x N column-major; b_k=0: N x K column-major
+        for mode in (0, GD_ATOMIC_ADD, GD_LOWER):
+            got = _gemm(lib, a_k, b_k, A_store, B_store, C0, mode)
+            want = C0 + Ap @ Bp if mode == GD_ATOMIC_ADD else C0 - Ap @ Bp
+            if mode == GD_LOWER:
+                assert np.array_equal(got[~lower], C0[~lower]), (b_k, mode)
+                got, want = got[lower], want[lower]
+            np.testing.assert_allclose(got, want, rtol=0, atol=1e-11 * max(1.0, np.sqrt(k)), err_msg=str((b_k, mode)))
 
 
 @pytest.mark.parametrize("n,e,b,cend", [

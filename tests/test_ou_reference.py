@@ -5,10 +5,13 @@ The closed forms are what the large-index GPU tests (``test_gpu_zz_large_index.p
 where no O(n^3) reference runs, so each quantity they use is pinned here at n <= 500: the factor's columns, log det,
 solves, the tridiagonal K^-1, ``z L^T``, ``D a``, the gradient terms (against ``einsum`` over the oracle's gradient
 tensor, which also fixes the factor 1/2 and the sign of the ``log m`` derivative), the predictive mean and variance,
-and the leave-one-out terms of ``test_gpu_zz_loo_closed_form.py`` (``K a``, alpha, d, beta, diag(A), g and its scale
-against the brute-force formula, the value and LOO predictive against refits without the point).
+the leave-one-out terms of ``test_gpu_zz_loo_closed_form.py`` (``K a``, alpha, d, beta, diag(A), g and its scale
+against the brute-force formula, the value and LOO predictive against refits without the point), and the Fisher
+information and input gradient of ``test_gpu_zz_fisher_grad_x_closed_form.py`` (F against the trace formula over the
+oracle's gradient tensor; dx and its scale against the contraction with the oracle's x-gradient, and against central
+differences of the log-likelihood, which do not go through that contraction).
 The differences are the float64 rounding of K's entries carried through cond(K) <= 10 (largest measured: 1.5e-15, in
-the LOO diag(A); bar 1e-14).
+the LOO diag(A); bar 1e-14); the central differences have their own bar.
 """
 import numpy as np
 import pytest
@@ -150,6 +153,77 @@ def test_loo_terms_match_the_longdouble_formula(oracle, n, c, m, gap):
         term = -np.log(2 * LD(np.pi) * var) / 2 - (r[i] - mu) ** 2 / (2 * var)
         own = -np.log(2 * LD(np.pi)) / 2 + np.log(t["d"][i]) / 2 - t["alpha"][i] ** 2 / (2 * t["d"][i])
         assert abs(float(own - term)) <= TOL * max(1.0, abs(float(term)))
+
+
+@pytest.mark.parametrize("n,c,m,gap", CASES)
+def test_fisher_matches_the_longdouble_trace(oracle, n, c, m, gap):
+    """``fisher`` against ``1/2 tr(K^-1 dK_p K^-1 dK_q)`` over the oracle's gradient tensor and ``1^T K^-1 1``, and
+    ``factor_terms`` against the log-likelihood of the longdouble factorisation."""
+    x, kernel, spec, K, ou = _case(n, c, m, gap)
+    L = hiprec.chol_ld(K)
+    Kinv = hiprec.solve_ld(L, np.eye(n))
+    dK = oracle.gradient_general(spec, [1, 1], x[:, None], x[:, None]).astype(LD)
+    KdK = [Kinv @ dK[:, :, p] for p in range(2)]
+    F_ref = np.zeros((3, 3), dtype=LD)
+    F_ref[0, 0] = np.sum(Kinv)
+    scale = np.zeros((3, 3), dtype=LD)
+    scale[0, 0] = np.sum(np.abs(Kinv))
+    for p in range(2):
+        for q in range(2):
+            F_ref[1 + p, 1 + q] = np.sum(KdK[p] * KdK[q].T) / 2
+            scale[1 + p, 1 + q] = np.sum(np.abs(KdK[p]) * np.abs(KdK[q].T)) / 2
+    F = ou.fisher()
+    assert np.all(np.abs(F - F_ref) <= TOL * scale), (F, F_ref)
+    assert np.all(F[0, 1:] == 0) and np.all(F[1:, 0] == 0)
+    assert np.array_equal(ou.fisher(mean=False), F[1:, 1:])
+    assert F[1, 1] == LD(n) / 2
+    assert abs(float(F[1, 2] - ou.trace_kinv_d() / 4)) <= TOL * float(scale[1, 2])
+
+    r = np.sin(x / np.sqrt(m)) + 0.5
+    ll_ref = -(r.astype(LD) @ hiprec.solve_ld(L, r.astype(LD)) + hiprec.logdet_ld(L) + n * np.log(2 * LD(np.pi))) / 2
+    ll = np.sum(ou.factor_terms(r))
+    assert abs(float(ll - ll_ref)) <= TOL * float(np.sum(np.abs(ou.factor_terms(r))))
+
+
+# Central differences in the scaled gaps, extrapolated twice (truncation O(h^6)): the rounding of the factor terms over
+# the step, ~1e-19 / FD_STEP, limits them (largest measured: 4.2e-14, the widely spaced case, where scale is smallest)
+FD_STEP = 1e-3
+FD_TOL = 5e-13
+
+
+@pytest.mark.parametrize("n,c,m,gap", CASES)
+def test_grad_x_matches_the_contraction_and_differences(oracle, n, c, m, gap):
+    """``grad_x`` against ``sum_j (alpha alpha^T - K^-1)_ij dk_ij/dx_i`` with the oracle's x-gradient and the
+    longdouble K^-1, and against central differences of the log-likelihood in each x_i (through ``factor_terms``,
+    whose sum is pinned to the factorisation's log-likelihood above); its scale bounds the contraction's terms."""
+    x, kernel, spec, K, ou = _case(n, c, m, gap)
+    L = hiprec.chol_ld(K)
+    Kinv = hiprec.solve_ld(L, np.eye(n))
+    Kinv = (Kinv + Kinv.T) / 2
+    dkdx = oracle.x_gradient_general(spec, 1, x[:, None], x[:, None])[:, :, 0].astype(LD)
+    r = np.sin(x / np.sqrt(m)) + 0.1 * np.random.default_rng(n + 6).standard_normal(n)
+    alpha = Kinv @ r.astype(LD)
+    A = np.outer(alpha, alpha) - Kinv
+    dx_ref = np.sum(A * dkdx, axis=1)
+    bound = np.sum(np.abs(A) * np.abs(dkdx), axis=1)
+    dx, scale = ou.grad_x(r)
+    assert np.all(np.abs(dx - dx_ref) <= TOL * scale), float(np.max(np.abs(dx - dx_ref) / scale))
+    assert np.all(scale >= bound * (1 - TOL)), (scale, bound)
+    assert np.sum(scale) <= 4 * np.sum(bound), (np.sum(scale), np.sum(bound))
+    assert abs(float(np.sum(dx))) <= TOL * float(np.sum(scale))
+
+    # d t_j / d gap_j per factor, then dx_i = G_i - G_{i+1}
+    def diff(h):
+        eta = LD(h)  # a step of h length scales in every gap
+        return (ou.factor_terms(r, ou.delta + eta) - ou.factor_terms(r, ou.delta - eta)) / (2 * h * ou.ell)
+
+    def richardson(h):
+        return (4 * diff(h / 2) - diff(h)) / 3
+    G = (16 * richardson(FD_STEP / 2) - richardson(FD_STEP)) / 15
+    G[0] = 0
+    dx_fd = G.copy()
+    dx_fd[:-1] -= G[1:]
+    assert np.all(np.abs(dx - dx_fd) <= FD_TOL * scale), float(np.max(np.abs(dx - dx_fd) / scale))
 
 
 @pytest.mark.parametrize("n,c,m,gap", CASES)
